@@ -1,10 +1,11 @@
-"""Benchmark of the RoHM denoising hot path on B200 (contract: see the task brief / DESIGN.md "Measurement").
+"""Benchmark of the RoHM denoising hot path on H100 (see DESIGN.md "Measurement").
 
   python bench.py --gpus 1 --steps 3 --warmup 3            # one process, cuda:0, BASELINE configs[1] (the headline)
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W            # one rank per GPU, NCCL
   python bench.py --impl reference ...                     # the reference algorithm on the host CPU cores
   python bench.py --config {posenet,trajcontrol,pipeline,respaced100,lbs}   # the other BASELINE configs (one line each)
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as DIR/<name>.npy
 
 Workloads (BASELINE.json configs, per GPU; clips shard over ranks, weak scaling, one all-gather of final outputs per step):
   posenet      configs[1]  PoseNet denoiser, 32 clips x 145 frames (T = 144 motion frames, 145 tokens), 1000 DDPM steps
@@ -67,7 +68,8 @@ def read_peaks():
         d = json.load(open(p))
         return {"bf16_tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops")), "bf16_burst": d.get("bf16_tflops"),
                 "hbm_gbs": d.get("hbm_gbs"), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_tflops": 1400.0, "bf16_burst": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (dense bf16, HBM3), not measured; a power-limited card reaches less
+    return {"bf16_tflops": 989.0, "bf16_burst": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (not measured)"}
 
 
 class ClockSampler:
@@ -403,6 +405,18 @@ class Workload:
     def run(self, batch):
         return getattr(self, "_run_" + self.args.config)(batch)
 
+    def outputs(self):
+        """What the last resident step handed its caller, by name."""
+        out = {"output": self.last_out}
+        if self.args.config == "respaced100":
+            out["traj_output"] = self._traj_out
+        elif self.args.config == "pipeline":
+            recon = self._recon if isinstance(self._recon, dict) else {"recon": self._recon}
+            out.update({f"recon_{k}": v for k, v in recon.items() if torch.is_tensor(v)})
+        elif self.args.config == "lbs":
+            out = {"joints": self._joints, "vertices": self.last_out}
+        return out
+
     def h2d_bytes(self):
         return int(sum(v.numel() * v.element_size() for v in self.host_in.values()))
 
@@ -417,7 +431,11 @@ def main():
     ap.add_argument("--traj-steps", type=int, default=100, help="TrajNet diffusion steps of the pipeline config "
                     "(100 = every shipped RoHM config; 1000 = BASELINE's wording)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last timed step (all ranks' clips) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        raise SystemExit("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         run_reference_arm(args)
         return
@@ -441,7 +459,7 @@ def main():
     # lbs: the host reads the joints back; the 575 MB of vertices stay on the device (rendering / metrics consume them there)
     out_host = torch.empty(w.out_shape if args.config != "lbs" else [B, w.T, 22, 3], dtype=torch.float32).pin_memory()
     gathered = torch.empty([world * B] + list(w.out_shape[1:]), device=dev) if (distributed and args.config != "lbs") else None
-    flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=dev)  # 256 MiB > 126 MB L2
+    flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=dev)  # 256 MiB > 50 MB L2
     torch.manual_seed(1234 + rank)
 
     def barrier():
@@ -453,6 +471,7 @@ def main():
         out = w.run(w.dev_in)
         if gathered is not None:
             dist.all_gather_into_tensor(gathered, out)
+        w.last_out = gathered if gathered is not None else out  # what the caller of the sharded path receives
         return out
 
     def one_step_e2e():
@@ -490,6 +509,17 @@ def main():
         barrier()
     ms_per_step = maxreduce(ms_total) / args.steps
     value = world * B / (ms_per_step / 1000.0)
+    if args.dump_outputs:
+        arrays = w.outputs()
+        if distributed:  # every array over the whole batch, as the caller of the sharded path sees the output
+            def gather(t):
+                t = t.contiguous()
+                g = torch.empty([world * t.shape[0]] + list(t.shape[1:]), dtype=t.dtype, device=t.device)
+                dist.all_gather_into_tensor(g, t)
+                return g
+            arrays = {k: (v if k == "output" and gathered is not None else gather(v)) for k, v in arrays.items()}
+        if rank == 0:
+            dump_outputs(args.dump_outputs, arrays)
 
     one_step_e2e()
     barrier()
@@ -512,7 +542,7 @@ def main():
         line = {
             "metric": w.cfg["metric"], "value": value, "unit": "clips/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": None, "dtype": dtype, "data": "synthetic", "config": workload_config(args, world, "B200"),
+            "vs_baseline": None, "dtype": dtype, "data": "synthetic", "config": workload_config(args, world, torch.cuda.get_device_name(dev)),
             "clocks": clocks.summary(),
             "e2e": {"value": e2e_value, "unit": "clips/s", "h2d_bytes_per_step": w.h2d_bytes(), "d2h_bytes_per_step": d2h},
             "gpu_launches": args.steps * launches,
@@ -525,8 +555,34 @@ def main():
         dist.destroy_process_group()
 
 
+DUMP_MAX_ELEMS = 2 * 1024 * 1024  # per array; larger outputs are stored as a fixed, seeded sample
+DUMP_MAX_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(directory, arrays):
+    """Writes each array as <directory>/<name>.npy, float64 as float64 and everything else as float32.  An array of more
+    than DUMP_MAX_ELEMS elements is replaced by the DUMP_MAX_ELEMS elements of its flattened form at the sorted indices
+    numpy.random.default_rng(0).choice(size, DUMP_MAX_ELEMS, replace=False) draws, the same on every run.  The total is
+    checked against DUMP_MAX_BYTES before anything is written."""
+    out = {}
+    for name, t in arrays.items():
+        a = t.detach().cpu()
+        a = (a.double() if a.dtype == torch.float64 else a.float()).numpy()
+        if a.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))
+            a = a.reshape(-1)[idx]
+        out[name] = a
+    total = sum(a.nbytes for a in out.values())
+    if total > DUMP_MAX_BYTES:
+        raise SystemExit(f"--dump-outputs: {total} bytes of outputs exceed {DUMP_MAX_BYTES}")
+    os.makedirs(directory, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(directory, f"{name}.npy"), a)
+
+
 # -------------------------------------------------------------------------------------------------------------
-# per-config roofline objects (measured live with CUDA events; ncu traffic figures come from profiles/)
+# per-config roofline objects (measured live with CUDA events; DRAM traffic figures are read from profiles/<name> when such an
+# ncu capture is present, and reported as null otherwise)
 # -------------------------------------------------------------------------------------------------------------
 def _traffic(name):
     tp = os.path.join(ROOT, "profiles", name)
@@ -579,8 +635,8 @@ def posenet_roofline(w, peaks, ms_per_step, model=None, B=None, T=None):
     achieved_graph = flops / (graph_ms * share / 1000.0) / 1e12  # GEMM share of the graph time (no per-launch event overhead)
     prec = engine.precision
     passes = 1 if prec == 1 else 3
-    kernel_kind = {3: "tcgen05 kind::tf32 on TF32 hi/lo pairs, 3 products", 2: "tcgen05 kind::f16 on fp16 hi/lo pairs, 3 products",
-                   1: "tcgen05 kind::tf32, single pass"}[prec]
+    kernel_kind = {3: "wgmma .tf32 on TF32 hi/lo pairs, 3 products", 2: "wgmma .f16 on fp16 hi/lo pairs, 3 products",
+                   1: "wgmma .tf32, single pass"}[prec]
     pipe_peak = peaks["bf16_tflops"] if prec == 2 else peaks["bf16_tflops"] / 2.0
     traffic, traffic_src = _traffic("r2_gemm_traffic.json")
     if traffic is None:
@@ -589,11 +645,13 @@ def posenet_roofline(w, peaks, ms_per_step, model=None, B=None, T=None):
         "kernel": f"gemm kernels ({kernel_kind}), {cat_n['gemm']} launches per PoseNet forward",
         # achieved = algorithmic GEMM FLOPs / (GEMM share of the forward x forward time as it runs in the loop).  The share comes
         # from CUDA events around every launch (rohm_posenet_profile: serialised, no PDL overlap, ~4 us of event overhead per
-        # launch -- so only the SHARE is taken from it, which the ncu launch list under profiles/ reproduces); the forward time
+        # launch -- so only the SHARE is taken from it); the forward time
         # is the captured graph timed with events on the launching stream, warm L2.  The raw event-timed figure is kept below.
         "bound": "tensor", "achieved": achieved_graph, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
         "frac": achieved_graph / peaks["bf16_tflops"], "traffic": traffic,
-        "traffic_source": traffic_src, "traffic_note": "cold-cache ncu figure; inside the loop operands are L2 hits",
+        "traffic_source": traffic_src,
+        "traffic_note": ("cold-cache ncu figure; inside the loop operands are L2 hits" if traffic is not None
+                         else "not captured (no ncu traffic file under profiles/)"),
         "peak_source": peaks["source"] + ", sustained bf16",
         "algorithmic_flops_per_forward": flops, "avg_launch_us": 1000.0 * graph_ms * share / max(cat_n["gemm"], 1),
         "achieved_event_timed": achieved, "frac_event_timed": (achieved / peaks["bf16_tflops"]) if achieved else None,
@@ -629,7 +687,7 @@ def trajnet_roofline(w, peaks, model, B, T, control):
     achieved = flops / (fwd_ms / 1000.0) / 1e12
     traffic, src = _traffic("r2_trajnet_traffic.json")
     return {
-        "kernel": f"TrajNet{'+TrajControl' if control else ''} forward: conv-as-GEMM tcgen05 kernels (fp16 hi/lo pairs, 3 products) + "
+        "kernel": f"TrajNet{'+TrajControl' if control else ''} forward: conv-as-GEMM wgmma kernels (fp16 hi/lo pairs, 3 products) + "
                   f"GroupNorm/Mish, {eng.launches_per_forward} launches, one CUDA graph",
         "bound": "tensor", "achieved": achieved, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
         "frac": achieved / peaks["bf16_tflops"], "traffic": traffic, "traffic_source": src,
@@ -657,7 +715,7 @@ def lbs_roofline(w, peaks, body, B, T):
     achieved = frames * LBS_BYTES_PER_FRAME / (ms / 1000.0) / 1e9
     traffic, src = _traffic("r2_lbs_traffic.json")
     return {
-        "kernel": "SMPL-X LBS: repr->axis-angle, 55-joint FK, pose/shape blend (tcgen05 GEMM on fp16 pairs) + skinning",
+        "kernel": "SMPL-X LBS: repr->axis-angle, 55-joint FK, pose/shape blend (wgmma GEMM on fp16 pairs) + skinning",
         "bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
         "traffic": traffic, "traffic_source": src, "peak_source": peaks["source"] + ", STREAM-style copy",
         "algorithmic_bytes_per_frame": LBS_BYTES_PER_FRAME, "frames": frames, "call_ms": ms,

@@ -1,4 +1,4 @@
-/* rohm_b200 -- C ABI of the B200-native RoHM hot path.
+/* rohm_b200 -- C ABI of the H100-native RoHM hot path.
  *
  * The reference (sanweiliti/RoHM) is pure Python/PyTorch and has no FFI; its boundary is a set of Python symbols
  * (SURVEY.md 8b, layer A).  This header is layer B: the plain-C entry points the Python drop-in
@@ -31,7 +31,7 @@ typedef enum {
   ROHM_OK = 0,
   ROHM_ERR_INVALID = -1,   /* bad argument / unsupported shape */
   ROHM_ERR_CUDA = -2,      /* CUDA runtime or driver error */
-  ROHM_ERR_NO_DEVICE = -3, /* no sm_100 device */
+  ROHM_ERR_NO_DEVICE = -3, /* no sm_90 (H100) device */
   ROHM_ERR_STATE = -4      /* call order violated (e.g. forward before set_cond) */
 } rohm_status;
 

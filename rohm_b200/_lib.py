@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI library (include/rohm_b200.h -> rohm_b200/librohm_b200.so).
 
-The product path has no CPU fallback: if the library is missing or no sm_100 device is present, every entry point
+The product path has no CPU fallback: if the library is missing or no sm_90 (H100) device is present, every entry point
 raises ``RohmB200Error`` with the reason.  Importing this module never touches the GPU; the library is loaded on
 first use.
 """
@@ -123,7 +123,7 @@ def ctx(device_index):
         rc = lib.rohm_ctx_create(int(device_index), C.byref(out))
         if rc != ROHM_OK:
             raise RohmB200Error(f"rohm_ctx_create(device={device_index}) failed with status {rc}: "
-                                "an sm_100 (B200) device is required; there is no CPU fallback")
+                                "an sm_90 (H100) device is required; there is no CPU fallback")
         _ctx[device_index] = out
     return _ctx[device_index]
 

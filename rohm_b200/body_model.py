@@ -264,7 +264,7 @@ class BodyModel(nn.Module):
             if isinstance(val, torch.Tensor):
                 if val.numel() and bool(torch.count_nonzero(val)):
                     raise RohmB200Error(f"BodyModel.forward: {name} must be all zeros (RoHM's call convention); the "
-                                        "B200 kernels do not evaluate hands / jaw / eyes / expression")
+                                        "CUDA kernels do not evaluate hands / jaw / eyes / expression")
             elif val is not None:
                 raise RohmB200Error(f"BodyModel.forward: unsupported argument {name}={val!r}")
         N = global_orient.shape[0]

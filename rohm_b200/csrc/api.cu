@@ -13,7 +13,7 @@ extern "C" int rohm_ctx_create(int device, rohm_ctx** out) {
   if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0 || device < 0 || device >= count) return ROHM_ERR_NO_DEVICE;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return ROHM_ERR_CUDA;
-  if (prop.major != 10) return ROHM_ERR_NO_DEVICE;  // kernels are sm_100a only
+  if (prop.major != 9 || prop.minor != 0) return ROHM_ERR_NO_DEVICE;  // kernels are sm_90a only
   rohm_ctx* ctx = new (std::nothrow) rohm_ctx();
   if (ctx == nullptr) return ROHM_ERR_INVALID;
   ctx->device = device;

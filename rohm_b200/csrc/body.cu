@@ -695,8 +695,8 @@ extern "C" int rohm_body_create(rohm_ctx* ctx, const float* v_template, const fl
     bd->a_frame_stride = round_up(F, 128);  // whole 128-frame row tiles: the epilogue's bulk copies never leave a row
     bd->A = bd->pool.floats(bd->a_frame_stride * kJ * 12);
     bd->feat_h = bd->pool.floats(F * kBlendK), bd->feat_l = bd->pool.floats(F * kBlendK);
-    // v_posed lives only for one chunk of kLbsChunk frames (48 MB): the blend GEMM writes it and the skinning kernel reads it
-    // back while it is still in the 126 MB L2, so the 2 x 531 MB round trip of a whole-batch intermediate never reaches HBM
+    // two-kernel path: v_posed lives for one chunk of frames at a time (the blend GEMM writes it, the skinning kernel reads
+    // it back); a chunk small enough for the 50 MB L2 (ROHM_B200_LBS_CHUNK=384: 48 MB) keeps that round trip out of HBM
     if (const char* env = getenv("ROHM_B200_LBS_CHUNK")) {  // developer switch: frames per chunk (multiple of 128)
       const long v = atol(env);
       if (v >= 128 && v % 128 == 0) bd->chunk = v;
@@ -815,8 +815,7 @@ extern "C" int rohm_body_create(rohm_ctx* ctx, const float* v_template, const fl
         k = GemmParams{};
         // The tensor maps end at the last live K column (200 -> 208: the rest of the fourth K block is zero-filled by TMA without
         // being read: 19 % less L2 -> SM operand traffic).  ROHM_B200_LBS_MULTICAST=1 additionally shares the A tile of a row
-        // stripe between the two CTAs of a pair; measured on B200 neither moves the launch (442 vs 434 us for 4576 frames): it is
-        // bound by the epilogue's load / store instruction count (4-byte accesses), not by operand traffic.
+        // stripe between the two CTAs of a pair.
         constexpr int kLiveK = (kPoseFeat + kBetas + 1 + 15) / 16 * 16;
         int rs = make_tmap_2d(&k.a_hi[0], bd->feat_h, F, kLiveK, kBlendK, kGemmBlockM, 1, bd->kind);
         rs |= make_tmap_2d(&k.a_lo[0], bd->feat_l, F, kLiveK, kBlendK, kGemmBlockM, 1, bd->kind);
@@ -896,7 +895,7 @@ extern "C" int rohm_body_forward(rohm_body* bd, const float* global_orient, cons
       verts ? bd->feat_l : nullptr, bd->kind == kKindF16 ? 1 : 0);
   ROHM_CUDA(ctx, cudaGetLastError());
   if (verts && bd->fused_lbs) {
-    // one launch: blend GEMM with the skinning epilogue (gemm.cu, EPI 4); v_posed stays in TMEM / registers
+    // one launch: blend GEMM with the skinning epilogue (gemm.cu, EPI 4); v_posed stays in registers / shared memory
     GemmParams g = bd->g_skin;
     g.M = static_cast<int>(N);
     g.out = vertices;
@@ -934,7 +933,7 @@ extern "C" int rohm_body_forward(rohm_body* bd, const float* global_orient, cons
     const int vblocks = (bd->V + 255) / 256;
     int occ = 0;  // resident CTAs per SM (registers / the 42 KB of shared memory decide)
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, skin_kernel, 256, 0) != cudaSuccess || occ < 1) occ = 3;
-    const int skin_y = std::max(1, (ctx->sm_count > 0 ? ctx->sm_count : 148) * occ / vblocks);  // one full wave
+    const int skin_y = std::max(1, (ctx->sm_count > 0 ? ctx->sm_count : 132) * occ / vblocks);  // one full wave
     const int64_t kChunk = bd->chunk;
     const int64_t chunks = (N + kChunk - 1) / kChunk;
     const bool overlap = bd->skin_stream != nullptr && chunks > 1;

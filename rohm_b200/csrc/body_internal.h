@@ -37,8 +37,7 @@ struct rohm_body {
   float* skin_w = nullptr;
   // full LBS pipeline: v_posed double buffer (one chunk each), second stream for the skinning kernels
   int64_t vposed_stride = 0;
-  // frames per chunk.  Measured on B200 (32 x 143 frames): chunking v_posed through L2 (384-frame chunks, with or without the
-  // second stream) is not faster than one pass (0.99 vs 0.85 ms): the skinning kernel is issue-bound, not HBM-bound.
+  // frames per chunk (ROHM_B200_LBS_CHUNK; the default is one pass over the batch)
   int64_t chunk = 4608;
   CUtensorMap st_out_b{};
   cudaStream_t skin_stream = nullptr;

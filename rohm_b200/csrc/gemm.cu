@@ -1,4 +1,4 @@
-// tcgen05 / TMA implementation of the segmented-A hi/lo-pair GEMM declared in gemm.cuh.
+// wgmma / TMA implementation of the segmented-A hi/lo-pair GEMM declared in gemm.cuh.
 #include "gemm.cuh"
 #include "ptx.cuh"
 
@@ -12,9 +12,11 @@ namespace rohm {
 
 namespace {
 
-constexpr int kEpiWarps = 8;
-constexpr int kThreads = 32 * (2 + kEpiWarps);
-constexpr int kSmemBudget = 192 * 1024;  // operand ring budget (BLOCK_N = 128, PASSES = 3: 6 x 32 KB or 3 x 64 KB)
+constexpr int kEpiWarps = 8;  // the two MMA warpgroups, which also run the epilogue
+constexpr int kFirstEpiWarp = 4;
+constexpr int kThreads = 32 * (kFirstEpiWarp + kEpiWarps);  // warpgroup 0: TMA producer (one lane); 1, 2: MMA + epilogue
+constexpr int kSmemLimit = 227 * 1024;  // H100: dynamic + static shared memory of one block
+constexpr int kStaticSmemReserve = 8 * 1024;  // barriers, per-column vectors, skinning tables
 constexpr int kEpiTileFloats = 32 * 32;   // per-epilogue-warp staging tile (32 x 32, XOR-swizzled columns): coalesced stores
 // fused skinning epilogue (EPI 4): one 128 x 96 fp32 staging tile for the whole CTA.  Pitch 100 floats: the 16-byte
 // row-per-thread writes (8 lanes per wavefront hit 8 distinct 16-byte bank groups: 25 r mod 8) and the 4-byte row-contiguous
@@ -24,27 +26,45 @@ constexpr int kSkinStageBytes = kGemmBlockM * kSkinPitch * 4;
 
 template <int BLOCK_N, int PASSES>
 struct TileCfg {
-  static constexpr int kABytes = kGemmBlockM * kGemmBlockK * 4;  // 16 KB
+  static constexpr int kABytes = kGemmBlockM * kGemmBlockK * 4;
   static constexpr int kBBytes = BLOCK_N * kGemmBlockK * 4;
   static constexpr int kSplit = (PASSES == 3) ? 2 : 1;
   static constexpr int kStageBytes = kSplit * (kABytes + kBBytes);
-  static constexpr int kStagesRaw = kSmemBudget / kStageBytes;
+  // The finished accumulator tile goes registers -> shared memory (fp32, 128 x BLOCK_N, pitch BLOCK_N + 4: the fragment
+  // writes and the row-per-thread 16-byte reads of the epilogue are at most 2-way conflicted) -> one row per thread.
+  static constexpr int kAccPitch = BLOCK_N + 4;
+  static constexpr int kAccBytes = kGemmBlockM * kAccPitch * 4;
+  // the epilogue staging area: per-warp 32 x 32 tiles, or (BLOCK_N = 96) the skinning epilogue's CTA-wide tile
+  static constexpr int kEpiBytes =
+      BLOCK_N == 96 && kSkinStageBytes > kEpiWarps * kEpiTileFloats * 4 ? kSkinStageBytes : kEpiWarps * kEpiTileFloats * 4;
+  static constexpr int kStagesRaw = (kSmemLimit - kStaticSmemReserve - 1024 - kAccBytes - kEpiBytes) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 10 ? 10 : kStagesRaw;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + kEpiWarps * kEpiTileFloats * 4;
-  // PASSES == 3 keeps two accumulators per stage: columns [0, BLOCK_N) take the leading hi*hi products, columns
-  // [BLOCK_N, 2*BLOCK_N) the two small cross terms.  The tensor core truncates when it adds into the
-  // accumulator, so keeping the ~2^-11-sized terms out of the big sum cuts the rounding count of the main
-  // accumulator by 3x (measured: error grows linearly with the number of accumulating MMAs).
-  static constexpr int kAccCols = (PASSES == 3 ? 2 : 1) * BLOCK_N;
-  // two accumulator stages: the epilogue drains tile i while the MMA warp already accumulates tile i+1
-  static constexpr int kAccStages = 2;
-  static constexpr int kTmemNeed = kAccStages * kAccCols;
-  static constexpr uint32_t kTmemCols = kTmemNeed <= 32 ? 32 : kTmemNeed <= 64 ? 64 : kTmemNeed <= 128 ? 128 : kTmemNeed <= 256 ? 256 : 512;
-  static_assert(kTmemNeed <= 512, "accumulators exceed TMEM");
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + kAccBytes + kEpiWarps * kEpiTileFloats * 4;
+  // PASSES == 3 keeps two register accumulators: one takes the leading hi*hi products, the other the two small cross
+  // terms.  The tensor core truncates when it adds into the accumulator, so keeping the ~2^-11-sized terms out of the big
+  // sum cuts the rounding count of the main accumulator by 3x.  They are added once, when the tile leaves the registers.
+  static constexpr int kAccRegs = BLOCK_N / 2;  // per thread and accumulator: m64 x BLOCK_N over a warpgroup
   static_assert(kStages >= 2, "need at least a double buffer");
-  static_assert(BLOCK_N % 16 == 0 && BLOCK_N >= 16 && BLOCK_N <= 256, "UMMA N constraint for M=128");
-  static_assert(BLOCK_N % 32 == 0, "epilogue walks TMEM in 32-column chunks");
+  static_assert(BLOCK_N % 32 == 0 && BLOCK_N >= 32 && BLOCK_N <= 128, "wgmma N and the epilogue's 32-column chunks");
 };
+
+// One wgmma step of the operand kind on an m64 x BLOCK_N accumulator.
+template <int KIND, int R>
+__device__ __forceinline__ void mma_step(float (&d)[R], uint64_t a, uint64_t b) {
+  if constexpr (KIND == kKindF16) ptx::wgmma_f16(d, a, b);
+  else ptx::wgmma_tf32(d, a, b);
+}
+
+// N consecutive accumulator columns of one row out of the shared-memory accumulator tile
+template <int PITCH, int N>
+__device__ __forceinline__ void acc_load(const float* acc, int row, int col, float (&v)[N]) {
+  const float4* src = reinterpret_cast<const float4*>(acc + row * PITCH + col);
+#pragma unroll
+  for (int j = 0; j < N / 4; ++j) {
+    const float4 t = src[j];
+    v[4 * j] = t.x, v[4 * j + 1] = t.y, v[4 * j + 2] = t.z, v[4 * j + 3] = t.w;
+  }
+}
 
 __device__ __forceinline__ void stamp(const GemmParams& p, int slot) {
   if (p.debug_ts != nullptr && blockIdx.x == 0) {
@@ -213,14 +233,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t full_bar[Cfg::kStages];
   __shared__ uint64_t empty_bar[Cfg::kStages];
-  __shared__ uint64_t tmem_full_bar[Cfg::kAccStages];
-  __shared__ uint64_t tmem_empty_bar[Cfg::kAccStages];
-  __shared__ uint32_t tmem_base_smem;
   // Epilogue parameters are copied from the (3 KB, tensor-map dominated) kernel parameter block into shared memory
-  // once: reading them late from the constant bank cost ~0.7 us per first touch (measured with %globaltimer stamps).
+  // once: reading them late from the constant bank is slow on first touch.
   __shared__ EpiParams epi_s;
-  // per-column vectors of the current tile (single-buffered, see the staging block of the epilogue; 227 KB are in use, every
-  // 512 bytes count): bias; LayerNorm folding: c_n of a consumer GEMM, or (EPI 3) gamma | beta of the residual's LayerNorm
+  // per-column vectors of the current tile (single-buffered, see the staging block of the epilogue): bias; LayerNorm
+  // folding: c_n of a consumer GEMM, or (EPI 3) gamma | beta of the residual's LayerNorm
   __shared__ __align__(16) float bias_s[BLOCK_N];
   __shared__ __align__(16) float corr_s[BLOCK_N];
   __shared__ __align__(16) float beta_s[EPI == 3 ? BLOCK_N : 4];
@@ -230,9 +247,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
   __shared__ int skin_bone_s[EPI == 4 ? 2 : 1][EPI == 4 ? kSkinTileBones : 1];
   __shared__ int skin_nb_s[2];
 
-  // SWIZZLE_128B tiles need 1024-byte alignment.
+  // 128B-swizzled tiles need 1024-byte alignment.
   const uint32_t raw_addr = ptx::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
+  float* const acc_s = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint8_t* const epi_smem = smem + Cfg::kStages * Cfg::kStageBytes + Cfg::kAccBytes;
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -258,20 +277,17 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
     }
     for (int i = 0; i < Cfg::kStages; ++i) {
       ptx::mbar_init(&full_bar[i], 1);
-      ptx::mbar_init(&empty_bar[i], p.multicast_a ? 2 : 1);  // multicast: the slot is refilled by both CTAs of the pair
-    }
-    for (int i = 0; i < Cfg::kAccStages; ++i) {
-      ptx::mbar_init(&tmem_full_bar[i], 1);
-      ptx::mbar_init(&tmem_empty_bar[i], kEpiWarps);
+      // one arrival per MMA warpgroup; multicast: the slot is refilled by both CTAs of the pair, so the warpgroups of both
+      // CTAs release it
+      ptx::mbar_init(&empty_bar[i], p.multicast_a ? 4 : 2);
     }
     if (EPI == 3)
       for (int i = 0; i < kEpiWarps; ++i) ptx::mbar_init(&res_bar[i], 1);
     ptx::fence_barrier_init();
   }
   // The B operand is a weight matrix that no kernel of the chain writes: the producer thread puts the B tiles of the first
-  // pipeline stages in flight right after it has initialised the barriers -- BEFORE the CTA-wide setup barrier (TMEM
-  // allocation, epilogue parameters) and before it waits for the previous grid -- so the pipeline fill (~1 us, tensor-map
-  // fetch included) overlaps both the setup and that grid's tail.
+  // pipeline stages in flight right after it has initialised the barriers -- BEFORE the CTA-wide setup barrier and before
+  // it waits for the previous grid -- so the pipeline fill overlaps both the setup and that grid's tail.
   int prefetched = 0;
   if (warp_idx == 0 && lane == 0 && !p.multicast_a && static_cast<int>(blockIdx.x) < num_work) {
     const int tile0 = static_cast<int>(blockIdx.x) / S;
@@ -287,10 +303,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         ptx::tma_load_2d(st + 2 * Cfg::kABytes + Cfg::kBBytes, &p.b_lo, &full_bar[i], (it_b + i) * kElemK, n0);
     }
   }
-  if (warp_idx == 1) {
-    ptx::tmem_alloc<Cfg::kTmemCols>(&tmem_base_smem);
-  }
-  if (warp_idx == 2 && lane == 0) {
+  if (warp_idx == kFirstEpiWarp && lane == 0) {
     epi_s.bias = p.bias, epi_s.residual = p.residual, epi_s.ldr = p.ldr, epi_s.out = p.out, epi_s.ldo = p.ldo;
     epi_s.out_hi = p.out_hi, epi_s.out_lo = p.out_lo, epi_s.lds = p.lds, epi_s.act = p.act, epi_s.M = p.M, epi_s.N = p.N;
     epi_s.out_row_mul = p.out_row_mul, epi_s.out_row_add = p.out_row_add, epi_s.clip_rows = p.clip_rows;
@@ -307,11 +320,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
       ptx::prefetch_tmap(&p.st_lo);
     }
   }
-  ptx::tc_fence_before_sync();
   __syncthreads();
   if (p.multicast_a) ptx::cluster_sync_all();  // the partner's barriers are initialised before anything is sent to them
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_smem;
 
   if (threadIdx.x == 0) stamp(p, 1);
   // Programmatic dependent launch: let the next kernel of the chain become resident as soon as SMs free up (its
@@ -320,9 +330,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
   ptx::pdl_launch_dependents();
   ptx::pdl_wait_prior_grid();
 
-  if (warp_idx == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (warp_idx < kFirstEpiWarp) {
+    // ===================== TMA producer (warpgroup 0, one lane) =====================
+    ptx::setmaxnreg_dec<40>();
+    if (warp_idx == 0 && lane == 0) {
       int it = 0, stage = 0;
       uint32_t phase = 0;
       for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
@@ -374,78 +385,89 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         }
       }
     }
-  } else if (warp_idx == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = ptx::make_idesc(KIND == kKindF16 ? /*F16*/ 0 : /*TF32*/ 2, kGemmBlockM, BLOCK_N);
-      constexpr uint32_t idesc_wide = ptx::make_idesc(KIND == kKindF16 ? 0 : 2, kGemmBlockM, BLOCK_N <= 128 ? 2 * BLOCK_N : BLOCK_N);
-      auto mma = [](uint32_t d, uint64_t a, uint64_t b, uint32_t id, uint32_t accumulate) {
-        if (KIND == kKindF16) ptx::mma_f16_ss(d, a, b, id, accumulate);
-        else ptx::mma_tf32_ss(d, a, b, id, accumulate);
-      };
-      int it = 0, tcount = 0, stage = 0;
-      uint32_t phase = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++tcount) {
-        const int acc_stage = tcount % Cfg::kAccStages;
-        const uint32_t acc_phase = (tcount / Cfg::kAccStages) & 1;
-        ptx::mbar_wait(&tmem_empty_bar[acc_stage], acc_phase ^ 1);  // epilogue has drained this accumulator
-        ptx::tc_fence_after_sync();
-        const uint32_t acc = tmem_base + static_cast<uint32_t>(acc_stage * Cfg::kAccCols);
-        const int it_b = (w % S) * per_split;
-        const int n_it = (total_iters < it_b + per_split ? total_iters : it_b + per_split) - it_b;
-        for (int ki = 0; ki < n_it; ++ki, ++it) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          if (it == 0) stamp(p, 3);
-          ptx::tc_fence_after_sync();
-          const uint32_t st = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint64_t a_hi = ptx::make_desc_kmajor<kGemmBlockK * 4>(st);
-          const uint64_t b_hi = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + Cfg::kSplit * Cfg::kABytes);
-          const uint64_t a_lo = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + Cfg::kABytes);
-          const uint64_t b_lo = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + 2 * Cfg::kABytes + Cfg::kBBytes);
-#pragma unroll
-          for (int k = 0; k < kGemmBlockK / 8; ++k) {
-            // advancing K by one instruction (8 fp32 / 16 fp16 = 32 bytes) inside the swizzle span: +2 in the (>>4)
-            // address field
-            const uint64_t koff = static_cast<uint64_t>(k * 2);
-            const uint32_t first = (ki > 0 || k > 0) ? 1u : 0u;
-            if (PASSES == 3 && BLOCK_N <= 128) {
-              // B_hi and B_lo are adjacent in the stage, and so are the two accumulators in TMEM: A_hi x [B_hi ; B_lo] is ONE
-              // instruction of twice the width (columns [0, BLOCK_N) = hi*hi, [BLOCK_N, 2 BLOCK_N) = hi*lo), which reads A_hi
-              // from shared memory once instead of twice.  The main loop is bound by the shared-memory port (TMA fill + operand
-              // reads, 128 B/clk), not by the tensor pipe: 20 KB instead of 24 KB of operand reads per k-step.
-              mma(acc, a_hi + koff, b_hi + koff, idesc_wide, first);
-              mma(acc + BLOCK_N, a_lo + koff, b_hi + koff, idesc, 1u);
-            } else if (PASSES == 3) {
-              mma(acc + BLOCK_N, a_lo + koff, b_hi + koff, idesc, first);
-              mma(acc + BLOCK_N, a_hi + koff, b_lo + koff, idesc, 1u);
-              mma(acc, a_hi + koff, b_hi + koff, idesc, first);
-            } else {
-              mma(acc, a_hi + koff, b_hi + koff, idesc, first);
-            }
-          }
-          // frees the smem slot once these MMAs have read it (multicast: in both CTAs of the pair, which both write into it)
-          if (p.multicast_a) ptx::mma_commit_multicast(&empty_bar[stage], 0x3);
-          else ptx::mma_commit(&empty_bar[stage]);
-          if (++stage == Cfg::kStages) stage = 0, phase ^= 1;
-        }
-        ptx::mma_commit(&tmem_full_bar[acc_stage]);  // accumulator complete
-        if (tcount == 0) stamp(p, 4);
-        stamp(p, 12);  // last write wins: all MMAs of this CTA issued
-        if (tcount < 8) stamp(p, 16 + tcount);
-      }
-    }
   } else {
-    // ===================== epilogue (warps 2..9) =====================
-    // TMEM lane quarter = warp_idx % 4 (hardware rule); the two warps sharing a quarter alternate 32-column chunks.
-    // Data path: TMEM -> registers (one row per thread) -> bias / activation / row mask / GroupNorm sums -> 32x32
-    // staging tile in shared memory -> re-read with 8 lanes per row -> residual add -> 128-byte-coalesced float4
-    // stores (fp32 and/or TF32 hi/lo).  The row-per-thread layout the TMEM load dictates would make every store
-    // instruction touch 32 different rows (measured: 11 us per 128x128 tile with three outputs).
+    // ===================== MMA + epilogue (warpgroups 1, 2) =====================
+    ptx::setmaxnreg_inc<232>();
+    const int ew = warp_idx - kFirstEpiWarp;  // epilogue warp 0..7
+    // MMA: warpgroup `half` computes rows [64 half, 64 half + 64) of the tile.  Epilogue: warp ew owns rows
+    // [32 q, 32 q + 32), one per lane, and the 32-column chunks half * 32 + 64 j.
+    const int q = ew & 3;
+    const int half = ew >> 2;
+    int mma_stage = 0;
+    uint32_t mma_phase = 0;
+    // Runs the K loop of work item w into registers, then publishes the finished tile in acc_s (a barrier over the two
+    // warpgroups: afterwards every epilogue thread may read any row).  The caller guarantees that no thread still reads
+    // acc_s for the previous tile.
+    auto mma_tile = [&](int w) {
+      float dm[Cfg::kAccRegs];
+      float dc[PASSES == 3 ? Cfg::kAccRegs : 1];
+#pragma unroll
+      for (int i = 0; i < Cfg::kAccRegs; ++i) dm[i] = 0.0f;
+#pragma unroll
+      for (int i = 0; i < (PASSES == 3 ? Cfg::kAccRegs : 1); ++i) dc[i] = 0.0f;
+      const int it_b = (w % S) * per_split;
+      const int n_it = (total_iters < it_b + per_split ? total_iters : it_b + per_split) - it_b;
+      const bool signaller = (threadIdx.x & 127) == 0;
+      auto release = [&](int stg) {
+        if (!signaller) return;
+        if (p.multicast_a) {
+          ptx::mbar_arrive_cluster(&empty_bar[stg], 0);
+          ptx::mbar_arrive_cluster(&empty_bar[stg], 1);
+        } else {
+          ptx::mbar_arrive(&empty_bar[stg]);
+        }
+      };
+      int prev = -1;
+      for (int ki = 0; ki < n_it; ++ki) {
+        ptx::mbar_wait(&full_bar[mma_stage], mma_phase);
+        if (ki == 0 && w == static_cast<int>(blockIdx.x)) stamp(p, 3);
+        const uint32_t st = ptx::smem_u32(smem + mma_stage * Cfg::kStageBytes);
+        const uint32_t a_off = static_cast<uint32_t>(half * (Cfg::kABytes / 2));  // this warpgroup's 64 rows
+        const uint64_t a_hi = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + a_off);
+        const uint64_t b_hi = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + Cfg::kSplit * Cfg::kABytes);
+        const uint64_t a_lo = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + Cfg::kABytes + a_off);
+        const uint64_t b_lo = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + 2 * Cfg::kABytes + Cfg::kBBytes);
+        ptx::wgmma_fence_regs(dm);
+        if (PASSES == 3) ptx::wgmma_fence_regs(dc);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kGemmBlockK / 8; ++k) {
+          // advancing K by one instruction (8 fp32 / 16 fp16 = 32 bytes) inside the swizzle span: +2 in the (>>4) address field
+          const uint64_t koff = static_cast<uint64_t>(k * 2);
+          mma_step<KIND>(dm, a_hi + koff, b_hi + koff);
+          if constexpr (PASSES == 3) {
+            mma_step<KIND>(dc, a_lo + koff, b_hi + koff);
+            mma_step<KIND>(dc, a_hi + koff, b_lo + koff);
+          }
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_fence_regs(dm);
+        if (PASSES == 3) ptx::wgmma_fence_regs(dc);
+        // keep this stage's MMAs in flight; the previous stage's have completed, so its slot goes back to the producer
+        ptx::wgmma_wait<1>();
+        if (prev >= 0) release(prev);
+        prev = mma_stage;
+        if (++mma_stage == Cfg::kStages) mma_stage = 0, mma_phase ^= 1;
+      }
+      ptx::wgmma_wait<0>();
+      ptx::wgmma_fence_regs(dm);
+      if (PASSES == 3) ptx::wgmma_fence_regs(dc);
+      if (prev >= 0) release(prev);
+      // fragment -> acc_s (the two accumulators of PASSES == 3 are added here)
+      const int r0 = half * 64 + q * 16 + (lane >> 2);
+      const int cc = 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        float v0 = dm[4 * j], v1 = dm[4 * j + 1], v2 = dm[4 * j + 2], v3 = dm[4 * j + 3];
+        if (PASSES == 3) v0 += dc[4 * j], v1 += dc[4 * j + 1], v2 += dc[4 * j + 2], v3 += dc[4 * j + 3];
+        *reinterpret_cast<float2*>(acc_s + r0 * Cfg::kAccPitch + 8 * j + cc) = make_float2(v0, v1);
+        *reinterpret_cast<float2*>(acc_s + (r0 + 8) * Cfg::kAccPitch + 8 * j + cc) = make_float2(v2, v3);
+      }
+      asm volatile("bar.sync 3, %0;" ::"n"(kEpiWarps * 32));
+    };
     const EpiParams e = epi_s;  // registers
-    const int q = warp_idx & 3;
-    const int half = (warp_idx - 2) >> 2;
     const bool vec_ok = ((e.N & 3) == 0);
-    float* tile = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes) + (warp_idx - 2) * kEpiTileFloats;
+    float* tile = reinterpret_cast<float*>(epi_smem) + ew * kEpiTileFloats;
     const int tr = lane >> 3, tc = (lane & 7) * 4;  // transposed mapping: rows tr, tr+4, ..., columns tc..tc+3
     int tcount = 0;
     if constexpr (EPI == 4) {
@@ -456,9 +478,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
       // requested right after that, so their L2 latency hides behind this tile's staging and stores.
       static_assert(BLOCK_N == 96 && PASSES == 3 && KIND == kKindF16, "skinning epilogue: 32 vertices x 3 per tile, fp16 pairs");
       constexpr int kSkinRegBones = 4;
-      const int i = (warp_idx - 2) * 32 + lane;
+      const int i = ew * 32 + lane;
       float4 sk[kSkinRegBones][3];
-      float* const stg = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
+      float* const stg = reinterpret_cast<float*>(epi_smem);
       auto fetch_tables = [&](int tile_n, float& w0, float& w1, int& bone, int& nbv) {
         const float* wsrc = p.skin_w + static_cast<int64_t>(tile_n) * (kSkinTileBones * 32);
         w0 = __ldg(wsrc + i), w1 = __ldg(wsrc + i + 256);
@@ -490,8 +512,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
       for (int tile_idx = blockIdx.x; tile_idx < num_tiles; tile_idx += gridDim.x, ++tcount, buf ^= 1) {
         const int m0 = (tile_idx / tiles_n) * kGemmBlockM;
         const int n0 = (tile_idx % tiles_n) * BLOCK_N;
-        const int acc_stage = tcount % Cfg::kAccStages;
-        const uint32_t acc_phase = (tcount / Cfg::kAccStages) & 1;
         const int m = m0 + q * 32 + lane;
         const int next = tile_idx + static_cast<int>(gridDim.x);
         const bool has_next = next < num_tiles;
@@ -499,9 +519,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         int nbone = 0, nnb = 0;
         if (has_next) fetch_tables(next % tiles_n, nw0, nw1, nbone, nnb);  // in flight during the accumulator wait and the compute
 
-        ptx::mbar_wait(&tmem_full_bar[acc_stage], acc_phase);
-        if (tcount == 1 && warp_idx == 2 && lane == 0) stamp(p, 5);
-        ptx::tc_fence_after_sync();
+        mma_tile(tile_idx);  // the previous tile's reads of acc_s are behind the bar.sync 1 of its compute phase
+        if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 5);
         // verts = sum_b w[v][b] (R_b v_posed + t_b).  Within a 32-vertex tile nearly every (vertex, bone) pair carries weight
         // (vertices are indexed by body part), so every vertex is updated per bone: no branches, 12 FMAs per (vertex, bone).
         // Two rounds of 8 vertices keep the live registers (transforms 48 + v_posed 24 + results 48) under the 168 available.
@@ -514,25 +533,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         for (int h2 = 0; h2 < 2; ++h2) {
           float vp[24];
           {
-            uint32_t a0[16], a1[8], c0[16], c1[8];
-            const uint32_t taddr = tmem_base + static_cast<uint32_t>(acc_stage * Cfg::kAccCols) +
-                                   (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(48 * half + 24 * h2);
-            ptx::tmem_ld_32x16(taddr, a0);
-            ptx::tmem_ld_32x8(taddr + 16, a1);
-            ptx::tmem_ld_32x16(taddr + BLOCK_N, c0);
-            ptx::tmem_ld_32x8(taddr + BLOCK_N + 16, c1);
-            ptx::tmem_ld_wait();
+            acc_load<Cfg::kAccPitch>(acc_s, q * 32 + lane, 48 * half + 24 * h2, vp);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) vp[j] = (__uint_as_float(a0[j]) + __uint_as_float(c0[j])) * e.acc_scale;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) vp[16 + j] = (__uint_as_float(a1[j]) + __uint_as_float(c1[j])) * e.acc_scale;
+            for (int j = 0; j < 24; ++j) vp[j] *= e.acc_scale;
           }
-          if (h2 == 1) {  // the accumulator is drained: the MMA warp may start the tile after next
-            if (tcount == 1 && warp_idx == 2 && lane == 0) stamp(p, 8);
-            ptx::tc_fence_before_sync();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc_stage]);
-          }
+          if (h2 == 1 && tcount == 1 && ew == 0 && lane == 0) stamp(p, 8);
           auto apply_bone = [&](const float4& r0, const float4& r1, const float4& r2, const float* wrow) {
 #pragma unroll
             for (int g = 0; g < 2; ++g) {
@@ -564,10 +569,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
             }
           }
         }
-        if (tcount == 1 && warp_idx == 2 && lane == 0) stamp(p, 9);
+        if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 9);
         if (has_next) publish_tables(buf ^ 1, nw0, nw1, nbone, nnb);
         // TMA-store variant: the previous tile's bulk stores (issued by this thread) have finished reading the staging tile
-        if (e.tma_store && warp_idx == 2 && lane == 0) ptx::bulk_wait_read_all();
+        if (e.tma_store && ew == 0 && lane == 0) ptx::bulk_wait_read_all();
         // one barrier: the next tile's tables are visible, and every warp has finished storing the previous tile's rows out of
         // the staging tile that is overwritten below
         asm volatile("bar.sync 1, %0;" ::"n"(kEpiWarps * 32));
@@ -587,14 +592,14 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
           }
           ptx::fence_proxy_async();
           asm volatile("bar.sync 2, %0;" ::"n"(kEpiWarps * 32));
-          if (tcount == 1 && warp_idx == 2 && lane == 0) stamp(p, 10);
-          if (warp_idx == 2 && lane == 0) {
+          if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 10);
+          if (ew == 0 && lane == 0) {
 #pragma unroll
             for (int j = 0; j < 3; ++j)
               if (n0 + 32 * j < e.N) ptx::tma_store_2d(&p.st_out, sb + j * (kGemmBlockM * 128), n0 + 32 * j, m0);
             ptx::bulk_commit();
           }
-          if (tcount == 1 && warp_idx == 2 && lane == 0) stamp(p, 11);
+          if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 11);
           continue;
         }
         // transpose through the CTA-wide staging tile: the output row pitch (3 V floats) is not a multiple of 16 bytes, so
@@ -605,9 +610,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
           for (int j = 0; j < 12; ++j) srow[j] = make_float4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
         }
         asm volatile("bar.sync 2, %0;" ::"n"(kEpiWarps * 32));
-        if (tcount == 1 && warp_idx == 2 && lane == 0) stamp(p, 10);
+        if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 10);
         {
-          const int w8 = warp_idx - 2;
+          const int w8 = ew;
 #pragma unroll 4
           for (int rr = 0; rr < kGemmBlockM / kEpiWarps; ++rr) {
             const int r = w8 * (kGemmBlockM / kEpiWarps) + rr;
@@ -622,7 +627,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
             }
           }
         }
-        if (tcount == 1 && warp_idx == 2 && lane == 0) stamp(p, 11);
+        if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 11);
       }
     }
     for (int wi = blockIdx.x; EPI != 4 && wi < num_work; wi += gridDim.x, ++tcount) {
@@ -631,8 +636,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
       const int split_rows = (wi - tile_idx * S) * (EPI == 2 ? p.split_row_stride : 0);
       const int m0 = (tile_idx / tiles_n) * kGemmBlockM;
       const int n0 = (tile_idx % tiles_n) * BLOCK_N;
-      const int acc_stage = tcount % Cfg::kAccStages;
-      const uint32_t acc_phase = (tcount / Cfg::kAccStages) & 1;
       const int m = m0 + q * 32 + lane;
       const bool row_ok = m < e.M;
       bool row_real = true;
@@ -644,10 +647,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
       const int64_t orow = static_cast<int64_t>(m) * e.out_row_mul + e.out_row_add + split_rows;
       const float bias_row = (e.bias != nullptr && e.bias_per_row && row_ok) ? __ldg(e.bias + m) : 0.0f;
 
-      // stage this tile's per-column vectors while the MMA warp is still accumulating.  Single-buffered: the first barrier
+      // stage this tile's per-column vectors before the main loop of the tile.  Single-buffered: the first barrier
       // keeps the writers off the vectors until every epilogue thread has finished the previous tile.
       {
-        const int i = (warp_idx - 2) * 32 + lane;
+        const int i = ew * 32 + lane;
         asm volatile("bar.sync 1, %0;" ::"n"(kEpiWarps * 32));
         if (i < BLOCK_N) {
           const bool col_ok = n0 + i < e.N;
@@ -673,8 +676,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         a_mean = mr.x, a_rstd = mr.y;
       }
       // LayerNorm folding, producer side: the residual tile (this thread: one row, 2 x 32 columns) arrives through TMA into
-      // the warp's staging tile -- with 225 KB of shared memory in use there is no L1, and per-thread 16-byte loads were
-      // measured to slow the operand stream by 40 % -- and is passed through the previous LayerNorm on the fly.
+      // the warp's staging tile -- nearly all of the shared memory is in use, so there is little L1 for per-thread loads --
+      // and is passed through the previous LayerNorm on the fly.
       float lnv[EPI == 3 ? 2 : 1][EPI == 3 ? 32 : 1];
       if constexpr (EPI == 3) {
         float r_mean = 0.0f, r_rstd = 1.0f;
@@ -683,7 +686,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
           r_mean = mr.x, r_rstd = mr.y;
         }
         uint8_t* tb = reinterpret_cast<uint8_t*>(tile);
-        uint64_t* rb = &res_bar[warp_idx - 2];
+        uint64_t* rb = &res_bar[ew];
 #pragma unroll
         for (int h2 = 0; h2 < 2; ++h2) {
           const int c0 = half * 32 + 64 * h2;
@@ -714,9 +717,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
           __syncwarp();
         }
       }
-      ptx::mbar_wait(&tmem_full_bar[acc_stage], acc_phase);
-      if (tcount == 0 && warp_idx == 2 && lane == 0) stamp(p, 5);
-      ptx::tc_fence_after_sync();
+      // the start-of-tile bar.sync 1 above keeps this tile's accumulator off acc_s until every thread has read the last one
+      mma_tile(wi);
+      if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 5);
 
       if constexpr (EPI == 3) {
         // ===== u = LN_prev(residual) + acc * 2^-s + bias, written in place as an fp16 pair + per-row partial statistics =====
@@ -726,26 +729,18 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
 #pragma unroll
         for (int h2 = 0; h2 < 2; ++h2) {
           const int c0 = half * 32 + 64 * h2;
-          uint32_t raw[32], raw2[32];
-          const uint32_t taddr = tmem_base + static_cast<uint32_t>(acc_stage * Cfg::kAccCols) +
-                                 (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(c0);
-          ptx::tmem_ld_32x32(taddr, raw);
-          ptx::tmem_ld_32x32(taddr + BLOCK_N, raw2);
-          ptx::tmem_ld_wait();
+          float raw[32];
+          acc_load<Cfg::kAccPitch>(acc_s, q * 32 + lane, c0, raw);
 #pragma unroll
           for (int j = 0; j < 32; j += 4) {
             const float4 b4 = *reinterpret_cast<const float4*>(&bias_s[c0 + j]);
-            v[h2][j] += fmaf(__uint_as_float(raw[j]) + __uint_as_float(raw2[j]), e.acc_scale, b4.x);
-            v[h2][j + 1] += fmaf(__uint_as_float(raw[j + 1]) + __uint_as_float(raw2[j + 1]), e.acc_scale, b4.y);
-            v[h2][j + 2] += fmaf(__uint_as_float(raw[j + 2]) + __uint_as_float(raw2[j + 2]), e.acc_scale, b4.z);
-            v[h2][j + 3] += fmaf(__uint_as_float(raw[j + 3]) + __uint_as_float(raw2[j + 3]), e.acc_scale, b4.w);
+            v[h2][j] += fmaf(raw[j], e.acc_scale, b4.x);
+            v[h2][j + 1] += fmaf(raw[j + 1], e.acc_scale, b4.y);
+            v[h2][j + 2] += fmaf(raw[j + 2], e.acc_scale, b4.z);
+            v[h2][j + 3] += fmaf(raw[j + 3], e.acc_scale, b4.w);
           }
         }
-        if (tcount == 0 && warp_idx == 2 && lane == 0) stamp(p, 8);
-        // the accumulator is drained: hand it back so that the MMA warp can start the next tile
-        ptx::tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc_stage]);
+        if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 8);
         uint8_t* tb = reinterpret_cast<uint8_t*>(tile);
         const bool group_full = (m0 + q * 32 + 32 <= e.M);
         auto store_chunk = [&](int h2) {
@@ -773,32 +768,21 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
           m2_i = fmaf(d0, d0, fmaf(d1, d1, m2_i));
         }
         if (row_ok) e.stats_out[static_cast<int64_t>(m) * 8 + tile_n * 2 + half] = make_float2(mean_i, m2_i);
-        if (tcount == 0 && warp_idx == 2 && lane == 0) stamp(p, 9);
+        if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 9);
         store_chunk(1);
-        if (tcount == 0 && warp_idx == 2 && lane == 0) stamp(p, 6);
+        if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 6);
         continue;
       }
 
 #pragma unroll 1
       for (int c0 = half * 32; c0 < BLOCK_N; c0 += 64) {
-        uint32_t raw[32], raw2[32];
-        const uint32_t taddr = tmem_base + static_cast<uint32_t>(acc_stage * Cfg::kAccCols) +
-                               (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(c0);
-        ptx::tmem_ld_32x32(taddr, raw);
-        if (PASSES == 3) ptx::tmem_ld_32x32(taddr + BLOCK_N, raw2);
         const int nb = n0 + c0;
         const bool full = vec_ok && (nb + 32 <= e.N);
         if (e.tma_store && full && (m0 + q * 32 + 32 <= e.M)) {
           // ---- TMA-store path: row-per-thread registers -> swizzled staging tile -> bulk tensor store ----
-          ptx::tmem_ld_wait();
           if (p.debug_flags & 1) continue;
           float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]);
-          if (PASSES == 3) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] += __uint_as_float(raw2[j]);
-          }
+          acc_load<Cfg::kAccPitch>(acc_s, q * 32 + lane, c0, v);
           if (KIND == kKindF16) {
 #pragma unroll
             for (int j = 0; j < 32; ++j) v[j] *= e.acc_scale;
@@ -878,7 +862,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
           }
           continue;
         }
-        // residual in the transposed (coalesced) layout: loads are issued before waiting on TMEM
+        // residual in the transposed (coalesced) layout
         float4 res[8];
         const bool use_res = e.residual != nullptr && full;
         if (use_res) {
@@ -891,15 +875,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
                   e.residual + (static_cast<int64_t>(mr) * e.out_row_mul + e.out_row_add) * e.ldr + nb + tc);
           }
         }
-        ptx::tmem_ld_wait();
-        if (tcount == 0 && warp_idx == 2 && lane == 0 && c0 == 0) stamp(p, 8);
+        if (tcount == 0 && ew == 0 && lane == 0 && c0 == 0) stamp(p, 8);
         float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]);
-        if (PASSES == 3) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += __uint_as_float(raw2[j]);
-        }
+        acc_load<Cfg::kAccPitch>(acc_s, q * 32 + lane, c0, v);
         if (KIND == kKindF16) {  // undo the power-of-two weight scale (exact)
 #pragma unroll
           for (int j = 0; j < 32; ++j) v[j] *= e.acc_scale;
@@ -920,7 +898,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
             }
           }
           // one warp-uniform branch per activation: a per-element switch compiles to ~3000 predicated-off
-          // instructions per chunk that are still issued when act == none (measured: 0.6 us per chunk)
+          // instructions per chunk that are still issued when act == none
           if (EPI == 0) {
           } else if (EPI == 1 || e.act == kActGelu) {
 #pragma unroll
@@ -947,7 +925,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         // ---- GroupNorm partial statistics over real rows ----
         if (!LEAN && e.gn_stats != nullptr) gn_partial_sums(v, e, nb, row_ok && row_real, clip, lane);
 
-        if (tcount == 0 && warp_idx == 2 && lane == 0 && c0 == 0) stamp(p, 9);
+        if (tcount == 0 && ew == 0 && lane == 0 && c0 == 0) stamp(p, 9);
         if (full) {
           // ---- coalesced path through the staging tile ----
           if (e.tma_store) {  // an earlier chunk's bulk store may still be reading the tile
@@ -957,7 +935,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
 #pragma unroll
           for (int j = 0; j < 32; ++j) tile[lane * 32 + (j ^ lane)] = v[j];  // column ^ row: conflict-free both ways
           __syncwarp();
-          if (tcount == 0 && warp_idx == 2 && lane == 0 && c0 == 0) stamp(p, 10);
+          if (tcount == 0 && ew == 0 && lane == 0 && c0 == 0) stamp(p, 10);
 #pragma unroll
           for (int rr = 0; rr < 8; ++rr) {
             const int r = rr * 4 + tr;
@@ -990,7 +968,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
             }
           }
           __syncwarp();
-          if (tcount == 0 && warp_idx == 2 && lane == 0 && c0 == 0) stamp(p, 11);
+          if (tcount == 0 && ew == 0 && lane == 0 && c0 == 0) stamp(p, 11);
         } else if (row_ok) {
           // ---- ragged N tail: scalar row-per-thread stores ----
           if (e.out != nullptr) {
@@ -1018,25 +996,17 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
           }
         }
       }
-      // all TMEM reads of this accumulator stage are complete (tcgen05.wait::ld above): hand it back
-      ptx::tc_fence_before_sync();
-      __syncwarp();
-      if (tcount == 0 && warp_idx == 2 && lane == 0) stamp(p, 6);
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc_stage]);
+      if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 6);
     }
-    if (warp_idx == 2 && lane == 0) stamp(p, 13);  // this warp's last tile drained
+    if (ew == 0 && lane == 0) stamp(p, 13);  // this warp's last tile drained
     // outstanding TMA stores of this warp must have finished reading the staging tile before the CTA's shared memory is
     // released; their global writes are ordered before the grid's completion like any other store
     if (lane == 0) ptx::bulk_wait_read_all();
-    if (warp_idx == 2 && lane == 0) stamp(p, 14);
+    if (ew == 0 && lane == 0) stamp(p, 14);
   }
 
   __syncthreads();
   if (p.multicast_a) ptx::cluster_sync_all();  // neither CTA leaves while the other may still send to it
-  if (warp_idx == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-  }
   if (threadIdx.x == 32) stamp(p, 7);
 }
 
@@ -1128,7 +1098,7 @@ cudaError_t launch_cfg(const GemmParams& p, int m_rows, int n_cols, cudaStream_t
           p.bias != nullptr || p.residual != nullptr || p.a_stats != nullptr || p.stats_out != nullptr)
         return cudaErrorInvalidValue;
       kern = gemm_tile_kernel<BLOCK_N, PASSES, 4, KIND>;
-      smem_bytes = Cfg::kStages * Cfg::kStageBytes + 1024 + kSkinStageBytes;
+      smem_bytes = Cfg::kStages * Cfg::kStageBytes + 1024 + Cfg::kAccBytes + kSkinStageBytes;
       static bool skin_attr_set = false;
       if (!skin_attr_set) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
@@ -1149,7 +1119,7 @@ cudaError_t launch_cfg(const GemmParams& p, int m_rows, int n_cols, cudaStream_t
   if (num_sms == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
+    if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
   }
   GemmParams q = p;
   q.grid_m_rows = m_rows;
@@ -1229,6 +1199,18 @@ static int encode_store_map(CUtensorMap* map, const void* base, int64_t rows, in
 
 int make_store_tmap(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld, bool half, int box_rows) {
   return encode_store_map(map, base, rows, cols, ld, half, box_rows);
+}
+
+int make_tile_tmap_f16_sw128(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
+  auto fn = get_encode_fn();
+  if (fn == nullptr) return -1;
+  cuuint64_t gdim[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ld) * 2};
+  cuuint32_t box[2] = {64u, static_cast<cuuint32_t>(box_rows)};
+  cuuint32_t estride[2] = {1u, 1u};
+  return static_cast<int>(fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estride,
+                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
 }
 
 int gemm_enable_multicast(GemmParams* p, const void* a_hi, const void* a_lo, int64_t rows, int64_t cols, int64_t ld, int n_cols,
@@ -1311,7 +1293,7 @@ cudaError_t f16_weight_scale(const float* w_dev, int64_t n, float* scale_out) {
   unsigned int bits = 0;
   e = cudaMemset(d_max, 0, sizeof(unsigned int));
   if (e == cudaSuccess) {
-    absmax_kernel<<<148, 256>>>(w_dev, n, d_max);
+    absmax_kernel<<<132, 256>>>(w_dev, n, d_max);
     e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaMemcpy(&bits, d_max, sizeof bits, cudaMemcpyDeviceToHost);
@@ -1333,7 +1315,7 @@ cudaError_t launch_split_f16(const float* x, void* hi, void* lo, int64_t n, floa
   if (n <= 0) return cudaSuccess;
   const int threads = 256;
   int64_t blocks = (n + threads - 1) / threads;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   split_f16_kernel<<<static_cast<unsigned>(blocks), threads, 0, stream>>>(x, static_cast<__half*>(hi), static_cast<__half*>(lo),
                                                                           n, scale);
   return cudaGetLastError();
@@ -1343,7 +1325,7 @@ cudaError_t launch_split_tf32(const float* x, float* hi, float* lo, int64_t n, c
   if (n <= 0) return cudaSuccess;
   const int threads = 256;
   int64_t blocks = (n + threads - 1) / threads;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   split_tf32_kernel<<<static_cast<unsigned>(blocks), threads, 0, stream>>>(x, hi, lo, n);
   return cudaGetLastError();
 }

@@ -1,4 +1,4 @@
-// Segmented-A GEMM on tcgen05 tensor cores with error-compensated hi/lo operand pairs for fp32-grade results.
+// Segmented-A GEMM on Hopper wgmma tensor cores with error-compensated hi/lo operand pairs for fp32-grade results.
 //
 //   C[m, n] = epilogue( sum_s sum_k A_s[m * row_mul_s + row_shift_s, k] * W[n, koff_s + k] )
 //
@@ -17,12 +17,12 @@
 //   fp32 stores at a per-split row offset and the consumer kernel adds them in split order (TrajNet's deep pyramid levels, where
 //   6-22 row tiles with 40-80 K blocks each would otherwise leave most SMs idle or force 32-wide tiles).
 //
-// Kernel shape: persistent, grid = min(#work items, #SMs), 128 x BLOCK_N output tiles, 320 threads per CTA:
-//   warp 0   : TMA producer (one elected lane)        smem ring of 64 KB stages: full[]/empty[] mbarriers
-//   warp 1   : TMEM allocator + tcgen05.mma issuer    two accumulator stages in TMEM (tmem_full[]/tmem_empty[])
-//   warps 2-9: epilogue (tcgen05.ld -> scale / bias / activation / row mask / GroupNorm sums -> swizzled smem tile ->
-//              TMA bulk store, or per-thread stores with a residual), draining tile i while the MMA warp already
-//              accumulates tile i+1
+// Kernel shape: persistent, grid = min(#work items, #SMs), 128 x BLOCK_N output tiles, 384 threads per CTA:
+//   warpgroup 0   : TMA producer (one lane)             smem ring of 2 x (A + B) stages: full[]/empty[] mbarriers
+//   warpgroups 1-2: wgmma, 64 rows each, accumulators in registers (two per thread with PASSES == 3); the finished tile
+//                   goes through a shared-memory accumulator tile to one row per thread, then the epilogue: scale / bias /
+//                   activation / row mask / GroupNorm sums -> swizzled smem tile -> TMA bulk store, or per-thread stores
+//                   with a residual.  The producer keeps filling the ring for the next tile during the epilogue.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -32,20 +32,19 @@ namespace rohm {
 
 constexpr int kSkinTileBones = 16;  // most distinct bones a 32-vertex column tile may touch (fused skinning epilogue)
 constexpr int kGemmBlockM = 128;
-// K extent of one pipeline stage in fp32 elements: 32 = 128-byte rows (SWIZZLE_128B), 64 KB stages, 3 in flight;
-// 16 = 64-byte rows (SWIZZLE_64B), 32 KB stages, 6 in flight.  Both are implemented and pass the self-test; measured on
-// B200 (N=512, 148 tiles): 0.51 us per 32 K-columns with BLOCK_K = 32 against 0.73 us with BLOCK_K = 16 (MMA-bound would
-// be 0.39 us) -- the per-stage handshake (full-barrier wait, descriptor setup, commit) costs ~250-350 cycles of tensor-
-// pipe bubble, so fewer, larger stages win even though fewer bytes are in flight.
+// K extent of one pipeline stage in fp32 elements: 32 = 128-byte rows (SWIZZLE_128B), 16 = 64-byte rows (SWIZZLE_64B).
+// Both are implemented.  16 is the default: next to the shared-memory accumulator tile (66 KB at BLOCK_N = 128) and the
+// epilogue staging tiles, the 227 KB of an H100 block hold three 32 KB stages of a 128-wide PASSES == 3 tile, where 64 KB
+// stages would leave a single one.
 #ifndef ROHM_GEMM_BLOCK_K
-#define ROHM_GEMM_BLOCK_K 32
+#define ROHM_GEMM_BLOCK_K 16
 #endif
 constexpr int kGemmBlockK = ROHM_GEMM_BLOCK_K;
 static_assert(kGemmBlockK == 16 || kGemmBlockK == 32, "one 64- or 128-byte swizzle span");
 constexpr int kMaxSegs = 10;
 
-// Operand element type of a GEMM.  kKindTf32: fp32 containers holding TF32 hi/lo pairs (tcgen05 kind::tf32, 8 K-columns
-// per instruction).  kKindF16: fp16 hi/lo pairs (kind::f16, 16 K-columns per instruction): the same 2 x 11 significant
+// Operand element type of a GEMM.  kKindTf32: fp32 containers holding TF32 hi/lo pairs (wgmma .tf32, 8 K-columns
+// per instruction).  kKindF16: fp16 hi/lo pairs (wgmma .f16, 16 K-columns per instruction): the same 2 x 11 significant
 // bits per value in half the bytes, so one 128-byte swizzle row -- one pipeline stage -- covers twice the K extent at the
 // same tensor-pipe and shared-memory-fill cost.  Weights are pre-scaled by a power of two into the middle of the fp16
 // range (GemmParams::acc_scale undoes it exactly in the epilogue); activations must stay below 1.3e5 in magnitude.
@@ -120,8 +119,7 @@ struct alignas(64) GemmParams {
   float ln_eps;
   // A-operand multicast (`multicast_a`, set by gemm_enable_multicast): CTAs run as clusters of two that own neighbouring
   // column tiles of the same 128-row stripe; each loads HALF of the stripe's A tile (64 rows, a_hi_half / a_lo_half) and
-  // multicasts it to both, so A crosses the L2 -> SM fabric once per pair.  Measured on B200 the main loop of these GEMMs is
-  // bound by that fabric (148 SMs x 64 KB per 0.51 us), not by the tensor pipe.  Requires one A segment, an even number
+  // multicasts it to both, so A crosses the L2 -> SM fabric once per pair.  Requires one A segment, an even number
   // of column tiles and PASSES == 3.
   CUtensorMap a_hi_half;
   CUtensorMap a_lo_half;
@@ -139,12 +137,12 @@ struct alignas(64) GemmParams {
   const float* skin_w;
   // optional: CTA 0 records %globaltimer at 8 milestones (developer instrumentation, see tools/gemm_selftest)
   unsigned long long* debug_ts;
-  // developer experiments (tools/gemm_selftest only; results are wrong when set): bit 0 = the epilogue only drains TMEM (no
+  // developer experiments (tools/gemm_selftest only; results are wrong when set): bit 0 = the epilogue only drains the accumulator (no
   // staging, no stores), bit 1 = staging writes but no TMA stores.  Slots 16.. of debug_ts: "all MMAs of tile i issued".
   int debug_flags;
   // Split-K (TrajNet convolutions on the deep pyramid levels; masked / GroupNorm epilogue variant only): the K iterations of
   // every output tile are cut into `k_splits` contiguous ranges, one work item each, so that a level with 6 to 22 row tiles
-  // still fills the 148 SMs with 128-wide tiles.  Split s stores its fp32 partial tile (no bias, no statistics) at output row
+  // still fills the SMs with 128-wide tiles.  Split s stores its fp32 partial tile (no bias, no statistics) at output row
   // m + s * split_row_stride of `out`; the consumer (gn_mish_split_kernel) adds the partials in a fixed order, so the result is
   // deterministic.  0 / 1 = off.  Every range must be non-empty: (k_splits - 1) * ceil(iters / k_splits) < iters.
   int k_splits;
@@ -174,6 +172,10 @@ int gemm_enable_multicast(GemmParams* p, const void* a_hi, const void* a_lo, int
 // Tensor map for box_rows x 32-element TMA store boxes over a row-major [rows, cols] matrix with pitch ld: fp32 with
 // SWIZZLE_128B (128-byte box rows) or fp16 with SWIZZLE_64B (64-byte box rows).  Returns 0 or a CUresult.
 int make_store_tmap(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld, bool half, int box_rows = 32);
+
+// Tensor map for box_rows x 64-element fp16 load boxes (128-byte rows, SWIZZLE_128B) over a row-major [rows, cols] matrix
+// with pitch ld: wgmma operand tiles of the attention kernel.  Returns 0 or a CUresult.
+int make_tile_tmap_f16_sw128(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows);
 
 // Launches the tile kernel.  block_n in {32, 64, 96, 128}; passes in {1, 3} (kKindF16: 3 only).
 // grid = ceil(M_tiles) x ceil(N_tiles) where M_tiles covers `m_rows` GEMM rows.

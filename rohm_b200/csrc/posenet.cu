@@ -2,12 +2,12 @@
 // (reference model/posenet.py:75-96, model/heads.py:112-176; torch nn.TransformerEncoderLayer post-norm, exact GELU).
 //
 // Token-major layout: every activation is a row-major [B*S, width] matrix, S = T + 1 tokens per clip (token 0 is the
-// timestep embedding), clips contiguous.  All linear layers run on the tcgen05 GEMM (gemm.cu); operands that feed a
+// timestep embedding), clips contiguous.  All linear layers run on the wgmma GEMM (gemm.cu); operands that feed a
 // tensor-core product are kept as hi/lo pairs (fp16 halves by default, TF32 in the tf32 modes) written by the
 // producing kernel's epilogue, so no separate conversion pass exists.
 //
 //   x_t [B,C,1,T] --pack--> A_in --GEMM(+bias+cond_embed+pe)--> X  (token 0 <- time-embedding table gather)
-//   8 x { X --GEMM--> Q|K|V --attention (tcgen05: S = QK^T, softmax from TMEM, O = PV)--> CTX --GEMM(+bias)--> Y
+//   8 x { X --GEMM--> Q|K|V --attention (wgmma: S = QK^T, softmax on the fragments, O = PV)--> CTX --GEMM(+bias)--> Y
 //         --LN(Y + X)--> X --GEMM(+bias,GELU)--> H --GEMM(+bias)--> Y --LN(Y + X)--> X }
 //   X --GEMM--> OUT_tok --unpack(+copy cond[:, :traj])--> out [B,C,1,T]
 // One forward = 61 launches, replayed as one CUDA graph with programmatic dependent launch along the chain.
@@ -31,7 +31,7 @@ namespace {
 __global__ void pack_tokens_kernel(const float* __restrict__ x, float* __restrict__ hi, float* __restrict__ lo, int C,
                                    int T, int S, int ld, int f16) {
   __shared__ float tile[32][33];
-  // programmatic dependent launch: the embedding GEMM behind this kernel may set itself up (barriers, TMEM, weight tiles)
+  // programmatic dependent launch: the embedding GEMM behind this kernel may set itself up (barriers, weight tiles)
   // while it runs; as a dependent (a no-op for a plain launch) nothing is read before the previous kernel has completed
   ptx::pdl_launch_dependents();
   ptx::pdl_wait_prior_grid();
@@ -778,301 +778,190 @@ __global__ void __launch_bounds__(32 * NK, 1) attention_f16_kernel(const __half*
 template <int DH>
 size_t attention_f16_smem_bytes(int NK) { return sizeof(__half) * 4 * 16 * NK * attn_f16_pitch<DH>(); }
 
-// ---- tcgen05 attention (ROHM_PRECISION_F16X2, head dim 128, clips of at most 160 tokens) ----------------------------
-// One CTA per (clip, head).  Q and K of the head are TMA-loaded as K-major SWIZZLE_128B tiles straight from the fused
-// Q|K|V projection's fp16 hi/lo output; S = Q K^T runs as UMMA 128 x 160 x 16 (two 128-row query tiles, 160 padded keys)
-// into TMEM; one thread per query row reads its logits back (tcgen05.ld), does the softmax in registers (two passes over
-// TMEM: max, then exp / sum) and writes the unnormalised P row as fp16 hi/lo into a K-major shared-memory tile; O = P V
-// runs as UMMA 128 x 128 x 16 with V read in place -- its natural [token][feature] layout is an MN-major B operand
-// (SWIZZLE_128B atoms of 8 keys x 64 features), so no transposition happens anywhere.
-// Every product is the 3-term hi/lo expansion; all three terms accumulate into one TMEM accumulator.
-//   TMEM columns: [32,192) S tile 0 (reused by O tile 1), [192,352) S tile 1, [352,480) O tile 0.
-//   smem: phase 1  Q {hi,lo} x {dh 0-63, 64-127} 4 x 20 KB | K likewise 4 x 20 KB
-//         phase 2  P {hi,lo} x 3 key chunks 6 x 20 KB (160 rows each: both query tiles side by side, so neither waits for
-//                  the other) | V {hi,lo} x {dh 0-63, 64-127} 4 x 20 KB -- both land over Q / K once every S MMA is done
-struct AttnTcParams {
-  CUtensorMap qkv_hi, qkv_lo;  // Q | K | V planes [rows, 3D] fp16, box {64 columns, 160 rows}
-  CUtensorMap st_hi, st_lo;    // ctx planes [rows, D] fp16, 32 x 32 store boxes
+// ---- wgmma attention (ROHM_PRECISION_F16X2, head dim 128, clips of at most 160 tokens) ----------------------------
+// One warpgroup per (clip, head, 64 queries).  Q (64 rows) and K / V (160 rows from the clip's first token) arrive by TMA
+// as 128B-swizzled hi/lo tiles (V on its own mbarrier).  S = Q K^T (wgmma m64n160k16) stays in registers, the softmax runs
+// on the fragments, and the fp16 hi/lo split of P is already the A operand of O = P V (wgmma m64n128k16, V read in place as
+// an MN-major B).  Three products each.  Keys past the clip get -inf logits and zeroed V rows.
+struct AttnWgParams {
+  CUtensorMap q_hi, q_lo;    // Q|K|V planes [rows, 3D] fp16, boxes of 64 columns x 64 rows
+  CUtensorMap kv_hi, kv_lo;  // the same planes, boxes of 64 columns x 160 rows
   __half* ctx_hi;
   __half* ctx_lo;
   int S, D, H;
   float scale;
-  int split_qk_load;             // Q / K arrive on two barriers, one per 64-wide head-dim half (ROHM_B200_ATTN_SPLIT_LOAD=0: one)
-  unsigned long long* debug_ts;  // developer instrumentation: CTA 0 records %globaltimer at 12 milestones
 };
-constexpr int kAtKeys = 160;                  // padded key count = UMMA N of the S product
-constexpr uint32_t kAtColS = 32, kAtColO0 = 32 + 2 * kAtKeys;  // TMEM column map (see above)
-constexpr int kAtQKBuf = kAtKeys * 128;       // bytes of one 160-row x 128-byte buffer: {plane, dh-chunk} of Q, K or V, {plane, key-chunk} of P
-constexpr int kAtTile = 128 * 128;            // bytes of the 128 rows of one query tile inside such a buffer
-constexpr int kAtSmemBytes = 10 * kAtQKBuf + 1024;
-constexpr int kAtThreads = 32 * (2 + 16);  // TMA warp, MMA warp, 2 query tiles x 4 lane quarters x 2 column halves
+constexpr int kAwKeys = 160;                 // padded key count = N of the S product
+constexpr int kAwQRows = 64;                 // queries per CTA = M of one wgmma
+constexpr int kAwQBuf = kAwQRows * 128;      // bytes of one {plane, 64-wide head-dim chunk} buffer of Q
+constexpr int kAwKBuf = kAwKeys * 128;       // the same for K or V
+constexpr int kAwSmemBytes = 4 * kAwQBuf + 8 * kAwKBuf + 1024;
 
-__device__ __forceinline__ void at_stamp(const AttnTcParams& p, int slot) {
-  if (p.debug_ts != nullptr && blockIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    p.debug_ts[slot] = t;
-  }
-}
-
-__global__ void __launch_bounds__(kAtThreads, 1) attention_tc_kernel(const __grid_constant__ AttnTcParams p) {
-  extern __shared__ uint8_t at_smem_raw[];
-  __shared__ uint64_t qk_full[2], v_full, s_full[2], p_ready[2], o_full[2];  // qk_full: one barrier per 64-wide head-dim half
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ float at_red[2][128][4];  // [tile][row][{max, max, sum, sum} of the two column halves]
-  const uint32_t raw_addr = ptx::smem_u32(at_smem_raw);
-  uint8_t* smem = at_smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = blockIdx.x / p.H, h_ = blockIdx.x % p.H;  // clip, head
+__global__ void __launch_bounds__(128, 1) attention_wgmma_kernel(const __grid_constant__ AttnWgParams p) {
+  extern __shared__ uint8_t aw_smem_raw[];
+  __shared__ uint64_t bar_qk, bar_v;
+  const uint32_t raw = ptx::smem_u32(aw_smem_raw);
+  uint8_t* const sm = aw_smem_raw + ((1024u - (raw & 1023u)) & 1023u);
+  uint8_t* const Qb = sm;                   // [plane][chunk]
+  uint8_t* const Kb = sm + 4 * kAwQBuf;     // [plane][chunk]
+  uint8_t* const Vb = Kb + 4 * kAwKBuf;     // [plane][chunk]
   const int S = p.S;
-  const int ntiles = S > 128 ? 2 : 1;
-  const int row0 = b * S;  // first token row of this clip
-  if (threadIdx.x == 0) at_stamp(p, 0);
-
-  if (warp_idx == 0 && lane == 0) {
-    ptx::prefetch_tmap(&p.qkv_hi), ptx::prefetch_tmap(&p.qkv_lo), ptx::prefetch_tmap(&p.st_hi), ptx::prefetch_tmap(&p.st_lo);
-    ptx::mbar_init(&qk_full[0], 1), ptx::mbar_init(&qk_full[1], 1), ptx::mbar_init(&v_full, 1);
-    for (int t = 0; t < 2; ++t) ptx::mbar_init(&s_full[t], 1), ptx::mbar_init(&p_ready[t], 8), ptx::mbar_init(&o_full[t], 1);
+  const int qtiles = (S + kAwQRows - 1) / kAwQRows;
+  const int qt = static_cast<int>(blockIdx.x) % qtiles;
+  const int bh = static_cast<int>(blockIdx.x) / qtiles;
+  const int h = bh % p.H, b = bh / p.H;
+  const int row0 = b * S, q0 = qt * kAwQRows;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    ptx::prefetch_tmap(&p.q_hi);
+    ptx::prefetch_tmap(&p.q_lo);
+    ptx::prefetch_tmap(&p.kv_hi);
+    ptx::prefetch_tmap(&p.kv_lo);
+    ptx::mbar_init(&bar_qk, 1);
+    ptx::mbar_init(&bar_v, 1);
     ptx::fence_barrier_init();
   }
-  if (warp_idx == 1) ptx::tmem_alloc<512>(&tmem_base_smem);
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_smem;
   ptx::pdl_launch_dependents();
   ptx::pdl_wait_prior_grid();
-  if (threadIdx.x == 0) at_stamp(p, 1);
+  if (threadIdx.x == 0) {
+    ptx::mbar_expect_tx(&bar_qk, 4 * kAwQBuf + 4 * kAwKBuf);
+    for (int pl = 0; pl < 2; ++pl)
+      for (int c = 0; c < 2; ++c) {
+        ptx::tma_load_2d(Qb + (pl * 2 + c) * kAwQBuf, pl ? &p.q_lo : &p.q_hi, &bar_qk, h * 128 + 64 * c, row0 + q0);
+        ptx::tma_load_2d(Kb + (pl * 2 + c) * kAwKBuf, pl ? &p.kv_lo : &p.kv_hi, &bar_qk, p.D + h * 128 + 64 * c, row0);
+      }
+    ptx::mbar_expect_tx(&bar_v, 4 * kAwKBuf);
+    for (int pl = 0; pl < 2; ++pl)
+      for (int c = 0; c < 2; ++c)
+        ptx::tma_load_2d(Vb + (pl * 2 + c) * kAwKBuf, pl ? &p.kv_lo : &p.kv_hi, &bar_v, 2 * p.D + h * 128 + 64 * c, row0);
+  }
 
-  uint8_t* const Qb = smem;                  // + (plane * 2 + kc) * kAtQKBuf
-  uint8_t* const Kb = smem + 4 * kAtQKBuf;
-  uint8_t* const Pb = smem;                  // + (plane * 3 + c) * kAtQKBuf, rows of tile t at + t * kAtTile
-  uint8_t* const Vb = smem + 6 * kAtQKBuf;   // + (plane * 2 + kc) * kAtQKBuf
+  // ---- S = Q K^T (64 x 160), three products per k-step ----
+  float s[80];
+#pragma unroll
+  for (int i = 0; i < 80; ++i) s[i] = 0.0f;
+  ptx::mbar_wait(&bar_qk, 0);
+  ptx::wgmma_fence_regs(s);
+  ptx::wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const int c = k >> 2;
+    const uint64_t ko = static_cast<uint64_t>((k & 3) * 2);  // 16 fp16 = 32 bytes inside the 128-byte swizzle span
+    const uint64_t qh = ptx::make_desc_kmajor<128>(ptx::smem_u32(Qb + c * kAwQBuf)) + ko;
+    const uint64_t ql = ptx::make_desc_kmajor<128>(ptx::smem_u32(Qb + (2 + c) * kAwQBuf)) + ko;
+    const uint64_t kh = ptx::make_desc_kmajor<128>(ptx::smem_u32(Kb + c * kAwKBuf)) + ko;
+    const uint64_t kl = ptx::make_desc_kmajor<128>(ptx::smem_u32(Kb + (2 + c) * kAwKBuf)) + ko;
+    ptx::wgmma_f16(s, ql, kh);
+    ptx::wgmma_f16(s, qh, kl);
+    ptx::wgmma_f16(s, qh, kh);
+  }
+  ptx::wgmma_commit();
+  ptx::wgmma_wait<0>();
+  ptx::wgmma_fence_regs(s);
 
-  if (warp_idx == 0) {
-    if (lane == 0) {
-      // head dims 0..63 of Q and K (both planes) first, on their own barrier: the S MMAs over that half start while the
-      // second half is still on its way (the load is bound by the SM's L2 read port: 148 KB at ~64 B/clk = 1.3 us)
-      for (int kc = 0; kc < 2; ++kc) {
-        uint64_t* bar = &qk_full[p.split_qk_load ? kc : 0];
-        if (p.split_qk_load || kc == 0) ptx::mbar_expect_tx(bar, (p.split_qk_load ? 4 : 8) * kAtQKBuf);
-        for (int pl = 0; pl < 2; ++pl) {
-          const CUtensorMap* m = pl == 0 ? &p.qkv_hi : &p.qkv_lo;
-          ptx::tma_load_2d(Qb + (pl * 2 + kc) * kAtQKBuf, m, bar, h_ * 128 + kc * 64, row0);
-          ptx::tma_load_2d(Kb + (pl * 2 + kc) * kAtQKBuf, m, bar, p.D + h_ * 128 + kc * 64, row0);
-        }
-      }
-      // V lands on top of K: wait until every S MMA has read it
-      ptx::mbar_wait(&s_full[ntiles - 1], 0);
-      ptx::mbar_expect_tx(&v_full, 4 * kAtQKBuf);
-      for (int pl = 0; pl < 2; ++pl) {
-        const CUtensorMap* m = pl == 0 ? &p.qkv_hi : &p.qkv_lo;
-        for (int kc = 0; kc < 2; ++kc)
-          ptx::tma_load_2d(Vb + (pl * 2 + kc) * kAtQKBuf, m, &v_full, 2 * p.D + h_ * 128 + kc * 64, row0);
-      }
-    }
-  } else if (warp_idx == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = ptx::make_idesc(/*F16*/ 0, 128, kAtKeys);
-      constexpr uint32_t idesc_o = ptx::make_idesc(/*F16*/ 0, 128, 128, /*b_mn_major=*/true);
-      ptx::mbar_wait(&qk_full[0], 0);
-      at_stamp(p, 2);
-      ptx::tc_fence_after_sync();
-      for (int t = 0; t < ntiles; ++t) {
-        const uint32_t acc = tmem_base + kAtColS + static_cast<uint32_t>(t * kAtKeys);
+  // ---- softmax on the fragments: this thread holds rows r and r + 8 (elements 4j, 4j+1 and 4j+2, 4j+3), keys 8j + c2 + {0,1}
+  const int c2 = 2 * (lane & 3);
+  float m0 = -INFINITY, m1 = -INFINITY;
 #pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {  // 16 head-dim columns per instruction
-          const int kc = ks >> 2;
-          if (t == 0 && ks == 4 && p.split_qk_load) {  // second head-dim half (its own barrier when the load is split)
-            ptx::mbar_wait(&qk_full[1], 0);
-            ptx::tc_fence_after_sync();
-          }
-          const uint64_t ko = static_cast<uint64_t>((ks & 3) * 2);
-          const uint64_t a_hi = ptx::make_desc_kmajor<128>(ptx::smem_u32(Qb + (0 * 2 + kc) * kAtQKBuf + t * kAtTile)) + ko;
-          const uint64_t a_lo = ptx::make_desc_kmajor<128>(ptx::smem_u32(Qb + (1 * 2 + kc) * kAtQKBuf + t * kAtTile)) + ko;
-          const uint64_t b_hi = ptx::make_desc_kmajor<128>(ptx::smem_u32(Kb + (0 * 2 + kc) * kAtQKBuf)) + ko;
-          const uint64_t b_lo = ptx::make_desc_kmajor<128>(ptx::smem_u32(Kb + (1 * 2 + kc) * kAtQKBuf)) + ko;
-          ptx::mma_f16_ss(acc, a_lo, b_hi, idesc_s, ks > 0 ? 1u : 0u);
-          ptx::mma_f16_ss(acc, a_hi, b_lo, idesc_s, 1u);
-          ptx::mma_f16_ss(acc, a_hi, b_hi, idesc_s, 1u);
-        }
-        ptx::mma_commit(&s_full[t]);
-      }
-      ptx::mbar_wait(&v_full, 0);
-      at_stamp(p, 4);
-      for (int t = 0; t < ntiles; ++t) {
-        ptx::mbar_wait(&p_ready[t], 0);
-        at_stamp(p, 6 + 3 * t);
-        ptx::tc_fence_after_sync();
-        const uint32_t acc = tmem_base + (t == 0 ? kAtColO0 : kAtColS);
+  for (int j = 0; j < 20; ++j) {
 #pragma unroll
-        for (int ks = 0; ks < kAtKeys / 16; ++ks) {  // 16 keys per instruction
-          const int c = ks >> 2;
-          const uint64_t ko = static_cast<uint64_t>((ks & 3) * 2);
-          const uint64_t a_hi = ptx::make_desc_kmajor<128>(ptx::smem_u32(Pb + (0 * 3 + c) * kAtQKBuf + t * kAtTile)) + ko;
-          const uint64_t a_lo = ptx::make_desc_kmajor<128>(ptx::smem_u32(Pb + (1 * 3 + c) * kAtQKBuf + t * kAtTile)) + ko;
-          // V[key][feature]: the 16 keys of this step are two 8-row atoms (1024 B apart); features 64..127 live in the
-          // next buffer (LBO)
-          const uint64_t b_hi = ptx::make_desc_mnmajor_sw128(ptx::smem_u32(Vb + 0 * kAtQKBuf + ks * 2048), kAtQKBuf, 1024);
-          const uint64_t b_lo = ptx::make_desc_mnmajor_sw128(ptx::smem_u32(Vb + 2 * kAtQKBuf + ks * 2048), kAtQKBuf, 1024);
-          ptx::mma_f16_ss(acc, a_lo, b_hi, idesc_o, ks > 0 ? 1u : 0u);
-          ptx::mma_f16_ss(acc, a_hi, b_lo, idesc_o, 1u);
-          ptx::mma_f16_ss(acc, a_hi, b_hi, idesc_o, 1u);
-        }
-        ptx::mma_commit(&o_full[t]);
-      }
-    }
-  } else {
-    // ===================== softmax + output warps: 8 per query tile, TWO threads per query row =====================
-    // tile t = (warp_idx - 2) / 8; TMEM lane quarter q = warp_idx % 4 (hardware rule); half h = ((warp_idx - 2) / 4) % 2:
-    // the two warps of a (tile, quarter) pair split the 160 key columns of their 32 rows (80 each: row maximum and row sum are
-    // exchanged through shared memory under a 64-thread named barrier) and, in the output phase, the 128 feature columns.
-    // One thread per row left the four schedulers with one latency-bound warp each for 4.2 us of the 12 us chain.
-    const int t = (warp_idx - 2) >> 3;
-    const int h = ((warp_idx - 2) >> 2) & 1;
-    const int q = warp_idx & 3;
-    const int row = q * 32 + lane;
-    const int grow = t * 128 + row;  // token index inside the clip
-    const bool valid = grow < S;
-    if (t < ntiles && t * 128 + q * 32 >= S) {
-      // no real query row in this pair's 32 lanes (the tail of tile 1): nothing to compute, just release the MMA warp
-      if (lane == 0) ptx::mbar_arrive(&p_ready[t]);
-    } else if (t < ntiles) {
-      const uint32_t lane_addr = static_cast<uint32_t>(q * 32) << 16;
-      const uint32_t s_addr = tmem_base + lane_addr + kAtColS + static_cast<uint32_t>(t * kAtKeys + 80 * h);
-      const int pair_bar = 1 + t * 4 + q;  // named barrier of this (tile, quarter) pair
-      constexpr int NC = 5;                // 16-column chunks per thread
-      uint32_t r0[16], r1[16];
-      ptx::mbar_wait(&s_full[t], 0);
-      if (t == 0 && warp_idx == 2 && lane == 0) at_stamp(p, 3);
-      ptx::tc_fence_after_sync();
-      // pass 1: maximum over this thread's real keys
-      float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-      ptx::tmem_ld_32x16(s_addr, r0);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < NC; ++c) {
-        uint32_t(&cur)[16] = (c & 1) ? r1 : r0;
-        uint32_t(&nxt)[16] = (c & 1) ? r0 : r1;
-        if (c + 1 < NC) ptx::tmem_ld_32x16(s_addr + (c + 1) * 16, nxt);
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-          if (80 * h + c * 16 + j < S) mx4[j & 3] = fmaxf(mx4[j & 3], __uint_as_float(cur[j]));
-        if (c + 1 < NC) ptx::tmem_ld_wait();
-      }
-      float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-      at_red[t][row][h] = mx;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      mx = fmaxf(mx, at_red[t][row][h ^ 1]);
-      if (t == 0 && warp_idx == 2 && lane == 0) at_stamp(p, 5);
-      // the P buffers overlap Q and K: every S MMA must have completed
-      ptx::mbar_wait(&s_full[ntiles - 1], 0);
-      // pass 2: p = exp(scale (s - max)), partial row sum, fp16 hi/lo -> K-major SWIZZLE_128B rows (16-byte unit u of row r at
-      // slot u ^ (r & 7))
-      float sum4[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-      const float sc2 = p.scale * 1.4426950408889634f;  // exp(x) = 2^(x log2 e): one FFMA + one MUFU.EX2 per element
-      const float ms2 = mx * sc2;
-      ptx::tmem_ld_32x16(s_addr, r0);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < NC; ++c) {
-        uint32_t(&cur)[16] = (c & 1) ? r1 : r0;
-        uint32_t(&nxt)[16] = (c & 1) ? r0 : r1;
-        if (c + 1 < NC) ptx::tmem_ld_32x16(s_addr + (c + 1) * 16, nxt);
-        const int k0 = 80 * h + 16 * c;  // first key of this chunk
-        float pv[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float x = fmaf(__uint_as_float(cur[j]), sc2, -ms2);  // <= 0
-          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(pv[j]) : "f"(x));
-        }
-        if (k0 + 15 >= S) {  // only the last chunk(s) hold padded keys
-#pragma unroll
-          for (int j = 0; j < 16; ++j) pv[j] = (k0 + j < S) ? pv[j] : 0.0f;
-        }
-#pragma unroll
-        for (int j = 0; j < 16; ++j) sum4[j & 3] += pv[j];
-        if (valid) {
-          uint8_t* ph = Pb + (0 * 3 + (k0 >> 6)) * kAtQKBuf + grow * 128;
-          uint8_t* pl = Pb + (1 * 3 + (k0 >> 6)) * kAtQKBuf + grow * 128;
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            uint32_t hw[4], lw[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) ptx::split_f16x2(pv[8 * u + 2 * i], pv[8 * u + 2 * i + 1], hw[i], lw[i]);
-            const int slot = ((((k0 & 63) >> 3) + u) ^ (row & 7)) << 4;
-            *reinterpret_cast<uint4*>(ph + slot) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-            *reinterpret_cast<uint4*>(pl + slot) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-          }
-        }
-        if (c + 1 < NC) ptx::tmem_ld_wait();
-      }
-      float sum = (sum4[0] + sum4[1]) + (sum4[2] + sum4[3]);
-      at_red[t][row][2 + h] = sum;
-      ptx::fence_proxy_async();  // generic-proxy writes of P -> visible to the tensor core's async-proxy reads
-      ptx::tc_fence_before_sync();
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      sum += at_red[t][row][2 + (h ^ 1)];
-      if (lane == 0) ptx::mbar_arrive(&p_ready[t]);
-
-      // output: O / sum -> fp16 hi/lo rows of ctx; this warp owns the 32-column chunks 2h and 2h + 1.  Full 32-row groups go
-      // through a SWIZZLE_64B staging tile (carved out of P buffer c, whose tile-0 rows are dead once the O MMAs of tile 0 have
-      // completed) and TMA stores; a group that straddles the end of the clip writes its real rows directly.
-      ptx::mbar_wait(&o_full[t], 0);
-      if (warp_idx == 4 + 8 * t && lane == 0) at_stamp(p, 7 + 3 * t);
-      ptx::tc_fence_after_sync();
-      const float inv = 1.0f / sum;
-      const uint32_t o_addr = tmem_base + lane_addr + (t == 0 ? kAtColO0 : kAtColS) + static_cast<uint32_t>(64 * h);
-      const int64_t o = (static_cast<int64_t>(row0) + grow) * p.D + h_ * 128 + 64 * h;
-      const bool group_full = t == 0 && (q * 32 + 32 <= S);  // tile 0 only: the staging area belongs to tile 0's P rows
-      ptx::tmem_ld_32x16(o_addr, r0);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {  // 16 columns per step; two steps per 32-column chunk
-        uint32_t(&cur)[16] = (cc & 1) ? r1 : r0;
-        uint32_t(&nxt)[16] = (cc & 1) ? r0 : r1;
-        if (cc + 1 < 4) ptx::tmem_ld_32x16(o_addr + (cc + 1) * 16, nxt);
-        const int c = 2 * h + (cc >> 1);  // 32-column chunk of the head's 128 features
-        uint32_t hw[8], lw[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          ptx::split_f16x2(__uint_as_float(cur[2 * i]) * inv, __uint_as_float(cur[2 * i + 1]) * inv, hw[i], lw[i]);
-        if (group_full) {
-          uint8_t* const tb = Pb + c * kAtQKBuf + q * 4096;
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            const int off = lane * 64 + (((2 * (cc & 1) + u) ^ ((lane >> 1) & 3)) << 4);
-            *reinterpret_cast<uint4*>(tb + off) = make_uint4(hw[4 * u], hw[4 * u + 1], hw[4 * u + 2], hw[4 * u + 3]);
-            *reinterpret_cast<uint4*>(tb + 2048 + off) = make_uint4(lw[4 * u], lw[4 * u + 1], lw[4 * u + 2], lw[4 * u + 3]);
-          }
-          if (cc & 1) {  // the 32-column chunk is complete
-            ptx::fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) {
-              ptx::tma_store_2d(&p.st_hi, tb, h_ * 128 + c * 32, row0 + q * 32);
-              ptx::tma_store_2d(&p.st_lo, tb + 2048, h_ * 128 + c * 32, row0 + q * 32);
-              ptx::bulk_commit();
-            }
-          }
-        } else if (valid) {
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            *reinterpret_cast<uint4*>(p.ctx_hi + o + cc * 16 + u * 8) = make_uint4(hw[4 * u], hw[4 * u + 1], hw[4 * u + 2], hw[4 * u + 3]);
-            *reinterpret_cast<uint4*>(p.ctx_lo + o + cc * 16 + u * 8) = make_uint4(lw[4 * u], lw[4 * u + 1], lw[4 * u + 2], lw[4 * u + 3]);
-          }
-        }
-        if (cc + 1 < 4) ptx::tmem_ld_wait();
-      }
-      if (group_full && lane == 0) ptx::bulk_wait_read_all();  // staging tiles must outlive the TMA reads, not the writes
-      ptx::tc_fence_before_sync();
-      if (warp_idx == 4 + 8 * t && lane == 0) at_stamp(p, 8 + 3 * t);
+    for (int e = 0; e < 2; ++e) {
+      const bool valid = 8 * j + c2 + e < S;
+      s[4 * j + e] = valid ? s[4 * j + e] : -INFINITY;
+      s[4 * j + 2 + e] = valid ? s[4 * j + 2 + e] : -INFINITY;
+      m0 = fmaxf(m0, s[4 * j + e]);
+      m1 = fmaxf(m1, s[4 * j + 2 + e]);
     }
   }
-  __syncthreads();
-  if (threadIdx.x == 0) at_stamp(p, 12);
-  if (warp_idx == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc<512>(tmem_base);
+#pragma unroll
+  for (int off = 1; off <= 2; off <<= 1) {
+    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, off));
+    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, off));
+  }
+  float l0 = 0.0f, l1 = 0.0f;
+#pragma unroll
+  for (int j = 0; j < 20; ++j) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const bool valid = 8 * j + c2 + e < S;
+      const float p0 = valid ? expf((s[4 * j + e] - m0) * p.scale) : 0.0f;
+      const float p1 = valid ? expf((s[4 * j + 2 + e] - m1) * p.scale) : 0.0f;
+      s[4 * j + e] = p0, s[4 * j + 2 + e] = p1;
+      l0 += p0, l1 += p1;
+    }
+  }
+#pragma unroll
+  for (int off = 1; off <= 2; off <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+  }
+  // P as fp16 hi/lo pairs in the A-fragment layout of k-step k (keys 16k..16k+15): {row r, keys 16k + c2}, {row r + 8,
+  // same keys}, {row r, keys 16k + 8 + c2}, {row r + 8, same keys} = accumulator elements 8k .. 8k + 7 in order
+  uint32_t ph[10][4], plo[10][4];
+#pragma unroll
+  for (int k = 0; k < 10; ++k)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) ptx::split_f16x2(s[8 * k + 2 * i], s[8 * k + 2 * i + 1], ph[k][i], plo[k][i]);
+#pragma unroll
+  for (int k = 0; k < 10; ++k)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(ph[k][i]), "+r"(plo[k][i])::"memory");
+
+  // ---- V: key rows past the clip are zeroed (0 x NaN of a neighbouring clip would otherwise leak into O) ----
+  ptx::mbar_wait(&bar_v, 0);
+  if (S < kAwKeys) {
+    const int n = (kAwKeys - S) * 8;  // 16-byte chunks per buffer
+    for (int i = threadIdx.x; i < 4 * n; i += 128) {
+      const int buf = i / n, r = i - buf * n;
+      *reinterpret_cast<uint4*>(Vb + buf * kAwKBuf + S * 128 + r * 16) = make_uint4(0u, 0u, 0u, 0u);
+    }
+    ptx::fence_proxy_async();
+    __syncthreads();
+  }
+
+  // ---- O = P V (64 x 128) ----
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.0f;
+  ptx::wgmma_fence_regs(o);
+  ptx::wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 10; ++k) {
+    // 16 keys = two 8-row atoms (SBO 1024 bytes); the two 64-wide head-dim chunks are one buffer apart (LBO)
+    const uint64_t vh = ptx::make_desc_mnmajor_sw128(ptx::smem_u32(Vb + k * 2048), kAwKBuf, 1024);
+    const uint64_t vl = ptx::make_desc_mnmajor_sw128(ptx::smem_u32(Vb + 2 * kAwKBuf + k * 2048), kAwKBuf, 1024);
+    ptx::wgmma_f16_rs_tb(o, plo[k], vh);
+    ptx::wgmma_f16_rs_tb(o, ph[k], vl);
+    ptx::wgmma_f16_rs_tb(o, ph[k], vh);
+  }
+  ptx::wgmma_commit();
+  ptx::wgmma_wait<0>();
+  ptx::wgmma_fence_regs(o);
+#pragma unroll
+  for (int k = 0; k < 10; ++k)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(ph[k][i]), "+r"(plo[k][i])::"memory");
+
+  // ---- normalise, split, store the context rows of this tile ----
+  const int ra = q0 + warp * 16 + (lane >> 2), rb = ra + 8;
+  const float ia = 1.0f / l0, ib = 1.0f / l1;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int col = h * 128 + 8 * j + c2;
+    uint32_t hi, lo;
+    if (ra < S) {
+      ptx::split_f16x2(o[4 * j] * ia, o[4 * j + 1] * ia, hi, lo);
+      const int64_t off = static_cast<int64_t>(row0 + ra) * p.D + col;
+      *reinterpret_cast<uint32_t*>(p.ctx_hi + off) = hi;
+      *reinterpret_cast<uint32_t*>(p.ctx_lo + off) = lo;
+    }
+    if (rb < S) {
+      ptx::split_f16x2(o[4 * j + 2] * ib, o[4 * j + 3] * ib, hi, lo);
+      const int64_t off = static_cast<int64_t>(row0 + rb) * p.D + col;
+      *reinterpret_cast<uint32_t*>(p.ctx_hi + off) = hi;
+      *reinterpret_cast<uint32_t*>(p.ctx_lo + off) = lo;
+    }
   }
 }
 
@@ -1134,10 +1023,11 @@ struct rohm_posenet {
   bool use_graph = true;
   bool use_pdl = true;
   bool use_tma_store = true;  // ROHM_B200_TMA_STORE=0 falls back to the per-thread store epilogue (developer switch)
-  // A-operand TMA multicast across CTA pairs (GemmParams::multicast_a).  Measured on B200: no gain (the main loop is bound by
-  // the shared-memory port, not by the L2 -> SM fabric: 0.7705 ms per forward with, 0.7633 ms without), so it is off by
-  // default; ROHM_B200_MULTICAST=1 turns it on.
+  // A-operand TMA multicast across CTA pairs (GemmParams::multicast_a); off by default, ROHM_B200_MULTICAST=1 turns it on.
   bool use_multicast = false;
+  // wgmma attention (F16X2, head dim 128, <= 160 tokens per clip; ROHM_B200_TC_ATTENTION=0 selects the mma.sync kernel)
+  bool tc_attention = false;
+  AttnWgParams attn_wg{};
   // LayerNorm folding (F16X2, d_model 512; ROHM_B200_FUSED_LN=0 keeps the separate layernorm_kernel): the residual stream
   // is stored un-normalised as an fp16 pair plus per-row partial statistics (stats1: after the attention sublayer, stats2:
   // after the feed-forward sublayer), LN(u) is never materialised: see GemmParams::stats_out / a_stats
@@ -1145,9 +1035,6 @@ struct rohm_posenet {
   float2* stats1 = nullptr;
   float2* stats2 = nullptr;
   float *out_c = nullptr, *out_d = nullptr;  // output head: c_n, d_n of the folded last LayerNorm
-  // tcgen05 attention (F16X2, head dim 128, <= 160 tokens per clip; ROHM_B200_TC_ATTENTION=0 selects the mma.sync kernel)
-  bool tc_attention = false;
-  AttnTcParams attn_tc{};
   cudaStream_t capture_stream = nullptr;
   ~rohm_posenet() {
     if (capture_stream) cudaStreamDestroy(capture_stream);
@@ -1318,7 +1205,7 @@ static int setup_linear(rohm_posenet* pn, GemmParams* g, const float* a_hi, cons
 static int run_gemm(rohm_posenet* pn, GemmParams& g, const PackedWeight& w, int rows, cudaStream_t st) {
   g.M = rows;
   prof_begin(pn, kCatGemm, st);
-  // programmatic dependent launch: this GEMM's prologue (barrier init, TMEM alloc, tensor-map prefetch) overlaps the
+  // programmatic dependent launch: this GEMM's prologue (barrier init, tensor-map prefetch, weight tiles) overlaps the
   // tail of the previous kernel; its griddepcontrol.wait orders all global reads/writes after that kernel
   ROHM_CUDA(pn->ctx, launch_gemm(g, rows, w.N, w.block_n, pn->passes, st, pn->use_pdl && !pn->profiling, w.kind));
   prof_end(pn, st);
@@ -1383,31 +1270,15 @@ static cudaError_t launch_attention_mma(rohm_posenet* pn, int B, int S, float sc
                       pn->CTXl, S, pn->D, pn->H, scale, pn->kind == kKindF16 ? 1 : 0);
 }
 
-static int run_attention_tc(rohm_posenet* pn, int B, int S, cudaStream_t st) {
-  AttnTcParams prm = pn->attn_tc;
+static int run_attention_wgmma(rohm_posenet* pn, int B, int S, cudaStream_t st) {
+  AttnWgParams prm = pn->attn_wg;
   prm.S = S;
-  static unsigned long long* d_ts = nullptr;
-  static int ts_calls = 0;
-  const bool want_ts = getenv("ROHM_B200_ATTN_TS") != nullptr && ++ts_calls == 12;  // a warm call, outside graph capture
-  if (want_ts) {
-    if (d_ts == nullptr) cudaMalloc(&d_ts, 16 * sizeof(unsigned long long));
-    prm.debug_ts = d_ts;
-  }
+  const int qtiles = (S + kAwQRows - 1) / kAwQRows;
   prof_begin(pn, kCatAttention, st);
-  cudaError_t e = launch_chain(attention_tc_kernel, dim3(B * pn->H), dim3(kAtThreads), kAtSmemBytes, st,
+  cudaError_t e = launch_chain(attention_wgmma_kernel, dim3(B * pn->H * qtiles), dim3(128), kAwSmemBytes, st,
                                pn->use_pdl && !pn->profiling, prm);
   prof_end(pn, st);
   ROHM_CUDA(pn->ctx, e);
-  if (want_ts) {
-    unsigned long long h[16];
-    cudaStreamSynchronize(st);
-    cudaMemcpy(h, d_ts, sizeof h, cudaMemcpyDeviceToHost);
-    fprintf(stderr,
-            "attention_tc CTA0 timeline (ns): prologue %llu | Q,K landed %llu | S0 done %llu | V^T landed %llu | pass1 done %llu | "
-            "P0 ready %llu | O0 done %llu | tile0 stored %llu | P1 ready %llu | O1 done %llu | tile1 stored %llu | exit %llu\n",
-            h[1] - h[0], h[2] - h[0], h[3] - h[0], h[4] - h[0], h[5] - h[0], h[6] - h[0], h[7] - h[0], h[8] - h[0], h[9] - h[0],
-            h[10] - h[0], h[11] - h[0], h[12] - h[0]);
-  }
   pn->launches++;
   return ROHM_OK;
 }
@@ -1708,23 +1579,21 @@ extern "C" int rohm_posenet_create(rohm_ctx* ctx, const rohm_posenet_weights* w,
     set_f16(attention_f16_kernel<128, 10>, attention_f16_smem_bytes<128>(10));
     set_f16(attention_f16_kernel<64, 4>, attention_f16_smem_bytes<64>(4));
     set_f16(attention_f16_kernel<64, 10>, attention_f16_smem_bytes<64>(10));
-    set_f16(attention_tc_kernel, kAtSmemBytes);
+    set_f16(attention_wgmma_kernel, kAwSmemBytes);
     if (pn->tc_attention) {
       __half* qkv_hi = reinterpret_cast<__half*>(pn->QKV);
       __half* qkv_lo = qkv_hi + R * 3 * D;
-      int rcm = make_tmap_2d(&pn->attn_tc.qkv_hi, qkv_hi, R, 3 * D, 3 * D, kAtKeys, 1, kKindF16);
-      rcm |= make_tmap_2d(&pn->attn_tc.qkv_lo, qkv_lo, R, 3 * D, 3 * D, kAtKeys, 1, kKindF16);
-      rcm |= make_store_tmap(&pn->attn_tc.st_hi, pn->CTXh, R, D, D, true);
-      rcm |= make_store_tmap(&pn->attn_tc.st_lo, pn->CTXl, R, D, D, true);
+      int rcm = make_tile_tmap_f16_sw128(&pn->attn_wg.q_hi, qkv_hi, R, 3 * D, 3 * D, kAwQRows);
+      rcm |= make_tile_tmap_f16_sw128(&pn->attn_wg.q_lo, qkv_lo, R, 3 * D, 3 * D, kAwQRows);
+      rcm |= make_tile_tmap_f16_sw128(&pn->attn_wg.kv_hi, qkv_hi, R, 3 * D, 3 * D, kAwKeys);
+      rcm |= make_tile_tmap_f16_sw128(&pn->attn_wg.kv_lo, qkv_lo, R, 3 * D, 3 * D, kAwKeys);
       if (rcm != 0) {
         delete pn;
-        return fail(ctx, ROHM_ERR_CUDA, "cuTensorMapEncodeTiled (attention store) failed (%d)", rcm);
+        return fail(ctx, ROHM_ERR_CUDA, "cuTensorMapEncodeTiled (attention tiles) failed (%d)", rcm);
       }
-      pn->attn_tc.ctx_hi = reinterpret_cast<__half*>(pn->CTXh), pn->attn_tc.ctx_lo = reinterpret_cast<__half*>(pn->CTXl);
-      pn->attn_tc.D = D, pn->attn_tc.H = pn->H;
-      pn->attn_tc.scale = 1.0f / sqrtf(static_cast<float>(dh));
-      const char* sq = getenv("ROHM_B200_ATTN_SPLIT_LOAD");
-      pn->attn_tc.split_qk_load = (sq == nullptr || sq[0] != '0') ? 1 : 0;
+      pn->attn_wg.ctx_hi = reinterpret_cast<__half*>(pn->CTXh), pn->attn_wg.ctx_lo = reinterpret_cast<__half*>(pn->CTXl);
+      pn->attn_wg.D = D, pn->attn_wg.H = pn->H;
+      pn->attn_wg.scale = 1.0f / sqrtf(static_cast<float>(dh));
     }
     if (ea != cudaSuccess) {
       delete pn;
@@ -1820,8 +1689,8 @@ static int forward_launches(rohm_posenet* pn, const float* x_t, const int64_t* t
   for (int l = 0; l < pn->L; ++l) {
     PoseNetLayerDev& d = pn->layers[l];
     if ((rc = run_gemm(pn, pn->g_qkv[l], d.qkv, rows, st)) != ROHM_OK) return rc;
-    if (pn->tc_attention && S <= kAtKeys) {
-      if ((rc = run_attention_tc(pn, B, S, st)) != ROHM_OK) return rc;
+    if (pn->tc_attention && S <= kAwKeys) {
+      if ((rc = run_attention_wgmma(pn, B, S, st)) != ROHM_OK) return rc;
     } else {
       if ((rc = run_attention(pn, B, S, st)) != ROHM_OK) return rc;
     }

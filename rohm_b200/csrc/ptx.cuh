@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), fences.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma, clusters, fences.
 // Everything here is device-only and header-only.
 #pragma once
 #include <cstdint>
@@ -128,106 +128,47 @@ __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bu
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads
+// wgmma: warpgroup MMA, operands in shared memory, FP32 accumulators in registers
 // ----------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: power of two in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// Register layout of an m64nN accumulator d[N / 2] in warp w (0..3) of the warpgroup, lane l: element i sits at row
+// 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + (i % 2).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
+// Keeps the compiler from touching accumulator registers across an asynchronous wgmma (they are written behind its back).
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// Register budget of a warpgroup (all four warps execute it): producers give registers back, MMA warpgroups take them.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
 }
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
 }
-// D[tmem] (+)= A[smem desc] * B[smem desc], TF32 inputs, FP32 accumulate, single CTA.
-__device__ __forceinline__ void mma_tf32_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
+// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      ".reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n\t"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(cta)
       : "memory");
 }
-// F16 / BF16 inputs (the instruction descriptor says which), FP32 accumulate.
-__device__ __forceinline__ void mma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed.
-// (Implies tcgen05.fence::before_thread_sync.)
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// The same arrival delivered to the mbarrier at this shared-memory offset in every CTA of the cluster selected by cta_mask.
-__device__ __forceinline__ void mma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp receives lane (base_lane + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x4(uint32_t taddr, uint32_t (&v)[4]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// ----------------------------------------------------------------------------------------------
-// Descriptors
-// ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a K-major tile whose rows are exactly one swizzle span of kRowBytes (128 ->
-// SWIZZLE_128B, 64 -> SWIZZLE_64B): 8-row core groups are 8 * kRowBytes apart.  Field layout of the sm_100 descriptor:
-// start_address[0,14) (>>4), LBO[16,30) (ignored for swizzled K-major, set to 1), SBO[32,46) (>>4), version[46,48)=1,
-// layout_type[61,64): 2 = SWIZZLE_128B, 4 = SWIZZLE_64B.
+// Shared-memory matrix descriptor of a K-major tile whose rows are exactly one swizzle span of kRowBytes (128 ->
+// 128B swizzle, 64 -> 64B swizzle), as TMA writes it: 8-row core groups are 8 * kRowBytes apart.  sm_90 layout:
+// start_address[0,14) (>>4), LBO[16,30) (unused for swizzled K-major, 1), SBO[32,46) (>>4), layout[62,64): 1 = 128B,
+// 2 = 64B.  Advancing K by 32 bytes inside the span is +2 on the descriptor.
 template <int kRowBytes>
 __device__ __forceinline__ uint64_t make_desc_kmajor(uint32_t smem_addr) {
   static_assert(kRowBytes == 128 || kRowBytes == 64, "row = one swizzle span");
@@ -235,26 +176,67 @@ __device__ __forceinline__ uint64_t make_desc_kmajor(uint32_t smem_addr) {
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>((8 * kRowBytes) >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(kRowBytes == 128 ? 2 : 4) << 61;
+  d |= static_cast<uint64_t>(kRowBytes == 128 ? 1 : 2) << 62;
   return d;
 }
-// MN-major operand (the MN extent is the contiguous one) in SWIZZLE_128B atoms of 8 K-rows x 128 bytes: LBO = byte distance
-// between atoms along MN (the next 64 16-bit elements), SBO = byte distance between atoms along K (the next 8 rows).
+
+// MN-major operand (the MN extent is contiguous) in 128B-swizzle atoms of 8 K-rows x 128 bytes: LBO = byte distance between
+// atoms along MN (the next 64 16-bit elements), SBO = byte distance between atoms along K (the next 8 rows).
 __device__ __forceinline__ uint64_t make_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor (32-bit): c_format[4,6), a_format[7,10), b_format[10,13), a_major[15], b_major[16],
-// n_dim[17,23) = N>>3, m_dim[24,29) = M>>4.  Formats: 0=F16, 1=BF16, 2=TF32; C: 1=F32.  Both operands K-major.
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t ab_format, uint32_t M, uint32_t N, bool b_mn_major = false) {
-  return (1u << 4) | (ab_format << 7) | (ab_format << 10) | (b_mn_major ? (1u << 16) : 0u) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
+
+// Operand lists of the wgmma wrappers below: accumulator registers %0.. in blocks of 16, "+f" constraints in blocks of 16.
+#define ROHM_R16_0 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+#define ROHM_R16_1 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define ROHM_R16_2 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+#define ROHM_R16_3 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define ROHM_R16_4 "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
+#define ROHM_F4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define ROHM_F16(i) ROHM_F4(i), ROHM_F4(i + 4), ROHM_F4(i + 8), ROHM_F4(i + 12)
+#define ROHM_PRED(n) "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #n ", 0;\n\t"
+
+// D (+)= A * B for one m64nNk16 (fp16) / m64nNk8 (tf32) step, both operands K-major in shared memory.
+#define ROHM_WGMMA_SS(KIND, INSTR, R, REGS, A, B, P, IMM, ...)                                                       \
+  __device__ __forceinline__ void wgmma_##KIND(float (&d)[R], uint64_t desc_a, uint64_t desc_b) {                 \
+    asm volatile(ROHM_PRED(P) INSTR " {" REGS "}, %" #A ", %" #B ", p" IMM ";\n\t}\n"                           \
+                 : __VA_ARGS__                                                                                    \
+                 : "l"(desc_a), "l"(desc_b), "r"(1));                                                             \
+  }
+ROHM_WGMMA_SS(f16, "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16", 16, ROHM_R16_0, 16, 17, 18, ", 1, 1, 0, 0",
+              ROHM_F16(0))
+ROHM_WGMMA_SS(f16, "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16", 32, ROHM_R16_0 ", " ROHM_R16_1, 32, 33, 34,
+              ", 1, 1, 0, 0", ROHM_F16(0), ROHM_F16(16))
+ROHM_WGMMA_SS(f16, "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16", 48,
+              ROHM_R16_0 ", " ROHM_R16_1 ", " ROHM_R16_2, 48, 49, 50, ", 1, 1, 0, 0", ROHM_F16(0), ROHM_F16(16), ROHM_F16(32))
+ROHM_WGMMA_SS(f16, "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16", 64,
+              ROHM_R16_0 ", " ROHM_R16_1 ", " ROHM_R16_2 ", " ROHM_R16_3, 64, 65, 66, ", 1, 1, 0, 0", ROHM_F16(0),
+              ROHM_F16(16), ROHM_F16(32), ROHM_F16(48))
+// m64n160k16: the S = Q K^T product of the attention kernel
+ROHM_WGMMA_SS(f16, "wgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16", 80,
+              ROHM_R16_0 ", " ROHM_R16_1 ", " ROHM_R16_2 ", " ROHM_R16_3 ", " ROHM_R16_4, 80, 81, 82, ", 1, 1, 0, 0",
+              ROHM_F16(0), ROHM_F16(16), ROHM_F16(32), ROHM_F16(48), ROHM_F16(64))
+ROHM_WGMMA_SS(tf32, "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32", 16, ROHM_R16_0, 16, 17, 18, ", 1, 1", ROHM_F16(0))
+ROHM_WGMMA_SS(tf32, "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32", 32, ROHM_R16_0 ", " ROHM_R16_1, 32, 33, 34,
+              ", 1, 1", ROHM_F16(0), ROHM_F16(16))
+ROHM_WGMMA_SS(tf32, "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32", 48, ROHM_R16_0 ", " ROHM_R16_1 ", " ROHM_R16_2,
+              48, 49, 50, ", 1, 1", ROHM_F16(0), ROHM_F16(16), ROHM_F16(32))
+ROHM_WGMMA_SS(tf32, "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32", 64,
+              ROHM_R16_0 ", " ROHM_R16_1 ", " ROHM_R16_2 ", " ROHM_R16_3, 64, 65, 66, ", 1, 1", ROHM_F16(0), ROHM_F16(16),
+              ROHM_F16(32), ROHM_F16(48))
+
+// m64n128k16 with A from registers (per warp the m16n8k16 A-fragment layout) and an MN-major B in shared memory: the
+// O = P V product of the attention kernel
+__device__ __forceinline__ void wgmma_f16_rs_tb(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b) {
+  asm volatile(ROHM_PRED(69) "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {" ROHM_R16_0 ", " ROHM_R16_1 ", " ROHM_R16_2
+               ", " ROHM_R16_3 "}, {%64, %65, %66, %67}, %68, p, 1, 1, 1;\n\t}\n"
+               : ROHM_F16(0), ROHM_F16(16), ROHM_F16(32), ROHM_F16(48)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
 }
 
 // Round-to-nearest TF32 (10-bit mantissa), result kept in an fp32 container.

@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(kThreads) ddpm_step_philox_kernel(const float*
 }
 
 int grid_for(const rohm_ctx* ctx, int64_t work_items) {
-  const int sms = ctx->sm_count > 0 ? ctx->sm_count : 148;
+  const int sms = ctx->sm_count > 0 ? ctx->sm_count : 132;
   int64_t blocks = (work_items + kThreads - 1) / kThreads;
   const int64_t cap = static_cast<int64_t>(sms) * 8;  // 8 resident CTAs of 256 threads per SM
   if (blocks > cap) blocks = cap;
@@ -145,7 +145,7 @@ extern "C" int rohm_ddpm_step(rohm_ctx* ctx, const float* x0, const float* x_t, 
   if (n_clips == 0 || clip_elems == 0) return ROHM_OK;
   const bool vec = (clip_elems % 4 == 0) && aligned16(x0) && aligned16(x_t) && aligned16(noise) && aligned16(out) &&
                    (n_grads < 1 || aligned16(grad0)) && (n_grads < 2 || aligned16(grad1));
-  const int sms = ctx->sm_count > 0 ? ctx->sm_count : 148;
+  const int sms = ctx->sm_count > 0 ? ctx->sm_count : 132;
   const int64_t items = vec ? clip_elems / 4 : clip_elems;
   int64_t bx = (items + kThreads - 1) / kThreads;
   const int64_t cap = (static_cast<int64_t>(sms) * 8 + n_clips - 1) / n_clips;  // ~8 resident CTAs per SM in total

@@ -7,9 +7,9 @@
 //   * channel concat [x, skip]  = two K-segments of one GEMM,
 //   * Downsample (k3, stride 2) = the same with a row-stride-2 TMA descriptor,
 //   * ConvTranspose (k4, s2)    = two GEMMs (even / odd output frames), 2 taps each, row-interleaved stores,
-// so every convolution is one launch of the tcgen05 segmented-A GEMM (gemm.cu) and no im2col / concat / transpose
+// so every convolution is one launch of the wgmma segmented-A GEMM (gemm.cu) and no im2col / concat / transpose
 // buffer exists.  The convolutions of the deep pyramid levels are cut along K into 3-6 ranges (pick_split: 128-wide tiles x K
-// ranges cover the 148 SMs where 6-22 row tiles alone cannot); one kernel per GroupNorm'd convolution (gn_mish_split_kernel, a
+// ranges cover the SMs where 6-22 row tiles alone cannot); one kernel per GroupNorm'd convolution (gn_mish_split_kernel, a
 // CTA per (clip, group)) adds bias + the fp32 partial(s) in split order, takes the group's statistics, applies GroupNorm + Mish
 // (+ time projection, + residual, + TrajControl residual) and emits the hi/lo operand pair of the next convolution.  The
 // step-invariant condition pyramid and control_zero_conv_0 run once per condition (set_cond).  rohm_trajnet_sample_step appends
@@ -90,7 +90,7 @@ __device__ __forceinline__ void trajnet_time_compute(float t, int b, int time_di
 }
 
 // Per step the embedding depends on the (integer) timestep only, so the whole path is tabulated at create time for
-// t in [0, table_rows) (the direct evaluation took 89 us per forward, latency-bound) and the per-forward kernel is a row
+// t in [0, table_rows) (the direct evaluation is latency-bound) and the per-forward kernel is a row
 // gather; timesteps outside the table are evaluated directly.  `table` == nullptr: always evaluate (used to build the table).
 __global__ void __launch_bounds__(256) trajnet_time_kernel(const int64_t* __restrict__ time, int time_dim,
                                                            const float* __restrict__ w1, const float* __restrict__ b1,
@@ -410,11 +410,11 @@ struct rohm_trajnet {
   float* scratchSplit[2] = {nullptr, nullptr};
   bool use_splitk = true;
   // GroupNorm statistics inside the GroupNorm kernel (one CTA per (clip, group), the split-K consumer with one "partial") for
-  // every GroupNorm'd convolution, instead of per-chunk double atomics in the GEMM epilogue: the epilogue of a small
-  // convolution drops from 3.4-5.0 us to 1.7-2.2 us (CTA timelines, ROHM_B200_TRAJ_TS).  ROHM_B200_TRAJ_GN_EPILOGUE=1: old path.
+  // every GroupNorm'd convolution, instead of per-chunk double atomics in the GEMM epilogue, which keeps the epilogue of a
+  // small convolution short.  ROHM_B200_TRAJ_GN_EPILOGUE=1: statistics in the GEMM epilogue.
   bool gn_in_kernel = true;
   // The forward is captured as a graph with parallel branches: the TrajControl branch next to the U-Net encoder, every
-  // block's 1x1 residual convolution next to its conv1 -> GroupNorm -> conv2 chain.  None of these GEMMs fills the 148 SMs
+  // block's 1x1 residual convolution next to its conv1 -> GroupNorm -> conv2 chain.  None of these GEMMs fills the 132 SMs
   // (11 to 96 tiles), so running them side by side shortens the critical path at no cost.  ROHM_B200_TRAJ_PARALLEL=0: serial.
   bool parallel = true;
   cudaStream_t side[3] = {nullptr, nullptr, nullptr};  // 0: TrajControl branch, 1 / 2: residual convolutions of branch 0 / 1
@@ -504,8 +504,10 @@ int make_act(rohm_trajnet* tn, const std::string& name, int C, int level, bool w
   return ROHM_OK;
 }
 
+constexpr int kModelSms = 132;  // H100 SXM: the wave size of the tile-count models below
+
 // Output-tile width of a convolution GEMM.  The deep pyramid levels have few 128-row tiles (11 at level 3 with 64 clips), so
-// 128-wide tiles would leave most of the 148 SMs idle; a narrower tile multiplies the tile count at a modest cost per tile
+// 128-wide tiles would leave most of the SMs idle; a narrower tile multiplies the tile count at a modest cost per tile
 // (operand fill per 32 K-columns: 32 KB of A + BLOCK_N / 4 KB of B).  Choose the width that minimises waves x fill.
 int pick_bn(int N, int64_t rows) {
   const int64_t m_tiles = (rows + kGemmBlockM - 1) / kGemmBlockM;
@@ -514,27 +516,29 @@ int pick_bn(int N, int64_t rows) {
   for (int bn : {128, 64, 32}) {
     if (bn > 32 && bn > N) continue;
     const int64_t tiles = m_tiles * ((N + bn - 1) / bn);
-    const double cost = static_cast<double>((tiles + 147) / 148) * (32.0 + bn / 4.0);
+    const double cost = static_cast<double>((tiles + kModelSms - 1) / kModelSms) * (32.0 + bn / 4.0);
     if (best == 0 || cost < best_cost) best = bn, best_cost = cost;
   }
   return best;
 }
 
-// Split-K choice for a GroupNorm'd convolution (conv1 / conv2 of a ResidualTemporalBlock) with `stages` K blocks.  On the deep
-// levels a tile's K loop (40 to 80 stages of 64 columns) is the whole launch: cutting it into S ranges lets 128-wide tiles
-// (the cheapest per flop: the A stripe is read once per 128 columns) still cover the 148 SMs.  Model, in us: one wave of work
-// items costs (stages / S) * t_stage(bn) + fixed launch / prologue / epilogue; the consumer reads S partials.
+// Split-K choice for a GroupNorm'd convolution (conv1 / conv2 of a ResidualTemporalBlock) with `stages` K blocks of `blk_cols`
+// columns.  On the deep levels a tile's K loop (2560 to 5120 columns) is the whole launch: cutting it into S ranges lets
+// 128-wide tiles (the cheapest per flop: the A stripe is read once per 128 columns) still cover the SMs.  Model, in us: one
+// wave of work items costs (columns / S / 64) * t64(bn) + fixed launch / prologue / epilogue; the consumer reads S partials.
+// The per-64-column times t64 and the fixed costs are estimates, not H100 measurements.
 // Returns S (1 = keep the single-pass path and pick_bn's width); *bn_out is only written when S > 1.
 constexpr int kMaxSplits = kMaxSplitsDev;
-int pick_split(int N, int64_t rows, int stages, int* bn_out, double extra_us = 0.0) {
-  if (stages < 16 || N % 32 != 0) return 1;
+int pick_split(int N, int64_t rows, int stages, int blk_cols, int* bn_out, double extra_us = 0.0) {
+  const double unit = blk_cols / 64.0;  // K blocks -> 64-column units of the model
+  if (stages * unit < 16 || N % 32 != 0) return 1;
   const int64_t m_tiles = (rows + kGemmBlockM - 1) / kGemmBlockM;
-  auto t_stage = [](int bn) { return bn == 128 ? 0.60 : bn == 64 ? 0.42 : 0.41; };  // measured (ROHM_B200_TRAJ_TS): A-bound below 128
+  auto t64 = [](int bn) { return bn == 128 ? 0.60 : bn == 64 ? 0.42 : 0.41; };  // A-bound below 128 (estimate)
   const double t_fixed = 4.5, t_partial = 0.4;
   auto cost = [&](int bn, int S) {
     const int64_t items = m_tiles * ((N + bn - 1) / bn) * S;
     const int per = (stages + S - 1) / S;
-    return static_cast<double>((items + 147) / 148) * (per * t_stage(bn) + t_fixed) + (S > 1 ? S * t_partial : 0.0);
+    return static_cast<double>((items + kModelSms - 1) / kModelSms) * (per * unit * t64(bn) + t_fixed) + (S > 1 ? S * t_partial : 0.0);
   };
   const int bn1 = pick_bn(N, rows);
   const double base = cost(bn1, 1);
@@ -544,7 +548,7 @@ int pick_split(int N, int64_t rows, int stages, int* bn_out, double extra_us = 0
     if (bn > N || N % bn != 0) continue;
     for (int S = 2; S <= kMaxSplits; ++S) {
       const int per = (stages + S - 1) / S;
-      if (per < 4 || (S - 1) * per >= stages) continue;  // at least 4 stages per item, no empty range
+      if (per * unit < 4 || (S - 1) * per >= stages) continue;  // at least 256 columns per item, no empty range
       const double c = cost(bn, S);
       if (c < best) best = c, best_bn = bn, best_S = S;
     }
@@ -589,7 +593,7 @@ int make_conv(rohm_trajnet* tn, const std::string& name, const std::string& wkey
   const bool can_split = tn->use_splitk && kind == 0 && out->ld == Cout && Cout % 4 == 0;
   if (can_split && ((with_stats && stride == 1 && out->f32 != nullptr && out->hi == nullptr) || (!with_stats && ks > 1))) {
     int bn = pw.block_n;
-    cv.splits = pick_split(Cout, rows_of(tn, out->level), Ktot / kblk, &bn, with_stats ? 0.0 : 4.0);
+    cv.splits = pick_split(Cout, rows_of(tn, out->level), Ktot / kblk, kblk, &bn, with_stats ? 0.0 : 4.0);
     if (cv.splits > 1) {
       pw.block_n = bn;
       if (!with_stats) cv.sum_after = true, cv.sum_out = *out;

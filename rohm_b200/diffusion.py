@@ -1,4 +1,4 @@
-"""Gaussian diffusion samplers for PoseNet and TrajNet on the B200 engines.
+"""Gaussian diffusion samplers for PoseNet and TrajNet on the CUDA engines.
 
 API-compatible with the reference classes (diffusion/gaussian_diffusion_posenet.py ``GaussianDiffusionPoseNet``,
 diffusion/gaussian_diffusion_trajnet.py ``GaussianDiffusionTrajNet``, diffusion/respace.py ``SpacedDiffusion*`` and

@@ -1,7 +1,7 @@
 """Shadows the reference's data_loaders/motion_representation.py: everything the drivers import from it with
 ``from data_loaders.motion_representation import *`` keeps coming from the reference's own file (found further down
 ``sys.path``: cano_seq_smplx, get_repr_smplx, foot_detect, ...), except ``recover_from_repr_smpl`` (:332-398), which is routed
-to the B200 kernels whenever its inputs live on a CUDA device (test_amass_full.py:292, 406, 416-418, 428).
+to the CUDA kernels whenever its inputs live on a CUDA device (test_amass_full.py:292, 406, 416-418, 428).
 """
 import importlib.util
 import os

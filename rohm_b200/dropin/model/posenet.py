@@ -1,2 +1,2 @@
-"""Shadows the reference's model/posenet.py with the B200 implementation."""
+"""Shadows the reference's model/posenet.py with the CUDA implementation."""
 from rohm_b200.posenet import PoseNet  # noqa: F401

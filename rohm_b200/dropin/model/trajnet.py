@@ -1,2 +1,2 @@
-"""Shadows the reference's model/trajnet.py with the B200 implementation."""
+"""Shadows the reference's model/trajnet.py with the CUDA implementation."""
 from rohm_b200.trajnet import ControlNet, TrajNet  # noqa: F401

@@ -1,4 +1,4 @@
-"""``recover_from_repr_smpl`` on the B200 kernels: drop-in for the one function of
+"""``recover_from_repr_smpl`` on the CUDA kernels: drop-in for the one function of
 data_loaders/motion_representation.py (:332-398) that the inference drivers call between and after the sampling loops
 (test_amass_full.py:292, 406, 416-418, 428; test_posenet.py / test_trajnet.py through compute_losses_with_smpl).
 
@@ -75,7 +75,7 @@ def recover_from_repr_smpl(data_dict, recover_mode='joint_abs_traj', smplx_model
         return j.reshape(lead + (22, 3))
     if return_full_joints:
         raise RohmB200Error("recover_from_repr_smpl(return_full_joints=True): the 72 landmark joints beyond the 55 "
-                            "kinematic ones are not evaluated by the B200 body kernels (no inference driver asks for them)")
+                            "kinematic ones are not evaluated by the CUDA body kernels (no inference driver asks for them)")
     if smplx_model is None:
         raise RohmB200Error("recover_from_repr_smpl('smplx_params') needs smplx_model")
     from .body_model import kernels_for

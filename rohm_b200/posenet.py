@@ -3,7 +3,7 @@ with the forward pass executed by the CUDA engine behind ``rohm_posenet_*`` (inc
 
 The module owns its parameters in torch containers named exactly like the reference so ``load_state_dict(strict=True)``
 works on released checkpoints; on the first forward (and whenever parameters change) they are repacked into the
-engine's TF32 hi/lo layout.  There is no eager / CPU forward: calling the model without a B200 raises.
+engine's TF32 hi/lo layout.  There is no eager / CPU forward: calling the model without an H100 raises.
 """
 import ctypes as C
 import os

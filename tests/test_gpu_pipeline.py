@@ -135,7 +135,7 @@ def test_pipeline_flag_variants_run(cuda_device):
 def test_guided_tail_at_benchmark_size(cuda_device):
     """Guided tail of the PoseNet sampler at the benchmark size: 32 clips x 143 frames, respaced steps t = 50 .. 0 of the
     1000-step schedule, in-loop skating guidance on every step, CUDA path vs the CPU oracle fed the same noise.
-    Free-running and teacher-forced errors are printed (committed under profiles/); only what is well-posed is asserted:
+    Free-running and teacher-forced errors are printed; only what is well-posed is asserted:
     every teacher-forced step and the unguided chain."""
     dev = cuda_device
     B, T = 32, 143

@@ -54,8 +54,8 @@ def test_forward_matches_reference_golden(posenet, cuda_device):
         assert err < TOL, (c, err)
 
 
-# T + 1 tokens per clip: 128 / 129 straddle the query-tile boundary of the tcgen05 attention kernel, 160 is its largest clip,
-# 161 and 201 take the mma.sync / SIMT fallbacks
+# T + 1 tokens per clip: 128 / 129 straddle a 64-query tile boundary of the wgmma attention kernel, 160 is its largest
+# clip, 161 and 201 take the mma.sync / SIMT fallbacks
 @pytest.mark.parametrize("B,T", [(1, 1), (2, 7), (3, 143), (5, 144), (2, 127), (2, 128), (3, 159), (1, 160), (2, 200)])
 def test_forward_matches_oracle(posenet, cuda_device, B, T):
     m, sd = posenet
@@ -363,7 +363,7 @@ def test_prox_guidance_schedule_runs_both_terms(posenet, cuda_device):
 
 def test_in_kernel_noise_is_torchs_own_stream(cuda_device):
     """rohm_ddpm_step_philox draws what torch.randn_like would have drawn (same values, same generator advance), for sizes
-    below / at / above one pass of torch's grid (148 SMs x 8 blocks x 256 threads x 4)."""
+    below / at / above one pass of torch's grid (SMs x 8 blocks x 256 threads x 4)."""
     dev = cuda_device
     gen = torch.cuda.default_generators[dev.index]
     for shape in [(1, 7, 1, 3), (2, 294, 1, 16), (32, 294, 1, 144), (128, 294, 1, 144), (64, 144, 13)]:

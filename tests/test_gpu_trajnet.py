@@ -1,4 +1,4 @@
-"""GPU parity tests for the TrajNet / TrajControl engine (conv-as-GEMM on tcgen05) and its sampling loop."""
+"""GPU parity tests for the TrajNet / TrajControl engine (conv-as-GEMM on wgmma) and its sampling loop."""
 import argparse
 
 import numpy as np

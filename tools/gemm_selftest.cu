@@ -1,5 +1,5 @@
-// Standalone numerics + timing check of the tcgen05 3xTF32 GEMM (rohm_b200/csrc/gemm.cu) against a CPU fp64
-// reference.  Build:  make -C tools   Run on a B200:  tools/gemm_selftest
+// Standalone numerics + timing check of the wgmma 3xTF32 GEMM (rohm_b200/csrc/gemm.cu) against a CPU fp64
+// reference.  Build:  make -C tools   Run on an H100:  tools/gemm_selftest
 // Cases: plain linear layers (PoseNet shapes), ragged K/N tails, multi-segment shifted reads (Conv1d k=5 over a
 // padded-clip layout), stride-2 reads (Downsample1d), GroupNorm statistics, hi/lo split outputs.
 #include <cmath>
@@ -264,7 +264,7 @@ static void case_linear_f16(int M, int N, int K, int block_n, int act, bool with
     printf("    timing: %.2f us/launch  -> %.1f TFLOP/s algorithmic (fp16 hi/lo, 3 tensor passes)\n", us, 2.0 * M * N * K / us * 1e-6);
     unsigned long long* dts;
     CK(cudaMalloc(&dts, 32 * sizeof(unsigned long long)));
-    // flags 1 / 2: developer experiments that break the result (epilogue drains TMEM only / stages without storing) -- they
+    // flags 1 / 2: developer experiments that break the result (epilogue drains the accumulator only / stages without storing) -- they
     // show how much of the main loop's steady-state slowdown comes from the concurrent epilogue of the previous tile
     for (int flags = 0; flags < (tma_mode == 2 && N >= 1024 ? 3 : 1); ++flags) {
       p.debug_flags = flags;
@@ -643,9 +643,9 @@ int main() {
     cudaEvent_t e0, e1;
     CK(cudaEventCreate(&e0));
     CK(cudaEventCreate(&e1));
-    for (int i = 0; i < 10; ++i) empty_kernel<<<148, 320>>>();
+    for (int i = 0; i < 10; ++i) empty_kernel<<<132, 384>>>();
     CK(cudaEventRecord(e0));
-    for (int i = 0; i < 200; ++i) empty_kernel<<<148, 320>>>();
+    for (int i = 0; i < 200; ++i) empty_kernel<<<132, 384>>>();
     CK(cudaEventRecord(e1));
     CK(cudaEventSynchronize(e1));
     float ms;

@@ -17,6 +17,6 @@ for row in rows[2:]:
     n += 1
 json.dump({"kernel": pattern, "launches_captured": n, "dram_bytes_per_launch": tot / n, "mean_us_under_ncu": us / n,
            "source": rep.split("/")[-1], "note": "ncu --set full, cold caches (ncu flushes L2 between replays): every "
-           "operand is fetched from DRAM once; in the running loop the weights and most activations stay in the 126 MB L2"},
+           "operand is fetched from DRAM once; in the running loop part of the weights and activations stays in the 50 MB L2"},
           open(dst, "w"), indent=1)
 print(open(dst).read())
