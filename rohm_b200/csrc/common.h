@@ -59,6 +59,24 @@ class DeviceGuard {
   bool restore_ = false;
 };
 
+// Kernel launch with the programmatic-dependent-launch attribute (the kernel must call griddepcontrol.wait before it
+// touches memory, which every kernel launched through here does).
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_chain(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl,
+                                Args... args) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = pdl ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+}
+
 // Owns a set of cudaMalloc'ed buffers; frees them on destruction.
 class DevicePool {
  public:

@@ -109,6 +109,54 @@ def test_mma_sync_attention_fallback_matches_oracle(posenet, cuda_device, monkey
     assert float((y - ref).abs().max()) < TOL
 
 
+@pytest.mark.parametrize("env", [{"ROHM_B200_TC_ATTENTION": "0"}, {"ROHM_B200_MULTICAST": "1"}, {"ROHM_B200_TMA_STORE": "0"},
+                                 {"ROHM_B200_FUSED_LN": "0"}])
+def test_engine_switches_match_oracle(posenet, cuda_device, monkeypatch, env):
+    """The engines behind the library's switches: ROHM_B200_TC_ATTENTION=0 routes f16x2 attention to the mma.sync m16n8k16
+    kernel, ROHM_B200_MULTICAST=1 shares the GEMMs' A tiles across CTA pairs, ROHM_B200_TMA_STORE=0 keeps the per-thread
+    store epilogue (and with it the separate LayerNorm kernel), ROHM_B200_FUSED_LN=0 the separate LayerNorm kernel alone.
+    32 clips x 145 tokens: 37 row tiles, so the persistent GEMMs run several rounds per launch."""
+    m, sd = posenet
+    B, T = 32, 144
+    gen = torch.Generator().manual_seed(31337)
+    x = torch.randn(B, 294, 1, T, generator=gen)
+    cond = synthetic.posenet_batch(B, T, 11)['cond']
+    ts = torch.randint(0, 1000, (B,), generator=gen)
+    ref = posenet_oracle.posenet_forward(sd, x, cond, ts)
+    for k, v in env.items():
+        monkeypatch.setenv(k, v)
+    m.invalidate_engine()
+    try:
+        y = m({'x_t': x.to(cuda_device), 'cond': cond.to(cuda_device)}, ts.to(cuda_device)).cpu()
+    finally:
+        for k in env:
+            monkeypatch.delenv(k)
+        m.invalidate_engine()
+    assert float((y - ref).abs().max()) < TOL
+
+
+def test_launch_switches_do_not_change_the_result(posenet, cuda_device):
+    """Programmatic dependent launch and CUDA-graph replay only change how the kernels are scheduled: the forward must be
+    bit-identical with either switched off (rohm_posenet_set_option 1 / 0)."""
+    m, _ = posenet
+    B, T = 5, 144
+    gen = torch.Generator().manual_seed(41)
+    x = torch.randn(B, 294, 1, T, generator=gen).to(cuda_device)
+    cond = synthetic.posenet_batch(B, T, 3)['cond'].to(cuda_device)
+    ts = torch.randint(0, 1000, (B,), generator=gen).to(cuda_device)
+    ref = m({'x_t': x, 'cond': cond}, ts).clone()
+    eng = m._engine
+    try:
+        for option in (1, 0):
+            assert eng.lib.rohm_posenet_set_option(eng.handle, option, 0) == 0
+            assert torch.equal(m({'x_t': x, 'cond': cond}, ts), ref)
+            assert eng.lib.rohm_posenet_set_option(eng.handle, option, 1) == 0
+            assert torch.equal(m({'x_t': x, 'cond': cond}, ts), ref)
+    finally:
+        eng.lib.rohm_posenet_set_option(eng.handle, 0, 1)
+        eng.lib.rohm_posenet_set_option(eng.handle, 1, 1)
+
+
 def test_forward_noncontiguous_inputs_and_cond_updates(posenet, cuda_device):
     """The driver builds cond by permute(0,2,1).unsqueeze(-2) (non-contiguous) and edits it in place between rounds."""
     m, sd = posenet
@@ -295,14 +343,15 @@ def test_recycled_condition_address_is_not_mistaken_for_the_cached_one(posenet, 
 
 def test_out_of_range_timestep_poisons_the_output(posenet, cuda_device):
     """The reference raises on pe[t] with a bad t; the kernel cannot raise, so it must not return a plausible embedding."""
-    m, _ = posenet
+    m, sd = posenet
     B, T = 2, 8
     cond = synthetic.posenet_batch(B, T, 9)['cond'].to(cuda_device)
     x = torch.randn(B, 294, 1, T, device=cuda_device)
     y = m({'x_t': x, 'cond': cond}, torch.tensor([5, 5000], device=cuda_device))
-    # (clips that share an attention key tile with the poisoned one may turn NaN too -- 0 x NaN in the masked key columns --
-    # which is still "the call failed", as the reference's IndexError is for the whole batch)
     assert bool(torch.isnan(y[1, 22:]).all())
+    # the poison stays in its clip: attention reads only the clip's own rows (the next clip lies inside clip 0's key tile)
+    ref0 = posenet_oracle.posenet_forward(sd, x[:1].cpu(), cond[:1].cpu(), torch.tensor([5]))
+    assert float((y[:1].cpu() - ref0).abs().max()) < TOL
     ok = m({'x_t': x, 'cond': cond}, torch.tensor([5, 4999], device=cuda_device))
     assert bool(torch.isfinite(ok).all())
     with pytest.raises(Exception):
