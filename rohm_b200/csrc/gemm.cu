@@ -12,9 +12,22 @@ namespace rohm {
 
 namespace {
 
-constexpr int kEpiWarps = 8;  // the two MMA warpgroups, which also run the epilogue
-constexpr int kFirstEpiWarp = 4;
-constexpr int kThreads = 32 * (kFirstEpiWarp + kEpiWarps);  // warpgroup 0: TMA producer (one lane); 1, 2: MMA + epilogue
+// Warp roles.  Warpgroup 0: TMA producer (one lane).  Warpgroups 1, 2 (warps 4-11): wgmma, 64 tile rows each.
+// EPI 0, 1, 3 (the lean variants the PoseNet forward runs): warpgroup 3 (warps 12-15) is a dedicated epilogue, one tile row
+// per thread, so the MMA warpgroups go straight on to the next tile's K loop while it runs (512 threads).
+// EPI 2 (TrajNet: split-K, GroupNorm sums, padded clips) and EPI 4 (skinning, ~168 registers per epilogue thread): the MMA
+// warpgroups run the epilogue themselves, after the tile's MMAs (384 threads) -- these epilogues do not fit the register
+// budget of an epilogue warpgroup next to two MMA warpgroups.
+constexpr int kFirstMmaWarp = 4;
+constexpr int kMmaWarps = 8;
+constexpr int kFirstEpiWarp = kFirstMmaWarp + kMmaWarps;  // the dedicated epilogue warpgroup
+__host__ __device__ constexpr bool epi_role(int epi) { return epi == 0 || epi == 1 || epi == 3; }
+__host__ __device__ constexpr int kernel_threads(int epi) { return 32 * (kFirstEpiWarp + (epi_role(epi) ? 4 : 0)); }
+// setmaxnreg budgets of the 512-thread variants: producer + epilogue + 2 x MMA <= 65536 / 128 registers per thread
+// (a launch starts every thread at 65536 / 512 = 128: the producer gives registers back, the other roles take them)
+constexpr int kProducerRegs = 40, kEpiRoleRegs = 152, kMmaRegs = 160;
+static_assert(kProducerRegs + kEpiRoleRegs + 2 * kMmaRegs <= 512, "register file of one SM");
+static_assert(kProducerRegs <= 128 && kEpiRoleRegs >= 128 && kMmaRegs >= 128, "setmaxnreg.dec / .inc direction");
 constexpr int kSmemLimit = 227 * 1024;  // H100: dynamic + static shared memory of one block
 constexpr int kStaticSmemReserve = 8 * 1024;  // barriers, per-column vectors, skinning tables
 constexpr int kEpiTileFloats = 32 * 32;   // per-epilogue-warp staging tile (32 x 32, XOR-swizzled columns): coalesced stores
@@ -24,8 +37,9 @@ constexpr int kEpiTileFloats = 32 * 32;   // per-epilogue-warp staging tile (32 
 constexpr int kSkinPitch = 100;
 constexpr int kSkinStageBytes = kGemmBlockM * kSkinPitch * 4;
 
-template <int BLOCK_N, int PASSES>
+template <int BLOCK_N, int PASSES, bool EPI_ROLE>
 struct TileCfg {
+  static constexpr int kEpiWarps = EPI_ROLE ? 4 : 8;  // warps that run the epilogue, 32 tile rows each
   static constexpr int kABytes = kGemmBlockM * kGemmBlockK * 4;
   static constexpr int kBBytes = BLOCK_N * kGemmBlockK * 4;
   static constexpr int kSplit = (PASSES == 3) ? 2 : 1;
@@ -34,9 +48,11 @@ struct TileCfg {
   // writes and the row-per-thread 16-byte reads of the epilogue are at most 2-way conflicted) -> one row per thread.
   static constexpr int kAccPitch = BLOCK_N + 4;
   static constexpr int kAccBytes = kGemmBlockM * kAccPitch * 4;
-  // the epilogue staging area: per-warp 32 x 32 tiles, or (BLOCK_N = 96) the skinning epilogue's CTA-wide tile
-  static constexpr int kEpiBytes =
-      BLOCK_N == 96 && kSkinStageBytes > kEpiWarps * kEpiTileFloats * 4 ? kSkinStageBytes : kEpiWarps * kEpiTileFloats * 4;
+  // the epilogue staging area: per-warp 32 x 32 tiles, or (BLOCK_N = 96, 384-thread variants) the skinning epilogue's
+  // CTA-wide tile.  The four epilogue-warpgroup tiles leave room for 4 stages at BLOCK_N = 128 (3 with eight tiles).
+  static constexpr int kEpiBytes = !EPI_ROLE && BLOCK_N == 96 && kSkinStageBytes > kEpiWarps * kEpiTileFloats * 4
+                                       ? kSkinStageBytes
+                                       : kEpiWarps * kEpiTileFloats * 4;
   static constexpr int kStagesRaw = (kSmemLimit - kStaticSmemReserve - 1024 - kAccBytes - kEpiBytes) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 10 ? 10 : kStagesRaw;
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + kAccBytes + kEpiWarps * kEpiTileFloats * 4;
@@ -225,11 +241,18 @@ __device__ __forceinline__ void stage_pair_chunk(const float (&v)[32], uint8_t* 
 // LayerNorm with the row statistics exchanged between the four column-tile CTAs of a row stripe (PoseNet out-proj / FFN2,
 // see GemmParams::ln_gamma).  Separate instantiations keep the hot variants' code small (the full
 // epilogue is ~7000 SASS instructions, most of them predicated-off activation code when unused).
+//
+// EPI 0 / 1 / 3 hand the finished accumulator tile over through acc_s and two mbarriers: the MMA warpgroups wait on
+// acc_empty (the epilogue has read the previous tile) before they write acc_s, then arrive on acc_full and start the next
+// work item's K loop; the epilogue warpgroup stages the next tile's per-column vectors, row statistics and (EPI 3) residual
+// while those MMAs run, waits on acc_full, and arrives on acc_empty once it has read the tile.
 template <int BLOCK_N, int PASSES, int EPI, int KIND>
-__global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_constant__ GemmParams p) {
+__global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const __grid_constant__ GemmParams p) {
   constexpr bool LEAN = EPI != 2;  // EPI: 0 bias / stores, 1 + exact GELU, 2 everything (TrajNet), 3 LayerNorm-folding producer, 4 skinning
-  constexpr int kElemK = gemm_block_k(KIND);  // K elements per pipeline stage (TMA coordinates are in elements)  // EPI: 0 = bias/residual/stores, 1 = the same + exact GELU, 2 = everything
-  using Cfg = TileCfg<BLOCK_N, PASSES>;
+  constexpr bool EPI_ROLE = epi_role(EPI);  // a dedicated epilogue warpgroup (see kFirstMmaWarp)
+  constexpr int kElemK = gemm_block_k(KIND);  // K elements per pipeline stage (TMA coordinates are in elements)
+  using Cfg = TileCfg<BLOCK_N, PASSES, EPI_ROLE>;
+  constexpr int kEpiWarps = Cfg::kEpiWarps;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t full_bar[Cfg::kStages];
   __shared__ uint64_t empty_bar[Cfg::kStages];
@@ -242,6 +265,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
   __shared__ __align__(16) float corr_s[BLOCK_N];
   __shared__ __align__(16) float beta_s[EPI == 3 ? BLOCK_N : 4];
   __shared__ uint64_t res_bar[EPI == 3 ? kEpiWarps : 1];  // EPI 3: one transaction barrier per epilogue warp (residual tile loads)
+  __shared__ uint64_t acc_full, acc_empty;  // EPI_ROLE: the acc_s hand-over between the MMA and the epilogue warpgroups
   // EPI 4 (skinning): the current column tile's bone list and dense [bone][vertex] weights
   __shared__ __align__(16) float skin_w_s[EPI == 4 ? 2 : 1][EPI == 4 ? kSkinTileBones * 32 : 4];  // double-buffered across tiles
   __shared__ int skin_bone_s[EPI == 4 ? 2 : 1][EPI == 4 ? kSkinTileBones : 1];
@@ -283,6 +307,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
     }
     if (EPI == 3)
       for (int i = 0; i < kEpiWarps; ++i) ptx::mbar_init(&res_bar[i], 1);
+    if (EPI_ROLE) {
+      ptx::mbar_init(&acc_full, kMmaWarps);  // one arrival per warp
+      ptx::mbar_init(&acc_empty, kEpiWarps);
+    }
     ptx::fence_barrier_init();
   }
   // The B operand is a weight matrix that no kernel of the chain writes: the producer thread puts the B tiles of the first
@@ -303,7 +331,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         ptx::tma_load_2d(st + 2 * Cfg::kABytes + Cfg::kBBytes, &p.b_lo, &full_bar[i], (it_b + i) * kElemK, n0);
     }
   }
-  if (warp_idx == kFirstEpiWarp && lane == 0) {
+  if (warp_idx == kFirstMmaWarp && lane == 0) {
     epi_s.bias = p.bias, epi_s.residual = p.residual, epi_s.ldr = p.ldr, epi_s.out = p.out, epi_s.ldo = p.ldo;
     epi_s.out_hi = p.out_hi, epi_s.out_lo = p.out_lo, epi_s.lds = p.lds, epi_s.act = p.act, epi_s.M = p.M, epi_s.N = p.N;
     epi_s.out_row_mul = p.out_row_mul, epi_s.out_row_add = p.out_row_add, epi_s.clip_rows = p.clip_rows;
@@ -330,9 +358,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
   ptx::pdl_launch_dependents();
   ptx::pdl_wait_prior_grid();
 
-  if (warp_idx < kFirstEpiWarp) {
+  if (warp_idx < kFirstMmaWarp) {
     // ===================== TMA producer (warpgroup 0, one lane) =====================
-    ptx::setmaxnreg_dec<40>();
+    ptx::setmaxnreg_dec<kProducerRegs>();
     if (warp_idx == 0 && lane == 0) {
       int it = 0, stage = 0;
       uint32_t phase = 0;
@@ -386,19 +414,27 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
       }
     }
   } else {
-    // ===================== MMA + epilogue (warpgroups 1, 2) =====================
-    ptx::setmaxnreg_inc<232>();
-    const int ew = warp_idx - kFirstEpiWarp;  // epilogue warp 0..7
-    // MMA: warpgroup `half` computes rows [64 half, 64 half + 64) of the tile.  Epilogue: warp ew owns rows
-    // [32 q, 32 q + 32), one per lane, and the 32-column chunks half * 32 + 64 j.
+    // ===================== MMA (warpgroups 1, 2) and epilogue (warpgroup 3, or 1 and 2) =====================
+    const bool mma_warp = warp_idx < kFirstEpiWarp;
+    // (EPI_ROLE: each role sets its budget inside its own branch below -- ptxas allocates code reached from both
+    // branches within the smaller budget)
+    if constexpr (!EPI_ROLE) ptx::setmaxnreg_inc<232>();
+    // MMA: warpgroup mhalf computes rows [64 mhalf, 64 mhalf + 64) of the tile, warp mq of it rows 16 mq + [0, 16).
+    const int mq = (warp_idx - kFirstMmaWarp) & 3;
+    const int mhalf = (warp_idx - kFirstMmaWarp) >> 2;
+    // Epilogue: warp ew owns rows [32 q, 32 q + 32), one per lane, and the 32-column chunks half * 32 + 64 j (384 threads)
+    // or all of them (EPI_ROLE: half = 0, chunks 32 j).
+    const int ew = warp_idx - (EPI_ROLE ? kFirstEpiWarp : kFirstMmaWarp);  // epilogue warp 0..kEpiWarps-1
     const int q = ew & 3;
-    const int half = ew >> 2;
+    const int half = EPI_ROLE ? 0 : ew >> 2;
+    constexpr int kChunkStep = EPI_ROLE ? 32 : 64;
     int mma_stage = 0;
     uint32_t mma_phase = 0;
-    // Runs the K loop of work item w into registers, then publishes the finished tile in acc_s (a barrier over the two
-    // warpgroups: afterwards every epilogue thread may read any row).  The caller guarantees that no thread still reads
-    // acc_s for the previous tile.
-    auto mma_tile = [&](int w) {
+    // Runs the K loop of work item w (the CTA's item number tc) into registers, then publishes the finished tile in acc_s.
+    // EPI_ROLE: waits on acc_empty before it writes acc_s and arrives on acc_full afterwards.  Otherwise a barrier over the
+    // two warpgroups publishes it (afterwards every epilogue thread may read any row), and the caller guarantees that no
+    // thread still reads acc_s for the previous tile.
+    auto mma_tile = [&](int w, int tc) {
       float dm[Cfg::kAccRegs];
       float dc[PASSES == 3 ? Cfg::kAccRegs : 1];
 #pragma unroll
@@ -422,7 +458,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         ptx::mbar_wait(&full_bar[mma_stage], mma_phase);
         if (ki == 0 && w == static_cast<int>(blockIdx.x)) stamp(p, 3);
         const uint32_t st = ptx::smem_u32(smem + mma_stage * Cfg::kStageBytes);
-        const uint32_t a_off = static_cast<uint32_t>(half * (Cfg::kABytes / 2));  // this warpgroup's 64 rows
+        const uint32_t a_off = static_cast<uint32_t>(mhalf * (Cfg::kABytes / 2));  // this warpgroup's 64 rows
         const uint64_t a_hi = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + a_off);
         const uint64_t b_hi = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + Cfg::kSplit * Cfg::kABytes);
         const uint64_t a_lo = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + Cfg::kABytes + a_off);
@@ -453,8 +489,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
       ptx::wgmma_fence_regs(dm);
       if (PASSES == 3) ptx::wgmma_fence_regs(dc);
       if (prev >= 0) release(prev);
+      if constexpr (EPI_ROLE) ptx::mbar_wait(&acc_empty, static_cast<uint32_t>((tc & 1) ^ 1));
       // fragment -> acc_s (the two accumulators of PASSES == 3 are added here)
-      const int r0 = half * 64 + q * 16 + (lane >> 2);
+      const int r0 = mhalf * 64 + mq * 16 + (lane >> 2);
       const int cc = 2 * (lane & 3);
 #pragma unroll
       for (int j = 0; j < BLOCK_N / 8; ++j) {
@@ -463,13 +500,38 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         *reinterpret_cast<float2*>(acc_s + r0 * Cfg::kAccPitch + 8 * j + cc) = make_float2(v0, v1);
         *reinterpret_cast<float2*>(acc_s + (r0 + 8) * Cfg::kAccPitch + 8 * j + cc) = make_float2(v2, v3);
       }
-      asm volatile("bar.sync 3, %0;" ::"n"(kEpiWarps * 32));
+      if constexpr (EPI_ROLE) {
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&acc_full);
+      } else {
+        asm volatile("bar.sync 3, %0;" ::"n"(kMmaWarps * 32));
+      }
     };
-    const EpiParams e = epi_s;  // registers
+    const bool epi_warp = !EPI_ROLE || !mma_warp;
+    if (!epi_warp) {
+      // MMA warpgroups of the EPI_ROLE variants: nothing but K loops and the hand-over (debug_ts slots 16 + i: tile i < 4
+      // published in acc_s, 12: the last one; the epilogue's slots 20 + i: prologue done, 24 + i: acc_full observed,
+      // 28 + i: tile stored)
+      ptx::setmaxnreg_inc<kMmaRegs>();
+      int tc = 0;
+      for (int wi = blockIdx.x; wi < num_work; wi += gridDim.x, ++tc) {
+        mma_tile(wi, tc);
+        if (warp_idx == kFirstMmaWarp && lane == 0 && tc < 4) stamp(p, 16 + tc);
+      }
+      if (warp_idx == kFirstMmaWarp && lane == 0) stamp(p, 12);
+    } else if constexpr (EPI_ROLE) {
+      ptx::setmaxnreg_inc<kEpiRoleRegs>();
+    }
+    // the 384-thread variants keep the epilogue parameters in registers; the epilogue warpgroup reads them from shared
+    // memory (its register budget goes to the row's values)
+    EpiParams e_regs;
+    if constexpr (!EPI_ROLE) e_regs = epi_s;
+    const EpiParams& e = EPI_ROLE ? epi_s : e_regs;
     const bool vec_ok = ((e.N & 3) == 0);
     float* tile = reinterpret_cast<float*>(epi_smem) + ew * kEpiTileFloats;
     const int tr = lane >> 3, tc = (lane & 7) * 4;  // transposed mapping: rows tr, tr+4, ..., columns tc..tc+3
     int tcount = 0;
+    uint32_t res_phase = 0;  // EPI 3: parity of this warp's next residual load on res_bar[ew]
     if constexpr (EPI == 4) {
       // ===== linear-blend skinning epilogue: thread = frame m, 16 of the tile's 32 vertices (warp half) =====
       // Software pipeline over the CTA's tiles: the next tile's tables (bones, dense weights) are fetched into registers at the
@@ -519,7 +581,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         int nbone = 0, nnb = 0;
         if (has_next) fetch_tables(next % tiles_n, nw0, nw1, nbone, nnb);  // in flight during the accumulator wait and the compute
 
-        mma_tile(tile_idx);  // the previous tile's reads of acc_s are behind the bar.sync 1 of its compute phase
+        mma_tile(tile_idx, tcount);  // the previous tile's reads of acc_s are behind the bar.sync 1 of its compute phase
         if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 5);
         // verts = sum_b w[v][b] (R_b v_posed + t_b).  Within a 32-vertex tile nearly every (vertex, bone) pair carries weight
         // (vertices are indexed by body part), so every vertex is updated per bone: no branches, 12 FMAs per (vertex, bone).
@@ -630,7 +692,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 11);
       }
     }
-    for (int wi = blockIdx.x; EPI != 4 && wi < num_work; wi += gridDim.x, ++tcount) {
+    for (int wi = blockIdx.x; EPI != 4 && epi_warp && wi < num_work; wi += gridDim.x, ++tcount) {
       const int tile_idx = wi / S;
       // split-K: the partial tile of split s goes to output rows m + s * split_row_stride
       const int split_rows = (wi - tile_idx * S) * (EPI == 2 ? p.split_row_stride : 0);
@@ -647,8 +709,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
       const int64_t orow = static_cast<int64_t>(m) * e.out_row_mul + e.out_row_add + split_rows;
       const float bias_row = (e.bias != nullptr && e.bias_per_row && row_ok) ? __ldg(e.bias + m) : 0.0f;
 
-      // stage this tile's per-column vectors before the main loop of the tile.  Single-buffered: the first barrier
-      // keeps the writers off the vectors until every epilogue thread has finished the previous tile.
+      // stage this tile's per-column vectors before its accumulator is ready (EPI_ROLE: while its MMAs run; otherwise
+      // before its main loop).  Single-buffered: the first barrier keeps the writers off the vectors until every epilogue
+      // thread has finished the previous tile.
       {
         const int i = ew * 32 + lane;
         asm volatile("bar.sync 1, %0;" ::"n"(kEpiWarps * 32));
@@ -664,8 +727,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         }
         if (e.residual != nullptr && row_ok) {
           const float* r = e.residual + orow * e.ldr + n0 + half * 32;
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(r));
-          if (BLOCK_N > 64) asm volatile("prefetch.global.L2 [%0];" ::"l"(r + 64));
+#pragma unroll
+          for (int c = 0; c < (EPI_ROLE ? BLOCK_N : (BLOCK_N > 64 ? 128 : 64)); c += kChunkStep)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(r + c));
         }
         asm volatile("bar.sync 1, %0;" ::"n"(kEpiWarps * 32));
       }
@@ -675,28 +739,26 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
         const float2 mr = combine_row_stats(e.a_stats + static_cast<int64_t>(m) * 8, e.ln_eps);
         a_mean = mr.x, a_rstd = mr.y;
       }
-      // LayerNorm folding, producer side: the residual tile (this thread: one row, 2 x 32 columns) arrives through TMA into
-      // the warp's staging tile -- nearly all of the shared memory is in use, so there is little L1 for per-thread loads --
-      // and is passed through the previous LayerNorm on the fly.
+      // LayerNorm folding, producer side: the residual tile (this thread: one row; the 2 x 32 columns of one 64-column
+      // statistics group at a time, columns g * 32 + 64 h2) arrives through TMA into the warp's staging tile -- nearly all
+      // of the shared memory is in use, so there is little L1 for per-thread loads -- and is passed through the previous
+      // LayerNorm on the fly.  Group 0 is loaded before the accumulator is ready, group 1 after group 0 has been stored.
       float lnv[EPI == 3 ? 2 : 1][EPI == 3 ? 32 : 1];
-      if constexpr (EPI == 3) {
-        float r_mean = 0.0f, r_rstd = 1.0f;
-        if (e.res_stats != nullptr && row_ok) {
-          const float2 mr = combine_row_stats(e.res_stats + static_cast<int64_t>(m) * 8, e.ln_eps);
-          r_mean = mr.x, r_rstd = mr.y;
-        }
+      float r_mean = 0.0f, r_rstd = 1.0f;
+      auto load_residual = [&](int g) {
         uint8_t* tb = reinterpret_cast<uint8_t*>(tile);
         uint64_t* rb = &res_bar[ew];
 #pragma unroll
         for (int h2 = 0; h2 < 2; ++h2) {
-          const int c0 = half * 32 + 64 * h2;
+          const int c0 = g * 32 + 64 * h2;
           if (lane == 0) {
-            ptx::bulk_wait_read_all();  // this warp's stores of the previous tile have finished reading the staging tile
+            ptx::bulk_wait_read_all();  // this warp's stores have finished reading the staging tile
             ptx::mbar_expect_tx(rb, 4096);
             ptx::tma_load_2d(tb, &p.st_hi, rb, n0 + c0, m0 + q * 32);
             ptx::tma_load_2d(tb + 2048, &p.st_lo, rb, n0 + c0, m0 + q * 32);
           }
-          ptx::mbar_wait(rb, static_cast<uint32_t>((2 * tcount + h2) & 1));
+          ptx::mbar_wait(rb, res_phase);
+          res_phase ^= 1;
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
             const int off = lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4);
@@ -716,66 +778,89 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
           ptx::fence_proxy_async();  // generic-proxy reads above, async-proxy writes (next load / the stores) below
           __syncwarp();
         }
+      };
+      if constexpr (EPI == 3) {
+        if (e.res_stats != nullptr && row_ok) {
+          const float2 mr = combine_row_stats(e.res_stats + static_cast<int64_t>(m) * 8, e.ln_eps);
+          r_mean = mr.x, r_rstd = mr.y;
+        }
+        load_residual(0);
       }
-      // the start-of-tile bar.sync 1 above keeps this tile's accumulator off acc_s until every thread has read the last one
-      mma_tile(wi);
+      if (EPI_ROLE && ew == 0 && lane == 0 && tcount < 4) stamp(p, 20 + tcount);  // prologue done
+      if constexpr (EPI_ROLE) {
+        ptx::mbar_wait(&acc_full, static_cast<uint32_t>(tcount & 1));
+        if (ew == 0 && lane == 0 && tcount < 4) stamp(p, 24 + tcount);
+      } else {
+        // the start-of-tile bar.sync 1 above keeps this tile's accumulator off acc_s until every thread has read the last one
+        mma_tile(wi, tcount);
+      }
       if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 5);
 
       if constexpr (EPI == 3) {
         // ===== u = LN_prev(residual) + acc * 2^-s + bias, written in place as an fp16 pair + per-row partial statistics =====
         static_assert(BLOCK_N == 128 && PASSES == 3 && KIND == kKindF16, "LayerNorm-folding producer: fp16 pairs, 128-wide tiles");
+        static_assert(EPI_ROLE, "one thread per row: both 64-column statistics groups");
         const int tile_n = tile_idx % tiles_n;
         float (&v)[2][32] = lnv;
-#pragma unroll
-        for (int h2 = 0; h2 < 2; ++h2) {
-          const int c0 = half * 32 + 64 * h2;
-          float raw[32];
-          acc_load<Cfg::kAccPitch>(acc_s, q * 32 + lane, c0, raw);
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b4 = *reinterpret_cast<const float4*>(&bias_s[c0 + j]);
-            v[h2][j] += fmaf(raw[j], e.acc_scale, b4.x);
-            v[h2][j + 1] += fmaf(raw[j + 1], e.acc_scale, b4.y);
-            v[h2][j + 2] += fmaf(raw[j + 2], e.acc_scale, b4.z);
-            v[h2][j + 3] += fmaf(raw[j + 3], e.acc_scale, b4.w);
-          }
-        }
-        if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 8);
         uint8_t* tb = reinterpret_cast<uint8_t*>(tile);
         const bool group_full = (m0 + q * 32 + 32 <= e.M);
-        auto store_chunk = [&](int h2) {
-          const int nb = n0 + half * 32 + 64 * h2;
-          if (group_full) {
-            stage_pair_chunk(v[h2], tb, lane, &p.st_hi, &p.st_lo, nb, m0 + q * 32);
-          } else if (row_ok) {  // ragged last row group: per-thread stores
-            __half* oh = static_cast<__half*>(e.out_hi) + static_cast<int64_t>(m) * e.lds + nb;
-            __half* ol = static_cast<__half*>(e.out_lo) + static_cast<int64_t>(m) * e.lds + nb;
+#pragma unroll 1
+        for (int g = 0; g < 2; ++g) {
+          if (g == 1) load_residual(1);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) ptx::split_f16(v[h2][j], oh[j], ol[j]);
+          for (int h2 = 0; h2 < 2; ++h2) {
+            const int c0 = g * 32 + 64 * h2;
+            float raw[32];
+            acc_load<Cfg::kAccPitch>(acc_s, q * 32 + lane, c0, raw);
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+              const float4 b4 = *reinterpret_cast<const float4*>(&bias_s[c0 + j]);
+              v[h2][j] += fmaf(raw[j], e.acc_scale, b4.x);
+              v[h2][j + 1] += fmaf(raw[j + 1], e.acc_scale, b4.y);
+              v[h2][j + 2] += fmaf(raw[j + 2], e.acc_scale, b4.z);
+              v[h2][j + 3] += fmaf(raw[j + 3], e.acc_scale, b4.w);
+            }
           }
-        };
-        store_chunk(0);
-        // partial row statistics over this thread's 64 columns for the consumers of LN(u) -- computed while the TMA engine
-        // reads the first chunk out of the staging tile (the second chunk has to wait for that anyway)
-        float s1 = 0.0f;
+          if (g == 1) {  // the last read of acc_s: the MMA warpgroups may write the next tile
+            __syncwarp();
+            if (lane == 0) ptx::mbar_arrive(&acc_empty);
+          }
+          if (tcount == 0 && g == 0 && ew == 0 && lane == 0) stamp(p, 8);
+          auto store_chunk = [&](int h2) {
+            const int nb = n0 + g * 32 + 64 * h2;
+            if (group_full) {
+              stage_pair_chunk(v[h2], tb, lane, &p.st_hi, &p.st_lo, nb, m0 + q * 32);
+            } else if (row_ok) {  // ragged last row group: per-thread stores
+              __half* oh = static_cast<__half*>(e.out_hi) + static_cast<int64_t>(m) * e.lds + nb;
+              __half* ol = static_cast<__half*>(e.out_lo) + static_cast<int64_t>(m) * e.lds + nb;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) s1 += v[0][j] + v[1][j];
-        const float mean_i = s1 * (1.0f / 64.0f);
-        float m2_i = 0.0f;
+              for (int j = 0; j < 32; ++j) ptx::split_f16(v[h2][j], oh[j], ol[j]);
+            }
+          };
+          store_chunk(0);
+          // partial row statistics over the group's 64 columns for the consumers of LN(u) -- computed while the TMA engine
+          // reads the first chunk out of the staging tile (the second chunk has to wait for that anyway)
+          float s1 = 0.0f;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float d0 = v[0][j] - mean_i, d1 = v[1][j] - mean_i;
-          m2_i = fmaf(d0, d0, fmaf(d1, d1, m2_i));
+          for (int j = 0; j < 32; ++j) s1 += v[0][j] + v[1][j];
+          const float mean_i = s1 * (1.0f / 64.0f);
+          float m2_i = 0.0f;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const float d0 = v[0][j] - mean_i, d1 = v[1][j] - mean_i;
+            m2_i = fmaf(d0, d0, fmaf(d1, d1, m2_i));
+          }
+          if (row_ok) e.stats_out[static_cast<int64_t>(m) * 8 + tile_n * 2 + g] = make_float2(mean_i, m2_i);
+          if (tcount == 0 && g == 0 && ew == 0 && lane == 0) stamp(p, 9);
+          store_chunk(1);
         }
-        if (row_ok) e.stats_out[static_cast<int64_t>(m) * 8 + tile_n * 2 + half] = make_float2(mean_i, m2_i);
-        if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 9);
-        store_chunk(1);
         if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 6);
+        if (ew == 0 && lane == 0 && tcount < 4) stamp(p, 28 + tcount);
         continue;
       }
 
 #pragma unroll 1
-      for (int c0 = half * 32; c0 < BLOCK_N; c0 += 64) {
+      for (int c0 = half * 32; c0 < BLOCK_N; c0 += kChunkStep) {
         const int nb = n0 + c0;
         const bool full = vec_ok && (nb + 32 <= e.N);
         if (e.tma_store && full && (m0 + q * 32 + 32 <= e.M)) {
@@ -996,6 +1081,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tile_kernel(const __grid_con
           }
         }
       }
+      if constexpr (EPI_ROLE) {  // every chunk has been read out of acc_s
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&acc_empty);
+        if (ew == 0 && lane == 0 && tcount < 4) stamp(p, 28 + tcount);
+      }
       if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 6);
     }
     if (ew == 0 && lane == 0) stamp(p, 13);  // this warp's last tile drained
@@ -1056,28 +1146,30 @@ PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
 
 template <int BLOCK_N, int PASSES, int KIND>
 static cudaError_t set_attr() {
+  constexpr int kRoleSmem = TileCfg<BLOCK_N, PASSES, true>::kSmemBytes;
   cudaError_t e = cudaFuncSetAttribute(gemm_tile_kernel<BLOCK_N, PASSES, 0, KIND>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<BLOCK_N, PASSES>::kSmemBytes);
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, kRoleSmem);
   if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(gemm_tile_kernel<BLOCK_N, PASSES, 1, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           TileCfg<BLOCK_N, PASSES>::kSmemBytes);
+  e = cudaFuncSetAttribute(gemm_tile_kernel<BLOCK_N, PASSES, 1, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRoleSmem);
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(gemm_tile_kernel<BLOCK_N, PASSES, 2, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           TileCfg<BLOCK_N, PASSES>::kSmemBytes);
+                           TileCfg<BLOCK_N, PASSES, false>::kSmemBytes);
   if (e != cudaSuccess) return e;
   if constexpr (BLOCK_N == 128 && PASSES == 3 && KIND == kKindF16)
-    e = cudaFuncSetAttribute(gemm_tile_kernel<BLOCK_N, PASSES, 3, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             TileCfg<BLOCK_N, PASSES>::kSmemBytes);
+    e = cudaFuncSetAttribute(gemm_tile_kernel<BLOCK_N, PASSES, 3, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRoleSmem);
   return e;
 }
 
 template <int BLOCK_N, int PASSES, int KIND>
 cudaError_t launch_cfg(const GemmParams& p, int m_rows, int n_cols, cudaStream_t stream, bool pdl) {
-  using Cfg = TileCfg<BLOCK_N, PASSES>;
+  using Cfg = TileCfg<BLOCK_N, PASSES, false>;  // the 384-thread variants (EPI 2, 4)
   const bool plain = p.clip_rows == 0 && p.gn_stats == nullptr;
-  auto kern = (plain && p.act == kActNone)   ? gemm_tile_kernel<BLOCK_N, PASSES, 0, KIND>
-              : (plain && p.act == kActGelu) ? gemm_tile_kernel<BLOCK_N, PASSES, 1, KIND>
-                                             : gemm_tile_kernel<BLOCK_N, PASSES, 2, KIND>;
+  const int epi = (plain && p.act == kActNone) ? 0 : (plain && p.act == kActGelu) ? 1 : 2;
+  auto kern = epi == 0 ? gemm_tile_kernel<BLOCK_N, PASSES, 0, KIND>
+              : epi == 1 ? gemm_tile_kernel<BLOCK_N, PASSES, 1, KIND>
+                         : gemm_tile_kernel<BLOCK_N, PASSES, 2, KIND>;
+  int threads = kernel_threads(epi);
+  int smem_bytes = epi_role(epi) ? TileCfg<BLOCK_N, PASSES, true>::kSmemBytes : Cfg::kSmemBytes;
   if (p.a_stats != nullptr && (!plain || p.a_corr == nullptr)) return cudaErrorInvalidValue;
   if (p.stats_out != nullptr) {
     // LayerNorm-folding producer: the output pair overwrites the residual pair tile by tile (st_hi / st_lo both ways), rows are
@@ -1087,17 +1179,19 @@ cudaError_t launch_cfg(const GemmParams& p, int m_rows, int n_cols, cudaStream_t
           p.out_hi == nullptr || p.a_stats != nullptr || (p.res_stats != nullptr && (p.res_gamma == nullptr || p.res_beta == nullptr)))
         return cudaErrorInvalidValue;
       kern = gemm_tile_kernel<BLOCK_N, PASSES, 3, KIND>;
+      threads = kernel_threads(3);
+      smem_bytes = TileCfg<BLOCK_N, PASSES, true>::kSmemBytes;
     } else {
       return cudaErrorInvalidValue;
     }
   }
-  int smem_bytes = Cfg::kSmemBytes;
   if (p.skin_A != nullptr) {
     if constexpr (BLOCK_N == 96 && PASSES == 3 && KIND == kKindF16) {
       if (!plain || p.act != kActNone || p.out == nullptr || p.skin_nb == nullptr || p.skin_bone == nullptr || p.skin_w == nullptr ||
           p.bias != nullptr || p.residual != nullptr || p.a_stats != nullptr || p.stats_out != nullptr)
         return cudaErrorInvalidValue;
       kern = gemm_tile_kernel<BLOCK_N, PASSES, 4, KIND>;
+      threads = kernel_threads(4);
       smem_bytes = Cfg::kStages * Cfg::kStageBytes + 1024 + Cfg::kAccBytes + kSkinStageBytes;
       static bool skin_attr_set = false;
       if (!skin_attr_set) {
@@ -1142,7 +1236,7 @@ cudaError_t launch_cfg(const GemmParams& p, int m_rows, int n_cols, cudaStream_t
   if (q.multicast_a && (PASSES != 3 || q.num_segs != 1 || tiles_n_ % 2 != 0 || grid < 2)) q.multicast_a = 0;
   if (q.multicast_a) grid -= grid % 2;  // pairs: tiles 2j, 2j+1 of a round are neighbouring column tiles of one stripe
   cfg.gridDim = dim3(grid, 1, 1);
-  cfg.blockDim = dim3(kThreads, 1, 1);
+  cfg.blockDim = dim3(threads, 1, 1);
   cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];

@@ -17,12 +17,15 @@
 //   fp32 stores at a per-split row offset and the consumer kernel adds them in split order (TrajNet's deep pyramid levels, where
 //   6-22 row tiles with 40-80 K blocks each would otherwise leave most SMs idle or force 32-wide tiles).
 //
-// Kernel shape: persistent, grid = min(#work items, #SMs), 128 x BLOCK_N output tiles, 384 threads per CTA:
-//   warpgroup 0   : TMA producer (one lane)             smem ring of 2 x (A + B) stages: full[]/empty[] mbarriers
+// Kernel shape: persistent, grid = min(#work items, #SMs), 128 x BLOCK_N output tiles:
+//   warpgroup 0   : TMA producer (one lane)             smem ring of (A + B) stages: full[]/empty[] mbarriers
 //   warpgroups 1-2: wgmma, 64 rows each, accumulators in registers (two per thread with PASSES == 3); the finished tile
-//                   goes through a shared-memory accumulator tile to one row per thread, then the epilogue: scale / bias /
-//                   activation / row mask / GroupNorm sums -> swizzled smem tile -> TMA bulk store, or per-thread stores
-//                   with a residual.  The producer keeps filling the ring for the next tile during the epilogue.
+//                   goes to a shared-memory accumulator tile (acc_s), read back one row per thread by the epilogue: scale /
+//                   bias / activation / row mask / GroupNorm sums -> swizzled smem tile -> TMA bulk store, or per-thread
+//                   stores with a residual.
+//   Lean variants (no masks / statistics: every PoseNet launch), 512 threads: warpgroup 3 runs the epilogue while
+//   warpgroups 1-2 run the next tile's MMAs (acc_full / acc_empty mbarriers around acc_s).  Masked / GroupNorm (TrajNet)
+//   and skinning variants, 384 threads: warpgroups 1-2 run the epilogue after their MMAs.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -135,10 +138,12 @@ struct alignas(64) GemmParams {
   const int* skin_nb;
   const int* skin_bone;
   const float* skin_w;
-  // optional: CTA 0 records %globaltimer at 8 milestones (developer instrumentation, see tools/gemm_selftest)
+  // optional: CTA 0 records %globaltimer at milestones into 32 slots (developer instrumentation, see tools/gemm_selftest);
+  // lean variants: slots 16 + i = tile i published by the MMA warpgroups, 20 + i / 24 + i / 28 + i = the epilogue's
+  // prologue done / accumulator observed / tile stored, for the CTA's first four tiles
   unsigned long long* debug_ts;
   // developer experiments (tools/gemm_selftest only; results are wrong when set): bit 0 = the epilogue only drains the accumulator (no
-  // staging, no stores), bit 1 = staging writes but no TMA stores.  Slots 16.. of debug_ts: "all MMAs of tile i issued".
+  // staging, no stores), bit 1 = staging writes but no TMA stores.
   int debug_flags;
   // Split-K (TrajNet convolutions on the deep pyramid levels; masked / GroupNorm epilogue variant only): the K iterations of
   // every output tile are cut into `k_splits` contiguous ranges, one work item each, so that a level with 6 to 22 row tiles

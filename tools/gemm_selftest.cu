@@ -156,6 +156,18 @@ static void case_linear(int M, int N, int K, int block_n, int act, bool with_res
 }
 
 
+
+// CTA 0's two timelines of the lean variants (EPI 0 / 1 / 3; gemm.cu debug_ts slots), first four tiles: MMA warpgroups --
+// tile i published in acc_s; epilogue warpgroup -- prologue of tile i done (ready), acc_full observed (start), tile i stored (done).  ns since
+// kernel start.
+static void print_role_timeline(const unsigned long long* h) {
+  printf("      MMA: first_full %llu | tile published:", h[3] - h[0]);
+  for (int i = 16; i < 20 && h[i] != 0; ++i) printf(" %llu", h[i] - h[0]);
+  printf("\n      EPI: ready/start/done per tile:");
+  for (int i = 0; i < 4 && h[28 + i] != 0; ++i) printf(" %llu/%llu/%llu", h[20 + i] - h[0], h[24 + i] - h[0], h[28 + i] - h[0]);
+  printf(" | end %llu\n", h[7] - h[0]);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Case 1b: the same linear layer on fp16 hi/lo pairs (kKindF16): A split as is, W scaled by a power of two into the
 // middle of the fp16 range, accumulator scaled back in the epilogue.  a_scale stresses the fp16 range of the activations.
@@ -282,12 +294,10 @@ static void case_linear_f16(int M, int N, int K, int block_n, int act, bool with
       CK(cudaDeviceSynchronize());
       unsigned long long h[32];
       CK(cudaMemcpy(h, dts, sizeof h, cudaMemcpyDeviceToHost));
-      printf("    [debug_flags %d: %.2f us/launch] CTA0 timeline (ns): setup %llu | first_tma %llu | first_full %llu | tile0 mma issued %llu | tile0 epi start %llu | "
-             "tile0 epi done %llu | all mma issued %llu | last epi done %llu | stores done %llu | end %llu | per-tile mma issued:",
-             flags, ms * 1000.0 / iters, h[1] - h[0], h[2] - h[0], h[3] - h[0], h[4] - h[0], h[5] - h[0], h[6] - h[0], h[12] - h[0],
-             h[13] - h[0], h[14] - h[0], h[7] - h[0]);
-      for (int i = 16; i < 24 && h[i] != 0; ++i) printf(" %llu", h[i] - h[0]);
-      printf("\n");
+      printf("    [debug_flags %d: %.2f us/launch] CTA0 timeline (ns): setup %llu | first_tma %llu | tile0 epi start %llu | tile0 epi done %llu | "
+             "all tiles published %llu | last epi done %llu | stores done %llu\n",
+             flags, ms * 1000.0 / iters, h[1] - h[0], h[2] - h[0], h[5] - h[0], h[6] - h[0], h[12] - h[0], h[13] - h[0], h[14] - h[0]);
+      print_role_timeline(h);
     }
     p.debug_flags = 0;
     p.debug_ts = nullptr;
@@ -458,15 +468,17 @@ static void case_linear_ln(int M, int K, bool timing) {
     }
     unsigned long long* dts;
     CK(cudaMalloc(&dts, 32 * sizeof(unsigned long long)));
+    CK(cudaMemset(dts, 0, 32 * sizeof(unsigned long long)));
     pc.debug_ts = dts;
     CK(launch_gemm(pc, M, D, 128, 3, 0, false, kKindF16));
     CK(launch_gemm(pc, M, D, 128, 3, 0, false, kKindF16));
     CK(cudaDeviceSynchronize());
-    unsigned long long h[16];
+    unsigned long long h[32];
     CK(cudaMemcpy(h, dts, sizeof h, cudaMemcpyDeviceToHost));
-    printf("    (C) CTA0 timeline (ns): setup %llu | first_tma %llu | first_full %llu | tile0 mma issued %llu | epi start %llu | acc added %llu | "
-           "stats written %llu | tile0 epi done %llu | all mma issued %llu | end %llu\n",
-           h[1] - h[0], h[2] - h[0], h[3] - h[0], h[4] - h[0], h[5] - h[0], h[8] - h[0], h[9] - h[0], h[6] - h[0], h[12] - h[0], h[7] - h[0]);
+    printf("    (C) CTA0 timeline (ns): setup %llu | first_tma %llu | tile0 epi start %llu | acc added %llu | stats written %llu | "
+           "tile0 epi done %llu | end %llu\n",
+           h[1] - h[0], h[2] - h[0], h[5] - h[0], h[8] - h[0], h[9] - h[0], h[6] - h[0], h[7] - h[0]);
+    print_role_timeline(h);
     cudaFree(dts);
   }
   for (float* q : {dA1, dA3, dR, db1, db3, dc2, dd2, dg, dbe, dY}) cudaFree(q);
