@@ -814,18 +814,12 @@ extern "C" int rohm_body_create(rohm_ctx* ctx, const float* v_template, const fl
         GemmParams& k = bd->g_skin;
         k = GemmParams{};
         // The tensor maps end at the last live K column (200 -> 208: the rest of the fourth K block is zero-filled by TMA without
-        // being read: 19 % less L2 -> SM operand traffic).  ROHM_B200_LBS_MULTICAST=1 additionally shares the A tile of a row
-        // stripe between the two CTAs of a pair.
+        // being read: 19 % less L2 -> SM operand traffic).
         constexpr int kLiveK = (kPoseFeat + kBetas + 1 + 15) / 16 * 16;
         int rs = make_tmap_2d(&k.a_hi[0], bd->feat_h, F, kLiveK, kBlendK, kGemmBlockM, 1, bd->kind);
         rs |= make_tmap_2d(&k.a_lo[0], bd->feat_l, F, kLiveK, kBlendK, kGemmBlockM, 1, bd->kind);
         rs |= make_tmap_2d(&k.b_hi, bd->blend.hi, bd->blend.Np, kLiveK, kBlendK, 96, 1, bd->kind);
         rs |= make_tmap_2d(&k.b_lo, bd->blend.lo, bd->blend.Np, kLiveK, kBlendK, 96, 1, bd->kind);
-        const char* mc = getenv("ROHM_B200_LBS_MULTICAST");
-        if (rs == 0 && mc != nullptr && mc[0] == '1') {
-          k.num_segs = 1, k.seg_row_mul[0] = 1;
-          rs |= gemm_enable_multicast(&k, bd->feat_h, bd->feat_l, F, kLiveK, kBlendK, bd->blend.Np, 96, bd->kind);
-        }
         k.num_segs = 1, k.seg_kblocks[0] = kBlendK / gemm_block_k(bd->kind), k.seg_row_mul[0] = 1;
         k.acc_scale = 1.0f / bd->blend.scale;
         k.ldo = V * 3, k.N = V * 3, k.out_row_mul = 1;

@@ -15,7 +15,7 @@ namespace {
 // Warp roles.  Warpgroup 0: TMA producer (one lane).  Warpgroups 1, 2 (warps 4-11): wgmma, 64 tile rows each.
 // EPI 0, 1, 3 (the lean variants the PoseNet forward runs): warpgroup 3 (warps 12-15) is a dedicated epilogue, one tile row
 // per thread, so the MMA warpgroups go straight on to the next tile's K loop while it runs (512 threads).
-// EPI 2 (TrajNet: split-K, GroupNorm sums, padded clips) and EPI 4 (skinning, ~168 registers per epilogue thread): the MMA
+// EPI 2 (TrajNet: split-K, activations, padded clips) and EPI 4 (skinning, ~168 registers per epilogue thread): the MMA
 // warpgroups run the epilogue themselves, after the tile's MMAs (384 threads) -- these epilogues do not fit the register
 // budget of an epilogue warpgroup next to two MMA warpgroups.
 constexpr int kFirstMmaWarp = 4;
@@ -146,52 +146,11 @@ struct EpiParams {
   float* out;
   void* out_hi;
   void* out_lo;
-  double* gn_stats;
   float acc_scale;
   int tma_store;
   int bias_per_row;
-  int ldr, ldo, lds, act, M, N, out_row_mul, out_row_add, clip_rows, clip_valid, gn_groups, gn_group_size;
+  int ldr, ldo, lds, act, M, N, out_row_mul, out_row_add, clip_rows, clip_valid;
 };
-
-// GroupNorm statistics of one 32-column chunk (one row per lane): per (clip, group) sum and sum of squares of the stored
-// values over the rows that contribute, added to e.gn_stats with double atomics (one per warp when the warp's rows all
-// belong to one clip).
-__device__ __forceinline__ void gn_partial_sums(const float (&v)[32], const EpiParams& e, int nb, bool contrib, int clip,
-                                                int lane) {
-  const int gs = e.gn_group_size;
-  const int clip0 = __shfl_sync(0xffffffffu, clip, 0);
-  const bool uniform = __all_sync(0xffffffffu, clip == clip0);
-  for (int jg = 0; jg < 32 && nb + jg < e.N; jg += (gs < 32 ? gs : 32)) {
-    const int span = gs < 32 ? gs : 32;
-    float s1 = 0.0f, s2 = 0.0f;
-    if (contrib) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        if (j >= jg && j < jg + span && nb + j < e.N) {
-          s1 += v[j];
-          s2 += v[j] * v[j];
-        }
-      }
-    }
-    const int g = (nb + jg) / gs;
-    if (uniform) {
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) {
-        s1 += __shfl_xor_sync(0xffffffffu, s1, off);
-        s2 += __shfl_xor_sync(0xffffffffu, s2, off);
-      }
-      if (lane == 0) {
-        double* dst = e.gn_stats + (static_cast<int64_t>(clip0) * e.gn_groups + g) * 2;
-        atomicAdd(dst, static_cast<double>(s1));
-        atomicAdd(dst + 1, static_cast<double>(s2));
-      }
-    } else if (contrib) {
-      double* dst = e.gn_stats + (static_cast<int64_t>(clip) * e.gn_groups + g) * 2;
-      atomicAdd(dst, static_cast<double>(s1));
-      atomicAdd(dst + 1, static_cast<double>(s2));
-    }
-  }
-}
 
 // (mean, rstd) of a 512-wide row from its 8 partial (mean_i, M2_i) over 64 columns each (Chan et al. pairwise combination);
 // row8: 64 contiguous bytes in global memory, written by the previous kernel.
@@ -237,7 +196,7 @@ __device__ __forceinline__ void stage_pair_chunk(const float (&v)[32], uint8_t* 
 // Persistent, warp-specialised: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ...
 // (N-tile index fastest, so CTAs running concurrently share the same A rows in L2).
 // Epilogue variants: 0 = bias + residual + fp32 / hi-lo stores (the PoseNet linears), 1 = the same + exact GELU (FFN1),
-// 2 = everything (other activations, padded-clip row masks, GroupNorm partial sums: TrajNet), 3 = bias + residual pair +
+// 2 = everything (other activations, padded-clip row masks, split-K partials: TrajNet), 3 = bias + residual pair +
 // LayerNorm with the row statistics exchanged between the four column-tile CTAs of a row stripe (PoseNet out-proj / FFN2,
 // see GemmParams::ln_gamma).  Separate instantiations keep the hot variants' code small (the full
 // epilogue is ~7000 SASS instructions, most of them predicated-off activation code when unused).
@@ -286,7 +245,7 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
 
   int total_iters = 0;
   for (int s = 0; s < p.num_segs; ++s) total_iters += p.seg_kblocks[s];
-  // Split-K (GemmParams::k_splits, masked / GroupNorm variant only): work item w = tile * S + split; split s runs the K
+  // Split-K (GemmParams::k_splits, masked variant only): work item w = tile * S + split; split s runs the K
   // iterations [s * per_split, min(total_iters, (s + 1) * per_split)).  S == 1 everywhere else: one item per tile.
   const int S = (EPI == 2 && p.k_splits > 1) ? p.k_splits : 1;
   const int per_split = (total_iters + S - 1) / S;
@@ -301,9 +260,7 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
     }
     for (int i = 0; i < Cfg::kStages; ++i) {
       ptx::mbar_init(&full_bar[i], 1);
-      // one arrival per MMA warpgroup; multicast: the slot is refilled by both CTAs of the pair, so the warpgroups of both
-      // CTAs release it
-      ptx::mbar_init(&empty_bar[i], p.multicast_a ? 4 : 2);
+      ptx::mbar_init(&empty_bar[i], 2);  // one arrival per MMA warpgroup
     }
     if (EPI == 3)
       for (int i = 0; i < kEpiWarps; ++i) ptx::mbar_init(&res_bar[i], 1);
@@ -317,7 +274,7 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
   // pipeline stages in flight right after it has initialised the barriers -- BEFORE the CTA-wide setup barrier and before
   // it waits for the previous grid -- so the pipeline fill overlaps both the setup and that grid's tail.
   int prefetched = 0;
-  if (warp_idx == 0 && lane == 0 && !p.multicast_a && static_cast<int>(blockIdx.x) < num_work) {
+  if (warp_idx == 0 && lane == 0 && static_cast<int>(blockIdx.x) < num_work) {
     const int tile0 = static_cast<int>(blockIdx.x) / S;
     const int it_b = (static_cast<int>(blockIdx.x) - tile0 * S) * per_split;
     const int cnt = (total_iters < it_b + per_split ? total_iters : it_b + per_split) - it_b;
@@ -335,8 +292,7 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
     epi_s.bias = p.bias, epi_s.residual = p.residual, epi_s.ldr = p.ldr, epi_s.out = p.out, epi_s.ldo = p.ldo;
     epi_s.out_hi = p.out_hi, epi_s.out_lo = p.out_lo, epi_s.lds = p.lds, epi_s.act = p.act, epi_s.M = p.M, epi_s.N = p.N;
     epi_s.out_row_mul = p.out_row_mul, epi_s.out_row_add = p.out_row_add, epi_s.clip_rows = p.clip_rows;
-    epi_s.clip_valid = p.clip_valid, epi_s.gn_stats = p.gn_stats, epi_s.gn_groups = p.gn_groups;
-    epi_s.gn_group_size = p.gn_group_size;
+    epi_s.clip_valid = p.clip_valid;
     epi_s.acc_scale = p.acc_scale == 0.0f ? 1.0f : p.acc_scale;
     epi_s.tma_store = p.tma_store;
     epi_s.bias_per_row = p.bias_per_row;
@@ -349,7 +305,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
     }
   }
   __syncthreads();
-  if (p.multicast_a) ptx::cluster_sync_all();  // the partner's barriers are initialised before anything is sent to them
 
   if (threadIdx.x == 0) stamp(p, 1);
   // Programmatic dependent launch: let the next kernel of the chain become resident as soon as SMs free up (its
@@ -389,23 +344,11 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
             ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
             if (it == 0) stamp(p, 2);
             ptx::mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-            if (PASSES == 3 && p.multicast_a) {
-              // my half of the stripe's A tile goes to both CTAs of the pair (the partner sends the other half)
-              const int half_rows = kGemmBlockM / 2;
-              const uint32_t rank = ptx::cluster_ctarank();
-              ptx::tma_load_2d_multicast(st + rank * (Cfg::kABytes / 2), &p.a_hi_half, &full_bar[stage], kb * kElemK,
-                                         row + static_cast<int>(rank) * half_rows, 0x3);
-              ptx::tma_load_2d_multicast(st + Cfg::kABytes + rank * (Cfg::kABytes / 2), &p.a_lo_half, &full_bar[stage],
-                                         kb * kElemK, row + static_cast<int>(rank) * half_rows, 0x3);
-              ptx::tma_load_2d(st + Cfg::kSplit * Cfg::kABytes, &p.b_hi, &full_bar[stage], kcol, n0);
+            ptx::tma_load_2d(st, &p.a_hi[s], &full_bar[stage], kb * kElemK, row);
+            ptx::tma_load_2d(st + Cfg::kSplit * Cfg::kABytes, &p.b_hi, &full_bar[stage], kcol, n0);
+            if (PASSES == 3) {
+              ptx::tma_load_2d(st + Cfg::kABytes, &p.a_lo[s], &full_bar[stage], kb * kElemK, row);
               ptx::tma_load_2d(st + 2 * Cfg::kABytes + Cfg::kBBytes, &p.b_lo, &full_bar[stage], kcol, n0);
-            } else {
-              ptx::tma_load_2d(st, &p.a_hi[s], &full_bar[stage], kb * kElemK, row);
-              ptx::tma_load_2d(st + Cfg::kSplit * Cfg::kABytes, &p.b_hi, &full_bar[stage], kcol, n0);
-              if (PASSES == 3) {
-                ptx::tma_load_2d(st + Cfg::kABytes, &p.a_lo[s], &full_bar[stage], kb * kElemK, row);
-                ptx::tma_load_2d(st + 2 * Cfg::kABytes + Cfg::kBBytes, &p.b_lo, &full_bar[stage], kcol, n0);
-              }
             }
             if (++stage == Cfg::kStages) stage = 0, phase ^= 1;
             if (++kb == p.seg_kblocks[s]) kb = 0, ++s;
@@ -445,13 +388,7 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
       const int n_it = (total_iters < it_b + per_split ? total_iters : it_b + per_split) - it_b;
       const bool signaller = (threadIdx.x & 127) == 0;
       auto release = [&](int stg) {
-        if (!signaller) return;
-        if (p.multicast_a) {
-          ptx::mbar_arrive_cluster(&empty_bar[stg], 0);
-          ptx::mbar_arrive_cluster(&empty_bar[stg], 1);
-        } else {
-          ptx::mbar_arrive(&empty_bar[stg]);
-        }
+        if (signaller) ptx::mbar_arrive(&empty_bar[stg]);
       };
       int prev = -1;
       for (int ki = 0; ki < n_it; ++ki) {
@@ -701,11 +638,7 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
       const int m = m0 + q * 32 + lane;
       const bool row_ok = m < e.M;
       bool row_real = true;
-      int clip = 0;
-      if (!LEAN && e.clip_rows > 0) {
-        clip = m / e.clip_rows;
-        row_real = (m - clip * e.clip_rows) < e.clip_valid;
-      }
+      if (!LEAN && e.clip_rows > 0) row_real = (m % e.clip_rows) < e.clip_valid;
       const int64_t orow = static_cast<int64_t>(m) * e.out_row_mul + e.out_row_add + split_rows;
       const float bias_row = (e.bias != nullptr && e.bias_per_row && row_ok) ? __ldg(e.bias + m) : 0.0f;
 
@@ -895,7 +828,7 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
 #pragma unroll
             for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
           }
-          if (!LEAN) {  // TrajNet: other activations, zeroed pad rows, GroupNorm partial sums
+          if (!LEAN) {  // TrajNet: other activations, zeroed pad rows
             if (e.act == kActGelu) {
 #pragma unroll
               for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
@@ -910,7 +843,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
 #pragma unroll
               for (int j = 0; j < 32; ++j) v[j] = 0.0f;
             }
-            if (e.gn_stats != nullptr) gn_partial_sums(v, e, nb, row_real, clip, lane);
           }
           // the previous chunk's bulk store must have finished reading the staging tile
           if (lane == 0) ptx::bulk_wait_read_all();
@@ -1007,9 +939,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
           }
         }
 
-        // ---- GroupNorm partial statistics over real rows ----
-        if (!LEAN && e.gn_stats != nullptr) gn_partial_sums(v, e, nb, row_ok && row_real, clip, lane);
-
         if (tcount == 0 && ew == 0 && lane == 0 && c0 == 0) stamp(p, 9);
         if (full) {
           // ---- coalesced path through the staging tile ----
@@ -1096,7 +1025,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
   }
 
   __syncthreads();
-  if (p.multicast_a) ptx::cluster_sync_all();  // neither CTA leaves while the other may still send to it
   if (threadIdx.x == 32) stamp(p, 7);
 }
 
@@ -1163,7 +1091,7 @@ static cudaError_t set_attr() {
 template <int BLOCK_N, int PASSES, int KIND>
 cudaError_t launch_cfg(const GemmParams& p, int m_rows, int n_cols, cudaStream_t stream, bool pdl) {
   using Cfg = TileCfg<BLOCK_N, PASSES, false>;  // the 384-thread variants (EPI 2, 4)
-  const bool plain = p.clip_rows == 0 && p.gn_stats == nullptr;
+  const bool plain = p.clip_rows == 0;
   const int epi = (plain && p.act == kActNone) ? 0 : (plain && p.act == kActGelu) ? 1 : 2;
   auto kern = epi == 0 ? gemm_tile_kernel<BLOCK_N, PASSES, 0, KIND>
               : epi == 1 ? gemm_tile_kernel<BLOCK_N, PASSES, 1, KIND>
@@ -1219,12 +1147,12 @@ cudaError_t launch_cfg(const GemmParams& p, int m_rows, int n_cols, cudaStream_t
   q.grid_m_rows = m_rows;
   q.grid_n_cols = n_cols;
   int tiles = ((n_cols + BLOCK_N - 1) / BLOCK_N) * ((m_rows + kGemmBlockM - 1) / kGemmBlockM);
-  if (q.k_splits > 1) {  // split-K: masked / GroupNorm variant, fp32 partials only, every K range non-empty
+  if (q.k_splits > 1) {  // split-K: masked variant, fp32 partials only, every K range non-empty
     int iters = 0;
     for (int s = 0; s < q.num_segs; ++s) iters += q.seg_kblocks[s];
     const int per = (iters + q.k_splits - 1) / q.k_splits;
-    if (plain || q.out == nullptr || q.out_hi != nullptr || q.bias != nullptr || q.residual != nullptr || q.gn_stats != nullptr ||
-        q.act != kActNone || q.out_row_mul != 1 || q.out_row_add != 0 || q.multicast_a || (q.k_splits - 1) * per >= iters ||
+    if (plain || q.out == nullptr || q.out_hi != nullptr || q.bias != nullptr || q.residual != nullptr ||
+        q.act != kActNone || q.out_row_mul != 1 || q.out_row_add != 0 || (q.k_splits - 1) * per >= iters ||
         q.split_row_stride < m_rows)
       return cudaErrorInvalidValue;
     tiles *= q.k_splits;
@@ -1232,23 +1160,15 @@ cudaError_t launch_cfg(const GemmParams& p, int m_rows, int n_cols, cudaStream_t
   cudaLaunchConfig_t cfg{};
   int grid = tiles < num_sms ? tiles : num_sms;
   if (p.stats_out != nullptr) grid -= grid % 4;  // a CTA keeps its column tile: tile % 4 == blockIdx % 4 on every round
-  const int tiles_n_ = (n_cols + BLOCK_N - 1) / BLOCK_N;
-  if (q.multicast_a && (PASSES != 3 || q.num_segs != 1 || tiles_n_ % 2 != 0 || grid < 2)) q.multicast_a = 0;
-  if (q.multicast_a) grid -= grid % 2;  // pairs: tiles 2j, 2j+1 of a round are neighbouring column tiles of one stripe
   cfg.gridDim = dim3(grid, 1, 1);
   cfg.blockDim = dim3(threads, 1, 1);
   cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   int na = 0;
   if (pdl) {
     attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  if (q.multicast_a) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = 2, attr[na].val.clusterDim.y = 1, attr[na].val.clusterDim.z = 1;
     ++na;
   }
   cfg.attrs = attr;
@@ -1305,17 +1225,6 @@ int make_tile_tmap_f16_sw128(CUtensorMap* map, const void* base, int64_t rows, i
   return static_cast<int>(fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estride,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
-}
-
-int gemm_enable_multicast(GemmParams* p, const void* a_hi, const void* a_lo, int64_t rows, int64_t cols, int64_t ld, int n_cols,
-                          int block_n, int kind) {
-  p->multicast_a = 0;
-  if (p->num_segs != 1 || p->seg_row_mul[0] != 1 || ((n_cols + block_n - 1) / block_n) % 2 != 0) return 0;
-  int rc = make_tmap_2d(&p->a_hi_half, a_hi, rows, cols, ld, kGemmBlockM / 2, 1, kind);
-  if (rc == 0) rc = make_tmap_2d(&p->a_lo_half, a_lo, rows, cols, ld, kGemmBlockM / 2, 1, kind);
-  if (rc != 0) return rc;
-  p->multicast_a = 1;
-  return 0;
 }
 
 int gemm_enable_tma_store(GemmParams* p, int64_t rows_total, int kind) {

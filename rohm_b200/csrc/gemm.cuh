@@ -13,7 +13,7 @@
 // * PASSES == 3: D += A_lo*W_hi + A_hi*W_lo + A_hi*W_hi  (drops only the lo*lo term, ~2^-22 relative).
 //   PASSES == 1: D += A_hi*W_hi (plain TF32, ~2^-11 relative) -- the documented fast mode.
 //
-// * Split-K (GemmParams::k_splits, masked / GroupNorm variant): a work item is a (tile, K range) pair; partial tiles are plain
+// * Split-K (GemmParams::k_splits, masked variant): a work item is a (tile, K range) pair; partial tiles are plain
 //   fp32 stores at a per-split row offset and the consumer kernel adds them in split order (TrajNet's deep pyramid levels, where
 //   6-22 row tiles with 40-80 K blocks each would otherwise leave most SMs idle or force 32-wide tiles).
 //
@@ -21,11 +21,11 @@
 //   warpgroup 0   : TMA producer (one lane)             smem ring of (A + B) stages: full[]/empty[] mbarriers
 //   warpgroups 1-2: wgmma, 64 rows each, accumulators in registers (two per thread with PASSES == 3); the finished tile
 //                   goes to a shared-memory accumulator tile (acc_s), read back one row per thread by the epilogue: scale /
-//                   bias / activation / row mask / GroupNorm sums -> swizzled smem tile -> TMA bulk store, or per-thread
-//                   stores with a residual.
-//   Lean variants (no masks / statistics: every PoseNet launch), 512 threads: warpgroup 3 runs the epilogue while
-//   warpgroups 1-2 run the next tile's MMAs (acc_full / acc_empty mbarriers around acc_s).  Masked / GroupNorm (TrajNet)
-//   and skinning variants, 384 threads: warpgroups 1-2 run the epilogue after their MMAs.
+//                   bias / activation / row mask -> swizzled smem tile -> TMA bulk store, or per-thread stores with a
+//                   residual.
+//   Lean variants (no masks: every PoseNet launch), 512 threads: warpgroup 3 runs the epilogue while warpgroups 1-2 run
+//   the next tile's MMAs (acc_full / acc_empty mbarriers around acc_s).  Masked (TrajNet) and skinning variants, 384
+//   threads: warpgroups 1-2 run the epilogue after their MMAs.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -89,10 +89,6 @@ struct alignas(64) GemmParams {
   // are real frames; the others are written as zeros so that they act as conv padding for the next layer.
   int clip_rows;  // 0 = disabled
   int clip_valid;
-  // GroupNorm statistics (TrajNet): per (clip, group) sum and sum of squares of the stored fp32 values.
-  double* gn_stats;  // [num_clips, gn_groups, 2] or nullptr
-  int gn_groups;
-  int gn_group_size;  // channels per group
   // TMA-store epilogue (gemm_enable_tma_store): 32 x 32 output chunks go registers -> swizzled shared-memory tile ->
   // cp.async.bulk.tensor store.  Eligible launches: no residual, identity output row map (not the transposed-conv
   // phases), and either only `out` (fp32) or only an fp16 out_hi/out_lo pair.  Chunks on a ragged M or N edge still take
@@ -120,13 +116,6 @@ struct alignas(64) GemmParams {
   const float* res_beta;    // [N]
   float2* stats_out;        // [rows][8], or nullptr: plain epilogue
   float ln_eps;
-  // A-operand multicast (`multicast_a`, set by gemm_enable_multicast): CTAs run as clusters of two that own neighbouring
-  // column tiles of the same 128-row stripe; each loads HALF of the stripe's A tile (64 rows, a_hi_half / a_lo_half) and
-  // multicasts it to both, so A crosses the L2 -> SM fabric once per pair.  Requires one A segment, an even number
-  // of column tiles and PASSES == 3.
-  CUtensorMap a_hi_half;
-  CUtensorMap a_lo_half;
-  int multicast_a;
   // Linear-blend skinning in the epilogue (`skin_A` != nullptr; BLOCK_N = 96 = 32 vertices x 3, fp16 pairs): the
   // accumulator row of frame m is v_posed[m][32 vertices]; the epilogue applies  verts[m][v] = sum_b w[v][b] (R[m][b] v_posed +
   // t[m][b])  with the bone transforms skin_A [55][12][skin_lda frames] (row-major 3 x 4 per bone, translation folded in; frames contiguous:
@@ -145,9 +134,9 @@ struct alignas(64) GemmParams {
   // developer experiments (tools/gemm_selftest only; results are wrong when set): bit 0 = the epilogue only drains the accumulator (no
   // staging, no stores), bit 1 = staging writes but no TMA stores.
   int debug_flags;
-  // Split-K (TrajNet convolutions on the deep pyramid levels; masked / GroupNorm epilogue variant only): the K iterations of
+  // Split-K (TrajNet convolutions on the deep pyramid levels; masked epilogue variant only): the K iterations of
   // every output tile are cut into `k_splits` contiguous ranges, one work item each, so that a level with 6 to 22 row tiles
-  // still fills the SMs with 128-wide tiles.  Split s stores its fp32 partial tile (no bias, no statistics) at output row
+  // still fills the SMs with 128-wide tiles.  Split s stores its fp32 partial tile (no bias) at output row
   // m + s * split_row_stride of `out`; the consumer (gn_mish_split_kernel) adds the partials in a fixed order, so the result is
   // deterministic.  0 / 1 = off.  Every range must be non-empty: (k_splits - 1) * ceil(iters / k_splits) < iters.
   int k_splits;
@@ -168,11 +157,6 @@ int make_tmap_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols,
 // buffers) and sets p.tma_store when the launch is eligible (see GemmParams); otherwise clears it.  Returns 0 or a
 // CUresult.
 int gemm_enable_tma_store(GemmParams* p, int64_t rows_total, int kind);
-
-// Builds the half-tile maps of segment 0 (same base / extents as a_hi[0], a_lo[0]; 64-row boxes) and sets p->multicast_a when
-// the launch is eligible, else clears it.  Returns 0 or a CUresult.
-int gemm_enable_multicast(GemmParams* p, const void* a_hi, const void* a_lo, int64_t rows, int64_t cols, int64_t ld, int n_cols,
-                          int block_n, int kind);
 
 // Tensor map for box_rows x 32-element TMA store boxes over a row-major [rows, cols] matrix with pitch ld: fp32 with
 // SWIZZLE_128B (128-byte box rows) or fp16 with SWIZZLE_64B (64-byte box rows).  Returns 0 or a CUresult.

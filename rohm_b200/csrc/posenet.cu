@@ -265,9 +265,6 @@ struct rohm_posenet {
   std::vector<FwdGraph> graphs;
   bool use_graph = true;
   bool use_pdl = true;
-  bool use_tma_store = true;  // ROHM_B200_TMA_STORE=0 falls back to the per-thread store epilogue (developer switch)
-  // A-operand TMA multicast across CTA pairs (GemmParams::multicast_a); off by default, ROHM_B200_MULTICAST=1 turns it on.
-  bool use_multicast = false;
   // wgmma attention (F16X2, head dim 128, <= 160 tokens per clip; ROHM_B200_TC_ATTENTION=0 selects the mma.sync kernel)
   bool tc_attention = false;
   AttnWgmmaMaps attn_wg{};
@@ -440,9 +437,6 @@ static int setup_linear(rohm_posenet* pn, GemmParams* g, const float* a_hi, cons
   g->N = w.N;
   g->out_row_mul = 1;
   g->out_row_add = 0;
-  if (pn->use_multicast && w.kind == kKindF16 && pn->passes == 3 &&
-      gemm_enable_multicast(g, a_hi, a_lo, rows, K, lda, w.N, w.block_n, w.kind) != 0)
-    return fail(pn->ctx, ROHM_ERR_CUDA, "cuTensorMapEncodeTiled failed (multicast maps)");
   return ROHM_OK;
 }
 
@@ -549,8 +543,6 @@ extern "C" int rohm_posenet_create(rohm_ctx* ctx, const rohm_posenet_weights* w,
   pn->D = w->d_model, pn->F = w->ff_size, pn->L = w->num_layers, pn->H = w->num_heads;
   pn->C = w->in_feats, pn->Cout = w->out_feats, pn->traj = w->traj_feats, pn->pe_len = w->pe_len;
   pn->kind = precision == ROHM_PRECISION_F16X2 ? kKindF16 : kKindTf32;
-  if (const char* env = getenv("ROHM_B200_TMA_STORE")) pn->use_tma_store = env[0] != '0';
-  if (const char* env = getenv("ROHM_B200_MULTICAST")) pn->use_multicast = env[0] != '0';
   pn->passes = precision == ROHM_PRECISION_TF32 ? 1 : 3;
   pn->max_batch = max_batch, pn->max_frames = max_frames;
   pn->max_rows = static_cast<int64_t>(max_batch) * (max_frames + 1);
@@ -563,7 +555,7 @@ extern "C" int rohm_posenet_create(rohm_ctx* ctx, const rohm_posenet_weights* w,
   const int64_t R = pn->max_rows;
   {
     const char* env = getenv("ROHM_B200_FUSED_LN");
-    pn->fused_ln = pn->kind == kKindF16 && D == 512 && pn->use_tma_store && (env == nullptr || env[0] != '0');
+    pn->fused_ln = pn->kind == kKindF16 && D == 512 && (env == nullptr || env[0] != '0');
     if (pn->fused_ln) {
       pn->stats1 = static_cast<float2*>(pn->pool.bytes(R * 8 * static_cast<int64_t>(sizeof(float2))));
       pn->stats2 = static_cast<float2*>(pn->pool.bytes(R * 8 * static_cast<int64_t>(sizeof(float2))));
@@ -695,14 +687,14 @@ extern "C" int rohm_posenet_create(rohm_ctx* ctx, const rohm_posenet_weights* w,
       producer(pn->g_ff2[l], pn->stats2, pn->stats1, d.n1_w, d.n1_b);  // u2 = LN1(u1) + ffn
     }
     for (GemmParams* g : {&pn->g_qkv[l], &pn->g_proj[l], &pn->g_ff1[l], &pn->g_ff2[l]}) {
-      if (pn->use_tma_store && gemm_enable_tma_store(g, R, pn->kind) != 0) {
+      if (gemm_enable_tma_store(g, R, pn->kind) != 0) {
         const int rc__ = fail(ctx, ROHM_ERR_CUDA, "cuTensorMapEncodeTiled (store map) failed");
         delete pn;
         return rc__;
       }
     }
   }
-  if (pn->use_tma_store && gemm_enable_tma_store(&pn->g_out, R, pn->kind) != 0) {
+  if (gemm_enable_tma_store(&pn->g_out, R, pn->kind) != 0) {
     const int rc__ = fail(ctx, ROHM_ERR_CUDA, "cuTensorMapEncodeTiled (store map) failed");
     delete pn;
     return rc__;

@@ -88,26 +88,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// The same load delivered to the same shared-memory offset (and signalling the mbarrier at the same offset) of every CTA
-// of the cluster whose bit is set in cta_mask: one L2 read feeds several SMs.
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0,
-                                                      int32_t c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
-      "%4}], [%2], %5;" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
 // 2-D tiled store shared -> global (bulk async group of the issuing thread); out-of-bounds parts of the box are clipped.
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
@@ -153,18 +133,6 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() {
   asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
 }
-// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 remote;\n\t"
-      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-
 // Shared-memory matrix descriptor of a K-major tile whose rows are exactly one swizzle span of kRowBytes (128 ->
 // 128B swizzle, 64 -> 64B swizzle), as TMA writes it: 8-row core groups are 8 * kRowBytes apart.  sm_90 layout:
 // start_address[0,14) (>>4), LBO[16,30) (unused for swizzled K-major, 1), SBO[32,46) (>>4), layout[62,64): 1 = 128B,

@@ -33,12 +33,10 @@ class Gemm(C.Structure):
                 ("w_rows", C.c_int64), ("w_cols", C.c_int), ("bias", C.c_void_p), ("residual", C.c_void_p), ("ldr", C.c_int),
                 ("out", C.c_void_p), ("ldo", C.c_int), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p), ("lds", C.c_int),
                 ("acc_scale", C.c_float), ("act", C.c_int), ("M", C.c_int), ("N", C.c_int), ("out_row_mul", C.c_int),
-                ("out_row_add", C.c_int), ("clip_rows", C.c_int), ("clip_valid", C.c_int), ("gn_stats", C.c_void_p),
-                ("gn_groups", C.c_int), ("gn_group_size", C.c_int), ("a_stats", C.c_void_p), ("a_corr", C.c_void_p),
-                ("res_stats", C.c_void_p), ("res_gamma", C.c_void_p), ("res_beta", C.c_void_p), ("stats_out", C.c_void_p),
-                ("ln_eps", C.c_float), ("k_splits", C.c_int), ("split_row_stride", C.c_int), ("want_tma_store", C.c_int),
-                ("store_rows", C.c_int64), ("want_multicast", C.c_int), ("pdl", C.c_int), ("tma_store", C.c_int),
-                ("multicast", C.c_int)]
+                ("out_row_add", C.c_int), ("clip_rows", C.c_int), ("clip_valid", C.c_int), ("a_stats", C.c_void_p),
+                ("a_corr", C.c_void_p), ("res_stats", C.c_void_p), ("res_gamma", C.c_void_p), ("res_beta", C.c_void_p),
+                ("stats_out", C.c_void_p), ("ln_eps", C.c_float), ("k_splits", C.c_int), ("split_row_stride", C.c_int),
+                ("want_tma_store", C.c_int), ("store_rows", C.c_int64), ("pdl", C.c_int), ("tma_store", C.c_int)]
 
 
 class Attn(C.Structure):
@@ -134,7 +132,7 @@ class Weight:
 
 def gemm(kind, w, segs, M, N, *, passes=3, m_rows=None, out=None, ldo=None, out_hi=None, out_lo=None, lds=None,
          bias=None, residual=None, ldr=None, act=ACT_NONE, out_row_mul=1, out_row_add=0, clip_rows=0, clip_valid=0,
-         gn_stats=None, gn_groups=0, tma_store=False, store_rows=None, multicast=False, k_splits=0, split_row_stride=0,
+         tma_store=False, store_rows=None, k_splits=0, split_row_stride=0,
          a_stats=None, a_corr=None, res_stats=None, res_gamma=None, res_beta=None, stats_out=None, ln_eps=1e-5,
          pdl=False, n_cols=None):
     """One launch_gemm; returns (rc, the filled Gemm struct).  segs: list of Seg."""
@@ -156,15 +154,11 @@ def gemm(kind, w, segs, M, N, *, passes=3, m_rows=None, out=None, ldo=None, out_
     g.act, g.M, g.N = act, M, N
     g.out_row_mul, g.out_row_add = out_row_mul, out_row_add
     g.clip_rows, g.clip_valid = clip_rows, clip_valid
-    g.gn_stats = _ptr(gn_stats)
-    g.gn_groups = gn_groups
-    g.gn_group_size = N // gn_groups if gn_groups else 0
     g.a_stats, g.a_corr, g.res_stats = _ptr(a_stats), _ptr(a_corr), _ptr(res_stats)
     g.res_gamma, g.res_beta, g.stats_out, g.ln_eps = _ptr(res_gamma), _ptr(res_beta), _ptr(stats_out), ln_eps
     g.k_splits, g.split_row_stride = k_splits, split_row_stride
     g.want_tma_store = int(tma_store)
     g.store_rows = store_rows if store_rows is not None else M
-    g.want_multicast = int(multicast)
     g.pdl = int(pdl)
     rc = lib().probe_gemm(C.byref(g))
     return rc, g

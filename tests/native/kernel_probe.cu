@@ -45,8 +45,6 @@ struct ProbeGemm {
   int M, N;
   int out_row_mul, out_row_add;
   int clip_rows, clip_valid;
-  double* gn_stats;
-  int gn_groups, gn_group_size;
   const float* a_stats;  // float2 [rows][8]
   const float* a_corr;
   const float* res_stats;  // float2 [rows][8]
@@ -57,11 +55,9 @@ struct ProbeGemm {
   int k_splits, split_row_stride;
   int want_tma_store;   // ask gemm_enable_tma_store for the bulk-store epilogue over store_rows rows
   int64_t store_rows;
-  int want_multicast;   // ask gemm_enable_multicast (segment 0 is the A operand)
   int pdl;
   // set by probe_gemm: what the library decided
   int tma_store;
-  int multicast;
 };
 
 int probe_gemm(ProbeGemm* g) {
@@ -88,19 +84,12 @@ int probe_gemm(ProbeGemm* g) {
   p.M = g->M, p.N = g->N;
   p.out_row_mul = g->out_row_mul, p.out_row_add = g->out_row_add;
   p.clip_rows = g->clip_rows, p.clip_valid = g->clip_valid;
-  p.gn_stats = g->gn_stats, p.gn_groups = g->gn_groups, p.gn_group_size = g->gn_group_size;
   p.a_stats = reinterpret_cast<const float2*>(g->a_stats), p.a_corr = g->a_corr;
   p.res_stats = reinterpret_cast<const float2*>(g->res_stats), p.res_gamma = g->res_gamma, p.res_beta = g->res_beta;
   p.stats_out = reinterpret_cast<float2*>(g->stats_out), p.ln_eps = g->ln_eps;
   p.k_splits = g->k_splits, p.split_row_stride = g->split_row_stride;
   if (g->want_tma_store && (rc = gemm_enable_tma_store(&p, g->store_rows, g->kind)) != 0) return -rc;
-  if (g->want_multicast) {
-    const ProbeSeg& s0 = g->seg[0];
-    rc = gemm_enable_multicast(&p, s0.hi, s0.lo, s0.rows, s0.cols, s0.ld, g->n_cols, g->block_n, g->kind);
-    if (rc != 0) return -rc;
-  }
   g->tma_store = p.tma_store;
-  g->multicast = p.multicast_a;
   return static_cast<int>(launch_gemm(p, g->m_rows, g->n_cols, g->block_n, g->passes, nullptr, g->pdl != 0, g->kind));
 }
 

@@ -228,19 +228,17 @@ LEVELS = [(144, 176, 13, 64), (72, 88, 128, 128), (36, 44, 256, 256), (18, 22, 5
 
 @pytest.mark.parametrize("kind", [F16, TF32])
 @pytest.mark.parametrize("level", range(5))
-def test_conv_k5_masks_and_groupnorm_sums(dev, kind, level):
-    """k = 5 taps (row shifts -2..+2) at the TrajNet level shapes, GroupNorm(8) sums in the epilogue, pad rows exactly 0;
-    levels 1 and 3 read a two-source channel concat (the decoder's skip connections)."""
+def test_conv_k5_masks(dev, kind, level):
+    """k = 5 taps (row shifts -2..+2) at the TrajNet level shapes, pad rows exactly 0; levels 1 and 3 read a two-source
+    channel concat (the decoder's skip connections)."""
     T, Tp, Cin, Cout = LEVELS[level]
-    B, groups = 3, 8
+    B = 3
     cins = [Cin // 2, Cin - Cin // 2] if level in (1, 3) else [Cin]
     block_n = 64 if Cout <= 64 else 128
     W, segs, W64, x64, pad, ops = _conv_setup(dev, kind, B, T, Tp, cins, Cout, 5, 1, block_n, 40 + level)
     bias = _randn((Cout,), 3, dev)
     out = torch.full((B * Tp, Cout), 777.0, device=dev)
-    stats = torch.zeros(B, groups, 2, dtype=torch.float64, device=dev)
-    rc, g = kp.gemm(kind, W, segs, B * Tp, Cout, out=out, bias=bias, clip_rows=Tp, clip_valid=T, gn_stats=stats,
-                    gn_groups=groups, tma_store=True)
+    rc, g = kp.gemm(kind, W, segs, B * Tp, Cout, out=out, bias=bias, clip_rows=Tp, clip_valid=T, tma_store=True)
     assert rc == 0 and g.tma_store == 1
     torch.cuda.synchronize()
     y = out.reshape(B, Tp, Cout)
@@ -249,12 +247,6 @@ def test_conv_k5_masks_and_groupnorm_sums(dev, kind, level):
     aw = F.conv1d(x64.abs(), W64.abs(), padding=pad).permute(0, 2, 1)
     ws = W64.abs().sum((1, 2))
     _check(y[:, :T], ref, _bound(aw, bias.double().abs(), ws) + 2.0 ** -23 * ref.abs(), "conv")
-    # statistics of the stored values, per (clip, group), in float64
-    v = y[:, :T].double().reshape(B, T, groups, Cout // groups)
-    s1, s2 = v.sum((1, 3)), (v * v).sum((1, 3))
-    a1, a2 = v.abs().sum((1, 3)), (v * v).sum((1, 3))
-    assert float(((stats[..., 0] - s1).abs() - 2.0 ** -19 * a1).max()) <= 0.0, "GroupNorm sums"
-    assert float(((stats[..., 1] - s2).abs() - 2.0 ** -19 * a2).max()) <= 0.0, "GroupNorm sums of squares"
 
 
 @pytest.mark.parametrize("kind", [F16, TF32])
@@ -360,21 +352,6 @@ def test_split_k_refusals_launch_nothing(dev, kind):
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("kind,M,N,block_n,eligible", [(F16, 4640, 1536, 128, True), (F16, 34, 512, 128, True),
-                                                        (F16, 4640, 1152, 128, False), (TF32, 1000, 256, 64, True),
-                                                        (F16, 300, 96, 32, False)])
-def test_a_operand_multicast(dev, kind, M, N, block_n, eligible):
-    """CTA pairs share the A tile; an odd number of column tiles clears the flag and runs the plain path."""
-    A, W, _, _ = _linear(dev, kind, M, N, 512, block_n, 130 + N)
-    out = torch.zeros(M, N, device=dev)
-    rc, g = kp.gemm(kind, W, [A.seg(W.kblocks[0])], M, N, out=out, multicast=True)
-    assert rc == 0 and g.multicast == int(eligible)
-    torch.cuda.synchronize()
-    rows = _rows(M, 8)
-    ref, aw, ab, ws = _ref_linear(A, W, rows)
-    _check(out[rows.to(dev)], ref, _bound(aw, ab, ws) + 2.0 ** -23 * ref.abs(), "multicast")
-
-
 @pytest.mark.parametrize("M", [34, 128, 1000, 4640])
 def test_layernorm_folding_chain(dev, M):
     """(A) producer u1 = R + A1 W1^T + b1 in place over the residual pair, with per-row partial statistics;

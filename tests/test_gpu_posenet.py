@@ -109,12 +109,12 @@ def test_mma_sync_attention_fallback_matches_oracle(posenet, cuda_device, monkey
     assert float((y - ref).abs().max()) < TOL
 
 
-@pytest.mark.parametrize("env", [{"ROHM_B200_TC_ATTENTION": "0"}, {"ROHM_B200_MULTICAST": "1"}, {"ROHM_B200_TMA_STORE": "0"},
-                                 {"ROHM_B200_FUSED_LN": "0"}])
+@pytest.mark.parametrize("env", [{"ROHM_B200_TC_ATTENTION": "0"}, {"ROHM_B200_PRECISION": "tf32x3"},
+                                 {"ROHM_B200_TC_ATTENTION": "0", "ROHM_B200_FUSED_LN": "0"}, {"ROHM_B200_FUSED_LN": "0"}])
 def test_engine_switches_match_oracle(posenet, cuda_device, monkeypatch, env):
     """The engines behind the library's switches: ROHM_B200_TC_ATTENTION=0 routes f16x2 attention to the mma.sync m16n8k16
-    kernel, ROHM_B200_MULTICAST=1 shares the GEMMs' A tiles across CTA pairs, ROHM_B200_TMA_STORE=0 keeps the per-thread
-    store epilogue (and with it the separate LayerNorm kernel), ROHM_B200_FUSED_LN=0 the separate LayerNorm kernel alone.
+    kernel, ROHM_B200_FUSED_LN=0 keeps the separate LayerNorm kernel, both together leave no f16x2-only path in the forward,
+    and ROHM_B200_PRECISION=tf32x3 runs TF32 pairs (TF32 GEMM variants, mma.sync TF32 attention, separate LayerNorm).
     32 clips x 145 tokens: 37 row tiles, so the persistent GEMMs run several rounds per launch."""
     m, sd = posenet
     B, T = 32, 144

@@ -14,9 +14,9 @@ from rohm_b200.trajnet import TrajNet
 pytestmark = pytest.mark.gpu
 
 
-def _build(control, dev, seed=2):
+def _build(control, dev, seed=2, mid_dim=512):
     ds = synthetic.make_dataset('traj')
-    m = TrajNet(time_dim=32, mid_dim=512, cond_dim=13, traj_feat_dim=13, trajcontrol=control, device=dev, dataset=ds,
+    m = TrajNet(time_dim=32, mid_dim=mid_dim, cond_dim=13, traj_feat_dim=13, trajcontrol=control, device=dev, dataset=ds,
                 repr_abs_only=True)
     sd = {k: v.cpu() for k, v in synthetic.synth_state_dict(m, seed).items()}
     m.load_state_dict(sd)
@@ -105,6 +105,17 @@ def test_rejects_bad_frame_count(nets, cuda_device):
     with pytest.raises(RohmB200Error):
         m({'x_t': torch.zeros(1, 20, 13, device=cuda_device), 'cond': torch.zeros(1, 20, 13, device=cuda_device)},
           torch.zeros(1, dtype=torch.long, device=cuda_device))
+
+
+def test_rejects_mid_dim_that_is_not_a_multiple_of_256(cuda_device):
+    """mid_dim = 128 makes the level-0 blocks 16 channels wide: GroupNorm(8) groups of 2 channels, which the GroupNorm kernel
+    (float4 units) cannot take.  The engine refuses such a network when it is built and names the rule."""
+    from rohm_b200 import RohmB200Error
+    m, _ = _build(False, cuda_device, mid_dim=128)
+    batch = {k: v.to(cuda_device) for k, v in synthetic.trajnet_batch(1, 16, 3).items()}
+    batch['x_t'] = torch.zeros(1, 16, 13, device=cuda_device)
+    with pytest.raises(RohmB200Error, match=r"mid_dim \(128\) must be a positive multiple of 256"):
+        m(batch, torch.zeros(1, dtype=torch.long, device=cuda_device))
 
 
 def test_config1_trajnet_50_steps_matches_reference_golden(nets, cuda_device):
@@ -206,14 +217,15 @@ def test_launch_switches_do_not_change_the_result(nets, cuda_device):
         eng.lib.rohm_trajnet_set_option(eng.handle, 1, 1)
 
 
-@pytest.mark.parametrize("env", [{"ROHM_B200_TRAJ_SPLITK": "0"}, {"ROHM_B200_TRAJ_GN_EPILOGUE": "1"},
-                                 {"ROHM_B200_TRAJ_SPLITK": "0", "ROHM_B200_TRAJ_GN_EPILOGUE": "1"}])
+@pytest.mark.parametrize("env", [{"ROHM_B200_TRAJ_SPLITK": "0"}, {"ROHM_B200_TRAJ_PARALLEL": "0"},
+                                 {"ROHM_B200_TRAJ_SPLITK": "0", "ROHM_B200_TRAJ_PARALLEL": "0"}])
 def test_split_k_and_in_kernel_statistics_agree_with_the_single_pass_paths(nets, cuda_device, monkeypatch, env):
     """The default engine cuts the deep-level convolutions into K ranges (fp32 partials added in split order by the GroupNorm
-    kernel) and takes every GroupNorm's statistics inside that kernel; the engines built with ROHM_B200_TRAJ_SPLITK=0 and / or
-    ROHM_B200_TRAJ_GN_EPILOGUE=1 (one K loop per tile, statistics as double atomics in the GEMM epilogue: the round-2a path)
-    compute the same function with a different summation order: both must agree with the oracle and with each other far
-    inside the parity tolerance, at a batch where the split path uses 3-6 ranges (64 clips) and at one where it uses 8 (2 clips)."""
+    kernel, which takes every GroupNorm's statistics itself) and runs its graph on several streams.  The engine built with
+    ROHM_B200_TRAJ_SPLITK=0 (one K loop per tile, the GroupNorm kernel reading the one fp32 result) computes the same function
+    with a different summation order: it must agree with the default and with the oracle far inside the parity tolerance.
+    ROHM_B200_TRAJ_PARALLEL=0 (one serial chain) only changes the scheduling, so on its own it must be bit-identical.  Checked
+    at a batch where the split path uses 3-6 ranges (64 clips) and at one where it uses 8 (2 clips)."""
     _, sd = nets[True]
     for B, seed in ((2, 51), (64, 52)):
         T = 144
@@ -231,6 +243,8 @@ def test_split_k_and_in_kernel_statistics_agree_with_the_single_pass_paths(nets,
         out_other = other_m(batch, ts.to(cuda_device)).cpu()
         for k in env:
             monkeypatch.delenv(k)
+        if "ROHM_B200_TRAJ_SPLITK" not in env:
+            assert torch.equal(out_default, out_other), "scheduling alone must not change the result"
         scale = float(out_default.abs().max())
         assert float((out_default - out_other).abs().max()) < 2e-5 * max(1.0, scale)
         if B == 2:
