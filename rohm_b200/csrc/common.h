@@ -105,13 +105,6 @@ class DevicePool {
   int64_t total_ = 0;
 };
 
-// sampler.cu: the Philox-fused ancestral update, for engines that append it to their forward graph
-const void* ddpm_step_philox_kernel_address();
-int ddpm_step_philox_policy(rohm_ctx* ctx, int64_t numel, int64_t* G, int* iters, unsigned long long* increment);
-cudaError_t launch_ddpm_step_philox(const float* x0, const float* x_t, float* out, int64_t numel, int64_t clip_elems,
-                                    const float* coef, unsigned long long seed, unsigned long long offset, int64_t G, int iters,
-                                    cudaStream_t st, bool pdl = false);
-
 // A weight matrix [N, K] repacked for the GEMM: zero-padded to [Np, Kp] and split into a hi / lo pair: TF32 values in
 // fp32 containers (kind 0) or fp16 values of w * scale (kind 1, scale a power of two; see gemm.cuh GemmKind).
 struct PackedWeight {

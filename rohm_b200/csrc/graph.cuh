@@ -1,0 +1,123 @@
+// Cached CUDA graphs of a denoiser engine's forward (posenet.cu, trajnet.cu).  A forward, optionally followed by the sampler
+// update, is captured once per shape and then issued as one cudaGraphLaunch.  The few kernels that touch caller memory (the
+// boundary kernels) get those arguments replaced before every replay.
+#pragma once
+#include <cstring>
+#include <functional>
+#include <memory>
+#include <tuple>
+#include <type_traits>
+#include <vector>
+
+#include "common.h"
+
+namespace rohm {
+
+// Argument I of a boundary kernel, set to `value` on every replay.
+template <size_t I, typename V>
+struct Arg {
+  V value;
+};
+template <size_t I, typename V>
+Arg<I, V> arg(V value) {
+  return {value};
+}
+
+// A boundary kernel and those of its arguments that change from call to call.  The kernel's function type gives the
+// argument count and the type of every patched parameter: an index past the end, or a value whose type is not the
+// parameter's (a pointer may gain const), does not compile.
+class KernelPatch {
+ public:
+  template <typename... P, size_t... I, typename... V>
+  KernelPatch(void (*kernel)(P...), Arg<I, V>... args)
+      : func_(reinterpret_cast<const void*>(kernel)), nargs_(sizeof...(P)) {
+    static_assert(sizeof...(P) <= kMaxArgs && sizeof...(I) <= kMaxPatched, "KernelPatch: raise kMaxArgs / kMaxPatched");
+    (put<std::tuple_element_t<I, std::tuple<P...>>>(I, args.value), ...);
+  }
+  const void* func() const { return func_; }
+  // Sets the arguments of `node` in `exec` to `captured` (the node's parameters as captured) with the patched ones replaced.
+  cudaError_t apply(cudaGraphExec_t exec, cudaGraphNode_t node, const cudaKernelNodeParams& captured) const;
+
+ private:
+  static constexpr int kMaxArgs = 32, kMaxPatched = 8;
+  struct Slot {
+    size_t index;
+    alignas(8) unsigned char bytes[8];
+  };
+  template <typename T, typename V>
+  void put(size_t index, const V& value) {
+    static_assert(std::is_same<V, T>::value || (std::is_pointer<V>::value && std::is_convertible<V, T>::value),
+                  "KernelPatch: the value's type is not the kernel parameter's");
+    static_assert(sizeof(T) <= sizeof(Slot::bytes), "KernelPatch: parameter wider than a slot");
+    const T v = value;
+    slots_[n_].index = index;
+    std::memcpy(slots_[n_].bytes, &v, sizeof v);
+    ++n_;
+  }
+  const void* func_;
+  int nargs_;
+  Slot slots_[kMaxPatched];
+  int n_ = 0;
+};
+
+// An engine's captured forwards, keyed by (B, T, with_step); at most kMaxGraphs, the oldest evicted first.
+class ForwardGraphs {
+ public:
+  static constexpr size_t kMaxGraphs = 8;
+  bool enabled = true;  // false: every forward is launched eagerly
+
+  ForwardGraphs() = default;
+  ForwardGraphs(const ForwardGraphs&) = delete;
+  ForwardGraphs& operator=(const ForwardGraphs&) = delete;
+  ~ForwardGraphs();
+
+  // Issues one forward on `st`.  launches(stream) issues its kernels on `stream`.  That runs directly on `st` when `eager`,
+  // when graphs are off, or when the caller is capturing `st`.  Otherwise the graph of (B, T, with_step) is replayed with
+  // the arguments of `patches` set; launches() is captured into it on first use.  Every call passes the same kernels in
+  // `patches` for the same key.
+  int run(rohm_ctx* ctx, int B, int T, bool with_step, bool eager, cudaStream_t st,
+          const std::function<int(cudaStream_t)>& launches, const std::vector<KernelPatch>& patches);
+  void clear() { graphs_.clear(); }  // the next run() of every key captures again
+
+ private:
+  struct DestroyGraph {
+    void operator()(cudaGraph_t g) const { cudaGraphDestroy(g); }
+  };
+  struct DestroyExec {
+    void operator()(cudaGraphExec_t e) const { cudaGraphExecDestroy(e); }
+  };
+  struct Entry {
+    int B = 0, T = 0;
+    bool with_step = false;
+    std::unique_ptr<std::remove_pointer_t<cudaGraph_t>, DestroyGraph> graph;  // owns the captured arguments in `params`
+    std::unique_ptr<std::remove_pointer_t<cudaGraphExec_t>, DestroyExec> exec;
+    std::vector<cudaGraphNode_t> nodes;  // the boundary nodes, in the order of the patches
+    std::vector<cudaKernelNodeParams> params;
+  };
+  int capture(rohm_ctx* ctx, const std::function<int(cudaStream_t)>& launches, const std::vector<KernelPatch>& patches,
+              Entry* e);
+
+  cudaStream_t capture_stream_ = nullptr;
+  std::vector<Entry> graphs_;
+};
+
+// sampler.cu: the Philox-fused ancestral update that the engines append to their forward (rohm_posenet_sample_step,
+// rohm_trajnet_sample_step).  x_next = coef_row-weighted x0, x_t and noise; the noise is what torch.randn_like would draw
+// from the generator state (seed, offset).
+struct DdpmStep {
+  const float* x0;  // the forward's output
+  const float* x_t;
+  float* x_next;
+  int64_t numel, clip_elems;
+  const float* coef_row;  // one row for every clip
+  unsigned long long seed, offset;
+  int64_t G = 0;  // launch geometry of torch's normal_ for numel, set by ddpm_step_plan
+  int iters = 0;
+};
+// Sets s->G and s->iters; *offset_increment (if not null) = what the generator's offset advances by.
+int ddpm_step_plan(rohm_ctx* ctx, DdpmStep* s, uint64_t* offset_increment);
+int launch_ddpm_step(rohm_ctx* ctx, const DdpmStep& s, cudaStream_t st, bool pdl);
+// The update node's per-call arguments in a replayed graph.
+KernelPatch ddpm_step_patch(const DdpmStep& s);
+
+}  // namespace rohm

@@ -10,7 +10,7 @@
 //   8 x { X --GEMM--> Q|K|V --attention (wgmma: S = QK^T, softmax on the fragments, O = PV)--> CTX --GEMM(+bias)--> Y
 //         --LN(Y + X)--> X --GEMM(+bias,GELU)--> H --GEMM(+bias)--> Y --LN(Y + X)--> X }
 //   X --GEMM--> OUT_tok --unpack(+copy cond[:, :traj])--> out [B,C,1,T]
-// One forward = 61 launches, replayed as one CUDA graph with programmatic dependent launch along the chain.
+// One forward = 45 launches, replayed as one CUDA graph with programmatic dependent launch along the chain.
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -19,6 +19,7 @@
 #include "attention.cuh"
 #include "common.h"
 #include "gemm.cuh"
+#include "graph.cuh"
 #include "ptx.cuh"
 
 namespace rohm {
@@ -59,6 +60,7 @@ __global__ void pack_tokens_kernel(const float* __restrict__ x, float* __restric
     }
   }
 }
+constexpr size_t kPackTokensX = 0;  // the argument replaced on every replay of a cached forward graph
 
 // Token rows -> [B, C, T]: channels [traj, traj+Cout) from tok[b*S+1+t][c - traj], channels [0, traj) from cond.
 __global__ void unpack_tokens_kernel(const float* __restrict__ tok, const float* __restrict__ cond_traj,
@@ -85,6 +87,7 @@ __global__ void unpack_tokens_kernel(const float* __restrict__ tok, const float*
     }
   }
 }
+constexpr size_t kUnpackTokensOut = 2;  // the argument replaced on every replay of a cached forward graph
 
 // rows[b*S + s][:] = pe[s][:]   (positional rows added to every token incl. the timestep token, posenet.py:90-91)
 __global__ void pe_rows_kernel(const float* __restrict__ pe, float* __restrict__ rows, int S, int D, int64_t total4) {
@@ -102,14 +105,10 @@ __global__ void pe_rows_kernel(const float* __restrict__ pe, float* __restrict__
 // over all pe_len timesteps); per step the token row (b, 0) is a gather.
 __global__ void time_token_gather_kernel(const int64_t* __restrict__ timesteps, const float* __restrict__ table,
                                          int table_rows, float* __restrict__ X, float* __restrict__ Xh,
-                                         float* __restrict__ Xl, int S, int D, int f16, unsigned int* __restrict__ zero_buf,
-                                         int zero_n) {
+                                         float* __restrict__ Xl, int S, int D, int f16) {
   ptx::pdl_launch_dependents();
   ptx::pdl_wait_prior_grid();  // the embedding GEMM (which also writes row (b, 0)) has completed
   const int b = blockIdx.x;
-  // once per forward: clear the arrival counters of the fused LayerNorm epilogues (GemmParams::ln_count)
-  if (b == 0)
-    for (int i = threadIdx.x; i < zero_n; i += blockDim.x) zero_buf[i] = 0u;
   int64_t t = timesteps[b];
   // The reference indexes pe[timesteps] and raises on a bad index (heads.py:145).  A kernel cannot raise, so an
   // out-of-range timestep poisons the clip's timestep token with NaN (which attention spreads over the whole clip's
@@ -136,6 +135,7 @@ __global__ void time_token_gather_kernel(const int64_t* __restrict__ timesteps, 
     }
   }
 }
+constexpr size_t kTimeTokenTimesteps = 0;  // the argument replaced on every replay of a cached forward graph
 
 __global__ void add_vec_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ out, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -252,18 +252,9 @@ struct rohm_posenet {
   float* cond_traj = nullptr;  // [B, traj, T] copy of cond[:, :traj] taken by set_cond (output channels [0,traj))
   int cond_B = -1, cond_T = -1;
   int launches = 0;
-  // CUDA graph of one forward per (B, T): 61 launches become one cudaGraphLaunch; the three nodes that touch caller
+  // CUDA graph of one forward per (B, T): 45 launches become one cudaGraphLaunch; the three nodes that touch caller
   // memory (pack: x_t, time-token gather: timesteps, unpack: out) get their pointers patched before every replay.
-  struct FwdGraph {
-    int B = 0, T = 0;
-    bool with_step = false;  // forward + Philox-fused ancestral update (rohm_posenet_sample_step)
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
-    cudaGraphNode_t n_pack = nullptr, n_time = nullptr, n_unpack = nullptr, n_step = nullptr;
-    cudaKernelNodeParams p_pack{}, p_time{}, p_unpack{}, p_step{};
-  };
-  std::vector<FwdGraph> graphs;
-  bool use_graph = true;
+  ForwardGraphs graphs;
   bool use_pdl = true;
   // wgmma attention (F16X2, head dim 128, <= 160 tokens per clip; ROHM_B200_TC_ATTENTION=0 selects the mma.sync kernel)
   bool tc_attention = false;
@@ -276,14 +267,6 @@ struct rohm_posenet {
   float2* stats1 = nullptr;
   float2* stats2 = nullptr;
   float *out_c = nullptr, *out_d = nullptr;  // output head: c_n, d_n of the folded last LayerNorm
-  cudaStream_t capture_stream = nullptr;
-  ~rohm_posenet() {
-    if (capture_stream) cudaStreamDestroy(capture_stream);
-    for (auto& g : graphs) {
-      if (g.exec) cudaGraphExecDestroy(g.exec);
-      if (g.graph) cudaGraphDestroy(g.graph);
-    }
-  }
   // optional per-kernel event timing (rohm_posenet_profile): category -> list of (start, stop) events
   bool profiling = false;
   std::vector<cudaEvent_t> prof_events;
@@ -797,7 +780,7 @@ static int forward_launches(rohm_posenet* pn, const float* x_t, const int64_t* t
   if ((rc = run_gemm(pn, pn->g_in, pn->w_in, rows, st)) != ROHM_OK) return rc;
   prof_begin(pn, kCatOther, st);
   ROHM_CUDA(ctx, launch_chain(time_token_gather_kernel, dim3(B), dim3(128), 0, st, pdl, timesteps, pn->time_table, pn->pe_len,
-                              pn->X, pn->Xh, pn->Xl, S, D, pn->kind == kKindF16 ? 1 : 0, nullptr, 0));
+                              pn->X, pn->Xh, pn->Xl, S, D, pn->kind == kKindF16 ? 1 : 0));
   prof_end(pn, st);
   ROHM_CUDA(ctx, cudaGetLastError());
   pn->launches++;
@@ -854,67 +837,9 @@ extern "C" int rohm_posenet_profile(rohm_posenet* pn, const float* x_t, const in
   return ROHM_OK;
 }
 
-struct StepArgs {  // the ancestral update appended to the forward (rohm_posenet_sample_step)
-  float* x_next;
-  const float* coef_row;
-  unsigned long long seed, offset;
-  int64_t G;
-  int iters;
-};
-
-static int build_forward_graph(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* out, int B, int T,
-                               cudaStream_t st, rohm_posenet::FwdGraph* fg, const StepArgs* step = nullptr) {
-  rohm_ctx* ctx = pn->ctx;
-  rohm::DeviceGuard device_guard__(ctx);
-  // Capture on a private stream: the caller's stream may be the legacy default stream, which cannot be captured.
-  // Nothing executes during capture; the instantiated graph is then launched on the caller's stream.
-  (void)st;
-  if (pn->capture_stream == nullptr)
-    ROHM_CUDA(ctx, cudaStreamCreateWithFlags(&pn->capture_stream, cudaStreamNonBlocking));
-  cudaStream_t cs = pn->capture_stream;
-  ROHM_CUDA(ctx, cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-  int rc = forward_launches(pn, x_t, timesteps, out, B, T, cs);
-  if (rc == ROHM_OK && step != nullptr) {
-    const int64_t clip_elems = static_cast<int64_t>(pn->C) * T;
-    if (launch_ddpm_step_philox(out, x_t, step->x_next, clip_elems * B, clip_elems, step->coef_row, step->seed, step->offset,
-                                step->G, step->iters, cs, pn->use_pdl) != cudaSuccess)
-      rc = fail(ctx, ROHM_ERR_CUDA, "ddpm step launch failed during capture");
-    pn->launches++;
-  }
-  cudaGraph_t graph = nullptr;
-  cudaError_t e = cudaStreamEndCapture(cs, &graph);
-  if (rc != ROHM_OK) {
-    if (graph) cudaGraphDestroy(graph);
-    return rc;
-  }
-  ROHM_CUDA(ctx, e);
-  size_t n = 0;
-  ROHM_CUDA(ctx, cudaGraphGetNodes(graph, nullptr, &n));
-  std::vector<cudaGraphNode_t> nodes(n);
-  ROHM_CUDA(ctx, cudaGraphGetNodes(graph, nodes.data(), &n));
-  fg->B = B, fg->T = T, fg->graph = graph, fg->with_step = step != nullptr;
-  for (cudaGraphNode_t node : nodes) {
-    cudaGraphNodeType ty;
-    ROHM_CUDA(ctx, cudaGraphNodeGetType(node, &ty));
-    if (ty != cudaGraphNodeTypeKernel) continue;
-    cudaKernelNodeParams kp{};
-    ROHM_CUDA(ctx, cudaGraphKernelNodeGetParams(node, &kp));
-    if (kp.func == reinterpret_cast<void*>(pack_tokens_kernel)) fg->n_pack = node, fg->p_pack = kp;
-    else if (kp.func == reinterpret_cast<void*>(time_token_gather_kernel)) fg->n_time = node, fg->p_time = kp;
-    else if (kp.func == reinterpret_cast<void*>(unpack_tokens_kernel)) fg->n_unpack = node, fg->p_unpack = kp;
-    else if (kp.func == const_cast<void*>(ddpm_step_philox_kernel_address())) fg->n_step = node, fg->p_step = kp;
-  }
-  if (!fg->n_pack || !fg->n_time || !fg->n_unpack || (step != nullptr && !fg->n_step)) {
-    cudaGraphDestroy(graph);
-    fg->graph = nullptr;
-    return fail(ctx, ROHM_ERR_CUDA, "forward graph: could not locate the boundary kernel nodes");
-  }
-  ROHM_CUDA(ctx, cudaGraphInstantiate(&fg->exec, graph, 0));
-  return ROHM_OK;
-}
-
+// One forward, with the ancestral update appended when `step` is given (rohm_posenet_sample_step).
 static int forward_or_step(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* out, int B, int T,
-                           void* stream, const StepArgs* step) {
+                           void* stream, const DdpmStep* step) {
   if (pn == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = pn->ctx;
   rohm::DeviceGuard device_guard__(ctx);
@@ -923,73 +848,17 @@ static int forward_or_step(rohm_posenet* pn, const float* x_t, const int64_t* ti
   if (B != pn->cond_B || T != pn->cond_T)
     return fail(ctx, ROHM_ERR_STATE, "rohm_posenet_forward: B=%d T=%d but set_cond was called with B=%d T=%d", B, T,
                 pn->cond_B, pn->cond_T);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  ROHM_CUDA(ctx, cudaStreamIsCapturing(st, &cap));
-  if (!pn->use_graph || pn->profiling || cap != cudaStreamCaptureStatusNone) {
-    int rc = forward_launches(pn, x_t, timesteps, out, B, T, st);
-    if (rc == ROHM_OK && step != nullptr) {
-      const int64_t clip_elems = static_cast<int64_t>(pn->C) * T;
-      ROHM_CUDA(ctx, launch_ddpm_step_philox(out, x_t, step->x_next, clip_elems * B, clip_elems, step->coef_row, step->seed,
-                                             step->offset, step->G, step->iters, st, pn->use_pdl && !pn->profiling));
-      pn->launches++;
-    }
-    return rc;
-  }
-
-  rohm_posenet::FwdGraph* fg = nullptr;
-  for (auto& g : pn->graphs)
-    if (g.B == B && g.T == T && g.with_step == (step != nullptr)) fg = &g;
-  if (fg == nullptr) {
-    rohm_posenet::FwdGraph ng;
-    int rc = build_forward_graph(pn, x_t, timesteps, out, B, T, st, &ng, step);
-    if (rc != ROHM_OK) return rc;
-    if (pn->graphs.size() >= 8) {  // bounded cache
-      if (pn->graphs.front().exec) cudaGraphExecDestroy(pn->graphs.front().exec);
-      if (pn->graphs.front().graph) cudaGraphDestroy(pn->graphs.front().graph);
-      pn->graphs.erase(pn->graphs.begin());
-    }
-    pn->graphs.push_back(ng);
-    fg = &pn->graphs.back();
-  }
-  // patch the caller-memory pointers (argument 0 of pack / time-token, arguments 0.. of unpack: tok, cond, out)
-  const void* a_x = x_t;
-  const void* a_t = timesteps;
-  void* a_o = out;
-  {
-    cudaKernelNodeParams kp = fg->p_pack;
-    std::vector<void*> args(kp.kernelParams, kp.kernelParams + 8);
-    args[0] = &a_x;
-    kp.kernelParams = args.data();
-    ROHM_CUDA(ctx, cudaGraphExecKernelNodeSetParams(fg->exec, fg->n_pack, &kp));
-  }
-  {
-    cudaKernelNodeParams kp = fg->p_time;
-    std::vector<void*> args(kp.kernelParams, kp.kernelParams + 11);
-    args[0] = &a_t;
-    kp.kernelParams = args.data();
-    ROHM_CUDA(ctx, cudaGraphExecKernelNodeSetParams(fg->exec, fg->n_time, &kp));
-  }
-  {
-    cudaKernelNodeParams kp = fg->p_unpack;
-    std::vector<void*> args(kp.kernelParams, kp.kernelParams + 9);
-    args[2] = &a_o;
-    kp.kernelParams = args.data();
-    ROHM_CUDA(ctx, cudaGraphExecKernelNodeSetParams(fg->exec, fg->n_unpack, &kp));
-  }
-  if (step != nullptr) {  // x0, x_t, out, coef row, Philox seed / offset of this step
-    cudaKernelNodeParams kp = fg->p_step;
-    std::vector<void*> args(kp.kernelParams, kp.kernelParams + 14);
-    const void* a_x0 = out;
-    void* a_next = step->x_next;
-    const void* a_coef = step->coef_row;
-    unsigned long long a_seed = step->seed, a_off = step->offset;
-    args[0] = &a_x0, args[1] = &a_x, args[5] = &a_next, args[8] = &a_coef, args[10] = &a_seed, args[11] = &a_off;
-    kp.kernelParams = args.data();
-    ROHM_CUDA(ctx, cudaGraphExecKernelNodeSetParams(fg->exec, fg->n_step, &kp));
-  }
-  ROHM_CUDA(ctx, cudaGraphLaunch(fg->exec, st));
-  return ROHM_OK;
+  auto launches = [&](cudaStream_t st) {
+    const int rc = forward_launches(pn, x_t, timesteps, out, B, T, st);
+    if (rc != ROHM_OK || step == nullptr) return rc;
+    pn->launches++;
+    return launch_ddpm_step(ctx, *step, st, pn->use_pdl && !pn->profiling);
+  };
+  std::vector<KernelPatch> patches = {{pack_tokens_kernel, arg<kPackTokensX>(x_t)},
+                                      {time_token_gather_kernel, arg<kTimeTokenTimesteps>(timesteps)},
+                                      {unpack_tokens_kernel, arg<kUnpackTokensOut>(out)}};
+  if (step != nullptr) patches.push_back(ddpm_step_patch(*step));
+  return pn->graphs.run(ctx, B, T, step != nullptr, pn->profiling, static_cast<cudaStream_t>(stream), launches, patches);
 }
 
 extern "C" int rohm_posenet_forward(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* out, int B,
@@ -1003,27 +872,22 @@ extern "C" int rohm_posenet_sample_step(rohm_posenet* pn, const float* x_t, cons
   if (pn == nullptr) return ROHM_ERR_INVALID;
   if (x_next == nullptr || coef_row == nullptr)
     return fail(pn->ctx, ROHM_ERR_INVALID, "rohm_posenet_sample_step: null pointer");
-  StepArgs sa{x_next, coef_row, seed, offset, 0, 0};
-  unsigned long long inc = 0;
-  int rc = ddpm_step_philox_policy(pn->ctx, static_cast<int64_t>(pn->C) * T * B, &sa.G, &sa.iters, &inc);
+  const int64_t clip_elems = static_cast<int64_t>(pn->C) * T;
+  DdpmStep step{x0_out, x_t, x_next, clip_elems * B, clip_elems, coef_row, seed, offset};
+  const int rc = ddpm_step_plan(pn->ctx, &step, offset_increment);
   if (rc != ROHM_OK) return rc;
-  if (offset_increment != nullptr) *offset_increment = inc;
-  return forward_or_step(pn, x_t, timesteps, x0_out, B, T, stream, &sa);
+  return forward_or_step(pn, x_t, timesteps, x0_out, B, T, stream, &step);
 }
 
 extern "C" int rohm_posenet_set_option(rohm_posenet* pn, int option, int value) {
   if (pn == nullptr) return ROHM_ERR_INVALID;
   if (option == 0) {
-    pn->use_graph = value != 0;
+    pn->graphs.enabled = value != 0;
     return ROHM_OK;
   }
   if (option == 1) {  // programmatic dependent launch on the GEMMs (graphs are re-captured)
+    if (pn->use_pdl != (value != 0)) pn->graphs.clear();
     pn->use_pdl = value != 0;
-    for (auto& g : pn->graphs) {
-      if (g.exec) cudaGraphExecDestroy(g.exec);
-      if (g.graph) cudaGraphDestroy(g.graph);
-    }
-    pn->graphs.clear();
     return ROHM_OK;
   }
   return fail(pn->ctx, ROHM_ERR_INVALID, "rohm_posenet_set_option: unknown option %d", option);

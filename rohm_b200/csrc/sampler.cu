@@ -4,7 +4,7 @@
 // (diffusion/gaussian_diffusion_posenet.py:212-234, 426-434, 461-479, 192-210, 696-715).
 #include <curand_kernel.h>
 
-#include "common.h"
+#include "graph.cuh"
 
 namespace rohm {
 namespace {
@@ -116,6 +116,8 @@ __global__ void __launch_bounds__(kThreads) ddpm_step_philox_kernel(const float*
     }
   }
 }
+// The arguments of ddpm_step_philox_kernel that change from step to step in a replayed graph (ddpm_step_patch)
+constexpr size_t kStepX0 = 0, kStepXt = 1, kStepOut = 5, kStepCoef = 8, kStepSeed = 10, kStepOffset = 11;
 
 int grid_for(const rohm_ctx* ctx, int64_t work_items) {
   const int sms = ctx->sm_count > 0 ? ctx->sm_count : 132;
@@ -202,25 +204,24 @@ extern "C" int rohm_ddpm_step_philox(rohm_ctx* ctx, const float* x0, const float
   return ROHM_OK;
 }
 
-// For the denoiser engines that append the update to their forward graph (posenet.cu): the kernel's address (to find its
-// graph node) and a launch with explicit geometry.
+// The update the denoiser engines append to their forward (graph.cuh DdpmStep).
 namespace rohm {
-const void* ddpm_step_philox_kernel_address() { return reinterpret_cast<const void*>(ddpm_step_philox_kernel); }
-int ddpm_step_philox_policy(rohm_ctx* ctx, int64_t numel, int64_t* G, int* iters, unsigned long long* increment) {
-  return torch_normal_policy(ctx, numel, G, iters, increment);
+int ddpm_step_plan(rohm_ctx* ctx, DdpmStep* s, uint64_t* offset_increment) {
+  unsigned long long inc = 0;
+  const int rc = torch_normal_policy(ctx, s->numel, &s->G, &s->iters, &inc);
+  if (rc != ROHM_OK) return rc;
+  if (offset_increment != nullptr) *offset_increment = inc;
+  return ROHM_OK;
 }
-cudaError_t launch_ddpm_step_philox(const float* x0, const float* x_t, float* out, int64_t numel, int64_t clip_elems,
-                                    const float* coef, unsigned long long seed, unsigned long long offset, int64_t G, int iters,
-                                    cudaStream_t st, bool pdl) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(G / kThreads)), cfg.blockDim = dim3(kThreads), cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr, cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, ddpm_step_philox_kernel, x0, x_t, static_cast<const float*>(nullptr),
-                            static_cast<const float*>(nullptr), 0, out, numel, clip_elems, coef, static_cast<int64_t>(0), seed,
-                            offset, G, iters);
+int launch_ddpm_step(rohm_ctx* ctx, const DdpmStep& s, cudaStream_t st, bool pdl) {
+  ROHM_CUDA(ctx, launch_chain(ddpm_step_philox_kernel, dim3(static_cast<unsigned>(s.G / kThreads)), dim3(kThreads), 0, st, pdl,
+                              s.x0, s.x_t, nullptr, nullptr, 0, s.x_next, s.numel, s.clip_elems, s.coef_row, 0, s.seed,
+                              s.offset, s.G, s.iters));
+  return ROHM_OK;
+}
+KernelPatch ddpm_step_patch(const DdpmStep& s) {
+  return {ddpm_step_philox_kernel, arg<kStepX0>(s.x0),         arg<kStepXt>(s.x_t),       arg<kStepOut>(s.x_next),
+          arg<kStepCoef>(s.coef_row), arg<kStepSeed>(s.seed), arg<kStepOffset>(s.offset)};
 }
 }  // namespace rohm
 

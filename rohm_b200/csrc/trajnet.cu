@@ -21,6 +21,7 @@
 
 #include "common.h"
 #include "gemm.cuh"
+#include "graph.cuh"
 #include "ptx.cuh"
 
 namespace rohm {
@@ -50,6 +51,7 @@ __global__ void pack_rows_kernel(const float* __restrict__ x, float* __restrict_
     lo[o] = v - h;
   }
 }
+constexpr size_t kPackRowsX = 0;  // the argument replaced on every replay of a cached forward graph
 
 // Timestep path of TrajNet (trajnet.py:120-125, 189) and the per-block time projections (heads.py:34-38, 51-52):
 //   temb = W3 mish(W1 sinusoid(t) + b1) + b3;  tp[b, :] = Wcat mish(temb) + bcat   (all blocks' Linear(32,out) stacked)
@@ -109,6 +111,7 @@ __global__ void __launch_bounds__(256) trajnet_time_kernel(const int64_t* __rest
   }
   trajnet_time_compute(static_cast<float>(ti), b, time_dim, w1, b1, w3, b3, wcat, bcat, total_out, tp, sm);
 }
+constexpr size_t kTrajnetTimeT = 0;  // the argument replaced on every replay of a cached forward graph
 
 constexpr int kMaxSplitsDev = 8;  // most K ranges a convolution is cut into (= kMaxSplits of the host-side choice)
 
@@ -259,6 +262,7 @@ __global__ void unpack_rows_kernel(const float* __restrict__ x, float* __restric
   const int64_t b = bt / T;
   out[i] = x[(b * Tp + t) * ld + c];
 }
+constexpr size_t kUnpackRowsOut = 1;  // the argument replaced on every replay of a cached forward graph
 
 // One segment of a convolution weight -> columns [seg_off, seg_off + Cs) of the packed [Np, Ktot] hi/lo pair.
 // conv:      w[co][src_off + c][tap]   (Conv1d weight [Cout, Cin, k])
@@ -349,36 +353,13 @@ struct rohm_trajnet {
   bool time_pending[2] = {false, false};
   int cond_B = -1;
   int launches = 0;
-  // CUDA graph of one forward per batch size
-  struct FwdGraph {
-    int B = 0;
-    bool with_step = false;  // forward + Philox-fused ancestral update (rohm_trajnet_sample_step)
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
-    cudaGraphNode_t n_pack = nullptr, n_time = nullptr, n_unpack = nullptr, n_step = nullptr;
-    cudaKernelNodeParams p_pack{}, p_time{}, p_unpack{}, p_step{};
-  };
-  std::vector<FwdGraph> graphs;
-  bool use_graph = true;
+  ForwardGraphs graphs;  // CUDA graph of one forward per batch size
   bool use_pdl = true;  // ROHM_B200_PDL / rohm_trajnet_set_option(1): programmatic dependent launch along the conv / GroupNorm chains
-  cudaStream_t capture_stream = nullptr;
-  void drop_graphs() {
-    for (auto& g : graphs) {
-      if (g.exec) cudaGraphExecDestroy(g.exec);
-      if (g.graph) cudaGraphDestroy(g.graph);
-    }
-    graphs.clear();
-  }
   ~rohm_trajnet() {
-    if (capture_stream) cudaStreamDestroy(capture_stream);
     for (cudaStream_t q : side)
       if (q) cudaStreamDestroy(q);
     for (cudaEvent_t e : events) cudaEventDestroy(e);
     if (time_ready) cudaEventDestroy(time_ready);
-    for (auto& g : graphs) {
-      if (g.exec) cudaGraphExecDestroy(g.exec);
-      if (g.graph) cudaGraphDestroy(g.graph);
-    }
   }
 };
 
@@ -1121,125 +1102,26 @@ static int trajnet_forward_launches(rohm_trajnet* tn, const float* x_t, const in
   return ROHM_OK;
 }
 
-struct TrajStepArgs {  // the ancestral update appended to the forward (rohm_trajnet_sample_step)
-  float* x_next;
-  const float* coef_row;
-  unsigned long long seed, offset;
-  int64_t G;
-  int iters;
-};
-
+// One forward, with the ancestral update appended when `step` is given (rohm_trajnet_sample_step).
 static int trajnet_forward_or_step(rohm_trajnet* tn, const float* x_t, const int64_t* time, float* out, int B, void* stream,
-                                   const TrajStepArgs* step) {
+                                   const DdpmStep* step) {
   if (tn == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = tn->ctx;
   rohm::DeviceGuard device_guard__(ctx);
   if (x_t == nullptr || time == nullptr || out == nullptr) return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_forward: null pointer");
   if (B != tn->cond_B)
     return fail(ctx, ROHM_ERR_STATE, "rohm_trajnet_forward: B=%d but set_cond was called with B=%d", B, tn->cond_B);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  ROHM_CUDA(ctx, cudaStreamIsCapturing(st, &cap));
-  const int64_t clip_elems = static_cast<int64_t>(tn->T) * tn->traj_dim;
-  auto launch_step = [&](cudaStream_t s_) {
-    return launch_ddpm_step_philox(out, x_t, step->x_next, clip_elems * B, clip_elems, step->coef_row, step->seed, step->offset,
-                                   step->G, step->iters, s_, tn->use_pdl);
+  auto launches = [&](cudaStream_t st) {
+    const int rc = trajnet_forward_launches(tn, x_t, time, out, B, st);
+    if (rc != ROHM_OK || step == nullptr) return rc;
+    tn->launches++;
+    return launch_ddpm_step(ctx, *step, st, tn->use_pdl);
   };
-  if (!tn->use_graph || cap != cudaStreamCaptureStatusNone) {
-    int rc = trajnet_forward_launches(tn, x_t, time, out, B, st);
-    if (rc == ROHM_OK && step != nullptr) {
-      ROHM_CUDA(ctx, launch_step(st));
-      tn->launches++;
-    }
-    return rc;
-  }
-
-  rohm_trajnet::FwdGraph* fg = nullptr;
-  for (auto& g : tn->graphs)
-    if (g.B == B && g.with_step == (step != nullptr)) fg = &g;
-  if (fg == nullptr) {
-    if (tn->capture_stream == nullptr) ROHM_CUDA(ctx, cudaStreamCreateWithFlags(&tn->capture_stream, cudaStreamNonBlocking));
-    cudaStream_t cs = tn->capture_stream;
-    ROHM_CUDA(ctx, cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-    int rc = trajnet_forward_launches(tn, x_t, time, out, B, cs);
-    if (rc == ROHM_OK && step != nullptr) {
-      if (launch_step(cs) != cudaSuccess) rc = fail(ctx, ROHM_ERR_CUDA, "ddpm step launch failed during capture");
-      tn->launches++;
-    }
-    cudaGraph_t graph = nullptr;
-    cudaError_t e = cudaStreamEndCapture(cs, &graph);
-    if (rc != ROHM_OK) {
-      if (graph) cudaGraphDestroy(graph);
-      return rc;
-    }
-    ROHM_CUDA(ctx, e);
-    rohm_trajnet::FwdGraph ng;
-    ng.B = B, ng.graph = graph, ng.with_step = step != nullptr;
-    size_t n = 0;
-    ROHM_CUDA(ctx, cudaGraphGetNodes(graph, nullptr, &n));
-    std::vector<cudaGraphNode_t> nodes(n);
-    ROHM_CUDA(ctx, cudaGraphGetNodes(graph, nodes.data(), &n));
-    for (cudaGraphNode_t node : nodes) {
-      cudaGraphNodeType ty;
-      ROHM_CUDA(ctx, cudaGraphNodeGetType(node, &ty));
-      if (ty != cudaGraphNodeTypeKernel) continue;
-      cudaKernelNodeParams kp{};
-      ROHM_CUDA(ctx, cudaGraphKernelNodeGetParams(node, &kp));
-      if (kp.func == reinterpret_cast<void*>(pack_rows_kernel)) ng.n_pack = node, ng.p_pack = kp;
-      else if (kp.func == reinterpret_cast<void*>(trajnet_time_kernel)) ng.n_time = node, ng.p_time = kp;
-      else if (kp.func == reinterpret_cast<void*>(unpack_rows_kernel)) ng.n_unpack = node, ng.p_unpack = kp;
-      else if (kp.func == const_cast<void*>(ddpm_step_philox_kernel_address())) ng.n_step = node, ng.p_step = kp;
-    }
-    if (!ng.n_pack || !ng.n_time || !ng.n_unpack || (step != nullptr && !ng.n_step)) {
-      cudaGraphDestroy(graph);
-      return fail(ctx, ROHM_ERR_CUDA, "trajnet graph: boundary nodes not found");
-    }
-    ROHM_CUDA(ctx, cudaGraphInstantiate(&ng.exec, graph, 0));
-    if (tn->graphs.size() >= 8) {
-      cudaGraphExecDestroy(tn->graphs.front().exec);
-      cudaGraphDestroy(tn->graphs.front().graph);
-      tn->graphs.erase(tn->graphs.begin());
-    }
-    tn->graphs.push_back(ng);
-    fg = &tn->graphs.back();
-  }
-  const void* a_x = x_t;
-  const void* a_t = time;
-  void* a_o = out;
-  {
-    cudaKernelNodeParams kp = fg->p_pack;
-    std::vector<void*> args(kp.kernelParams, kp.kernelParams + 9);
-    args[0] = &a_x;
-    kp.kernelParams = args.data();
-    ROHM_CUDA(ctx, cudaGraphExecKernelNodeSetParams(fg->exec, fg->n_pack, &kp));
-  }
-  {
-    cudaKernelNodeParams kp = fg->p_time;
-    std::vector<void*> args(kp.kernelParams, kp.kernelParams + 12);
-    args[0] = &a_t;
-    kp.kernelParams = args.data();
-    ROHM_CUDA(ctx, cudaGraphExecKernelNodeSetParams(fg->exec, fg->n_time, &kp));
-  }
-  {
-    cudaKernelNodeParams kp = fg->p_unpack;
-    std::vector<void*> args(kp.kernelParams, kp.kernelParams + 7);
-    args[1] = &a_o;
-    kp.kernelParams = args.data();
-    ROHM_CUDA(ctx, cudaGraphExecKernelNodeSetParams(fg->exec, fg->n_unpack, &kp));
-  }
-  if (step != nullptr) {  // x0, x_t, out, coef row, Philox seed / offset of this step (ddpm_step_philox_kernel's argument list)
-    cudaKernelNodeParams kp = fg->p_step;
-    std::vector<void*> args(kp.kernelParams, kp.kernelParams + 14);
-    const void* a_x0 = out;
-    void* a_next = step->x_next;
-    const void* a_coef = step->coef_row;
-    unsigned long long a_seed = step->seed, a_off = step->offset;
-    args[0] = &a_x0, args[1] = &a_x, args[5] = &a_next, args[8] = &a_coef, args[10] = &a_seed, args[11] = &a_off;
-    kp.kernelParams = args.data();
-    ROHM_CUDA(ctx, cudaGraphExecKernelNodeSetParams(fg->exec, fg->n_step, &kp));
-  }
-  ROHM_CUDA(ctx, cudaGraphLaunch(fg->exec, st));
-  return ROHM_OK;
+  std::vector<KernelPatch> patches = {{pack_rows_kernel, arg<kPackRowsX>(x_t)},
+                                      {trajnet_time_kernel, arg<kTrajnetTimeT>(time)},
+                                      {unpack_rows_kernel, arg<kUnpackRowsOut>(out)}};
+  if (step != nullptr) patches.push_back(ddpm_step_patch(*step));
+  return tn->graphs.run(ctx, B, tn->T, step != nullptr, false, static_cast<cudaStream_t>(stream), launches, patches);
 }
 
 // TrajNet.forward (trajnet.py:177-275).  x_t: [B, T, traj_dim]; time: int64 [B]; out: [B, T, traj_dim].
@@ -1256,22 +1138,21 @@ extern "C" int rohm_trajnet_sample_step(rohm_trajnet* tn, const float* x_t, cons
   if (tn == nullptr) return ROHM_ERR_INVALID;
   if (x_next == nullptr || coef_row == nullptr)
     return fail(tn->ctx, ROHM_ERR_INVALID, "rohm_trajnet_sample_step: null pointer");
-  TrajStepArgs sa{x_next, coef_row, seed, offset, 0, 0};
-  unsigned long long inc = 0;
-  int rc = ddpm_step_philox_policy(tn->ctx, static_cast<int64_t>(tn->T) * tn->traj_dim * B, &sa.G, &sa.iters, &inc);
+  const int64_t clip_elems = static_cast<int64_t>(tn->T) * tn->traj_dim;
+  DdpmStep step{x0_out, x_t, x_next, clip_elems * B, clip_elems, coef_row, seed, offset};
+  const int rc = ddpm_step_plan(tn->ctx, &step, offset_increment);
   if (rc != ROHM_OK) return rc;
-  if (offset_increment != nullptr) *offset_increment = inc;
-  return trajnet_forward_or_step(tn, x_t, time, x0_out, B, stream, &sa);
+  return trajnet_forward_or_step(tn, x_t, time, x0_out, B, stream, &step);
 }
 
 extern "C" int rohm_trajnet_set_option(rohm_trajnet* tn, int option, int value) {
   if (tn == nullptr) return ROHM_ERR_INVALID;
   if (option == 0) {
-    tn->use_graph = value != 0;
+    tn->graphs.enabled = value != 0;
     return ROHM_OK;
   }
   if (option == 1) {  // programmatic dependent launch along the convolution / GroupNorm chains (captured graphs are rebuilt)
-    if (tn->use_pdl != (value != 0)) tn->drop_graphs();
+    if (tn->use_pdl != (value != 0)) tn->graphs.clear();
     tn->use_pdl = value != 0;
     return ROHM_OK;
   }
