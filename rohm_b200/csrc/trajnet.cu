@@ -15,7 +15,7 @@
 // step-invariant condition pyramid and control_zero_conv_0 run once per condition (set_cond).  rohm_trajnet_sample_step appends
 // the in-kernel-noise sampler update to the forward graph.
 #include <cmath>
-#include <map>
+#include <memory>
 #include <new>
 #include <string>
 
@@ -296,10 +296,24 @@ struct Act {  // one activation tensor at pyramid level `level`
   int C = 0, ld = 0, level = 0;
 };
 
+// Scratch buffer `a` viewed as a [rows, C] matrix at `level` (row pitch C)
+Act view(Act a, int C, int level) {
+  a.C = C, a.ld = C, a.level = level;
+  return a;
+}
+
+enum ConvKind : int {
+  kConv,            // Conv1d(ks, stride, pad = ks/2 for stride 1, 1 for the stride-2 k3 downsample)
+  kTransposedEven,  // even output phase of ConvTranspose1d(k4, s2, p1) (GEMM rows = input level rows)
+  kTransposedOdd,   // odd output phase
+};
+
 struct Conv {
+  std::string name;  // for error messages and ROHM_B200_TRAJ_TS
   GemmParams g{};
   PackedWeight w;
   float* bias = nullptr;
+  Act out;
   int level_out = 0;   // GEMM rows are the rows of this level (for transposed convs: the INPUT level)
   // GroupNorm'd convolutions store the GEMM result without bias in `partial`, and gn_mish_split_kernel adds bias, takes the
   // statistics and applies GroupNorm.  Split-K (deep pyramid levels): `splits` fp32 partial results of [split_rows, Cout]
@@ -307,8 +321,26 @@ struct Conv {
   int splits = 1;
   float* partial = nullptr;
   int64_t split_rows = 0;
-  bool sum_after = false;  // no GroupNorm behind it: sum_split_kernel writes `sum_out` right after the GEMM
-  Act sum_out;
+  bool sum_after = false;  // no GroupNorm behind it: sum_split_kernel writes `out` right after the GEMM
+  int ts_runs = 0;         // ROHM_B200_TRAJ_TS: launches outside stream capture so far
+};
+
+struct GroupNorm {
+  float* gamma = nullptr;
+  float* beta = nullptr;
+};
+
+// ResidualTemporalBlock: out = Mish(GN(conv2(Mish(GN(conv1(x))) + time))) + residual [+ extra]
+struct Rtb {
+  std::string name;  // state-dict prefix, e.g. "diff_enc1."
+  Conv c1, c2, res;
+  bool has_res = false;  // the block changes the width: `res` is its 1x1 residual convolution
+  GroupNorm gn[2];
+  int tp_off = -1;  // offset of its rows in the stacked time projection; -1: no time input
+  Act a1;           // Mish(GN(conv1(x))) + time: conv2's input
+  const float* residual = nullptr;  // res's output, or the block's input
+  const float* extra = nullptr;     // the TrajControl residual added by the U-Net's mid_block2 and decoder
+  Act out;
 };
 
 }  // namespace
@@ -325,19 +357,30 @@ struct rohm_trajnet {
   int kind = kKindTf32;  // operand element type of the convolution GEMMs (kKindF16 in ROHM_PRECISION_F16X2)
   int max_batch = 0, T = 0;
   int Tl[kLevels], Tp[kLevels];
-  std::map<std::string, std::pair<const float*, int64_t>> sd;  // caller's tensors, valid during create only
+  // caller's parameters by state-dict key, valid during create only
+  int n_params = 0;
+  const char* const* names = nullptr;
+  const float* const* ptrs = nullptr;
+  const int64_t* numels = nullptr;
   // time path
   float *w1 = nullptr, *b1 = nullptr, *w3 = nullptr, *b3 = nullptr, *wcat = nullptr, *bcat = nullptr, *tp = nullptr;
   float* time_table = nullptr;  // [kTimeTableRows, tp_total]: the stacked projections of every tabulated timestep
   int tp_total = 0;
-  std::map<std::string, int> tp_off;  // block prefix -> offset in the stacked time projection
-  // activations
-  std::map<std::string, Act> acts;
-  std::map<std::string, Conv> convs;
-  std::map<std::string, std::pair<float*, float*>> norms;  // GroupNorm gamma/beta by conv-block prefix
+  // the network (trajnet.py); U-Net decoder arrays are indexed by the level they write, like the encoder's
+  Act xin, cin, kin;  // packed x_t, cond, control_cond
+  Rtb cond_enc[4];    // condition pyramid
+  Conv cond_down[3];
+  Rtb enc[4], mid_block[2], dec[4];  // U-Net
+  Conv down[4], up_even[4], up_odd[4];
+  Conv final_c, final_o;
+  GroupNorm final_gn;
+  Act f1;  // final GroupNorm's output
+  struct {
+    Conv z0, zero[4], down[4], zero_mid;
+    Rtb enc[4], mid_block[2];
+  } ctl;  // TrajControl
   // RTB-internal scratch, one set per concurrently running branch (0: U-Net, 1: TrajControl)
-  float *scratchY[2] = {nullptr, nullptr}, *scratchRes[2] = {nullptr, nullptr};
-  Act scratchA[2];
+  Act scratchY[2], scratchRes[2], scratchA[2];
   // Split-K partials of the GroupNorm'd convolutions (ROHM_B200_TRAJ_SPLITK=0 turns split-K off): kMaxSplits x the largest
   // 128-row-padded [rows, C] level matrix, per branch
   float* scratchSplit[2] = {nullptr, nullptr};
@@ -349,8 +392,6 @@ struct rohm_trajnet {
   cudaStream_t side[3] = {nullptr, nullptr, nullptr};  // 0: TrajControl branch, 1 / 2: residual convolutions of branch 0 / 1
   std::vector<cudaEvent_t> events;
   size_t ev_next = 0;
-  cudaEvent_t time_ready = nullptr;     // recorded after the time kernel; each branch waits for it before its first GroupNorm
-  bool time_pending[2] = {false, false};
   int cond_B = -1;
   int launches = 0;
   ForwardGraphs graphs;  // CUDA graph of one forward per batch size
@@ -359,52 +400,49 @@ struct rohm_trajnet {
     for (cudaStream_t q : side)
       if (q) cudaStreamDestroy(q);
     for (cudaEvent_t e : events) cudaEventDestroy(e);
-    if (time_ready) cudaEventDestroy(time_ready);
   }
 };
+
+#define TRY(expr)                     \
+  do {                                \
+    const int rc__ = (expr);          \
+    if (rc__ != ROHM_OK) return rc__; \
+  } while (0)
 
 namespace {
 
 int64_t rows_of(const rohm_trajnet* tn, int level) { return static_cast<int64_t>(tn->max_batch) * tn->Tp[level]; }
 
-const float* param(rohm_trajnet* tn, const std::string& key, int64_t expect_numel, int* rc) {
-  auto it = tn->sd.find(key);
-  if (it == tn->sd.end()) {
-    *rc = fail(tn->ctx, ROHM_ERR_INVALID, "rohm_trajnet_create: missing parameter '%s'", key.c_str());
-    return nullptr;
+int param(rohm_trajnet* tn, const std::string& key, int64_t expect_numel, const float** out) {
+  for (int i = 0; i < tn->n_params; ++i) {
+    if (key != tn->names[i]) continue;
+    if (tn->numels[i] != expect_numel)
+      return fail(tn->ctx, ROHM_ERR_INVALID, "rohm_trajnet_create: parameter '%s' has %lld elements, expected %lld",
+                  key.c_str(), static_cast<long long>(tn->numels[i]), static_cast<long long>(expect_numel));
+    *out = tn->ptrs[i];
+    return ROHM_OK;
   }
-  if (expect_numel >= 0 && it->second.second != expect_numel) {
-    *rc = fail(tn->ctx, ROHM_ERR_INVALID, "rohm_trajnet_create: parameter '%s' has %lld elements, expected %lld",
-               key.c_str(), static_cast<long long>(it->second.second), static_cast<long long>(expect_numel));
-    return nullptr;
-  }
-  return it->second.first;
+  return fail(tn->ctx, ROHM_ERR_INVALID, "rohm_trajnet_create: missing parameter '%s'", key.c_str());
 }
 
-float* dev_copy(rohm_trajnet* tn, const float* src, int64_t n, int* rc) {
-  float* d = tn->pool.floats(n);
-  if (d == nullptr) {
-    *rc = fail(tn->ctx, ROHM_ERR_CUDA, "alloc failed: %s", cudaGetErrorString(tn->pool.last_error()));
-    return nullptr;
-  }
-  cudaError_t e = cudaMemcpy(d, src, static_cast<size_t>(n) * sizeof(float), cudaMemcpyDeviceToDevice);
-  if (e != cudaSuccess) {
-    *rc = fail(tn->ctx, ROHM_ERR_CUDA, "memcpy failed: %s", cudaGetErrorString(e));
-    return nullptr;
-  }
-  return d;
+// The engine's own copy of parameter `key`
+int dev_copy(rohm_trajnet* tn, const std::string& key, int64_t n, float** out) {
+  const float* src = nullptr;
+  TRY(param(tn, key, n, &src));
+  *out = tn->pool.floats(n);
+  if (*out == nullptr) return fail(tn->ctx, ROHM_ERR_CUDA, "alloc failed: %s", cudaGetErrorString(tn->pool.last_error()));
+  ROHM_CUDA(tn->ctx, cudaMemcpy(*out, src, static_cast<size_t>(n) * sizeof(float), cudaMemcpyDeviceToDevice));
+  return ROHM_OK;
 }
 
 // Allocates an activation (fp32 and/or hi/lo) at a level.
-int make_act(rohm_trajnet* tn, const std::string& name, int C, int level, bool want_f32, bool want_split) {
-  Act a;
+int make_act(rohm_trajnet* tn, Act& a, int C, int level, bool want_f32, bool want_split) {
   a.C = C, a.level = level, a.ld = static_cast<int>(round_up(C, tn->kind == kKindF16 ? 8 : 4));  // 16-byte row pitch
   const int64_t n = rows_of(tn, level) * a.ld;
   if (want_f32) a.f32 = tn->pool.floats(n);
   if (want_split) a.hi = tn->pool.floats(n), a.lo = tn->pool.floats(n);
   if ((want_f32 && !a.f32) || (want_split && (!a.hi || !a.lo)))
     return fail(tn->ctx, ROHM_ERR_CUDA, "activation alloc failed: %s", cudaGetErrorString(tn->pool.last_error()));
-  tn->acts[name] = a;
   return ROHM_OK;
 }
 
@@ -462,25 +500,23 @@ int pick_split(int N, int64_t rows, int stages, int blk_cols, int* bn_out, doubl
   return best_S;
 }
 
-// Builds one convolution as a segmented GEMM.
-//   kind 0: Conv1d(ks, stride, pad = ks/2 for stride 1, 1 for the stride-2 k3 downsample)
-//   kind 1 / 2: even / odd output phase of ConvTranspose1d(k4, s2, p1) (GEMM rows = input level rows)
-int make_conv(rohm_trajnet* tn, const std::string& name, const std::string& wkey, std::vector<const Act*> srcs, int Cout,
-              int ks, int stride, int kind, const Act* out, bool with_stats) {
-  int rc = ROHM_OK;
+// Builds one convolution as a segmented GEMM writing `out` (Cout = out.C) from the channel concat of `srcs`.
+// group_normed: gn_mish_split_kernel follows and adds the bias; branch: whose split-K partial scratch it uses.
+int make_conv(rohm_trajnet* tn, Conv& cv, const std::string& name, const std::string& wkey, std::vector<const Act*> srcs,
+              const Act& out, int ks, int stride, ConvKind kind, bool group_normed, int branch) {
+  const int Cout = out.C;
   int Cin = 0;
   for (auto* s : srcs) Cin += s->C;
-  const float* w = param(tn, wkey + ".weight", static_cast<int64_t>(Cout) * Cin * ks, &rc);
-  if (rc != ROHM_OK) return rc;
-  const float* b = param(tn, wkey + ".bias", Cout, &rc);
-  if (rc != ROHM_OK) return rc;
-  Conv cv;
+  const float* w = nullptr;
+  TRY(param(tn, wkey + ".weight", static_cast<int64_t>(Cout) * Cin * ks, &w));
+  cv.name = name;
+  cv.out = out;
   // taps: (weight tap index, row shift)
   std::vector<std::pair<int, int>> taps;
-  if (kind == 0) {
+  if (kind == kConv) {
     const int pad = (stride == 2) ? 1 : ks / 2;
     for (int j = 0; j < ks; ++j) taps.push_back({j, j - pad});
-  } else if (kind == 1) {  // out[2u] = W[1] x[u] + W[3] x[u-1]
+  } else if (kind == kTransposedEven) {  // out[2u] = W[1] x[u] + W[3] x[u-1]
     taps = {{1, 0}, {3, -1}};
   } else {  // out[2u+1] = W[0] x[u+1] + W[2] x[u]
     taps = {{0, 1}, {2, 0}};
@@ -491,16 +527,19 @@ int make_conv(rohm_trajnet* tn, const std::string& name, const std::string& wkey
   int Ktot = 0;
   for (size_t i = 0; i < taps.size(); ++i)
     for (auto* s : srcs) Ktot += static_cast<int>(round_up(s->C, kblk));
+  // GEMM rows: output level rows, except transposed convs whose rows are the input level's
+  const int in_level = srcs[0]->level;
+  const int row_level = (kind == kConv) ? out.level : in_level;
   PackedWeight& pw = cv.w;
   pw.N = Cout, pw.K = Ktot, pw.Kp = Ktot;
-  pw.block_n = pick_bn(Cout, rows_of(tn, (kind == 0) ? out->level : srcs[0]->level));
-  const bool can_split = tn->use_splitk && kind == 0 && out->ld == Cout && Cout % 4 == 0;
-  if (can_split && ((with_stats && stride == 1 && out->f32 != nullptr && out->hi == nullptr) || (!with_stats && ks > 1))) {
+  pw.block_n = pick_bn(Cout, rows_of(tn, row_level));
+  const bool can_split = tn->use_splitk && kind == kConv && out.ld == Cout && Cout % 4 == 0;
+  if (can_split && ((group_normed && stride == 1 && out.f32 != nullptr && out.hi == nullptr) || (!group_normed && ks > 1))) {
     int bn = pw.block_n;
-    cv.splits = pick_split(Cout, rows_of(tn, out->level), Ktot / kblk, kblk, &bn, with_stats ? 0.0 : 4.0);
+    cv.splits = pick_split(Cout, rows_of(tn, out.level), Ktot / kblk, kblk, &bn, group_normed ? 0.0 : 4.0);
     if (cv.splits > 1) {
       pw.block_n = bn;
-      if (!with_stats) cv.sum_after = true, cv.sum_out = *out;
+      cv.sum_after = !group_normed;
     }
   }
   pw.Np = static_cast<int>(round_up(Cout, pw.block_n));
@@ -509,13 +548,10 @@ int make_conv(rohm_trajnet* tn, const std::string& name, const std::string& wkey
   pw.lo = static_cast<float*>(tn->pool.bytes(static_cast<int64_t>(pw.Np) * Ktot * gemm_elem_bytes(tn->kind)));
   if (!pw.hi || !pw.lo) return fail(tn->ctx, ROHM_ERR_CUDA, "weight alloc failed");
   if (tn->kind == kKindF16) ROHM_CUDA(tn->ctx, f16_weight_scale(w, static_cast<int64_t>(Cout) * Cin * ks, &pw.scale));
-  cv.bias = dev_copy(tn, b, Cout, &rc);
-  if (rc != ROHM_OK) return rc;
+  TRY(dev_copy(tn, wkey + ".bias", Cout, &cv.bias));
 
   GemmParams& g = cv.g;
-  g = GemmParams{};
   int seg = 0, seg_off = 0;
-  const int in_level = srcs[0]->level;
   for (auto& tap : taps) {
     int src_off = 0;
     for (auto* s : srcs) {
@@ -523,9 +559,9 @@ int make_conv(rohm_trajnet* tn, const std::string& name, const std::string& wkey
         return fail(tn->ctx, ROHM_ERR_INVALID, "conv '%s': bad source", name.c_str());
       const int Cs = s->C;
       const int64_t n = static_cast<int64_t>(Cout) * Cs;
-      pack_conv_segment_kernel<<<static_cast<unsigned>((n + 255) / 256), 256>>>(w, pw.hi, pw.lo, Cout, Cin, ks, src_off,
-                                                                              Cs, tap.first, seg_off, Ktot, kind != 0,
-                                                                              tn->kind == kKindF16 ? 1 : 0, pw.scale);
+      pack_conv_segment_kernel<<<static_cast<unsigned>((n + 255) / 256), 256>>>(
+          w, pw.hi, pw.lo, Cout, Cin, ks, src_off, Cs, tap.first, seg_off, Ktot, kind != kConv,
+          tn->kind == kKindF16 ? 1 : 0, pw.scale);
       int e1 = make_tmap_2d(&g.a_hi[seg], s->hi, rows_of(tn, in_level), Cs, s->ld, kGemmBlockM, stride, tn->kind);
       int e2 = make_tmap_2d(&g.a_lo[seg], s->lo, rows_of(tn, in_level), Cs, s->ld, kGemmBlockM, stride, tn->kind);
       if (e1 || e2) return fail(tn->ctx, ROHM_ERR_CUDA, "tensor map failed for conv '%s' (%d, %d)", name.c_str(), e1, e2);
@@ -545,92 +581,85 @@ int make_conv(rohm_trajnet* tn, const std::string& name, const std::string& wkey
     return fail(tn->ctx, ROHM_ERR_CUDA, "tensor map failed for weights of '%s'", name.c_str());
   g.bias = cv.bias;
   g.N = Cout;
-  // GEMM rows: output level rows, except transposed convs whose rows are the input level's
-  const int row_level = (kind == 0) ? out->level : in_level;
   cv.level_out = row_level;
   g.clip_rows = tn->Tp[row_level];
   g.clip_valid = tn->Tl[row_level];
-  g.out_row_mul = (kind == 0) ? 1 : 2;
-  g.out_row_add = (kind == 2) ? 1 : 0;
-  if (out->f32) g.out = out->f32, g.ldo = out->ld;
-  if (out->hi) g.out_hi = out->hi, g.out_lo = out->lo, g.lds = out->ld;
+  g.out_row_mul = (kind == kConv) ? 1 : 2;
+  g.out_row_add = (kind == kTransposedOdd) ? 1 : 0;
+  if (out.f32) g.out = out.f32, g.ldo = out.ld;
+  if (out.hi) g.out_hi = out.hi, g.out_lo = out.lo, g.lds = out.ld;
   if (cv.splits > 1) {
     // partial results instead of the block's fp32 scratch; bias / statistics / GroupNorm happen in gn_mish_split_kernel
-    const int br = (name.rfind("controlnet.", 0) == 0 || name[0] == 'k') ? 1 : 0;  // TrajControl convolutions: "controlnet.*", "k*"
     cv.split_rows = static_cast<int64_t>(round_up(rows_of(tn, row_level), kGemmBlockM));
-    cv.partial = tn->scratchSplit[br];
+    cv.partial = tn->scratchSplit[branch];
     g.out = cv.partial, g.ldo = Cout, g.out_hi = nullptr, g.out_lo = nullptr;
     g.bias = nullptr;
     g.k_splits = cv.splits;
     g.split_row_stride = static_cast<int>(cv.split_rows);
-  } else if (with_stats) {
+  } else if (group_normed) {
     // y = conv without bias; bias + statistics + GroupNorm in gn_mish_split_kernel (one "partial").  Every GroupNorm'd output
     // is an fp32-only [rows, Cout] scratch whose width is a multiple of 4 * kGroups (rohm_trajnet_create's mid_dim rule).
-    cv.partial = out->f32;
+    cv.partial = out.f32;
     g.bias = nullptr;
   }
   // fp32-only or fp16-pair-only outputs with the identity row map leave through TMA bulk stores (the transposed-conv phases
   // and the few convolutions that write both forms keep the per-thread epilogue)
   if (gemm_enable_tma_store(&g, cv.splits > 1 ? cv.splits * cv.split_rows : rows_of(tn, row_level), tn->kind) != 0)
     return fail(tn->ctx, ROHM_ERR_CUDA, "store tensor map failed for conv '%s'", name.c_str());
-  tn->convs[name] = cv;
   return ROHM_OK;
 }
 
-int load_norm(rohm_trajnet* tn, const std::string& block_prefix, int C) {
-  int rc = ROHM_OK;
-  const float* g = param(tn, block_prefix + "block.2.weight", C, &rc);
-  if (rc != ROHM_OK) return rc;
-  const float* b = param(tn, block_prefix + "block.2.bias", C, &rc);
-  if (rc != ROHM_OK) return rc;
-  float* dg = dev_copy(tn, g, C, &rc);
-  if (rc != ROHM_OK) return rc;
-  float* db = dev_copy(tn, b, C, &rc);
-  if (rc != ROHM_OK) return rc;
-  tn->norms[block_prefix] = {dg, db};
-  return ROHM_OK;
+int load_norm(rohm_trajnet* tn, GroupNorm& gn, const std::string& block_prefix, int C) {
+  TRY(dev_copy(tn, block_prefix + "block.2.weight", C, &gn.gamma));
+  return dev_copy(tn, block_prefix + "block.2.bias", C, &gn.beta);
 }
 
-// Declares the convolutions of a ResidualTemporalBlock named `p` (e.g. "diff_enc1.") reading `srcs`, writing `out`.
-int make_rtb(rohm_trajnet* tn, const std::string& p, std::vector<const Act*> srcs, int Cout, int level) {
+// Declares the ResidualTemporalBlock `p` (its state-dict prefix, e.g. "diff_enc1.") reading `srcs` and writing `out`, with the
+// RTB-internal scratch of `branch`.  timed: the block has a time input; it takes the next rows of the stacked time projection
+// and is appended to *timed.
+int make_rtb(rohm_trajnet* tn, Rtb& r, const std::string& p, std::vector<const Act*> srcs, const Act& out, int branch,
+             std::vector<const Rtb*>* timed, const float* extra = nullptr) {
   int Cin = 0;
   for (auto* s : srcs) Cin += s->C;
-  int rc;
-  Act y;  // fp32 scratch view with this block's width
-  const int br = p.rfind("controlnet.", 0) == 0 ? 1 : 0;
-  y.f32 = tn->scratchY[br], y.C = Cout, y.ld = Cout, y.level = level;
-  Act a1 = tn->scratchA[br];
-  a1.C = Cout, a1.ld = Cout, a1.level = level;
-  tn->acts[p + "#y"] = y;
-  tn->acts[p + "#a1"] = a1;
-  if ((rc = make_conv(tn, p + "c1", p + "blocks.0.block.0", srcs, Cout, 5, 1, 0, &tn->acts[p + "#y"], true)) != ROHM_OK) return rc;
-  if ((rc = make_conv(tn, p + "c2", p + "blocks.1.block.0", {&tn->acts[p + "#a1"]}, Cout, 5, 1, 0, &tn->acts[p + "#y"], true)) != ROHM_OK) return rc;
-  if ((rc = load_norm(tn, p + "blocks.0.", Cout)) != ROHM_OK) return rc;
-  if ((rc = load_norm(tn, p + "blocks.1.", Cout)) != ROHM_OK) return rc;
-  if (Cin != Cout) {
-    Act r;
-    r.f32 = tn->scratchRes[br], r.C = Cout, r.ld = Cout, r.level = level;
-    tn->acts[p + "#res"] = r;
-    if ((rc = make_conv(tn, p + "res", p + "residual_conv", srcs, Cout, 1, 1, 0, &tn->acts[p + "#res"], false)) != ROHM_OK) return rc;
+  const int Cout = out.C, level = out.level;
+  const Act y = view(tn->scratchY[branch], Cout, level);
+  r.name = p;
+  r.a1 = view(tn->scratchA[branch], Cout, level);
+  r.extra = extra;
+  r.out = out;
+  TRY(make_conv(tn, r.c1, p + "c1", p + "blocks.0.block.0", srcs, y, 5, 1, kConv, true, branch));
+  TRY(make_conv(tn, r.c2, p + "c2", p + "blocks.1.block.0", {&r.a1}, y, 5, 1, kConv, true, branch));
+  TRY(load_norm(tn, r.gn[0], p + "blocks.0.", Cout));
+  TRY(load_norm(tn, r.gn[1], p + "blocks.1.", Cout));
+  r.has_res = Cin != Cout;
+  if (r.has_res) {
+    const Act res = view(tn->scratchRes[branch], Cout, level);
+    TRY(make_conv(tn, r.res, p + "res", p + "residual_conv", srcs, res, 1, 1, kConv, false, branch));
+    r.residual = res.f32;
+  } else {
+    if (srcs.size() != 1 || srcs[0]->f32 == nullptr)
+      return fail(tn->ctx, ROHM_ERR_INVALID, "block '%s': the identity residual needs one fp32 input", p.c_str());
+    r.residual = srcs[0]->f32;
+  }
+  if (timed != nullptr) {
+    r.tp_off = tn->tp_total;
+    tn->tp_total += Cout;
+    timed->push_back(&r);
   }
   return ROHM_OK;
 }
 
-int run_conv(rohm_trajnet* tn, const std::string& name, int B, cudaStream_t st) {
-  auto it = tn->convs.find(name);
-  if (it == tn->convs.end()) return fail(tn->ctx, ROHM_ERR_STATE, "unknown conv '%s'", name.c_str());
-  Conv& cv = it->second;
+int run_conv(rohm_trajnet* tn, Conv& cv, int B, cudaStream_t st) {
   const int rows = B * tn->Tp[cv.level_out];
   cv.g.M = rows;
   // developer instrumentation: ROHM_B200_TRAJ_TS=<conv name>[,<conv name>...] prints CTA 0's %globaltimer stamps of that convolution's third
   // launch outside stream capture (use with ROHM_B200_GRAPH=0)
   unsigned long long* d_ts = nullptr;
   if (const char* want = getenv("ROHM_B200_TRAJ_TS")) {
-    static std::map<std::string, int> ts_calls;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     cudaStreamIsCapturing(st, &cap);
-    const bool listed = ("," + std::string(want) + ",").find("," + name + ",") != std::string::npos;  // comma-separated names
-    if (listed && cap == cudaStreamCaptureStatusNone && ++ts_calls[name] == 3 &&
+    const bool listed = ("," + std::string(want) + ",").find("," + cv.name + ",") != std::string::npos;  // comma-separated names
+    if (listed && cap == cudaStreamCaptureStatusNone && ++cv.ts_runs == 3 &&
         cudaMalloc(&d_ts, 32 * sizeof(unsigned long long)) == cudaSuccess) {
       cudaMemset(d_ts, 0, 32 * sizeof(unsigned long long));
       cudaStreamSynchronize(st);
@@ -649,50 +678,35 @@ int run_conv(rohm_trajnet* tn, const std::string& name, int B, cudaStream_t st) 
     for (int sgi = 0; sgi < cv.g.num_segs; ++sgi) iters += cv.g.seg_kblocks[sgi];
     fprintf(stderr, "conv %s (rows %d, N %d, block_n %d, %d K blocks, %d splits) CTA0 timeline (ns): setup %llu | first A tma %llu | "
             "first stage landed %llu | item0 mma issued %llu | item0 acc ready %llu | item0 epilogue done %llu | all mma issued %llu | "
-            "last item drained %llu | stores done %llu | end %llu\n", name.c_str(), rows, cv.w.N, cv.w.block_n, iters, cv.splits,
+            "last item drained %llu | stores done %llu | end %llu\n", cv.name.c_str(), rows, cv.w.N, cv.w.block_n, iters, cv.splits,
             h[1] - h[0], h[2] - h[0], h[3] - h[0], h[4] - h[0], h[5] - h[0], h[6] - h[0], h[12] - h[0], h[13] - h[0], h[14] - h[0],
             h[7] - h[0]);
   }
   if (cv.sum_after) {
     const int C = cv.w.N;
     const int64_t total4 = static_cast<int64_t>(rows) * C / 4;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>((total4 + 255) / 256)), cfg.blockDim = dim3(256), cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr, cfg.numAttrs = tn->use_pdl ? 1 : 0;
-    ROHM_CUDA(tn->ctx, cudaLaunchKernelEx(&cfg, sum_split_kernel, static_cast<const float*>(cv.partial), cv.splits,
-                                          static_cast<int64_t>(cv.split_rows) * C, static_cast<const float*>(cv.bias),
-                                          cv.sum_out.f32, cv.sum_out.hi, cv.sum_out.lo, C, tn->Tp[cv.level_out],
-                                          tn->Tl[cv.level_out], total4, tn->kind == kKindF16 ? 1 : 0));
+    ROHM_CUDA(tn->ctx, launch_chain(sum_split_kernel, dim3(static_cast<unsigned>((total4 + 255) / 256)), dim3(256), 0, st,
+                                    tn->use_pdl, cv.partial, cv.splits, cv.split_rows * C, cv.bias, cv.out.f32, cv.out.hi,
+                                    cv.out.lo, C, tn->Tp[cv.level_out], tn->Tl[cv.level_out], total4,
+                                    tn->kind == kKindF16 ? 1 : 0));
     tn->launches++;
   }
   return ROHM_OK;
 }
 
-// partial(s) + bias -> statistics -> GroupNorm / Mish of a GroupNorm'd convolution, one CTA per (clip, group)
-int run_gn(rohm_trajnet* tn, const std::string& conv_name, const std::string& norm_prefix, int C, int level, int B,
-           const float* tp, const float* r1, const float* r2, const Act* out, cudaStream_t st) {
-  const Conv& cv = tn->convs[conv_name];
-  auto nb = tn->norms[norm_prefix];
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(B * kGroups)), cfg.blockDim = dim3(256), cfg.stream = st;
-  cfg.dynamicSmemBytes = static_cast<size_t>(tn->Tl[level]) * (C / kGroups) * sizeof(float);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr, cfg.numAttrs = tn->use_pdl ? 1 : 0;
-  ROHM_CUDA(tn->ctx, cudaLaunchKernelEx(&cfg, gn_mish_split_kernel, static_cast<const float*>(cv.partial), cv.splits,
-                                        static_cast<int64_t>(cv.split_rows) * C, static_cast<const float*>(cv.bias),
-                                        static_cast<const float*>(nb.first), static_cast<const float*>(nb.second), tp,
-                                        tn->tp_total, r1, r2, out->f32, out->hi, out->lo, C, tn->Tp[level], tn->Tl[level],
-                                        kGroups, tn->kind == kKindF16 ? 1 : 0));
+// partial(s) + bias -> statistics -> GroupNorm / Mish of the GroupNorm'd convolution `cv`, one CTA per (clip, group)
+int run_gn(rohm_trajnet* tn, const Conv& cv, const GroupNorm& gn, int B, const float* tp, const float* r1, const float* r2,
+           const Act& out, cudaStream_t st) {
+  const int C = cv.w.N, level = cv.level_out;
+  ROHM_CUDA(tn->ctx, launch_chain(gn_mish_split_kernel, dim3(static_cast<unsigned>(B * kGroups)), dim3(256),
+                                  static_cast<size_t>(tn->Tl[level]) * (C / kGroups) * sizeof(float), st, tn->use_pdl,
+                                  cv.partial, cv.splits, cv.split_rows * C, cv.bias, gn.gamma, gn.beta, tp, tn->tp_total, r1,
+                                  r2, out.f32, out.hi, out.lo, C, tn->Tp[level], tn->Tl[level], kGroups,
+                                  tn->kind == kKindF16 ? 1 : 0));
   tn->launches++;
   return ROHM_OK;
 }
 
-// Executes a ResidualTemporalBlock: out = Mish(GN(conv2(Mish(GN(conv1(x))) + time))) + res(x) [+ extra]
 // fork: everything recorded on `from` so far happens-before what is launched on `to` afterwards (event record + wait; during
 // stream capture this adds a graph edge)
 int order_after(rohm_trajnet* tn, cudaStream_t from, cudaStream_t to) {
@@ -708,34 +722,18 @@ int order_after(rohm_trajnet* tn, cudaStream_t from, cudaStream_t to) {
   return ROHM_OK;
 }
 
-int run_rtb(rohm_trajnet* tn, const std::string& p, const float* identity_res, const Act* out, const float* extra, int B,
-            cudaStream_t st, cudaStream_t side = nullptr, int branch = 0) {
-  int rc;
-  const Act& y = tn->acts[p + "#y"];
-  const Act& a1 = tn->acts[p + "#a1"];
-  const int C = y.C, level = y.level;
-  const bool has_res = tn->convs.count(p + "res") != 0;
-  if (side == nullptr) side = st;
-  if (has_res) {  // the 1x1 residual convolution only reads the block's input: run it next to the main chain
-    if ((rc = order_after(tn, st, side)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, p + "res", B, side)) != ROHM_OK) return rc;
+// Executes a ResidualTemporalBlock on `st`, its 1x1 residual convolution on `side`
+int run_rtb(rohm_trajnet* tn, Rtb& r, int B, cudaStream_t st, cudaStream_t side) {
+  if (r.has_res) {  // the 1x1 residual convolution only reads the block's input: run it next to the main chain
+    TRY(order_after(tn, st, side));
+    TRY(run_conv(tn, r.res, B, side));
   }
-  if ((rc = run_conv(tn, p + "c1", B, st)) != ROHM_OK) return rc;
-  const float* tp = nullptr;
-  auto t = tn->tp_off.find(p);
-  if (t != tn->tp_off.end()) tp = tn->tp + t->second;
-  if (tp != nullptr && tn->time_pending[branch]) {  // first use of the time projections on this branch
-    ROHM_CUDA(tn->ctx, cudaStreamWaitEvent(st, tn->time_ready, 0));
-    tn->time_pending[branch] = false;
-  }
-  if ((rc = run_gn(tn, p + "c1", p + "blocks.0.", C, level, B, tp, nullptr, nullptr, &a1, st)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, p + "c2", B, st)) != ROHM_OK) return rc;
-  const float* res = identity_res;
-  if (has_res) {
-    if ((rc = order_after(tn, side, st)) != ROHM_OK) return rc;
-    res = tn->acts[p + "#res"].f32;
-  }
-  return run_gn(tn, p + "c2", p + "blocks.1.", C, level, B, nullptr, res, extra, out, st);
+  TRY(run_conv(tn, r.c1, B, st));
+  const float* tp = r.tp_off >= 0 ? tn->tp + r.tp_off : nullptr;
+  TRY(run_gn(tn, r.c1, r.gn[0], B, tp, nullptr, nullptr, r.a1, st));
+  TRY(run_conv(tn, r.c2, B, st));
+  if (r.has_res) TRY(order_after(tn, side, st));
+  return run_gn(tn, r.c2, r.gn[1], B, nullptr, r.residual, r.extra, r.out, st);
 }
 
 }  // namespace
@@ -759,7 +757,8 @@ extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* cons
   if (precision != ROHM_PRECISION_TF32X3 && precision != ROHM_PRECISION_TF32 && precision != ROHM_PRECISION_F16X2)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_create: precision must be 3 (TF32x3), 2 (F16x2) or 1 (TF32)");
   ROHM_CUDA(ctx, gemm_init_attributes());
-  rohm_trajnet* tn = new (std::nothrow) rohm_trajnet();
+  std::unique_ptr<rohm_trajnet> owner(new (std::nothrow) rohm_trajnet());
+  rohm_trajnet* tn = owner.get();
   if (tn == nullptr) return fail(ctx, ROHM_ERR_INVALID, "out of host memory");
   tn->ctx = ctx;
   tn->time_dim = time_dim, tn->cond_dim = cond_dim, tn->traj_dim = traj_feat_dim, tn->mid = mid_dim;
@@ -767,211 +766,151 @@ extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* cons
   tn->kind = precision == ROHM_PRECISION_F16X2 ? kKindF16 : kKindTf32;
   tn->max_batch = max_batch, tn->T = frames;
   for (int l = 0; l < kLevels; ++l) tn->Tl[l] = frames >> l, tn->Tp[l] = (frames + 32) >> l;
-  for (int i = 0; i < n_params; ++i) tn->sd[names[i]] = {ptrs[i], numels[i]};
+  tn->n_params = n_params, tn->names = names, tn->ptrs = ptrs, tn->numels = numels;
   const int m = mid_dim, td = time_dim;
-  int rc = ROHM_OK;
-
-#define TRY(expr)          \
-  do {                     \
-    rc = (expr);           \
-    if (rc != ROHM_OK) {   \
-      delete tn;           \
-      return rc;           \
-    }                      \
-  } while (0)
 
   // ---- scratch ----
-  int64_t max_elems = 0;
-  {
-    const int widths[kLevels] = {m / 8, m / 4, m / 2, m, 2 * m};
-    for (int l = 0; l < kLevels; ++l) max_elems = std::max<int64_t>(max_elems, rows_of(tn, l) * widths[l]);
+  int64_t max_elems = 0, max_padded = 0;  // the largest [rows, C] level matrix, unpadded and with 128-row-padded rows
+  const int widths[kLevels] = {m / 8, m / 4, m / 2, m, 2 * m};
+  for (int l = 0; l < kLevels; ++l) {
+    max_elems = std::max<int64_t>(max_elems, rows_of(tn, l) * widths[l]);
+    max_padded = std::max<int64_t>(max_padded, static_cast<int64_t>(round_up(rows_of(tn, l), kGemmBlockM)) * widths[l]);
   }
   for (int br = 0; br < 2; ++br) {
-    tn->scratchY[br] = tn->pool.floats(max_elems);
-    tn->scratchRes[br] = tn->pool.floats(max_elems);
+    tn->scratchY[br].f32 = tn->pool.floats(max_elems);
+    tn->scratchRes[br].f32 = tn->pool.floats(max_elems);
     tn->scratchA[br].hi = tn->pool.floats(max_elems);
     tn->scratchA[br].lo = tn->pool.floats(max_elems);
+    if (!tn->scratchY[br].f32 || !tn->scratchRes[br].f32 || !tn->scratchA[br].hi || !tn->scratchA[br].lo)
+      return fail(ctx, ROHM_ERR_CUDA, "scratch alloc failed");
   }
   if (const char* env = getenv("ROHM_B200_TRAJ_PARALLEL")) tn->parallel = env[0] != '0';
   if (const char* env = getenv("ROHM_B200_TRAJ_SPLITK")) tn->use_splitk = env[0] != '0';
   if (tn->use_splitk) {
-    int64_t max_padded = 0;
-    const int widths[kLevels] = {m / 8, m / 4, m / 2, m, 2 * m};
-    for (int l = 0; l < kLevels; ++l)
-      max_padded = std::max<int64_t>(max_padded, static_cast<int64_t>(round_up(rows_of(tn, l), kGemmBlockM)) * widths[l]);
     for (int br = 0; br < 2; ++br) {
       tn->scratchSplit[br] = tn->pool.floats(kMaxSplits * max_padded);
-      if (!tn->scratchSplit[br]) {
-        delete tn;
-        return fail(ctx, ROHM_ERR_CUDA, "split-K scratch alloc failed");
-      }
+      if (!tn->scratchSplit[br]) return fail(ctx, ROHM_ERR_CUDA, "split-K scratch alloc failed");
     }
-  }
-  if (!tn->scratchY[1] || !tn->scratchRes[1] || !tn->scratchA[1].hi || !tn->scratchA[1].lo || !tn->scratchY[0] ||
-      !tn->scratchRes[0] || !tn->scratchA[0].hi || !tn->scratchA[0].lo) {
-    delete tn;
-    return fail(ctx, ROHM_ERR_CUDA, "scratch alloc failed");
   }
 
   // ---- activations ----
-  TRY(make_act(tn, "xin", traj_feat_dim, 0, false, true));
-  TRY(make_act(tn, "cin", cond_dim, 0, false, true));
+  // c: condition pyramid (skip into the U-Net / control), cd: its downsamplings, d: U-Net encoder outputs (skips),
+  // e: downsampled concats, mb: mid blocks, up: upsamplings, u: decoder outputs; k, z, ke, kmb: the TrajControl counterparts
+  Act c[4], cd[3], d[4], e[4], mb[2], up[4], u[4], outp, k0, k[4], z[4], ke[4], kmb[2], zm;
+  TRY(make_act(tn, tn->xin, traj_feat_dim, 0, false, true));
+  TRY(make_act(tn, tn->cin, cond_dim, 0, false, true));
   const int enc_w[4] = {m / 8, m / 4, m / 2, m};
   for (int l = 0; l < 4; ++l) {
-    const std::string L = std::to_string(l + 1);
-    TRY(make_act(tn, "c" + L, enc_w[l], l, false, true));           // cond pyramid level (skip into the U-Net / control)
-    if (l < 3) TRY(make_act(tn, "cd" + L, enc_w[l], l + 1, true, true));  // cond downsample (identity residual never needed, f32 for safety)
-    TRY(make_act(tn, "d" + L, enc_w[l], l, false, true));           // U-Net encoder output (skip connection)
-    TRY(make_act(tn, "e" + L, 2 * enc_w[l], l + 1, true, true));    // downsampled concat (identity residual of next RTB)
+    TRY(make_act(tn, c[l], enc_w[l], l, false, true));
+    if (l < 3) TRY(make_act(tn, cd[l], enc_w[l], l + 1, true, true));  // identity residual never needed, f32 for safety
+    TRY(make_act(tn, d[l], enc_w[l], l, false, true));
+    TRY(make_act(tn, e[l], 2 * enc_w[l], l + 1, true, true));  // f32: identity residual of the next RTB
   }
-  TRY(make_act(tn, "m1", m, 4, true, true));
-  TRY(make_act(tn, "m2", m, 4, false, true));
+  TRY(make_act(tn, mb[0], m, 4, true, true));
+  TRY(make_act(tn, mb[1], m, 4, false, true));
   const int dec_w[4] = {32, m / 8, m / 4, m / 2};  // dec1..dec4 output widths
   for (int l = 3; l >= 0; --l) {
-    const std::string L = std::to_string(l + 1);
-    TRY(make_act(tn, "up" + L, (l == 3 ? m : dec_w[l + 1]), l, false, true));
-    TRY(make_act(tn, "u" + L, dec_w[l], l, false, true));
+    TRY(make_act(tn, up[l], (l == 3 ? m : dec_w[l + 1]), l, false, true));
+    TRY(make_act(tn, u[l], dec_w[l], l, false, true));
   }
-  TRY(make_act(tn, "f1", 32, 0, false, true));
-  TRY(make_act(tn, "outp", traj_feat_dim, 0, true, false));
+  TRY(make_act(tn, tn->f1, 32, 0, false, true));
+  TRY(make_act(tn, outp, traj_feat_dim, 0, true, false));
   if (tn->control) {
-    TRY(make_act(tn, "kin", control_cond_dim, 0, false, true));
-    TRY(make_act(tn, "k0", traj_feat_dim, 0, false, true));
+    TRY(make_act(tn, tn->kin, control_cond_dim, 0, false, true));
+    TRY(make_act(tn, k0, traj_feat_dim, 0, false, true));
     const int zw[4] = {32, m / 8, m / 4, m / 2};
     for (int l = 0; l < 4; ++l) {
-      const std::string L = std::to_string(l + 1);
-      TRY(make_act(tn, "k" + L, enc_w[l], l, false, true));
-      TRY(make_act(tn, "z" + L, zw[l], l, true, false));
-      TRY(make_act(tn, "ke" + L, 2 * enc_w[l], l + 1, true, true));
+      TRY(make_act(tn, k[l], enc_w[l], l, false, true));
+      TRY(make_act(tn, z[l], zw[l], l, true, false));
+      TRY(make_act(tn, ke[l], 2 * enc_w[l], l + 1, true, true));
     }
-    TRY(make_act(tn, "km1", m, 4, true, true));
-    TRY(make_act(tn, "km2", m, 4, false, true));
-    TRY(make_act(tn, "zm", m, 4, true, false));
-  }
-  auto A = [&](const std::string& n) { return &tn->acts[n]; };
-
-  // ---- time path: stacked Linear(time_dim -> out) of every block with input_t ----
-  {
-    std::vector<std::pair<std::string, int>> blocks = {
-        {"diff_enc1.", m / 8}, {"diff_enc2.", m / 4}, {"diff_enc3.", m / 2}, {"diff_enc4.", m},
-        {"diff_mid_block1.", m}, {"diff_mid_block2.", m}, {"diff_dec4.", m / 2}, {"diff_dec3.", m / 4},
-        {"diff_dec2.", m / 8}, {"diff_dec1.", 32}};
-    if (tn->control) {
-      blocks.insert(blocks.end(), {{"controlnet.control_enc1.", m / 8}, {"controlnet.control_enc2.", m / 4},
-                                   {"controlnet.control_enc3.", m / 2}, {"controlnet.control_enc4.", m},
-                                   {"controlnet.control_mid_block1.", m}, {"controlnet.control_mid_block2.", m}});
-    }
-    int total = 0;
-    for (auto& b : blocks) tn->tp_off[b.first] = total, total += b.second;
-    tn->tp_total = total;
-    tn->wcat = tn->pool.floats(static_cast<int64_t>(total) * td);
-    tn->bcat = tn->pool.floats(total);
-    tn->tp = tn->pool.floats(static_cast<int64_t>(max_batch) * total);
-    if (!tn->wcat || !tn->bcat || !tn->tp) {
-      delete tn;
-      return fail(ctx, ROHM_ERR_CUDA, "time projection alloc failed");
-    }
-    for (auto& b : blocks) {
-      const float* w = param(tn, b.first + "time_mlp.1.weight", static_cast<int64_t>(b.second) * td, &rc);
-      if (rc != ROHM_OK) { delete tn; return rc; }
-      const float* bb = param(tn, b.first + "time_mlp.1.bias", b.second, &rc);
-      if (rc != ROHM_OK) { delete tn; return rc; }
-      const int off = tn->tp_off[b.first];
-      cudaMemcpy(tn->wcat + static_cast<int64_t>(off) * td, w, sizeof(float) * b.second * td, cudaMemcpyDeviceToDevice);
-      cudaMemcpy(tn->bcat + off, bb, sizeof(float) * b.second, cudaMemcpyDeviceToDevice);
-    }
-    const float* p1 = param(tn, "time_mlp.1.weight", static_cast<int64_t>(4) * td * td, &rc);
-    if (rc != ROHM_OK) { delete tn; return rc; }
-    tn->w1 = dev_copy(tn, p1, static_cast<int64_t>(4) * td * td, &rc);
-    const float* p2 = param(tn, "time_mlp.1.bias", 4 * td, &rc);
-    if (rc != ROHM_OK) { delete tn; return rc; }
-    tn->b1 = dev_copy(tn, p2, 4 * td, &rc);
-    const float* p3 = param(tn, "time_mlp.3.weight", static_cast<int64_t>(4) * td * td, &rc);
-    if (rc != ROHM_OK) { delete tn; return rc; }
-    tn->w3 = dev_copy(tn, p3, static_cast<int64_t>(4) * td * td, &rc);
-    const float* p4 = param(tn, "time_mlp.3.bias", td, &rc);
-    if (rc != ROHM_OK) { delete tn; return rc; }
-    tn->b3 = dev_copy(tn, p4, td, &rc);
-    if (rc != ROHM_OK) { delete tn; return rc; }
-    // tabulate the whole time path for t = 0 .. kTimeTableRows-1 with the direct-evaluation branch of the kernel
-    tn->time_table = tn->pool.floats(static_cast<int64_t>(kTimeTableRows) * total);
-    std::vector<int64_t> ts(kTimeTableRows);
-    for (int i = 0; i < kTimeTableRows; ++i) ts[i] = i;
-    int64_t* d_ts = static_cast<int64_t*>(tn->pool.bytes(sizeof(int64_t) * kTimeTableRows));
-    if (!tn->time_table || !d_ts) { delete tn; return fail(ctx, ROHM_ERR_CUDA, "time table alloc failed"); }
-    cudaMemcpy(d_ts, ts.data(), sizeof(int64_t) * kTimeTableRows, cudaMemcpyHostToDevice);
-    trajnet_time_kernel<<<dim3(kTimeTableRows, 8), 256, sizeof(float) * 6 * td>>>(d_ts, td, tn->w1, tn->b1, tn->w3, tn->b3, tn->wcat,
-                                                                                tn->bcat, total, tn->time_table, nullptr, 0);
-    if (cudaDeviceSynchronize() != cudaSuccess) { delete tn; return fail(ctx, ROHM_ERR_CUDA, "time table build failed"); }
+    TRY(make_act(tn, kmb[0], m, 4, true, true));
+    TRY(make_act(tn, kmb[1], m, 4, false, true));
+    TRY(make_act(tn, zm, m, 4, true, false));
   }
 
   // ---- convolutions ----
+  std::vector<const Rtb*> timed;  // blocks with a time input, in the order of the stacked time projection
   // condition pyramid (trajnet.py:192-208): RTBs without time input
-  TRY(make_rtb(tn, "cond_enc1.", {A("cin")}, m / 8, 0));
-  TRY(make_conv(tn, "cond_down1", "cond_downsample1.conv", {A("c1")}, m / 8, 3, 2, 0, A("cd1"), false));
-  TRY(make_rtb(tn, "cond_enc2.", {A("cd1")}, m / 4, 1));
-  TRY(make_conv(tn, "cond_down2", "cond_downsample2.conv", {A("c2")}, m / 4, 3, 2, 0, A("cd2"), false));
-  TRY(make_rtb(tn, "cond_enc3.", {A("cd2")}, m / 2, 2));
-  TRY(make_conv(tn, "cond_down3", "cond_downsample3.conv", {A("c3")}, m / 2, 3, 2, 0, A("cd3"), false));
-  TRY(make_rtb(tn, "cond_enc4.", {A("cd3")}, m, 3));
+  for (int l = 0; l < 4; ++l) {
+    const std::string L = std::to_string(l + 1);
+    TRY(make_rtb(tn, tn->cond_enc[l], "cond_enc" + L + ".", {l == 0 ? &tn->cin : &cd[l - 1]}, c[l], 0, nullptr));
+    if (l < 3)
+      TRY(make_conv(tn, tn->cond_down[l], "cond_down" + L, "cond_downsample" + L + ".conv", {&c[l]}, cd[l], 3, 2, kConv,
+                    false, 0));
+  }
   // U-Net (trajnet.py:216-275)
-  TRY(make_rtb(tn, "diff_enc1.", {A("xin")}, m / 8, 0));
-  TRY(make_conv(tn, "diff_down1", "diff_downsample1.conv", {A("d1"), A("c1")}, m / 4, 3, 2, 0, A("e1"), false));
-  TRY(make_rtb(tn, "diff_enc2.", {A("e1")}, m / 4, 1));
-  TRY(make_conv(tn, "diff_down2", "diff_downsample2.conv", {A("d2"), A("c2")}, m / 2, 3, 2, 0, A("e2"), false));
-  TRY(make_rtb(tn, "diff_enc3.", {A("e2")}, m / 2, 2));
-  TRY(make_conv(tn, "diff_down3", "diff_downsample3.conv", {A("d3"), A("c3")}, m, 3, 2, 0, A("e3"), false));
-  TRY(make_rtb(tn, "diff_enc4.", {A("e3")}, m, 3));
-  TRY(make_conv(tn, "diff_down4", "diff_downsample4.conv", {A("d4"), A("c4")}, 2 * m, 3, 2, 0, A("e4"), false));
-  TRY(make_rtb(tn, "diff_mid_block1.", {A("e4")}, m, 4));
-  TRY(make_rtb(tn, "diff_mid_block2.", {A("m1")}, m, 4));
-  TRY(make_conv(tn, "up4e", "diff_upsample4.conv", {A("m2")}, m, 4, 1, 1, A("up4"), false));
-  TRY(make_conv(tn, "up4o", "diff_upsample4.conv", {A("m2")}, m, 4, 1, 2, A("up4"), false));
-  TRY(make_rtb(tn, "diff_dec4.", {A("up4"), A("d4")}, m / 2, 3));
-  TRY(make_conv(tn, "up3e", "diff_upsample3.conv", {A("u4")}, m / 2, 4, 1, 1, A("up3"), false));
-  TRY(make_conv(tn, "up3o", "diff_upsample3.conv", {A("u4")}, m / 2, 4, 1, 2, A("up3"), false));
-  TRY(make_rtb(tn, "diff_dec3.", {A("up3"), A("d3")}, m / 4, 2));
-  TRY(make_conv(tn, "up2e", "diff_upsample2.conv", {A("u3")}, m / 4, 4, 1, 1, A("up2"), false));
-  TRY(make_conv(tn, "up2o", "diff_upsample2.conv", {A("u3")}, m / 4, 4, 1, 2, A("up2"), false));
-  TRY(make_rtb(tn, "diff_dec2.", {A("up2"), A("d2")}, m / 8, 1));
-  TRY(make_conv(tn, "up1e", "diff_upsample1.conv", {A("u2")}, m / 8, 4, 1, 1, A("up1"), false));
-  TRY(make_conv(tn, "up1o", "diff_upsample1.conv", {A("u2")}, m / 8, 4, 1, 2, A("up1"), false));
-  TRY(make_rtb(tn, "diff_dec1.", {A("up1"), A("d1")}, 32, 0));
-  {
-    Act y;
-    y.f32 = tn->scratchY[0], y.C = 32, y.ld = 32, y.level = 0;
-    tn->acts["final#y"] = y;
-    TRY(make_conv(tn, "final_c", "diff_final_conv.0.block.0", {A("u1")}, 32, 5, 1, 0, A("final#y"), true));
-    TRY(load_norm(tn, "diff_final_conv.0.", 32));
-    TRY(make_conv(tn, "final_o", "diff_final_conv.1", {A("f1")}, traj_feat_dim, 1, 1, 0, A("outp"), false));
+  for (int l = 0; l < 4; ++l) {
+    const std::string L = std::to_string(l + 1);
+    TRY(make_rtb(tn, tn->enc[l], "diff_enc" + L + ".", {l == 0 ? &tn->xin : &e[l - 1]}, d[l], 0, &timed));
+    TRY(make_conv(tn, tn->down[l], "diff_down" + L, "diff_downsample" + L + ".conv", {&d[l], &c[l]}, e[l], 3, 2, kConv,
+                  false, 0));
   }
+  TRY(make_rtb(tn, tn->mid_block[0], "diff_mid_block1.", {&e[3]}, mb[0], 0, &timed));
+  TRY(make_rtb(tn, tn->mid_block[1], "diff_mid_block2.", {&mb[0]}, mb[1], 0, &timed, zm.f32));
+  for (int l = 3; l >= 0; --l) {
+    const std::string L = std::to_string(l + 1);
+    const Act* x = l == 3 ? &mb[1] : &u[l + 1];
+    TRY(make_conv(tn, tn->up_even[l], "up" + L + "e", "diff_upsample" + L + ".conv", {x}, up[l], 4, 1,
+                  kTransposedEven, false, 0));
+    TRY(make_conv(tn, tn->up_odd[l], "up" + L + "o", "diff_upsample" + L + ".conv", {x}, up[l], 4, 1,
+                  kTransposedOdd, false, 0));
+    TRY(make_rtb(tn, tn->dec[l], "diff_dec" + L + ".", {&up[l], &d[l]}, u[l], 0, &timed, z[l].f32));
+  }
+  TRY(make_conv(tn, tn->final_c, "final_c", "diff_final_conv.0.block.0", {&u[0]}, view(tn->scratchY[0], 32, 0), 5, 1, kConv,
+                true, 0));
+  TRY(load_norm(tn, tn->final_gn, "diff_final_conv.0.", 32));
+  TRY(make_conv(tn, tn->final_o, "final_o", "diff_final_conv.1", {&tn->f1}, outp, 1, 1, kConv, false, 0));
   if (tn->control) {  // trajnet.py:43-75
-    const std::string c = "controlnet.";
-    TRY(make_conv(tn, "kz0", c + "control_zero_conv_0", {A("kin")}, traj_feat_dim, 1, 1, 0, A("k0"), false));
-    TRY(make_rtb(tn, c + "control_enc1.", {A("k0")}, m / 8, 0));
-    TRY(make_conv(tn, "kz1", c + "control_zero_conv_1", {A("k1")}, 32, 1, 1, 0, A("z1"), false));
-    TRY(make_conv(tn, "kd1", c + "control_downsample1.conv", {A("k1"), A("c1")}, m / 4, 3, 2, 0, A("ke1"), false));
-    TRY(make_rtb(tn, c + "control_enc2.", {A("ke1")}, m / 4, 1));
-    TRY(make_conv(tn, "kz2", c + "control_zero_conv_2", {A("k2")}, m / 8, 1, 1, 0, A("z2"), false));
-    TRY(make_conv(tn, "kd2", c + "control_downsample2.conv", {A("k2"), A("c2")}, m / 2, 3, 2, 0, A("ke2"), false));
-    TRY(make_rtb(tn, c + "control_enc3.", {A("ke2")}, m / 2, 2));
-    TRY(make_conv(tn, "kz3", c + "control_zero_conv_3", {A("k3")}, m / 4, 1, 1, 0, A("z3"), false));
-    TRY(make_conv(tn, "kd3", c + "control_downsample3.conv", {A("k3"), A("c3")}, m, 3, 2, 0, A("ke3"), false));
-    TRY(make_rtb(tn, c + "control_enc4.", {A("ke3")}, m, 3));
-    TRY(make_conv(tn, "kz4", c + "control_zero_conv_4", {A("k4")}, m / 2, 1, 1, 0, A("z4"), false));
-    TRY(make_conv(tn, "kd4", c + "control_downsample4.conv", {A("k4"), A("c4")}, 2 * m, 3, 2, 0, A("ke4"), false));
-    TRY(make_rtb(tn, c + "control_mid_block1.", {A("ke4")}, m, 4));
-    TRY(make_rtb(tn, c + "control_mid_block2.", {A("km1")}, m, 4));
-    TRY(make_conv(tn, "kzm", c + "control_zero_conv_mid", {A("km2")}, m, 1, 1, 0, A("zm"), false));
+    const std::string cn = "controlnet.";
+    auto& ctl = tn->ctl;
+    TRY(make_conv(tn, ctl.z0, "kz0", cn + "control_zero_conv_0", {&tn->kin}, k0, 1, 1, kConv, false, 1));
+    for (int l = 0; l < 4; ++l) {
+      const std::string L = std::to_string(l + 1);
+      TRY(make_rtb(tn, ctl.enc[l], cn + "control_enc" + L + ".", {l == 0 ? &k0 : &ke[l - 1]}, k[l], 1, &timed));
+      TRY(make_conv(tn, ctl.zero[l], "kz" + L, cn + "control_zero_conv_" + L, {&k[l]}, z[l], 1, 1, kConv, false, 1));
+      TRY(make_conv(tn, ctl.down[l], "kd" + L, cn + "control_downsample" + L + ".conv", {&k[l], &c[l]}, ke[l], 3, 2, kConv,
+                    false, 1));
+    }
+    TRY(make_rtb(tn, ctl.mid_block[0], cn + "control_mid_block1.", {&ke[3]}, kmb[0], 1, &timed));
+    TRY(make_rtb(tn, ctl.mid_block[1], cn + "control_mid_block2.", {&kmb[0]}, kmb[1], 1, &timed));
+    TRY(make_conv(tn, ctl.zero_mid, "kzm", cn + "control_zero_conv_mid", {&kmb[1]}, zm, 1, 1, kConv, false, 1));
   }
-#undef TRY
-  cudaError_t e = cudaDeviceSynchronize();
-  tn->sd.clear();
-  if (e != cudaSuccess) {
-    delete tn;
-    return fail(ctx, ROHM_ERR_CUDA, "weight packing failed: %s", cudaGetErrorString(e));
+
+  // ---- time path: stacked Linear(time_dim -> out) of every block with input_t ----
+  const int total = tn->tp_total;
+  tn->wcat = tn->pool.floats(static_cast<int64_t>(total) * td);
+  tn->bcat = tn->pool.floats(total);
+  tn->tp = tn->pool.floats(static_cast<int64_t>(max_batch) * total);
+  if (!tn->wcat || !tn->bcat || !tn->tp) return fail(ctx, ROHM_ERR_CUDA, "time projection alloc failed");
+  for (const Rtb* r : timed) {
+    const float *w = nullptr, *b = nullptr;
+    TRY(param(tn, r->name + "time_mlp.1.weight", static_cast<int64_t>(r->out.C) * td, &w));
+    TRY(param(tn, r->name + "time_mlp.1.bias", r->out.C, &b));
+    ROHM_CUDA(ctx, cudaMemcpy(tn->wcat + static_cast<int64_t>(r->tp_off) * td, w, sizeof(float) * r->out.C * td,
+                              cudaMemcpyDeviceToDevice));
+    ROHM_CUDA(ctx, cudaMemcpy(tn->bcat + r->tp_off, b, sizeof(float) * r->out.C, cudaMemcpyDeviceToDevice));
   }
-  *out = tn;
+  TRY(dev_copy(tn, "time_mlp.1.weight", static_cast<int64_t>(4) * td * td, &tn->w1));
+  TRY(dev_copy(tn, "time_mlp.1.bias", 4 * td, &tn->b1));
+  TRY(dev_copy(tn, "time_mlp.3.weight", static_cast<int64_t>(4) * td * td, &tn->w3));
+  TRY(dev_copy(tn, "time_mlp.3.bias", td, &tn->b3));
+  // tabulate the whole time path for t = 0 .. kTimeTableRows-1 with the direct-evaluation branch of the kernel
+  tn->time_table = tn->pool.floats(static_cast<int64_t>(kTimeTableRows) * total);
+  std::vector<int64_t> ts(kTimeTableRows);
+  for (int i = 0; i < kTimeTableRows; ++i) ts[i] = i;
+  int64_t* d_ts = static_cast<int64_t*>(tn->pool.bytes(sizeof(int64_t) * kTimeTableRows));
+  if (!tn->time_table || !d_ts) return fail(ctx, ROHM_ERR_CUDA, "time table alloc failed");
+  ROHM_CUDA(ctx, cudaMemcpy(d_ts, ts.data(), sizeof(int64_t) * kTimeTableRows, cudaMemcpyHostToDevice));
+  trajnet_time_kernel<<<dim3(kTimeTableRows, 8), 256, sizeof(float) * 6 * td>>>(d_ts, td, tn->w1, tn->b1, tn->w3, tn->b3, tn->wcat,
+                                                                              tn->bcat, total, tn->time_table, nullptr, 0);
+  ROHM_CUDA(ctx, cudaGetLastError());
+
+  cudaError_t err = cudaDeviceSynchronize();
+  tn->n_params = 0;
+  if (err != cudaSuccess)
+    return fail(ctx, ROHM_ERR_CUDA, "weight packing / time table build failed: %s", cudaGetErrorString(err));
+  *out = owner.release();
   return ROHM_OK;
 }
 
@@ -997,19 +936,15 @@ extern "C" int rohm_trajnet_set_cond(rohm_trajnet* tn, const float* cond, const 
   if (cond == nullptr || B <= 0 || B > tn->max_batch || (tn->control && control_cond == nullptr))
     return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_set_cond: bad arguments (B=%d, capacity %d)", B, tn->max_batch);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc;
   const int saved = tn->launches;
-  if ((rc = trajnet_pack(tn, cond, tn->acts["cin"], B, st)) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "cond_enc1.", nullptr, &tn->acts["c1"], nullptr, B, st)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, "cond_down1", B, st)) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "cond_enc2.", nullptr, &tn->acts["c2"], nullptr, B, st)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, "cond_down2", B, st)) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "cond_enc3.", nullptr, &tn->acts["c3"], nullptr, B, st)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, "cond_down3", B, st)) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "cond_enc4.", nullptr, &tn->acts["c4"], nullptr, B, st)) != ROHM_OK) return rc;
+  TRY(trajnet_pack(tn, cond, tn->cin, B, st));
+  for (int l = 0; l < 4; ++l) {
+    TRY(run_rtb(tn, tn->cond_enc[l], B, st, st));
+    if (l < 3) TRY(run_conv(tn, tn->cond_down[l], B, st));
+  }
   if (tn->control) {
-    if ((rc = trajnet_pack(tn, control_cond, tn->acts["kin"], B, st)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kz0", B, st)) != ROHM_OK) return rc;
+    TRY(trajnet_pack(tn, control_cond, tn->kin, B, st));
+    TRY(run_conv(tn, tn->ctl.z0, B, st));
   }
   tn->launches = saved;
   tn->cond_B = B;
@@ -1020,10 +955,8 @@ static int trajnet_forward_launches(rohm_trajnet* tn, const float* x_t, const in
                                     cudaStream_t st) {
   rohm_ctx* ctx = tn->ctx;
   rohm::DeviceGuard device_guard__(ctx);
-  int rc;
   tn->launches = 0;
-  auto A = [&](const char* n) { return &tn->acts[n]; };
-  if ((rc = trajnet_pack(tn, x_t, *A("xin"), B, st)) != ROHM_OK) return rc;
+  TRY(trajnet_pack(tn, x_t, tn->xin, B, st));
   const int td = tn->time_dim;
   trajnet_time_kernel<<<dim3(B, 8), 256, sizeof(float) * 6 * td, st>>>(time, td, tn->w1, tn->b1, tn->w3, tn->b3, tn->wcat, tn->bcat,
                                                             tn->tp_total, tn->tp, tn->time_table, kTimeTableRows);
@@ -1040,61 +973,36 @@ static int trajnet_forward_launches(rohm_trajnet* tn, const float* x_t, const in
   cudaStream_t r0 = tn->parallel ? tn->side[1] : st;
   cudaStream_t r1 = tn->parallel ? tn->side[2] : sC;
   if (tn->control) {
-    const std::string c = "controlnet.";
-    if ((rc = order_after(tn, st, sC)) != ROHM_OK) return rc;  // fork after pack + time
-    if ((rc = run_rtb(tn, c + "control_enc1.", nullptr, A("k1"), nullptr, B, sC, r1, 1)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kz1", B, sC)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kd1", B, sC)) != ROHM_OK) return rc;
-    if ((rc = run_rtb(tn, c + "control_enc2.", A("ke1")->f32, A("k2"), nullptr, B, sC, r1, 1)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kz2", B, sC)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kd2", B, sC)) != ROHM_OK) return rc;
-    if ((rc = run_rtb(tn, c + "control_enc3.", A("ke2")->f32, A("k3"), nullptr, B, sC, r1, 1)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kz3", B, sC)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kd3", B, sC)) != ROHM_OK) return rc;
-    if ((rc = run_rtb(tn, c + "control_enc4.", A("ke3")->f32, A("k4"), nullptr, B, sC, r1, 1)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kz4", B, sC)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kd4", B, sC)) != ROHM_OK) return rc;
-    if ((rc = run_rtb(tn, c + "control_mid_block1.", nullptr, A("km1"), nullptr, B, sC, r1, 1)) != ROHM_OK) return rc;
-    if ((rc = run_rtb(tn, c + "control_mid_block2.", A("km1")->f32, A("km2"), nullptr, B, sC, r1, 1)) != ROHM_OK) return rc;
-    if ((rc = run_conv(tn, "kzm", B, sC)) != ROHM_OK) return rc;
+    auto& ctl = tn->ctl;
+    TRY(order_after(tn, st, sC));  // fork after pack + time
+    for (int l = 0; l < 4; ++l) {
+      TRY(run_rtb(tn, ctl.enc[l], B, sC, r1));
+      TRY(run_conv(tn, ctl.zero[l], B, sC));
+      TRY(run_conv(tn, ctl.down[l], B, sC));
+    }
+    for (Rtb& r : ctl.mid_block) TRY(run_rtb(tn, r, B, sC, r1));
+    TRY(run_conv(tn, ctl.zero_mid, B, sC));
   }
-  const float* z1 = tn->control ? A("z1")->f32 : nullptr;
-  const float* z2 = tn->control ? A("z2")->f32 : nullptr;
-  const float* z3 = tn->control ? A("z3")->f32 : nullptr;
-  const float* z4 = tn->control ? A("z4")->f32 : nullptr;
-  const float* zm = tn->control ? A("zm")->f32 : nullptr;
 
-  if ((rc = run_rtb(tn, "diff_enc1.", nullptr, A("d1"), nullptr, B, st, r0, 0)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, "diff_down1", B, st)) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "diff_enc2.", A("e1")->f32, A("d2"), nullptr, B, st, r0, 0)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, "diff_down2", B, st)) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "diff_enc3.", A("e2")->f32, A("d3"), nullptr, B, st, r0, 0)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, "diff_down3", B, st)) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "diff_enc4.", A("e3")->f32, A("d4"), nullptr, B, st, r0, 0)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, "diff_down4", B, st)) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "diff_mid_block1.", nullptr, A("m1"), nullptr, B, st, r0, 0)) != ROHM_OK) return rc;
-  if (tn->control && (rc = order_after(tn, sC, st)) != ROHM_OK) return rc;  // join: the decoder adds the TrajControl residuals
-  if ((rc = run_rtb(tn, "diff_mid_block2.", A("m1")->f32, A("m2"), zm, B, st, r0, 0)) != ROHM_OK) return rc;
-  // ConvTranspose1d = two independent GEMMs (even / odd output frames) with row-interleaved stores
-  auto upsample = [&](const char* even, const char* odd) -> int {
-    int r;
-    if ((r = order_after(tn, st, r0)) != ROHM_OK) return r;
-    if ((r = run_conv(tn, odd, B, r0)) != ROHM_OK) return r;
-    if ((r = run_conv(tn, even, B, st)) != ROHM_OK) return r;
-    return order_after(tn, r0, st);
-  };
-  if ((rc = upsample("up4e", "up4o")) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "diff_dec4.", nullptr, A("u4"), z4, B, st, r0, 0)) != ROHM_OK) return rc;
-  if ((rc = upsample("up3e", "up3o")) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "diff_dec3.", nullptr, A("u3"), z3, B, st, r0, 0)) != ROHM_OK) return rc;
-  if ((rc = upsample("up2e", "up2o")) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "diff_dec2.", nullptr, A("u2"), z2, B, st, r0, 0)) != ROHM_OK) return rc;
-  if ((rc = upsample("up1e", "up1o")) != ROHM_OK) return rc;
-  if ((rc = run_rtb(tn, "diff_dec1.", nullptr, A("u1"), z1, B, st, r0, 0)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, "final_c", B, st)) != ROHM_OK) return rc;
-  if ((rc = run_gn(tn, "final_c", "diff_final_conv.0.", 32, 0, B, nullptr, nullptr, nullptr, A("f1"), st)) != ROHM_OK) return rc;
-  if ((rc = run_conv(tn, "final_o", B, st)) != ROHM_OK) return rc;
-  const Act& o = *A("outp");
+  for (int l = 0; l < 4; ++l) {
+    TRY(run_rtb(tn, tn->enc[l], B, st, r0));
+    TRY(run_conv(tn, tn->down[l], B, st));
+  }
+  TRY(run_rtb(tn, tn->mid_block[0], B, st, r0));
+  if (tn->control) TRY(order_after(tn, sC, st));  // join: the decoder adds the TrajControl residuals
+  TRY(run_rtb(tn, tn->mid_block[1], B, st, r0));
+  for (int l = 3; l >= 0; --l) {
+    // ConvTranspose1d = two independent GEMMs (even / odd output frames) with row-interleaved stores
+    TRY(order_after(tn, st, r0));
+    TRY(run_conv(tn, tn->up_odd[l], B, r0));
+    TRY(run_conv(tn, tn->up_even[l], B, st));
+    TRY(order_after(tn, r0, st));
+    TRY(run_rtb(tn, tn->dec[l], B, st, r0));
+  }
+  TRY(run_conv(tn, tn->final_c, B, st));
+  TRY(run_gn(tn, tn->final_c, tn->final_gn, B, nullptr, nullptr, nullptr, tn->f1, st));
+  TRY(run_conv(tn, tn->final_o, B, st));
+  const Act& o = tn->final_o.out;
   const int64_t total = static_cast<int64_t>(B) * tn->T * o.C;
   unpack_rows_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(o.f32, out, tn->T, tn->Tp[0], o.C, o.ld, total);
   ROHM_CUDA(ctx, cudaGetLastError());

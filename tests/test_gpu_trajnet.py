@@ -8,7 +8,7 @@ import torch
 from helpers import NoiseTape, TOL, golden
 from oracle import diffusion_oracle as do
 from oracle import trajnet_oracle
-from rohm_b200 import diffusion, synthetic
+from rohm_b200 import diffusion, synthetic, trajnet_engine
 from rohm_b200.trajnet import TrajNet
 
 pytestmark = pytest.mark.gpu
@@ -215,6 +215,22 @@ def test_launch_switches_do_not_change_the_result(nets, cuda_device):
     finally:
         eng.lib.rohm_trajnet_set_option(eng.handle, 0, 1)
         eng.lib.rohm_trajnet_set_option(eng.handle, 1, 1)
+
+
+@pytest.mark.parametrize("control,forward,step", [(False, 64, 65), (True, 99, 100)])
+def test_launches_per_forward_at_config3_size(nets, cuda_device, control, forward, step):
+    """Kernel launches of one forward and of one fused sample step (forward + sampler update) at 64 clips x 144 frames, the
+    size of BASELINE configs[2]: the cheapest guard that the forward graph keeps its shape."""
+    m, _ = nets[control]
+    B, T = 64, 144
+    batch = {k: v.to(cuda_device) for k, v in synthetic.trajnet_batch(B, T, 5, control=control).items()}
+    batch['x_t'] = torch.zeros(B, T, 13, device=cuda_device)
+    m._engine = None  # an engine sized for exactly 64 clips: the split-K choices depend on its capacity
+    e, x, ts = trajnet_engine.prepare(m, batch, torch.zeros(B, dtype=torch.int64, device=cuda_device))
+    e.forward(x, ts)
+    assert e.launches_per_forward == forward
+    e.sample_step(x, ts, torch.zeros(8, device=cuda_device))
+    assert e.launches_per_forward == step
 
 
 @pytest.mark.parametrize("env", [{"ROHM_B200_TRAJ_SPLITK": "0"}, {"ROHM_B200_TRAJ_PARALLEL": "0"},
