@@ -134,7 +134,12 @@ typedef struct {
 } rohm_posenet_weights;
 
 /* Copies and repacks the weights (TF32 hi/lo split, K-padded) into library-owned device memory and allocates the
- * activation workspace for up to max_batch clips of max_frames frames. */
+ * activation workspace for up to max_batch clips of max_frames frames.
+ * Clip length (S = max_frames + 1 tokens): S <= pe_len always.  ROHM_PRECISION_F16X2 with head dim 128 (RoHM's
+ * configuration) reaches S = pe_len (4999 frames with the 5000-row table) on the streaming wgmma attention kernel.
+ * ROHM_PRECISION_TF32X3 / ROHM_PRECISION_TF32, and head dim 64, run clips above 160 tokens on the SIMT attention kernel,
+ * which keeps the clip's K and V in shared memory: at most 211 frames at head dim 128 and 255 at head dim 64.  A longer
+ * clip returns ROHM_ERR_INVALID with the rule in the message. */
 ROHM_API int rohm_posenet_create(rohm_ctx* ctx, const rohm_posenet_weights* w, int max_batch, int max_frames, int precision,
                         rohm_posenet** out);
 ROHM_API void rohm_posenet_destroy(rohm_posenet* pn);

@@ -761,6 +761,219 @@ __global__ void __launch_bounds__(128, 1) attention_wgmma_kernel(const __grid_co
   }
 }
 
+// ---- streaming wgmma attention (ROHM_PRECISION_F16X2, head dim 128, any clip length) ---------------------------------
+// One warpgroup per (clip, head, 64 queries), like attention_wgmma_kernel, but K and V stream through a two-stage TMA ring
+// in blocks of 64 keys (the 64 x 64 boxes of the Q maps) and the softmax is online: per block S_blk = Q K_blk^T (wgmma
+// m64n64k16, the same three products in the same order), an fp32 running max m and running sum l, O and l rescaled by
+// exp((m_old - m_new) scale), and P split into fp16 hi/lo registers as the A operand of O += P V_blk (V MN-major in place,
+// three products).  Shared memory does not grow with the clip.  Keys past the clip get -inf logits and their V rows are
+// zeroed before the P V product of the last block.  A stage is refilled as soon as its last reader has finished: the K
+// half after the S product, the V half after the P V product.
+struct AttnStreamParams {
+  CUtensorMap hi, lo;  // Q|K|V planes [rows, 3D] fp16, boxes of 64 columns x 64 rows (AttnWgmmaMaps::q_hi / q_lo)
+  __half* ctx_hi;
+  __half* ctx_lo;
+  int S, D, H;
+  float scale;
+};
+constexpr int kAsBlock = 64;                  // keys per block = queries per CTA
+constexpr int kAsBuf = kAsBlock * 128;        // bytes of one {plane, 64-wide head-dim chunk} tile
+constexpr int kAsTile = 4 * kAsBuf;           // Q, or one K or V block: two planes x two chunks
+constexpr int kAsStages = 2;
+constexpr int kAsSmemBytes = (1 + 2 * kAsStages) * kAsTile + 1024;
+
+__global__ void __launch_bounds__(128, 1) attention_wgmma_stream_kernel(const __grid_constant__ AttnStreamParams p) {
+  extern __shared__ uint8_t as_smem_raw[];
+  __shared__ uint64_t bar_q, bar_k[kAsStages], bar_v[kAsStages];
+  const uint32_t raw = ptx::smem_u32(as_smem_raw);
+  uint8_t* const sm = as_smem_raw + ((1024u - (raw & 1023u)) & 1023u);
+  uint8_t* const Qb = sm;                             // [plane][chunk]
+  uint8_t* const Kb = sm + kAsTile;                   // [stage][plane][chunk]
+  uint8_t* const Vb = Kb + kAsStages * kAsTile;       // [stage][plane][chunk]
+  const int S = p.S;
+  const int nblk = (S + kAsBlock - 1) / kAsBlock;     // key blocks = query tiles
+  const int qt = static_cast<int>(blockIdx.x) % nblk;
+  const int bh = static_cast<int>(blockIdx.x) / nblk;
+  const int h = bh % p.H, b = bh / p.H;
+  const int row0 = b * S, q0 = qt * kAsBlock;
+  const int kcol = p.D + h * 128, vcol = 2 * p.D + h * 128;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    ptx::prefetch_tmap(&p.hi);
+    ptx::prefetch_tmap(&p.lo);
+    ptx::mbar_init(&bar_q, 1);
+    for (int s = 0; s < kAsStages; ++s) ptx::mbar_init(&bar_k[s], 1), ptx::mbar_init(&bar_v[s], 1);
+    ptx::fence_barrier_init();
+  }
+  __syncthreads();
+  ptx::pdl_launch_dependents();
+  ptx::pdl_wait_prior_grid();
+  // one 64-row tile of a column range: hi and lo plane, two 64-wide chunks each
+  auto load_tile = [&](uint8_t* dst, uint64_t* bar, int col, int row) {
+    ptx::mbar_expect_tx(bar, kAsTile);
+    for (int pl = 0; pl < 2; ++pl)
+      for (int c = 0; c < 2; ++c) ptx::tma_load_2d(dst + (pl * 2 + c) * kAsBuf, pl ? &p.lo : &p.hi, bar, col + 64 * c, row);
+  };
+  if (threadIdx.x == 0) {
+    load_tile(Qb, &bar_q, h * 128, row0 + q0);
+    for (int j = 0; j < kAsStages && j < nblk; ++j) {
+      load_tile(Kb + j * kAsTile, &bar_k[j], kcol, row0 + j * kAsBlock);
+      load_tile(Vb + j * kAsTile, &bar_v[j], vcol, row0 + j * kAsBlock);
+    }
+  }
+
+  // this thread holds rows r and r + 8 of the tile: accumulator elements 4j, 4j+1 (row r) and 4j+2, 4j+3 (row r + 8),
+  // columns 8j + c2 + {0,1}
+  const int c2 = 2 * (lane & 3);
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.0f;
+  float m0 = -INFINITY, m1 = -INFINITY;  // running max of the raw logits (rows r, r + 8), equal across the quad
+  float l0 = 0.0f, l1 = 0.0f;            // running sum of this thread's columns, reduced over the quad at the end
+  ptx::mbar_wait(&bar_q, 0);
+#pragma unroll 1
+  for (int j = 0; j < nblk; ++j) {
+    const int st = j % kAsStages;
+    const uint32_t phase = (j / kAsStages) & 1;
+    uint8_t* const Ks = Kb + st * kAsTile;
+    uint8_t* const Vs = Vb + st * kAsTile;
+    const int kb = j * kAsBlock;
+
+    // ---- S_blk = Q K_blk^T (64 x 64), three products per k-step ----
+    float s[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = 0.0f;
+    ptx::mbar_wait(&bar_k[st], phase);
+    ptx::wgmma_fence_regs(s);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int c = k >> 2;
+      const uint64_t ko = static_cast<uint64_t>((k & 3) * 2);  // 16 fp16 = 32 bytes inside the 128-byte swizzle span
+      const uint64_t qh = ptx::make_desc_kmajor<128>(ptx::smem_u32(Qb + c * kAsBuf)) + ko;
+      const uint64_t ql = ptx::make_desc_kmajor<128>(ptx::smem_u32(Qb + (2 + c) * kAsBuf)) + ko;
+      const uint64_t kh = ptx::make_desc_kmajor<128>(ptx::smem_u32(Ks + c * kAsBuf)) + ko;
+      const uint64_t kl = ptx::make_desc_kmajor<128>(ptx::smem_u32(Ks + (2 + c) * kAsBuf)) + ko;
+      ptx::wgmma_f16(s, ql, kh);
+      ptx::wgmma_f16(s, qh, kl);
+      ptx::wgmma_f16(s, qh, kh);
+    }
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::wgmma_fence_regs(s);
+    __syncthreads();  // every warp's share of the S product has read the K stage
+    if (threadIdx.x == 0 && j + kAsStages < nblk) load_tile(Ks, &bar_k[st], kcol, row0 + kb + kAsStages * kAsBlock);
+
+    // ---- online softmax: new running max, rescale factor of the old O and l, P of the block ----
+    float n0 = m0, n1 = m1;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const bool valid = kb + 8 * jj + c2 + e < S;
+        s[4 * jj + e] = valid ? s[4 * jj + e] : -INFINITY;
+        s[4 * jj + 2 + e] = valid ? s[4 * jj + 2 + e] : -INFINITY;
+        n0 = fmaxf(n0, s[4 * jj + e]);
+        n1 = fmaxf(n1, s[4 * jj + 2 + e]);
+      }
+    }
+#pragma unroll
+    for (int off = 1; off <= 2; off <<= 1) {
+      n0 = fmaxf(n0, __shfl_xor_sync(0xffffffffu, n0, off));
+      n1 = fmaxf(n1, __shfl_xor_sync(0xffffffffu, n1, off));
+    }
+    const float a0 = expf((m0 - n0) * p.scale), a1 = expf((m1 - n1) * p.scale);  // 0 on the first block (m = -inf)
+    m0 = n0, m1 = n1;
+    float b0 = 0.0f, b1 = 0.0f;  // the block's sum first: two roundings of the running sum per block, not sixteen
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const bool valid = kb + 8 * jj + c2 + e < S;
+        const float p0 = valid ? expf((s[4 * jj + e] - m0) * p.scale) : 0.0f;
+        const float p1 = valid ? expf((s[4 * jj + 2 + e] - m1) * p.scale) : 0.0f;
+        s[4 * jj + e] = p0, s[4 * jj + 2 + e] = p1;
+        b0 += p0, b1 += p1;
+      }
+    }
+    l0 = l0 * a0 + b0, l1 = l1 * a1 + b1;
+    // P as fp16 hi/lo pairs in the A-fragment layout of k-step k (keys 16k..16k+15) = accumulator elements 8k..8k+7
+    uint32_t ph[4][4], plo[4][4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) ptx::split_f16x2(s[8 * k + 2 * i], s[8 * k + 2 * i + 1], ph[k][i], plo[k][i]);
+
+    // ---- V: key rows past the clip are zeroed (0 x NaN of a neighbouring clip would otherwise leak into O) ----
+    ptx::mbar_wait(&bar_v[st], phase);
+    if (kb + kAsBlock > S) {
+      const int n = (kb + kAsBlock - S) * 8;  // 16-byte chunks per buffer
+      for (int i = threadIdx.x; i < 4 * n; i += 128) {
+        const int buf = i / n, r = i - buf * n;
+        *reinterpret_cast<uint4*>(Vs + buf * kAsBuf + (S - kb) * 128 + r * 16) = make_uint4(0u, 0u, 0u, 0u);
+      }
+      ptx::fence_proxy_async();
+      __syncthreads();
+    }
+
+    // ---- O = O exp((m_old - m_new) scale) + P V_blk (64 x 128) ----
+    // The block's product gets an accumulator of its own and is folded into O with one rounded fma: accumulating all
+    // blocks in the wgmma accumulator would put 12 tensor-core additions per block on the running O (thousands over a
+    // long clip), where the fold puts one.
+    float ob[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) ob[i] = 0.0f;
+    ptx::wgmma_fence_regs(ob);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      // 16 keys = two 8-row atoms (SBO 1024 bytes); the two 64-wide head-dim chunks are one buffer apart (LBO)
+      const uint64_t vh = ptx::make_desc_mnmajor_sw128(ptx::smem_u32(Vs + k * 2048), kAsBuf, 1024);
+      const uint64_t vl = ptx::make_desc_mnmajor_sw128(ptx::smem_u32(Vs + 2 * kAsBuf + k * 2048), kAsBuf, 1024);
+      ptx::wgmma_f16_rs_tb(ob, plo[k], vh);
+      ptx::wgmma_f16_rs_tb(ob, ph[k], vl);
+      ptx::wgmma_f16_rs_tb(ob, ph[k], vh);
+    }
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::wgmma_fence_regs(ob);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] = fmaf(o[i], (i & 2) ? a1 : a0, ob[i]);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(ph[k][i]), "+r"(plo[k][i])::"memory");
+    __syncthreads();  // every warp's share of the P V product has read the V stage
+    if (threadIdx.x == 0 && j + kAsStages < nblk) load_tile(Vs, &bar_v[st], vcol, row0 + kb + kAsStages * kAsBlock);
+  }
+
+  // ---- normalise, split, store the context rows of this tile ----
+#pragma unroll
+  for (int off = 1; off <= 2; off <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+  }
+  const int ra = q0 + warp * 16 + (lane >> 2), rb = ra + 8;
+  const float ia = 1.0f / l0, ib = 1.0f / l1;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int col = h * 128 + 8 * j + c2;
+    uint32_t hi, lo;
+    if (ra < S) {
+      ptx::split_f16x2(o[4 * j] * ia, o[4 * j + 1] * ia, hi, lo);
+      const int64_t off = static_cast<int64_t>(row0 + ra) * p.D + col;
+      *reinterpret_cast<uint32_t*>(p.ctx_hi + off) = hi;
+      *reinterpret_cast<uint32_t*>(p.ctx_lo + off) = lo;
+    }
+    if (rb < S) {
+      ptx::split_f16x2(o[4 * j + 2] * ib, o[4 * j + 3] * ib, hi, lo);
+      const int64_t off = static_cast<int64_t>(row0 + rb) * p.D + col;
+      *reinterpret_cast<uint32_t*>(p.ctx_hi + off) = hi;
+      *reinterpret_cast<uint32_t*>(p.ctx_lo + off) = lo;
+    }
+  }
+}
+
 size_t attention_mma_smem_bytes(int NT) { return sizeof(float) * 2 * 8 * NT * kAttnPitch; }
 
 template <int DH, int NT>
@@ -823,9 +1036,13 @@ cudaError_t attention_init_attributes(int max_tokens, int dh) {
   set(attention_f16_kernel<64, 4>, attention_f16_smem_bytes<64>(4));
   set(attention_f16_kernel<64, 10>, attention_f16_smem_bytes<64>(10));
   set(attention_wgmma_kernel, kAwSmemBytes);
-  if (dh == 128) set(attention_kernel<128>, attention_smem_bytes(max_tokens, 128));
-  else if (dh == 64) set(attention_kernel<64>, attention_smem_bytes(max_tokens, 64));
-  else if (ea == cudaSuccess) ea = cudaErrorInvalidValue;
+  set(attention_wgmma_stream_kernel, kAsSmemBytes);
+  if (dh != 64 && dh != 128) return ea == cudaSuccess ? cudaErrorInvalidValue : ea;
+  // the SIMT kernel serves at most 256 tokens whose K and V fit in shared memory; longer clips never reach it
+  int simt_tokens = max_tokens < kAttnSimtMaxTokens ? max_tokens : kAttnSimtMaxTokens;
+  while (simt_tokens > 1 && attention_smem_bytes(simt_tokens, dh) > kAttnSmemLimit) --simt_tokens;
+  if (dh == 128) set(attention_kernel<128>, attention_smem_bytes(simt_tokens, 128));
+  else set(attention_kernel<64>, attention_smem_bytes(simt_tokens, 64));
   return ea;
 }
 
@@ -836,9 +1053,20 @@ cudaError_t launch_attention(const AttnArgs& a, int which, const AttnWgmmaMaps* 
   if (dh != 64 && dh != 128) return cudaErrorInvalidValue;
   const bool f16 = a.kind == kKindF16;
   const bool wg_ok = f16 && dh == 128 && a.S <= kAwKeys && wg != nullptr;
+  const bool stream_ok = f16 && dh == 128 && wg != nullptr;
   const bool mma_ok = a.S <= kAttnWgmmaMaxTokens;  // register budget of the S / P fragments
-  if (which == kAttnAuto) which = wg_ok ? kAttnWgmma : !mma_ok ? kAttnSimt : f16 ? kAttnMmaF16 : kAttnMmaTf32;
+  if (which == kAttnAuto)
+    which = wg_ok ? kAttnWgmma : (stream_ok && !mma_ok) ? kAttnWgmmaStream : !mma_ok ? kAttnSimt : f16 ? kAttnMmaF16 : kAttnMmaTf32;
   const int S = a.S;
+  if (which == kAttnWgmmaStream) {
+    if (!stream_ok) return cudaErrorInvalidValue;
+    AttnStreamParams prm;
+    prm.hi = wg->q_hi, prm.lo = wg->q_lo;
+    prm.ctx_hi = static_cast<__half*>(a.ctx_hi), prm.ctx_lo = static_cast<__half*>(a.ctx_lo);
+    prm.S = S, prm.D = a.D, prm.H = a.H, prm.scale = a.scale;
+    const int qtiles = (S + kAsBlock - 1) / kAsBlock;
+    return launch_chain(attention_wgmma_stream_kernel, dim3(a.B * a.H * qtiles), dim3(128), kAsSmemBytes, st, pdl, prm);
+  }
   if (which == kAttnWgmma) {
     if (!wg_ok) return cudaErrorInvalidValue;
     AttnWgParams prm;
@@ -872,7 +1100,7 @@ cudaError_t launch_attention(const AttnArgs& a, int which, const AttnWgmmaMaps* 
   }
   if (which == kAttnSimt) {
     const size_t smem = attention_smem_bytes(S, dh);
-    if (S > 256 || smem > 227 * 1024) return cudaErrorInvalidValue;
+    if (S > kAttnSimtMaxTokens || smem > kAttnSmemLimit) return cudaErrorInvalidValue;
     auto kern = dh == 128 ? attention_kernel<128> : attention_kernel<64>;
     return launch_chain(kern, dim3(a.B * a.H), dim3(256), smem, st, pdl, static_cast<const float*>(a.qkv_hi),
                         static_cast<const float*>(a.qkv_lo), static_cast<float*>(a.ctx_hi), static_cast<float*>(a.ctx_lo), S,

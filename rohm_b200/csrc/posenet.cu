@@ -256,8 +256,10 @@ struct rohm_posenet {
   // memory (pack: x_t, time-token gather: timesteps, unpack: out) get their pointers patched before every replay.
   ForwardGraphs graphs;
   bool use_pdl = true;
-  // wgmma attention (F16X2, head dim 128, <= 160 tokens per clip; ROHM_B200_TC_ATTENTION=0 selects the mma.sync kernel)
+  // wgmma attention (F16X2, head dim 128): the maps serve both wgmma kernels; ROHM_B200_TC_ATTENTION=0 selects the
+  // mma.sync kernel for clips of at most 160 tokens, longer clips always take the streaming wgmma kernel
   bool tc_attention = false;
+  bool attn_maps = false;
   AttnWgmmaMaps attn_wg{};
   AttnArgs attn{};  // Q|K|V planes and context pair of every layer (B and S set per forward)
   // LayerNorm folding (F16X2, d_model 512; ROHM_B200_FUSED_LN=0 keeps the separate layernorm_kernel): the residual stream
@@ -458,13 +460,15 @@ static int run_ln(rohm_posenet* pn, const float* in, const float* res, const flo
   return ROHM_OK;
 }
 
-// Attention of one layer (attention.cu): the wgmma kernel when the engine prepared its tensor maps and the clip fits,
-// else the mma.sync kernel of the operand kind, else (more than 160 tokens) the SIMT kernel.
+// Attention of one layer (attention.cu): on fp16 pairs of head dim 128 the wgmma kernel up to 160 tokens (unless
+// ROHM_B200_TC_ATTENTION=0) and the streaming wgmma kernel above; else the mma.sync kernel of the operand kind up to 160
+// tokens and the SIMT kernel above.
 static int run_attention(rohm_posenet* pn, int B, int S, cudaStream_t st) {
   AttnArgs a = pn->attn;
   a.B = B, a.S = S;
+  const bool maps = pn->attn_maps && (pn->tc_attention || S > kAttnWgmmaMaxTokens);
   prof_begin(pn, kCatAttention, st);
-  const cudaError_t e = launch_attention(a, kAttnAuto, pn->tc_attention ? &pn->attn_wg : nullptr, st, pn->use_pdl && !pn->profiling);
+  const cudaError_t e = launch_attention(a, kAttnAuto, maps ? &pn->attn_wg : nullptr, st, pn->use_pdl && !pn->profiling);
   prof_end(pn, st);
   ROHM_CUDA(pn->ctx, e);
   pn->launches++;
@@ -517,8 +521,21 @@ extern "C" int rohm_posenet_create(rohm_ctx* ctx, const rohm_posenet_weights* w,
     return fail(ctx, ROHM_ERR_INVALID, "rohm_posenet_create: d_model must be a multiple of 128, ff_size of 64");
   const int dh = w->d_model / w->num_heads;
   if (dh != 64 && dh != 128) return fail(ctx, ROHM_ERR_INVALID, "rohm_posenet_create: head dim must be 64 or 128");
-  if (max_frames + 1 > 256) return fail(ctx, ROHM_ERR_INVALID, "rohm_posenet_create: at most 255 frames per clip");
-  if (max_frames + 1 > w->pe_len) return fail(ctx, ROHM_ERR_INVALID, "rohm_posenet_create: clip longer than pe table");
+  if (max_frames + 1 > w->pe_len)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_posenet_create: %d frames need %d rows of the positional table, which has %d",
+                max_frames, max_frames + 1, w->pe_len);
+  // Clip length: fp16 pairs with head dim 128 stream K / V through the attention kernel and reach pe_len - 1 frames; the
+  // TF32 precisions and head dim 64 run clips of more than 160 tokens on the SIMT kernel, whose K and V of the whole clip
+  // must fit in shared memory (and at most 256 tokens).
+  if (!(precision == ROHM_PRECISION_F16X2 && dh == 128)) {
+    int simt_frames = kAttnSimtMaxTokens - 1;
+    while (attention_smem_bytes(simt_frames + 1, dh) > kAttnSmemLimit) --simt_frames;
+    if (max_frames > simt_frames)
+      return fail(ctx, ROHM_ERR_INVALID,
+                  "rohm_posenet_create: %d frames per clip: precision f16x2 with head dim 128 reaches pe_len - 1 = %d "
+                  "frames; the tf32x3 / tf32 precisions and head dim 64 reach %d frames at head dim %d",
+                  max_frames, w->pe_len - 1, simt_frames, dh);
+  }
 
   rohm_posenet* pn = new (std::nothrow) rohm_posenet();
   if (pn == nullptr) return fail(ctx, ROHM_ERR_INVALID, "out of host memory");
@@ -685,11 +702,6 @@ extern "C" int rohm_posenet_create(rohm_ctx* ctx, const rohm_posenet_weights* w,
 #undef TRY
 
   // attention kernels need > 48 KB of dynamic shared memory
-  const size_t smem_max = attention_smem_bytes(max_frames + 1, dh);
-  if (smem_max > 227 * 1024) {
-    delete pn;
-    return fail(ctx, ROHM_ERR_INVALID, "clip too long for the attention kernel (%zu B smem)", smem_max);
-  }
   {
     cudaError_t ea = gemm_init_attributes();
     if (ea == cudaSuccess) ea = attention_init_attributes(max_frames + 1, dh);
@@ -706,7 +718,8 @@ extern "C" int rohm_posenet_create(rohm_ctx* ctx, const rohm_posenet_weights* w,
   pn->attn.D = D, pn->attn.H = pn->H;
   pn->attn.scale = 1.0f / sqrtf(static_cast<float>(dh));
   pn->attn.kind = pn->kind;
-  if (pn->tc_attention) {
+  pn->attn_maps = pn->kind == kKindF16 && dh == 128;
+  if (pn->attn_maps) {
     const int rcm = attention_wgmma_maps(&pn->attn_wg, pn->attn);
     if (rcm != 0) {
       delete pn;

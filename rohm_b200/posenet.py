@@ -391,6 +391,11 @@ class PoseNet(nn.Module):
         if timesteps.is_floating_point():
             # the reference indexes pe[timesteps]: a float index raises there too (rescale_timesteps is never enabled)
             raise RohmB200Error("PoseNet: timesteps must be an integer tensor (they index the positional table)")
+        pe_rows = self.sequence_pos_encoder.pe.shape[0]
+        if x_t.shape[3] + 1 > pe_rows:
+            # T frames + the timestep token take T + 1 rows of the table; the reference's pe[:T + 1] add fails there too
+            raise RohmB200Error(f"PoseNet: a clip of {x_t.shape[3]} frames needs {x_t.shape[3] + 1} rows of the positional "
+                                f"table sequence_pos_encoder.pe, which has {pe_rows} (at most {pe_rows - 1} frames)")
         e = self.prepare_cond(cond)
         x = x_t if (x_t.is_contiguous() and x_t.dtype == torch.float32) else x_t.contiguous().float()
         ts = timesteps.to(device=x.device, dtype=torch.int64).contiguous()
