@@ -181,8 +181,12 @@ ROHM_API int rohm_posenet_launches_per_forward(const rohm_posenet* pn);
 /* Parameters are handed over by their reference state-dict key ("diff_enc1.blocks.0.block.0.weight",
  * "controlnet.control_zero_conv_0.bias", "time_mlp.1.weight", ...): `names[i]` (host strings), `ptrs[i]` (device fp32),
  * `numels[i]`.  Every key the architecture needs must be present with the reference's shape; extra keys (e.g. the
- * never-evaluated cond_downsample4.*) are ignored.  `frames` must be a multiple of 16.  The library repacks all
- * convolution weights into GEMM layout (TF32 hi/lo, tap-major K) and owns its copies. */
+ * never-evaluated cond_downsample4.*) are ignored.  `frames` must be a multiple of 16, and a GroupNorm group of the widest
+ * levels (frames x mid_dim / 64 values) must fit the shared memory of a cluster of 8 CTAs:
+ * frames <= 8 x floor(M / (mid_dim / 16)), M = the device's opt-in shared memory per block less the GroupNorm kernel's
+ * static shared memory -- about 58 000 frames at mid_dim 512 on an H100.  A longer clip is refused with ROHM_ERR_INVALID
+ * before anything is allocated.  The library repacks all convolution weights into GEMM layout (TF32 hi/lo, tap-major K) and
+ * owns its copies. */
 ROHM_API int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* const* names, const float* const* ptrs,
                                  const int64_t* numels, int time_dim, int cond_dim, int traj_feat_dim, int mid_dim,
                                  int trajcontrol, int control_cond_dim, int max_batch, int frames, int precision,
@@ -286,14 +290,15 @@ ROHM_API int rohm_projection_guidance(rohm_body* bd, const float* x0, const floa
  * traj_dim = 13 for repr_abs_only else <= 22) is scattered into repr_clean [B,T,294] -> composite_out [B,T,294]
  * (z-scored with the trajectory dataset's mean/std) -> SMPL-X joints (rot6d -> axis-angle -> FK) -> get_repr_smplx
  * (data_loaders/motion_representation.py:187-282: forward direction, root quaternion incl. the first-NaN repair, velocities,
- * global-orient 6-D / angular velocity, translation) -> traj_full_out [B,T-1,22], z-scored with the pose dataset's stats. */
+ * global-orient 6-D / angular velocity, translation) -> traj_full_out [B,T-1,22], z-scored with the pose dataset's stats.
+ * 2 <= T <= 8192 (one cluster of at most 8 CTAs of 1024 frames per clip). */
 ROHM_API int rohm_traj_glue(rohm_body* bd, const float* traj_out, int traj_dim, const float* repr_clean,
                             const float* traj_mean, const float* traj_std, const float* pose_mean, const float* pose_std,
                             int B, int T, float* composite_out, float* traj_full_out, void* stream);
 
 /* The last stage of rohm_traj_glue on its own: get_repr_smplx's trajectory block (motion_representation.py:187-282) from
  * joints [B,T,22,3], global-orient axis-angles [B*T,3] and translations [B*T,3] -> traj_full_out [B,T-1,22], z-scored with
- * mean/stdv (the first 22 entries are read). */
+ * mean/stdv (the first 22 entries are read).  2 <= T <= 8192, as rohm_traj_glue. */
 ROHM_API int rohm_traj_repr_from_joints(rohm_ctx* ctx, const float* joints, const float* global_orient_aa,
                                         const float* transl, const float* mean, const float* stdv, int B, int T,
                                         float* traj_full_out, void* stream);

@@ -59,21 +59,40 @@ class DeviceGuard {
   bool restore_ = false;
 };
 
+// Launch attributes of launch_chain: programmatic dependent launch, and a thread-block cluster of `cluster` CTAs along x
+// (1: no cluster attribute; the grid's x dimension must be a multiple of it).
+struct ChainAttrs {
+  ChainAttrs(bool pdl_, unsigned cluster_ = 1) : pdl(pdl_), cluster(cluster_) {}  // implicit: a bare bool is PDL only
+  bool pdl;
+  unsigned cluster;
+};
+
 // Kernel launch with the programmatic-dependent-launch attribute (the kernel must call griddepcontrol.wait before it
-// touches memory, which every kernel launched through here does).
+// touches memory, which every kernel launched through here does) and optionally a cluster dimension.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_chain(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl,
+inline cudaError_t launch_chain(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, ChainAttrs at,
                                 Args... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  unsigned na = 0;
+  if (at.pdl) {
+    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[na].val.programmaticStreamSerializationAllowed = 1;
+    ++na;
+  }
+  if (at.cluster > 1) {
+    attr[na].id = cudaLaunchAttributeClusterDimension;
+    attr[na].val.clusterDim.x = at.cluster;
+    attr[na].val.clusterDim.y = 1;
+    attr[na].val.clusterDim.z = 1;
+    ++na;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
+  cfg.numAttrs = na;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 

@@ -11,8 +11,12 @@
 //   rohm_projection_guidance    model/posenet.py:260-317 guide_2d_projection_with_smpl, analytic VJP instead of autograd
 #include <cmath>
 
+#include <cooperative_groups.h>
+
 #include "body_internal.h"
 #include "kin.cuh"
+
+namespace cg = cooperative_groups;
 
 namespace rohm {
 namespace {
@@ -75,23 +79,35 @@ __device__ __forceinline__ M3 rotvec_to_mat(V3 r) {
   return R;
 }
 
-// get_repr_smplx, trajectory block only (channels 0..21 of REPR_LIST), one CTA per clip, one thread per frame.
-// joints: [B, T, 22, 3]; go: [B*T, 3] axis-angle global orient; transl: [B*T, 3]; out: [B, T-1, 22] z-scored with the
-// PoseNet dataset statistics.
+constexpr int kReprFramesPerCta = 1024;  // frames (threads) per CTA of traj_full_repr_kernel
+constexpr int kReprMaxCluster = 8;       // CTAs per clip: clips of up to 8192 frames
+
+// get_repr_smplx, trajectory block only (channels 0..21 of REPR_LIST): one cluster of n = ceil(T / 1024) CTAs per clip, one
+// thread per frame; CTA `rank` holds frames [rank * ceil(T / n), ...) and their root quaternions in its shared memory.  The
+// clip-wide first NaN frame (rank 0's first_nan) and the quaternions of frames in other CTAs are reached through
+// distributed shared memory.  joints: [B, T, 22, 3]; go: [B*T, 3] axis-angle global orient; transl: [B*T, 3]; out:
+// [B, T-1, 22] z-scored with the PoseNet dataset statistics.
 __global__ void traj_full_repr_kernel(const float* __restrict__ joints, const float* __restrict__ go,
                                       const float* __restrict__ transl, const float* __restrict__ mean,
                                       const float* __restrict__ stdv, int T, float* __restrict__ out) {
   extern __shared__ float sm[];
-  float* qw = sm;            // root quaternion (w, 0, 0, z) per frame
-  float* qz = sm + T;
+  cg::cluster_group cluster = cg::this_cluster();
+  const int ncta = static_cast<int>(cluster.num_blocks()), rank = static_cast<int>(cluster.block_rank());
+  const int rows = (T + ncta - 1) / ncta;  // frames per CTA
+  float* qw = sm;                    // root quaternion (w, 0, 0, z) per frame of this CTA
+  float* qz = sm + rows;
   __shared__ int first_nan;
-  const int b = blockIdx.x;
-  const int t = threadIdx.x;
-  if (t == 0) first_nan = T;
-  __syncthreads();
-  const float* P = joints + (static_cast<int64_t>(b) * T + (t < T ? t : 0)) * kBodyJ * 3;
+  // this CTA's shared address p as seen in CTA r (a single CTA is its own cluster)
+  auto peer = [&](auto* p, int r) { return ncta > 1 ? cluster.map_shared_rank(p, r) : p; };
+  auto sync = [&] { ncta > 1 ? cluster.sync() : __syncthreads(); };
+  const int b = blockIdx.x / ncta;
+  const int t = rank * rows + threadIdx.x;
+  const bool mine = threadIdx.x < rows && t < T;  // this thread's frame exists and belongs to this CTA
+  if (rank == 0 && threadIdx.x == 0) first_nan = T;
+  sync();
+  const float* P = joints + (static_cast<int64_t>(b) * T + (mine ? t : 0)) * kBodyJ * 3;
   auto J = [&](const float* base, int j) { return V3{base[j * 3], base[j * 3 + 1], base[j * 3 + 2]}; };
-  if (t < T) {
+  if (mine) {
     // forward direction from hips (2 = right, 1 = left) and shoulders (17 = right, 16 = left)
     V3 across = (J(P, 1) - J(P, 2)) + (J(P, 17) - J(P, 16));
     across = (1.0f / sqrtf(dot(across, across))) * across;
@@ -102,63 +118,78 @@ __global__ void traj_full_repr_kernel(const float* __restrict__ joints, const fl
     const float w = sqrtf(dot(fwd, fwd) * 1.0f) + fwd.y;
     const float n = sqrtf(w * w + vx * vx + vz * vz);
     const float q0 = w / n, q1 = vx / n, q3 = vz / n;
-    qw[t] = q0, qz[t] = q3;
-    if (isnan(q0) || isnan(q1) || isnan(q3)) atomicMin(&first_nan, t);
+    qw[threadIdx.x] = q0, qz[threadIdx.x] = q3;
+    if (isnan(q0) || isnan(q1) || isnan(q3)) atomicMin(peer(&first_nan, 0), t);
   }
-  __syncthreads();
-  if (t == 0) {
+  sync();
+  if (rank == 0 && threadIdx.x == 0) {
     // "several frames have nan values": the reference repairs the FIRST one only, with its predecessor
     // (frame -1 = the last frame when the first frame is the bad one), then pins frame 0 to the identity
     if (first_nan < T) {
-      const int src = first_nan > 0 ? first_nan - 1 : T - 1;
-      qw[first_nan] = qw[src], qz[first_nan] = qz[src];
+      const int dst = first_nan, src = first_nan > 0 ? first_nan - 1 : T - 1;
+      peer(qw, dst / rows)[dst % rows] = peer(qw, src / rows)[src % rows];
+      peer(qz, dst / rows)[dst % rows] = peer(qz, src / rows)[src % rows];
     }
     qw[0] = 1.0f, qz[0] = 0.0f;
   }
-  __syncthreads();
-  if (t >= T - 1) return;
-  const float* P1 = P + kBodyJ * 3;
-  const int64_t f = static_cast<int64_t>(b) * T + t;
-  float o[kTrajFull];
-  const float w0 = qw[t], z0 = qz[t], w1 = qw[t + 1], z1 = qz[t + 1];
-  o[kChAngle] = atan2f(z0, w0);
-  // q[t+1] * conj(q[t]) for rotations about z
-  o[kChAngleVel] = atan2f(w0 * z1 - z0 * w1, w1 * w0 + z1 * z0);
-  const V3 r0 = J(P, 0), r1 = J(P1, 0);
-  o[kChRootPos] = r0.x, o[kChRootPos + 1] = r0.y;
-  {
-    // qrot(q[t+1], r1 - r0), qvec = (0, 0, z1)
-    const V3 v = r1 - r0;
-    const V3 qv = {0.0f, 0.0f, z1};
-    const V3 uv = cross(qv, v);
-    const V3 uuv = cross(qv, uv);
-    o[kChRootVel] = v.x + 2.0f * (w1 * uv.x + uuv.x);
-    o[kChRootVel + 1] = v.y + 2.0f * (w1 * uv.y + uuv.y);
-  }
-  o[kChHeight] = r0.z;
-  const M3 R0 = rotvec_to_mat({go[f * 3], go[f * 3 + 1], go[f * 3 + 2]});
-  const M3 R1 = rotvec_to_mat({go[(f + 1) * 3], go[(f + 1) * 3 + 1], go[(f + 1) * 3 + 2]});
-  // rot6d = R[:, :2] row-major
-  o[kChRot6d] = R0.c0.x, o[kChRot6d + 1] = R0.c1.x, o[kChRot6d + 2] = R0.c0.y, o[kChRot6d + 3] = R0.c1.y;
-  o[kChRot6d + 4] = R0.c0.z, o[kChRot6d + 5] = R0.c1.z;
-  {
-    // estimate_angular_velocity_np: w_mat = dR R^T; entries (i,j) = sum_k dR[i][k] R[j][k]
-    const M3 dR = {R1.c0 - R0.c0, R1.c1 - R0.c1, R1.c2 - R0.c2};
-    auto rowd = [&](int i) { return i == 0 ? V3{dR.c0.x, dR.c1.x, dR.c2.x} : (i == 1 ? V3{dR.c0.y, dR.c1.y, dR.c2.y} : V3{dR.c0.z, dR.c1.z, dR.c2.z}); };
-    auto rowr = [&](int i) { return i == 0 ? V3{R0.c0.x, R0.c1.x, R0.c2.x} : (i == 1 ? V3{R0.c0.y, R0.c1.y, R0.c2.y} : V3{R0.c0.z, R0.c1.z, R0.c2.z}); };
-    auto wm = [&](int i, int j) { return dot(rowd(i), rowr(j)); };
-    o[13] = (-wm(1, 2) + wm(2, 1)) / 2.0f;
-    o[14] = (wm(0, 2) - wm(2, 0)) / 2.0f;
-    o[15] = (-wm(0, 1) + wm(1, 0)) / 2.0f;
-  }
-  for (int k = 0; k < 3; ++k) {
-    const float a = transl[f * 3 + k], c = transl[(f + 1) * 3 + k];
-    o[kChTrans + k] = a;
-    o[19 + k] = c - a;
-  }
-  float* dst = out + (static_cast<int64_t>(b) * (T - 1) + t) * kTrajFull;
+  sync();
+  if (mine && t < T - 1) {
+    const float* P1 = P + kBodyJ * 3;
+    const int64_t f = static_cast<int64_t>(b) * T + t;
+    float o[kTrajFull];
+    // frame t + 1 is the next CTA's first when t is this CTA's last
+    const int u = threadIdx.x + 1 < rows ? threadIdx.x + 1 : 0, ur = threadIdx.x + 1 < rows ? rank : rank + 1;
+    const float w0 = qw[threadIdx.x], z0 = qz[threadIdx.x], w1 = peer(qw, ur)[u], z1 = peer(qz, ur)[u];
+    o[kChAngle] = atan2f(z0, w0);
+    // q[t+1] * conj(q[t]) for rotations about z
+    o[kChAngleVel] = atan2f(w0 * z1 - z0 * w1, w1 * w0 + z1 * z0);
+    const V3 r0 = J(P, 0), r1 = J(P1, 0);
+    o[kChRootPos] = r0.x, o[kChRootPos + 1] = r0.y;
+    {
+      // qrot(q[t+1], r1 - r0), qvec = (0, 0, z1)
+      const V3 v = r1 - r0;
+      const V3 qv = {0.0f, 0.0f, z1};
+      const V3 uv = cross(qv, v);
+      const V3 uuv = cross(qv, uv);
+      o[kChRootVel] = v.x + 2.0f * (w1 * uv.x + uuv.x);
+      o[kChRootVel + 1] = v.y + 2.0f * (w1 * uv.y + uuv.y);
+    }
+    o[kChHeight] = r0.z;
+    const M3 R0 = rotvec_to_mat({go[f * 3], go[f * 3 + 1], go[f * 3 + 2]});
+    const M3 R1 = rotvec_to_mat({go[(f + 1) * 3], go[(f + 1) * 3 + 1], go[(f + 1) * 3 + 2]});
+    // rot6d = R[:, :2] row-major
+    o[kChRot6d] = R0.c0.x, o[kChRot6d + 1] = R0.c1.x, o[kChRot6d + 2] = R0.c0.y, o[kChRot6d + 3] = R0.c1.y;
+    o[kChRot6d + 4] = R0.c0.z, o[kChRot6d + 5] = R0.c1.z;
+    {
+      // estimate_angular_velocity_np: w_mat = dR R^T; entries (i,j) = sum_k dR[i][k] R[j][k]
+      const M3 dR = {R1.c0 - R0.c0, R1.c1 - R0.c1, R1.c2 - R0.c2};
+      auto rowd = [&](int i) { return i == 0 ? V3{dR.c0.x, dR.c1.x, dR.c2.x} : (i == 1 ? V3{dR.c0.y, dR.c1.y, dR.c2.y} : V3{dR.c0.z, dR.c1.z, dR.c2.z}); };
+      auto rowr = [&](int i) { return i == 0 ? V3{R0.c0.x, R0.c1.x, R0.c2.x} : (i == 1 ? V3{R0.c0.y, R0.c1.y, R0.c2.y} : V3{R0.c0.z, R0.c1.z, R0.c2.z}); };
+      auto wm = [&](int i, int j) { return dot(rowd(i), rowr(j)); };
+      o[13] = (-wm(1, 2) + wm(2, 1)) / 2.0f;
+      o[14] = (wm(0, 2) - wm(2, 0)) / 2.0f;
+      o[15] = (-wm(0, 1) + wm(1, 0)) / 2.0f;
+    }
+    for (int k = 0; k < 3; ++k) {
+      const float a = transl[f * 3 + k], c = transl[(f + 1) * 3 + k];
+      o[kChTrans + k] = a;
+      o[19 + k] = c - a;
+    }
+    float* dst = out + (static_cast<int64_t>(b) * (T - 1) + t) * kTrajFull;
 #pragma unroll
-  for (int c = 0; c < kTrajFull; ++c) dst[c] = (o[c] - mean[c]) / stdv[c];
+    for (int c = 0; c < kTrajFull; ++c) dst[c] = (o[c] - mean[c]) / stdv[c];
+  }
+  if (ncta > 1) cluster.sync();  // peers may still read this CTA's quaternions
+}
+
+// B clusters of ceil(T / 1024) CTAs; T <= kReprFramesPerCta * kReprMaxCluster (checked by the callers)
+cudaError_t launch_traj_full_repr(const float* joints, const float* go, const float* transl, const float* mean,
+                                  const float* stdv, int B, int T, float* out, cudaStream_t st) {
+  const int n = (T + kReprFramesPerCta - 1) / kReprFramesPerCta;
+  const int rows = (T + n - 1) / n;
+  return launch_chain(traj_full_repr_kernel, dim3(static_cast<unsigned>(B * n)), dim3((rows + 31) / 32 * 32),
+                      2 * rows * sizeof(float), st, ChainAttrs(false, static_cast<unsigned>(n)), joints, go, transl, mean,
+                      stdv, T, out);
 }
 
 // control_cond[b, t, :] = pose_out[b, 22 + c, 0, min(t, Tp-1)]   (Tp = T-1 frames of PoseNet output; last frame repeated)
@@ -433,9 +464,12 @@ extern "C" int rohm_traj_glue(rohm_body* bd, const float* traj_out, int traj_dim
   rohm::DeviceGuard device_guard__(ctx);
   const int64_t N = static_cast<int64_t>(B) * T;
   if (!traj_out || !repr_clean || !traj_mean || !traj_std || !pose_mean || !pose_std || !composite_out || !traj_full_out ||
-      B <= 0 || T < 2 || T > 1024 || N > bd->max_frames || (traj_dim != 13 && (traj_dim < 1 || traj_dim > kTrajFull)))
+      B <= 0 || T < 2 || N > bd->max_frames || (traj_dim != 13 && (traj_dim < 1 || traj_dim > kTrajFull)))
     return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_glue: bad arguments (B=%d T=%d traj_dim=%d capacity %lld frames)", B, T,
                 traj_dim, static_cast<long long>(bd->max_frames));
+  if (T > kReprFramesPerCta * kReprMaxCluster)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_glue: T=%d frames exceeds %d (one cluster of at most %d CTAs of %d frames "
+                "per clip)", T, kReprFramesPerCta * kReprMaxCluster, kReprMaxCluster, kReprFramesPerCta);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t total = N * kC;
   compose_repr_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(traj_out, traj_dim, repr_clean,
@@ -443,10 +477,7 @@ extern "C" int rohm_traj_glue(rohm_body* bd, const float* traj_out, int traj_dim
   ROHM_CUDA(ctx, cudaGetLastError());
   int rc = rohm_body_from_repr_layout(bd, composite_out, 1, traj_mean, traj_std, B, T, bd->jwork, kBodyJ, nullptr, stream);
   if (rc != ROHM_OK) return rc;
-  const int threads = (T + 31) / 32 * 32;
-  traj_full_repr_kernel<<<B, threads, 2 * T * sizeof(float), st>>>(bd->jwork, bd->go, bd->transl, pose_mean, pose_std, T,
-                                                                  traj_full_out);
-  ROHM_CUDA(ctx, cudaGetLastError());
+  ROHM_CUDA(ctx, launch_traj_full_repr(bd->jwork, bd->go, bd->transl, pose_mean, pose_std, B, T, traj_full_out, st));
   return ROHM_OK;
 }
 
@@ -455,12 +486,13 @@ extern "C" int rohm_traj_repr_from_joints(rohm_ctx* ctx, const float* joints, co
                                           float* traj_full_out, void* stream) {
   if (ctx == nullptr) return ROHM_ERR_INVALID;
   rohm::DeviceGuard device_guard__(ctx);
-  if (!joints || !global_orient_aa || !transl || !mean || !stdv || !traj_full_out || B <= 0 || T < 2 || T > 1024)
+  if (!joints || !global_orient_aa || !transl || !mean || !stdv || !traj_full_out || B <= 0 || T < 2)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_repr_from_joints: bad arguments");
-  const int threads = (T + 31) / 32 * 32;
-  traj_full_repr_kernel<<<B, threads, 2 * T * sizeof(float), static_cast<cudaStream_t>(stream)>>>(
-      joints, global_orient_aa, transl, mean, stdv, T, traj_full_out);
-  ROHM_CUDA(ctx, cudaGetLastError());
+  if (T > kReprFramesPerCta * kReprMaxCluster)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_repr_from_joints: T=%d frames exceeds %d (one cluster of at most %d CTAs "
+                "of %d frames per clip)", T, kReprFramesPerCta * kReprMaxCluster, kReprMaxCluster, kReprFramesPerCta);
+  ROHM_CUDA(ctx, launch_traj_full_repr(joints, global_orient_aa, transl, mean, stdv, B, T, traj_full_out,
+                                       static_cast<cudaStream_t>(stream)));
   return ROHM_OK;
 }
 

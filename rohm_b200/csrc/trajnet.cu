@@ -9,8 +9,9 @@
 //   * ConvTranspose (k4, s2)    = two GEMMs (even / odd output frames), 2 taps each, row-interleaved stores,
 // so every convolution is one launch of the wgmma segmented-A GEMM (gemm.cu) and no im2col / concat / transpose
 // buffer exists.  The convolutions of the deep pyramid levels are cut along K into 3-6 ranges (pick_split: 128-wide tiles x K
-// ranges cover the SMs where 6-22 row tiles alone cannot); one kernel per GroupNorm'd convolution (gn_mish_split_kernel, a
-// CTA per (clip, group)) adds bias + the fp32 partial(s) in split order, takes the group's statistics, applies GroupNorm + Mish
+// ranges cover the SMs where 6-22 row tiles alone cannot); one kernel per GroupNorm'd convolution (gn_mish_split_kernel in
+// groupnorm.cu, a cluster of CTAs per (clip, group)) adds bias + the fp32 partial(s) in split order, takes the group's
+// statistics, applies GroupNorm + Mish
 // (+ time projection, + residual, + TrajControl residual) and emits the hi/lo operand pair of the next convolution.  The
 // step-invariant condition pyramid and control_zero_conv_0 run once per condition (set_cond).  rohm_trajnet_sample_step appends
 // the in-kernel-noise sampler update to the forward graph.
@@ -22,15 +23,11 @@
 #include "common.h"
 #include "gemm.cuh"
 #include "graph.cuh"
+#include "groupnorm.cuh"
 #include "ptx.cuh"
 
 namespace rohm {
 namespace {
-
-__device__ __forceinline__ float mish_f(float x) {
-  const float sp = x > 20.0f ? x : log1pf(expf(x));
-  return x * tanhf(sp);
-}
 
 // [B, T, C] channels-last API tensor -> padded-clip hi/lo rows (b * Tp + t), pitch ld.  Pad rows stay zero.
 __global__ void pack_rows_kernel(const float* __restrict__ x, float* __restrict__ hi, float* __restrict__ lo, int T,
@@ -113,25 +110,6 @@ __global__ void __launch_bounds__(256) trajnet_time_kernel(const int64_t* __rest
 }
 constexpr size_t kTrajnetTimeT = 0;  // the argument replaced on every replay of a cached forward graph
 
-constexpr int kMaxSplitsDev = 8;  // most K ranges a convolution is cut into (= kMaxSplits of the host-side choice)
-
-// One float4 of an activation in its stored forms: fp32 and / or the hi/lo operand pair of the next convolution.
-__device__ __forceinline__ void store_act4(float* out, float* out_hi, float* out_lo, int64_t idx, const float4& v, int f16) {
-  if (out != nullptr) reinterpret_cast<float4*>(out)[idx] = v;
-  if (out_hi != nullptr && f16) {
-    uint2 h, l;
-    ptx::split_f16x4(v, h, l);
-    reinterpret_cast<uint2*>(out_hi)[idx] = h;
-    reinterpret_cast<uint2*>(out_lo)[idx] = l;
-  } else if (out_hi != nullptr) {
-    float4 h, l;
-    h.x = ptx::to_tf32(v.x), h.y = ptx::to_tf32(v.y), h.z = ptx::to_tf32(v.z), h.w = ptx::to_tf32(v.w);
-    l.x = v.x - h.x, l.y = v.y - h.y, l.z = v.z - h.z, l.w = v.w - h.w;
-    reinterpret_cast<float4*>(out_hi)[idx] = h;
-    reinterpret_cast<float4*>(out_lo)[idx] = l;
-  }
-}
-
 // Split-K convolution without a GroupNorm behind it (the stride-2 downsampling convolutions): out = bias + the partials (in
 // split order) on real rows, 0 on pad rows.  4 channels per thread over the [B * Tp, C] output.
 __global__ void __launch_bounds__(256) sum_split_kernel(const float* __restrict__ part, int splits, int64_t split_stride,
@@ -158,97 +136,6 @@ __global__ void __launch_bounds__(256) sum_split_kernel(const float* __restrict_
       if (sp < splits) v.x += a[sp].x, v.y += a[sp].y, v.z += a[sp].z, v.w += a[sp].w;
   }
   store_act4(out, out_hi, out_lo, i, v, f16);
-}
-
-// GroupNorm + Mish behind every GroupNorm'd convolution: one CTA per (clip, group).  y = bias + the `splits` fp32 partials
-// (added in split order: deterministic; an un-split convolution passes its output as the one partial) of the group's
-// T x (C / groups) real elements is formed once into shared memory, its mean / variance are reduced inside the CTA (the
-// producing GEMM writes no statistics), then out = Mish(GroupNorm(y)) [+ tp] [+ r1] [+ r2]; pad rows are written as zeros.
-// part: [splits][split_stride] floats, each a [B * Tp, C] matrix.  C / groups must be a multiple of 4 (float4 units).
-__global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restrict__ part, int splits, int64_t split_stride,
-                                                            const float* __restrict__ bias, const float* __restrict__ gamma,
-                                                            const float* __restrict__ beta, const float* __restrict__ tp,
-                                                            int tp_stride, const float* __restrict__ r1,
-                                                            const float* __restrict__ r2, float* __restrict__ out,
-                                                            float* __restrict__ out_hi, float* __restrict__ out_lo, int C, int Tp,
-                                                            int T, int groups, int f16) {
-  extern __shared__ float4 gn_vals[];  // T * (C / groups) / 4
-  __shared__ double red[2][8];
-  ptx::pdl_launch_dependents();
-  ptx::pdl_wait_prior_grid();
-  const int b = blockIdx.x / groups, g = blockIdx.x - b * groups;
-  const int gs = C / groups, gs4 = gs / 4;
-  const int n4 = T * gs4;
-  const int c4 = C / 4;
-  const int64_t row0 = static_cast<int64_t>(b) * Tp;
-  double s1 = 0.0, s2 = 0.0;
-  for (int i = threadIdx.x; i < n4; i += blockDim.x) {
-    const int t = i / gs4;
-    const int c = g * gs + (i - t * gs4) * 4;
-    const int64_t idx = (row0 + t) * c4 + c / 4;
-    // all partials of this float4 are requested before the first is used (one L2 round trip instead of `splits`); they are
-    // still added in split order
-    float4 a[kMaxSplitsDev];
-#pragma unroll
-    for (int sp = 0; sp < kMaxSplitsDev; ++sp)
-      if (sp < splits) a[sp] = __ldcg(reinterpret_cast<const float4*>(part + sp * split_stride) + idx);
-    float4 v = *reinterpret_cast<const float4*>(bias + c);
-#pragma unroll
-    for (int sp = 0; sp < kMaxSplitsDev; ++sp)
-      if (sp < splits) v.x += a[sp].x, v.y += a[sp].y, v.z += a[sp].z, v.w += a[sp].w;
-    gn_vals[i] = v;
-    s1 += static_cast<double>(v.x) + static_cast<double>(v.y) + static_cast<double>(v.z) + static_cast<double>(v.w);
-    s2 += static_cast<double>(v.x) * v.x + static_cast<double>(v.y) * v.y + static_cast<double>(v.z) * v.z +
-          static_cast<double>(v.w) * v.w;
-  }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) {
-    s1 += __shfl_xor_sync(0xffffffffu, s1, off);
-    s2 += __shfl_xor_sync(0xffffffffu, s2, off);
-  }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) red[0][warp] = s1, red[1][warp] = s2;
-  __syncthreads();
-  s1 = 0.0, s2 = 0.0;
-  for (int wv = 0; wv < static_cast<int>(blockDim.x >> 5); ++wv) s1 += red[0][wv], s2 += red[1][wv];
-  const double n = static_cast<double>(gs) * static_cast<double>(T);
-  const double mean = s1 / n;
-  double var = s2 / n - mean * mean;
-  var = var < 0.0 ? 0.0 : var;
-  const float mu = static_cast<float>(mean);
-  const float rstd = static_cast<float>(1.0 / sqrt(var + 1e-5));
-  for (int i = threadIdx.x; i < n4; i += blockDim.x) {
-    const int t = i / gs4;
-    const int c = g * gs + (i - t * gs4) * 4;
-    const int64_t idx = (row0 + t) * c4 + c / 4;
-    const float4 x = gn_vals[i];
-    const float4 ga = *reinterpret_cast<const float4*>(gamma + c);
-    const float4 be = *reinterpret_cast<const float4*>(beta + c);
-    float4 v;
-    v.x = mish_f((x.x - mu) * rstd * ga.x + be.x);
-    v.y = mish_f((x.y - mu) * rstd * ga.y + be.y);
-    v.z = mish_f((x.z - mu) * rstd * ga.z + be.z);
-    v.w = mish_f((x.w - mu) * rstd * ga.w + be.w);
-    if (tp != nullptr) {
-      const float4 a = *reinterpret_cast<const float4*>(tp + static_cast<int64_t>(b) * tp_stride + c);
-      v.x += a.x, v.y += a.y, v.z += a.z, v.w += a.w;
-    }
-    if (r1 != nullptr) {
-      const float4 a = reinterpret_cast<const float4*>(r1)[idx];
-      v.x += a.x, v.y += a.y, v.z += a.z, v.w += a.w;
-    }
-    if (r2 != nullptr) {
-      const float4 a = reinterpret_cast<const float4*>(r2)[idx];
-      v.x += a.x, v.y += a.y, v.z += a.z, v.w += a.w;
-    }
-    store_act4(out, out_hi, out_lo, idx, v, f16);
-  }
-  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int i = threadIdx.x; i < (Tp - T) * gs4; i += blockDim.x) {  // pad rows: the next convolution's zero padding
-    const int t = T + i / gs4;
-    const int c = g * gs + (i % gs4) * 4;
-    store_act4(out, out_hi, out_lo, (row0 + t) * c4 + c / 4, zero, f16);
-  }
 }
 
 // padded-clip rows [B * Tp, ld] -> compact [B, T, C]
@@ -322,6 +209,7 @@ struct Conv {
   float* partial = nullptr;
   int64_t split_rows = 0;
   bool sum_after = false;  // no GroupNorm behind it: sum_split_kernel writes `out` right after the GEMM
+  int gn_cluster = 1;      // GroupNorm'd: CTAs per (clip, group) of its gn_mish_split_kernel launch (gn_pick_cluster)
   int ts_runs = 0;         // ROHM_B200_TRAJ_TS: launches outside stream capture so far
 };
 
@@ -396,6 +284,8 @@ struct rohm_trajnet {
   int launches = 0;
   ForwardGraphs graphs;  // CUDA graph of one forward per batch size
   bool use_pdl = true;  // ROHM_B200_PDL / rohm_trajnet_set_option(1): programmatic dependent launch along the conv / GroupNorm chains
+  size_t gn_budget = 0;    // gn_mish_split_kernel's default dynamic shared-memory budget per CTA
+  size_t gn_smem_max = 0;  // the largest slice of any of its launches
   ~rohm_trajnet() {
     for (cudaStream_t q : side)
       if (q) cudaStreamDestroy(q);
@@ -602,6 +492,10 @@ int make_conv(rohm_trajnet* tn, Conv& cv, const std::string& name, const std::st
     cv.partial = out.f32;
     g.bias = nullptr;
   }
+  if (group_normed) {
+    cv.gn_cluster = gn_pick_cluster(tn->Tl[row_level], Cout, kGroups, tn->gn_budget);
+    tn->gn_smem_max = std::max(tn->gn_smem_max, gn_slice_bytes(tn->Tl[row_level], Cout, kGroups, cv.gn_cluster));
+  }
   // fp32-only or fp16-pair-only outputs with the identity row map leave through TMA bulk stores (the transposed-conv phases
   // and the few convolutions that write both forms keep the per-thread epilogue)
   if (gemm_enable_tma_store(&g, cv.splits > 1 ? cv.splits * cv.split_rows : rows_of(tn, row_level), tn->kind) != 0)
@@ -694,15 +588,14 @@ int run_conv(rohm_trajnet* tn, Conv& cv, int B, cudaStream_t st) {
   return ROHM_OK;
 }
 
-// partial(s) + bias -> statistics -> GroupNorm / Mish of the GroupNorm'd convolution `cv`, one CTA per (clip, group)
+// partial(s) + bias -> statistics -> GroupNorm / Mish of the GroupNorm'd convolution `cv`, one cluster of cv.gn_cluster
+// CTAs per (clip, group)
 int run_gn(rohm_trajnet* tn, const Conv& cv, const GroupNorm& gn, int B, const float* tp, const float* r1, const float* r2,
            const Act& out, cudaStream_t st) {
   const int C = cv.w.N, level = cv.level_out;
-  ROHM_CUDA(tn->ctx, launch_chain(gn_mish_split_kernel, dim3(static_cast<unsigned>(B * kGroups)), dim3(256),
-                                  static_cast<size_t>(tn->Tl[level]) * (C / kGroups) * sizeof(float), st, tn->use_pdl,
-                                  cv.partial, cv.splits, cv.split_rows * C, cv.bias, gn.gamma, gn.beta, tp, tn->tp_total, r1,
-                                  r2, out.f32, out.hi, out.lo, C, tn->Tp[level], tn->Tl[level], kGroups,
-                                  tn->kind == kKindF16 ? 1 : 0));
+  const GnArgs a{cv.partial, cv.splits, cv.split_rows * C, cv.bias, gn.gamma, gn.beta, tp, tn->tp_total, r1, r2,
+                 out.f32, out.hi, out.lo, C, tn->Tp[level], tn->Tl[level], kGroups, tn->kind == kKindF16 ? 1 : 0};
+  ROHM_CUDA(tn->ctx, launch_gn_mish(a, B, cv.gn_cluster, st, tn->use_pdl));
   tn->launches++;
   return ROHM_OK;
 }
@@ -756,6 +649,17 @@ extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* cons
                 "groups of its mid_dim / 8-wide level need a multiple of 4 channels each), time_dim even and <= 64", mid_dim);
   if (precision != ROHM_PRECISION_TF32X3 && precision != ROHM_PRECISION_TF32 && precision != ROHM_PRECISION_F16X2)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_create: precision must be 3 (TF32x3), 2 (F16x2) or 1 (TF32)");
+  // GroupNorm: a group of the widest levels (frames x mid_dim / 8 values at level 0, and the same count at levels 1-3) is
+  // spread over a cluster of at most kGnMaxCluster CTAs, each of which holds its slice in shared memory
+  size_t gn_budget = 0, gn_max = 0;
+  ROHM_CUDA(ctx, gn_smem_budgets(&gn_budget, &gn_max));
+  const int64_t gn_row_bytes = static_cast<int64_t>(mid_dim / 8 / kGroups) * sizeof(float);
+  const int64_t max_frames = static_cast<int64_t>(gn_max) / gn_row_bytes * kGnMaxCluster / 16 * 16;
+  if (frames > max_frames)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_create: frames (%d) exceeds %lld at mid_dim %d: a GroupNorm group of "
+                "the widest levels holds frames x mid_dim / 64 values, spread over at most %d CTAs of %zu bytes of shared "
+                "memory each (frames <= %d x floor(%zu / (mid_dim / 16)), a multiple of 16)", frames,
+                static_cast<long long>(max_frames), mid_dim, kGnMaxCluster, gn_max, kGnMaxCluster, gn_max);
   ROHM_CUDA(ctx, gemm_init_attributes());
   std::unique_ptr<rohm_trajnet> owner(new (std::nothrow) rohm_trajnet());
   rohm_trajnet* tn = owner.get();
@@ -765,6 +669,7 @@ extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* cons
   tn->control = trajcontrol != 0, tn->control_dim = control_cond_dim, tn->passes = precision == ROHM_PRECISION_TF32 ? 1 : 3;
   tn->kind = precision == ROHM_PRECISION_F16X2 ? kKindF16 : kKindTf32;
   tn->max_batch = max_batch, tn->T = frames;
+  tn->gn_budget = gn_budget;
   for (int l = 0; l < kLevels; ++l) tn->Tl[l] = frames >> l, tn->Tp[l] = (frames + 32) >> l;
   tn->n_params = n_params, tn->names = names, tn->ptrs = ptrs, tn->numels = numels;
   const int m = mid_dim, td = time_dim;
@@ -876,6 +781,9 @@ extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* cons
     TRY(make_rtb(tn, ctl.mid_block[1], cn + "control_mid_block2.", {&kmb[0]}, kmb[1], 1, &timed));
     TRY(make_conv(tn, ctl.zero_mid, "kzm", cn + "control_zero_conv_mid", {&kmb[1]}, zm, 1, 1, kConv, false, 1));
   }
+
+  // one attribute for every GroupNorm launch of the engine; only needed when a slice exceeds the default budget (n = 8)
+  if (tn->gn_smem_max > gn_budget) ROHM_CUDA(ctx, gn_reserve_smem(tn->gn_smem_max));
 
   // ---- time path: stacked Linear(time_dim -> out) of every block with input_t ----
   const int total = tn->tp_total;
