@@ -903,24 +903,7 @@ extern "C" int rohm_body_forward(rohm_body* bd, const float* global_orient, cons
       g.st_hi = g.st_out, g.st_lo = g.st_out;
       g.tma_store = 1;
     }
-    static int ts_calls = 0;
-    unsigned long long* d_ts = nullptr;
-    if (getenv("ROHM_B200_LBS_TS") != nullptr && ++ts_calls == 3) {  // developer instrumentation: CTA 0's %globaltimer stamps
-      if (cudaMalloc(&d_ts, 32 * sizeof(unsigned long long)) == cudaSuccess) cudaMemset(d_ts, 0, 32 * sizeof(unsigned long long));
-      g.debug_ts = d_ts;
-    }
     ROHM_CUDA(ctx, launch_gemm(g, static_cast<int>(N), bd->blend.Np, 96, bd->passes, st, false, bd->kind));
-    if (d_ts != nullptr) {
-      unsigned long long h[32];
-      cudaStreamSynchronize(st);
-      cudaMemcpy(h, d_ts, sizeof h, cudaMemcpyDeviceToHost);
-      cudaFree(d_ts);
-      fprintf(stderr, "fused LBS CTA0 timeline (ns): setup %llu | first_full %llu | tile1: acc ready %llu | drained %llu | skinned %llu | "
-              "staged %llu | stored %llu || mma issued per tile:", h[1] - h[0], h[3] - h[0], h[5] - h[0], h[8] - h[0], h[9] - h[0],
-              h[10] - h[0], h[11] - h[0]);
-      for (int i = 16; i < 24 && h[i] != 0; ++i) fprintf(stderr, " %llu", h[i] - h[0]);
-      fprintf(stderr, " | all mma issued %llu | end %llu\n", h[12] - h[0], h[7] - h[0]);
-    }
   } else if (verts) {
     // Pipeline over chunks of kLbsChunk frames: blend GEMM of chunk i on the caller's stream into v_posed buffer i % 2,
     // skinning of chunk i on a second stream (HBM-bound next to the tensor-bound GEMM of chunk i + 1).

@@ -82,14 +82,6 @@ __device__ __forceinline__ void acc_load(const float* acc, int row, int col, flo
   }
 }
 
-__device__ __forceinline__ void stamp(const GemmParams& p, int slot) {
-  if (p.debug_ts != nullptr && blockIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    p.debug_ts[slot] = t;
-  }
-}
-
 __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == kActGelu) {
     return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));  // exact (erf) GELU, nn.GELU default
@@ -238,7 +230,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) stamp(p, 0);
   const int tiles_n = (p.grid_n_cols + BLOCK_N - 1) / BLOCK_N;
   const int tiles_m = (p.grid_m_rows + kGemmBlockM - 1) / kGemmBlockM;
   const int num_tiles = tiles_m * tiles_n;
@@ -306,7 +297,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
   }
   __syncthreads();
 
-  if (threadIdx.x == 0) stamp(p, 1);
   // Programmatic dependent launch: let the next kernel of the chain become resident as soon as SMs free up (its
   // prologue then overlaps this kernel's tail; it blocks in its own griddepcontrol.wait until this grid has completed
   // and flushed), then order everything below after the previous kernel.
@@ -334,7 +324,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
             const int row = m0 * p.seg_row_mul[s] + p.seg_row_shift[s];
             uint8_t* st = smem + stage * Cfg::kStageBytes;
             if (it < prefetched) {  // B of this stage is already in flight (see above): only A is missing
-              if (it == 0) stamp(p, 2);
               ptx::tma_load_2d(st, &p.a_hi[s], &full_bar[stage], kb * kElemK, row);
               if (PASSES == 3) ptx::tma_load_2d(st + Cfg::kABytes, &p.a_lo[s], &full_bar[stage], kb * kElemK, row);
               if (++stage == Cfg::kStages) stage = 0, phase ^= 1;
@@ -342,7 +331,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
               continue;
             }
             ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-            if (it == 0) stamp(p, 2);
             ptx::mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
             ptx::tma_load_2d(st, &p.a_hi[s], &full_bar[stage], kb * kElemK, row);
             ptx::tma_load_2d(st + Cfg::kSplit * Cfg::kABytes, &p.b_hi, &full_bar[stage], kcol, n0);
@@ -393,7 +381,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
       int prev = -1;
       for (int ki = 0; ki < n_it; ++ki) {
         ptx::mbar_wait(&full_bar[mma_stage], mma_phase);
-        if (ki == 0 && w == static_cast<int>(blockIdx.x)) stamp(p, 3);
         const uint32_t st = ptx::smem_u32(smem + mma_stage * Cfg::kStageBytes);
         const uint32_t a_off = static_cast<uint32_t>(mhalf * (Cfg::kABytes / 2));  // this warpgroup's 64 rows
         const uint64_t a_hi = ptx::make_desc_kmajor<kGemmBlockK * 4>(st + a_off);
@@ -446,16 +433,10 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
     };
     const bool epi_warp = !EPI_ROLE || !mma_warp;
     if (!epi_warp) {
-      // MMA warpgroups of the EPI_ROLE variants: nothing but K loops and the hand-over (debug_ts slots 16 + i: tile i < 4
-      // published in acc_s, 12: the last one; the epilogue's slots 20 + i: prologue done, 24 + i: acc_full observed,
-      // 28 + i: tile stored)
+      // MMA warpgroups of the EPI_ROLE variants: nothing but K loops and the hand-over
       ptx::setmaxnreg_inc<kMmaRegs>();
       int tc = 0;
-      for (int wi = blockIdx.x; wi < num_work; wi += gridDim.x, ++tc) {
-        mma_tile(wi, tc);
-        if (warp_idx == kFirstMmaWarp && lane == 0 && tc < 4) stamp(p, 16 + tc);
-      }
-      if (warp_idx == kFirstMmaWarp && lane == 0) stamp(p, 12);
+      for (int wi = blockIdx.x; wi < num_work; wi += gridDim.x, ++tc) mma_tile(wi, tc);
     } else if constexpr (EPI_ROLE) {
       ptx::setmaxnreg_inc<kEpiRoleRegs>();
     }
@@ -519,7 +500,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
         if (has_next) fetch_tables(next % tiles_n, nw0, nw1, nbone, nnb);  // in flight during the accumulator wait and the compute
 
         mma_tile(tile_idx, tcount);  // the previous tile's reads of acc_s are behind the bar.sync 1 of its compute phase
-        if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 5);
         // verts = sum_b w[v][b] (R_b v_posed + t_b).  Within a 32-vertex tile nearly every (vertex, bone) pair carries weight
         // (vertices are indexed by body part), so every vertex is updated per bone: no branches, 12 FMAs per (vertex, bone).
         // Two rounds of 8 vertices keep the live registers (transforms 48 + v_posed 24 + results 48) under the 168 available.
@@ -536,7 +516,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
 #pragma unroll
             for (int j = 0; j < 24; ++j) vp[j] *= e.acc_scale;
           }
-          if (h2 == 1 && tcount == 1 && ew == 0 && lane == 0) stamp(p, 8);
           auto apply_bone = [&](const float4& r0, const float4& r1, const float4& r2, const float* wrow) {
 #pragma unroll
             for (int g = 0; g < 2; ++g) {
@@ -568,7 +547,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
             }
           }
         }
-        if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 9);
         if (has_next) publish_tables(buf ^ 1, nw0, nw1, nbone, nnb);
         // TMA-store variant: the previous tile's bulk stores (issued by this thread) have finished reading the staging tile
         if (e.tma_store && ew == 0 && lane == 0) ptx::bulk_wait_read_all();
@@ -591,14 +569,12 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
           }
           ptx::fence_proxy_async();
           asm volatile("bar.sync 2, %0;" ::"n"(kEpiWarps * 32));
-          if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 10);
           if (ew == 0 && lane == 0) {
 #pragma unroll
             for (int j = 0; j < 3; ++j)
               if (n0 + 32 * j < e.N) ptx::tma_store_2d(&p.st_out, sb + j * (kGemmBlockM * 128), n0 + 32 * j, m0);
             ptx::bulk_commit();
           }
-          if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 11);
           continue;
         }
         // transpose through the CTA-wide staging tile: the output row pitch (3 V floats) is not a multiple of 16 bytes, so
@@ -609,7 +585,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
           for (int j = 0; j < 12; ++j) srow[j] = make_float4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
         }
         asm volatile("bar.sync 2, %0;" ::"n"(kEpiWarps * 32));
-        if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 10);
         {
           const int w8 = ew;
 #pragma unroll 4
@@ -626,7 +601,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
             }
           }
         }
-        if (tcount == 1 && ew == 0 && lane == 0) stamp(p, 11);
       }
     }
     for (int wi = blockIdx.x; EPI != 4 && epi_warp && wi < num_work; wi += gridDim.x, ++tcount) {
@@ -719,15 +693,12 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
         }
         load_residual(0);
       }
-      if (EPI_ROLE && ew == 0 && lane == 0 && tcount < 4) stamp(p, 20 + tcount);  // prologue done
       if constexpr (EPI_ROLE) {
         ptx::mbar_wait(&acc_full, static_cast<uint32_t>(tcount & 1));
-        if (ew == 0 && lane == 0 && tcount < 4) stamp(p, 24 + tcount);
       } else {
         // the start-of-tile bar.sync 1 above keeps this tile's accumulator off acc_s until every thread has read the last one
         mma_tile(wi, tcount);
       }
-      if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 5);
 
       if constexpr (EPI == 3) {
         // ===== u = LN_prev(residual) + acc * 2^-s + bias, written in place as an fp16 pair + per-row partial statistics =====
@@ -758,7 +729,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
             __syncwarp();
             if (lane == 0) ptx::mbar_arrive(&acc_empty);
           }
-          if (tcount == 0 && g == 0 && ew == 0 && lane == 0) stamp(p, 8);
           auto store_chunk = [&](int h2) {
             const int nb = n0 + g * 32 + 64 * h2;
             if (group_full) {
@@ -784,11 +754,8 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
             m2_i = fmaf(d0, d0, fmaf(d1, d1, m2_i));
           }
           if (row_ok) e.stats_out[static_cast<int64_t>(m) * 8 + tile_n * 2 + g] = make_float2(mean_i, m2_i);
-          if (tcount == 0 && g == 0 && ew == 0 && lane == 0) stamp(p, 9);
           store_chunk(1);
         }
-        if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 6);
-        if (ew == 0 && lane == 0 && tcount < 4) stamp(p, 28 + tcount);
         continue;
       }
 
@@ -798,7 +765,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
         const bool full = vec_ok && (nb + 32 <= e.N);
         if (e.tma_store && full && (m0 + q * 32 + 32 <= e.M)) {
           // ---- TMA-store path: row-per-thread registers -> swizzled staging tile -> bulk tensor store ----
-          if (p.debug_flags & 1) continue;
           float v[32];
           acc_load<Cfg::kAccPitch>(acc_s, q * 32 + lane, c0, v);
           if (KIND == kKindF16) {
@@ -868,7 +834,7 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
           }
           ptx::fence_proxy_async();
           __syncwarp();
-          if (lane == 0 && !(p.debug_flags & 2)) {
+          if (lane == 0) {
             if (e.out != nullptr) {
               ptx::tma_store_2d(&p.st_out, tb, nb, m0 + q * 32 + split_rows);
             } else {
@@ -892,7 +858,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
                   e.residual + (static_cast<int64_t>(mr) * e.out_row_mul + e.out_row_add) * e.ldr + nb + tc);
           }
         }
-        if (tcount == 0 && ew == 0 && lane == 0 && c0 == 0) stamp(p, 8);
         float v[32];
         acc_load<Cfg::kAccPitch>(acc_s, q * 32 + lane, c0, v);
         if (KIND == kKindF16) {  // undo the power-of-two weight scale (exact)
@@ -939,7 +904,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
           }
         }
 
-        if (tcount == 0 && ew == 0 && lane == 0 && c0 == 0) stamp(p, 9);
         if (full) {
           // ---- coalesced path through the staging tile ----
           if (e.tma_store) {  // an earlier chunk's bulk store may still be reading the tile
@@ -949,7 +913,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
 #pragma unroll
           for (int j = 0; j < 32; ++j) tile[lane * 32 + (j ^ lane)] = v[j];  // column ^ row: conflict-free both ways
           __syncwarp();
-          if (tcount == 0 && ew == 0 && lane == 0 && c0 == 0) stamp(p, 10);
 #pragma unroll
           for (int rr = 0; rr < 8; ++rr) {
             const int r = rr * 4 + tr;
@@ -982,7 +945,6 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
             }
           }
           __syncwarp();
-          if (tcount == 0 && ew == 0 && lane == 0 && c0 == 0) stamp(p, 11);
         } else if (row_ok) {
           // ---- ragged N tail: scalar row-per-thread stores ----
           if (e.out != nullptr) {
@@ -1013,19 +975,14 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
       if constexpr (EPI_ROLE) {  // every chunk has been read out of acc_s
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(&acc_empty);
-        if (ew == 0 && lane == 0 && tcount < 4) stamp(p, 28 + tcount);
       }
-      if (tcount == 0 && ew == 0 && lane == 0) stamp(p, 6);
     }
-    if (ew == 0 && lane == 0) stamp(p, 13);  // this warp's last tile drained
     // outstanding TMA stores of this warp must have finished reading the staging tile before the CTA's shared memory is
     // released; their global writes are ordered before the grid's completion like any other store
     if (lane == 0) ptx::bulk_wait_read_all();
-    if (ew == 0 && lane == 0) stamp(p, 14);
   }
 
   __syncthreads();
-  if (threadIdx.x == 32) stamp(p, 7);
 }
 
 __global__ void split_tf32_kernel(const float* __restrict__ x, float* __restrict__ hi, float* __restrict__ lo,
@@ -1190,8 +1147,7 @@ int make_tmap_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols,
   cuuint32_t estride[2] = {1u, static_cast<cuuint32_t>(row_elem_stride)};
   CUresult r = fn(map, kind == kKindF16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
                   const_cast<void*>(base), gdim, gstride, box, estride,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, kGemmBlockK == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return static_cast<int>(r);
 }

@@ -35,15 +35,10 @@ namespace rohm {
 
 constexpr int kSkinTileBones = 16;  // most distinct bones a 32-vertex column tile may touch (fused skinning epilogue)
 constexpr int kGemmBlockM = 128;
-// K extent of one pipeline stage in fp32 elements: 32 = 128-byte rows (SWIZZLE_128B), 16 = 64-byte rows (SWIZZLE_64B).
-// Both are implemented.  16 is the default: next to the shared-memory accumulator tile (66 KB at BLOCK_N = 128) and the
-// epilogue staging tiles, the 227 KB of an H100 block hold three 32 KB stages of a 128-wide PASSES == 3 tile, where 64 KB
-// stages would leave a single one.
-#ifndef ROHM_GEMM_BLOCK_K
-#define ROHM_GEMM_BLOCK_K 16
-#endif
-constexpr int kGemmBlockK = ROHM_GEMM_BLOCK_K;
-static_assert(kGemmBlockK == 16 || kGemmBlockK == 32, "one 64- or 128-byte swizzle span");
+// K extent of one pipeline stage in fp32 elements: 16 = 64-byte rows (SWIZZLE_64B).  Next to the shared-memory accumulator
+// tile (66 KB at BLOCK_N = 128) and the epilogue staging tiles, the 227 KB of an H100 block hold three 32 KB stages of a
+// 128-wide PASSES == 3 tile, where 128-byte rows (64 KB stages) would leave a single one.
+constexpr int kGemmBlockK = 16;
 constexpr int kMaxSegs = 10;
 
 // Operand element type of a GEMM.  kKindTf32: fp32 containers holding TF32 hi/lo pairs (wgmma .tf32, 8 K-columns
@@ -127,13 +122,6 @@ struct alignas(64) GemmParams {
   const int* skin_nb;
   const int* skin_bone;
   const float* skin_w;
-  // optional: CTA 0 records %globaltimer at milestones into 32 slots (developer instrumentation, see tools/gemm_selftest);
-  // lean variants: slots 16 + i = tile i published by the MMA warpgroups, 20 + i / 24 + i / 28 + i = the epilogue's
-  // prologue done / accumulator observed / tile stored, for the CTA's first four tiles
-  unsigned long long* debug_ts;
-  // developer experiments (tools/gemm_selftest only; results are wrong when set): bit 0 = the epilogue only drains the accumulator (no
-  // staging, no stores), bit 1 = staging writes but no TMA stores.
-  int debug_flags;
   // Split-K (TrajNet convolutions on the deep pyramid levels; masked epilogue variant only): the K iterations of
   // every output tile are cut into `k_splits` contiguous ranges, one work item each, so that a level with 6 to 22 row tiles
   // still fills the SMs with 128-wide tiles.  Split s stores its fp32 partial tile (no bias) at output row
@@ -148,7 +136,7 @@ struct alignas(64) GemmParams {
 
 // Host side ------------------------------------------------------------------------------------
 // Fills a 2-D fp32 tensor map: inner dim `cols` (contiguous), outer dim `rows`, row pitch `ld` elements,
-// box = {kGemmBlockK, box_rows}, SWIZZLE_64B/128B to match, zero OOB fill, optional row traversal stride.
+// box = {gemm_block_k(kind), box_rows}, SWIZZLE_64B, zero OOB fill, optional row traversal stride.
 // Returns 0 on success, a CUresult otherwise.
 int make_tmap_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows,
                  int row_elem_stride = 1, int kind = kKindTf32);

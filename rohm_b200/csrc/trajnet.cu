@@ -196,7 +196,7 @@ enum ConvKind : int {
 };
 
 struct Conv {
-  std::string name;  // for error messages and ROHM_B200_TRAJ_TS
+  std::string name;  // for error messages
   GemmParams g{};
   PackedWeight w;
   float* bias = nullptr;
@@ -210,7 +210,6 @@ struct Conv {
   int64_t split_rows = 0;
   bool sum_after = false;  // no GroupNorm behind it: sum_split_kernel writes `out` right after the GEMM
   int gn_cluster = 1;      // GroupNorm'd: CTAs per (clip, group) of its gn_mish_split_kernel launch (gn_pick_cluster)
-  int ts_runs = 0;         // ROHM_B200_TRAJ_TS: launches outside stream capture so far
 };
 
 struct GroupNorm {
@@ -546,36 +545,8 @@ int make_rtb(rohm_trajnet* tn, Rtb& r, const std::string& p, std::vector<const A
 int run_conv(rohm_trajnet* tn, Conv& cv, int B, cudaStream_t st) {
   const int rows = B * tn->Tp[cv.level_out];
   cv.g.M = rows;
-  // developer instrumentation: ROHM_B200_TRAJ_TS=<conv name>[,<conv name>...] prints CTA 0's %globaltimer stamps of that convolution's third
-  // launch outside stream capture (use with ROHM_B200_GRAPH=0)
-  unsigned long long* d_ts = nullptr;
-  if (const char* want = getenv("ROHM_B200_TRAJ_TS")) {
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cap);
-    const bool listed = ("," + std::string(want) + ",").find("," + cv.name + ",") != std::string::npos;  // comma-separated names
-    if (listed && cap == cudaStreamCaptureStatusNone && ++cv.ts_runs == 3 &&
-        cudaMalloc(&d_ts, 32 * sizeof(unsigned long long)) == cudaSuccess) {
-      cudaMemset(d_ts, 0, 32 * sizeof(unsigned long long));
-      cudaStreamSynchronize(st);
-    }
-  }
-  GemmParams launch_params = cv.g;
-  launch_params.debug_ts = d_ts;
-  ROHM_CUDA(tn->ctx, launch_gemm(launch_params, rows, cv.w.N, cv.w.block_n, tn->passes, st, tn->use_pdl, tn->kind));
+  ROHM_CUDA(tn->ctx, launch_gemm(cv.g, rows, cv.w.N, cv.w.block_n, tn->passes, st, tn->use_pdl, tn->kind));
   tn->launches++;
-  if (d_ts != nullptr) {
-    unsigned long long h[32];
-    cudaStreamSynchronize(st);
-    cudaMemcpy(h, d_ts, sizeof h, cudaMemcpyDeviceToHost);
-    cudaFree(d_ts);
-    int iters = 0;
-    for (int sgi = 0; sgi < cv.g.num_segs; ++sgi) iters += cv.g.seg_kblocks[sgi];
-    fprintf(stderr, "conv %s (rows %d, N %d, block_n %d, %d K blocks, %d splits) CTA0 timeline (ns): setup %llu | first A tma %llu | "
-            "first stage landed %llu | item0 mma issued %llu | item0 acc ready %llu | item0 epilogue done %llu | all mma issued %llu | "
-            "last item drained %llu | stores done %llu | end %llu\n", cv.name.c_str(), rows, cv.w.N, cv.w.block_n, iters, cv.splits,
-            h[1] - h[0], h[2] - h[0], h[3] - h[0], h[4] - h[0], h[5] - h[0], h[6] - h[0], h[12] - h[0], h[13] - h[0], h[14] - h[0],
-            h[7] - h[0]);
-  }
   if (cv.sum_after) {
     const int C = cv.w.N;
     const int64_t total4 = static_cast<int64_t>(rows) * C / 4;

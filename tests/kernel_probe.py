@@ -1,5 +1,6 @@
-"""ctypes driver of tests/native/libkernel_probe.so: the GEMM (rohm_b200/csrc/gemm.cu) and attention (attention.cu) kernels
-launched directly on torch device tensors, plus the operand packing the engines do (not collected by pytest)."""
+"""ctypes driver of tests/native/libkernel_probe.so: the GEMM (rohm_b200/csrc/gemm.cu), attention (attention.cu) and
+GroupNorm + Mish (groupnorm.cu) kernels launched directly on torch device tensors, plus the operand packing the engines do
+(not collected by pytest).  The launching functions take `reps`: that many launches back to back on the default stream."""
 import ctypes as C
 import os
 
@@ -14,7 +15,7 @@ BLOCK_M = 128
 MAX_SEGS = 10
 CUDA_ERROR_INVALID_VALUE = 1
 # attention.cuh AttnKernel
-ATTN_AUTO, ATTN_WGMMA, ATTN_MMA_F16, ATTN_MMA_TF32, ATTN_SIMT = 0, 1, 2, 3, 4
+ATTN_AUTO, ATTN_WGMMA, ATTN_MMA_F16, ATTN_MMA_TF32, ATTN_SIMT, ATTN_WGMMA_STREAM = 0, 1, 2, 3, 4, 5
 
 
 def block_k(kind):
@@ -45,6 +46,14 @@ class Attn(C.Structure):
                 ("kind", C.c_int), ("which", C.c_int), ("pdl", C.c_int)]
 
 
+class GnArgs(C.Structure):  # rohm_b200/csrc/groupnorm.cuh GnArgs
+    _fields_ = [("part", C.c_void_p), ("splits", C.c_int), ("split_stride", C.c_int64), ("bias", C.c_void_p),
+                ("gamma", C.c_void_p), ("beta", C.c_void_p), ("tp", C.c_void_p), ("tp_stride", C.c_int),
+                ("r1", C.c_void_p), ("r2", C.c_void_p), ("out", C.c_void_p), ("out_hi", C.c_void_p),
+                ("out_lo", C.c_void_p), ("C", C.c_int), ("Tp", C.c_int), ("T", C.c_int), ("groups", C.c_int),
+                ("f16", C.c_int)]
+
+
 _lib = None
 
 
@@ -55,10 +64,12 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise FileNotFoundError(f"{LIB_PATH} is missing: run __graft_entry__.build()")
         _lib = C.CDLL(LIB_PATH)
-        _lib.probe_gemm.argtypes = [C.POINTER(Gemm)]
+        _lib.probe_gemm.argtypes = [C.POINTER(Gemm), C.c_int]
         _lib.probe_split.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float]
         _lib.probe_f16_weight_scale.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_float)]
-        _lib.probe_attention.argtypes = [C.POINTER(Attn)]
+        _lib.probe_attention.argtypes = [C.POINTER(Attn), C.c_int]
+        _lib.probe_group_norm.argtypes = [C.POINTER(GnArgs), C.c_int, C.c_int, C.c_int]
+        _lib.probe_group_norm_cluster.argtypes = [C.c_int, C.c_int, C.c_int]
     return _lib
 
 
@@ -134,8 +145,8 @@ def gemm(kind, w, segs, M, N, *, passes=3, m_rows=None, out=None, ldo=None, out_
          bias=None, residual=None, ldr=None, act=ACT_NONE, out_row_mul=1, out_row_add=0, clip_rows=0, clip_valid=0,
          tma_store=False, store_rows=None, k_splits=0, split_row_stride=0,
          a_stats=None, a_corr=None, res_stats=None, res_gamma=None, res_beta=None, stats_out=None, ln_eps=1e-5,
-         pdl=False, n_cols=None):
-    """One launch_gemm; returns (rc, the filled Gemm struct).  segs: list of Seg."""
+         pdl=False, n_cols=None, reps=1):
+    """launch_gemm, `reps` times; returns (rc, the filled Gemm struct).  segs: list of Seg."""
     g = Gemm()
     g.kind, g.passes, g.block_n = kind, passes, w.block_n
     g.m_rows = M if m_rows is None else m_rows
@@ -160,10 +171,26 @@ def gemm(kind, w, segs, M, N, *, passes=3, m_rows=None, out=None, ldo=None, out_
     g.want_tma_store = int(tma_store)
     g.store_rows = store_rows if store_rows is not None else M
     g.pdl = int(pdl)
-    rc = lib().probe_gemm(C.byref(g))
+    rc = lib().probe_gemm(C.byref(g), reps)
     return rc, g
 
 
-def attention(qkv_hi, qkv_lo, ctx_hi, ctx_lo, B, S, D, H, scale, kind, which, pdl=False):
+def attention(qkv_hi, qkv_lo, ctx_hi, ctx_lo, B, S, D, H, scale, kind, which, pdl=False, reps=1):
+    """launch_attention for clips of any length, `reps` times; returns 0 or the error code."""
     a = Attn(_ptr(qkv_hi), _ptr(qkv_lo), qkv_hi.shape[0], _ptr(ctx_hi), _ptr(ctx_lo), B, S, D, H, scale, kind, which, int(pdl))
-    return lib().probe_attention(C.byref(a))
+    return lib().probe_attention(C.byref(a), reps)
+
+
+def group_norm(part, splits, split_stride, bias, gamma, beta, tp, tp_stride, r1, r2, out, out_hi, out_lo, C_, Tp, T, B, n,
+               f16, groups=8, reps=1):
+    """gn_mish_split_kernel over B clips with clusters of n CTAs per (clip, group), `reps` times (tensors or None);
+    returns 0 or the CUDA error code."""
+    p = _ptr
+    a = GnArgs(p(part), splits, split_stride, p(bias), p(gamma), p(beta), p(tp), tp_stride, p(r1), p(r2), p(out), p(out_hi),
+               p(out_lo), C_, Tp, T, groups, int(f16))
+    return lib().probe_group_norm(C.byref(a), B, n, reps)
+
+
+def group_norm_cluster(T, C_, groups=8):
+    """The cluster size the TrajNet engine chooses for groups of T rows of C_ / groups channels."""
+    return lib().probe_group_norm_cluster(T, C_, groups)

@@ -1,13 +1,28 @@
-// Test-only entry points into the GEMM and attention kernels (rohm_b200/csrc/gemm.cu, attention.cu), driven from Python
-// through ctypes by tests/kernel_probe.py.  Every function takes plain structs / device pointers, builds the tensor maps
-// itself with the library's own helpers and returns 0, a cudaError_t (> 0) or -CUresult of a failed tensor-map encoding.
-// The product library (librohm_b200.so, include/rohm_b200.h) exports none of this.
+// Test-only entry points into the GEMM, attention and GroupNorm kernels (rohm_b200/csrc/gemm.cu, attention.cu,
+// groupnorm.cu), driven from Python through ctypes by tests/kernel_probe.py and linked against the product's own objects of
+// those sources.  Every function takes plain structs / device pointers, builds the tensor maps itself with the library's own
+// helpers and returns 0, a cudaError_t (> 0) or -CUresult of a failed tensor-map encoding.  The launching probes run their
+// launch `reps` >= 1 times back to back on the default stream, set-up done once, so that tools can time them.  The product
+// library (librohm_b200.so, include/rohm_b200.h) exports none of this.
 #include <cstdint>
 
 #include "../../rohm_b200/csrc/attention.cuh"
 #include "../../rohm_b200/csrc/gemm.cuh"
+#include "../../rohm_b200/csrc/groupnorm.cuh"
 
 using namespace rohm;
+
+namespace {
+
+// `reps` calls of launch(), stopping at the first error
+template <class F>
+int repeat(int reps, F launch) {
+  cudaError_t rc = cudaSuccess;
+  for (int i = 0; i < reps && rc == cudaSuccess; ++i) rc = launch();
+  return static_cast<int>(rc);
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -60,7 +75,8 @@ struct ProbeGemm {
   int tma_store;
 };
 
-int probe_gemm(ProbeGemm* g) {
+int probe_gemm(ProbeGemm* g, int reps) {
+  if (reps < 1) return static_cast<int>(cudaErrorInvalidValue);
   GemmParams p{};
   for (int s = 0; s < g->num_segs; ++s) {
     const ProbeSeg& sg = g->seg[s];
@@ -90,7 +106,7 @@ int probe_gemm(ProbeGemm* g) {
   p.k_splits = g->k_splits, p.split_row_stride = g->split_row_stride;
   if (g->want_tma_store && (rc = gemm_enable_tma_store(&p, g->store_rows, g->kind)) != 0) return -rc;
   g->tma_store = p.tma_store;
-  return static_cast<int>(launch_gemm(p, g->m_rows, g->n_cols, g->block_n, g->passes, nullptr, g->pdl != 0, g->kind));
+  return repeat(reps, [&] { return launch_gemm(p, g->m_rows, g->n_cols, g->block_n, g->passes, nullptr, g->pdl != 0, g->kind); });
 }
 
 // The library's operand splits: fp32 -> TF32 pair (kind 0) or fp16 pair of x * scale (kind 1).
@@ -117,27 +133,44 @@ struct ProbeAttn {
   int pdl;
 };
 
-int probe_attention(const ProbeAttn* q) {
+// Clips of any length: the shared-memory limits of every attention kernel are raised for S tokens (the SIMT kernel's is
+// capped at what it can serve), and the wgmma tensor maps are built for both wgmma kernels; whatever launch_attention
+// cannot run, it refuses.
+int probe_attention(const ProbeAttn* q, int reps) {
   AttnArgs a{};
   a.qkv_hi = q->qkv_hi, a.qkv_lo = q->qkv_lo, a.rows = q->rows;
   a.ctx_hi = q->ctx_hi, a.ctx_lo = q->ctx_lo;
   a.B = q->B, a.S = q->S, a.D = q->D, a.H = q->H;
   a.scale = q->scale, a.kind = q->kind;
-  if (q->H <= 0 || q->D % q->H != 0) return static_cast<int>(cudaErrorInvalidValue);
+  if (q->H <= 0 || q->D % q->H != 0 || reps < 1) return static_cast<int>(cudaErrorInvalidValue);
   const int dh = q->D / q->H;
-  // the SIMT kernel's shared memory grows with the clip; anything it cannot hold is refused by launch_attention
-  if (attention_smem_bytes(q->S, dh) <= 227 * 1024) {
-    const cudaError_t e = attention_init_attributes(q->S, dh);
-    if (e != cudaSuccess) return static_cast<int>(e);
-  }
+  const cudaError_t e = attention_init_attributes(q->S, dh);
+  if (e != cudaSuccess) return static_cast<int>(e);
   AttnWgmmaMaps maps;
   const AttnWgmmaMaps* wg = nullptr;
-  if (q->kind == kKindF16 && dh == 128 && (q->which == kAttnWgmma || q->which == kAttnAuto)) {
+  if (q->kind == kKindF16 && dh == 128 &&
+      (q->which == kAttnWgmma || q->which == kAttnWgmmaStream || q->which == kAttnAuto)) {
     const int rc = attention_wgmma_maps(&maps, a);
     if (rc != 0) return -rc;
     wg = &maps;
   }
-  return static_cast<int>(launch_attention(a, q->which, wg, nullptr, q->pdl != 0));
+  return repeat(reps, [&] { return launch_attention(a, q->which, wg, nullptr, q->pdl != 0); });
+}
+
+// GroupNorm + Mish over B clips with clusters of n CTAs per (clip, group), the kernel's shared-memory limit raised to the
+// slice first (so n = 1 also runs groups above the default 48 KB).
+int probe_group_norm(const GnArgs* a, int B, int n, int reps) {
+  if (reps < 1 || B < 1) return static_cast<int>(cudaErrorInvalidValue);
+  const cudaError_t e = gn_reserve_smem(gn_slice_bytes(a->T, a->C, a->groups, n));
+  if (e != cudaSuccess) return static_cast<int>(e);
+  return repeat(reps, [&] { return launch_gn_mish(*a, B, n, nullptr, false); });
+}
+
+// The cluster size rohm_trajnet_create chooses for a (clip, group) of T rows of C / groups channels; 0 on error.
+int probe_group_norm_cluster(int T, int C, int groups) {
+  size_t budget = 0, max_budget = 0;
+  if (gn_smem_budgets(&budget, &max_budget) != cudaSuccess) return 0;
+  return gn_pick_cluster(T, C, groups, budget);
 }
 
 }  // extern "C"

@@ -109,7 +109,9 @@ LINEAR_CASES = [
     (TF32, 3, 32, 34, 13, 40),
     (TF32, 3, 64, 129, 100, 5120),
     (TF32, 3, 128, 18560, 256, 512),
+    (TF32, 3, 128, 4640, 1536, 512),
     (TF32, 1, 128, 4640, 512, 512),
+    (TF32, 1, 96, 300, 272, 294),
     (TF32, 1, 64, 127, 272, 294),
     (TF32, 1, 32, 1, 13, 40),
 ]
@@ -352,7 +354,7 @@ def test_split_k_refusals_launch_nothing(dev, kind):
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("M", [34, 128, 1000, 4640])
+@pytest.mark.parametrize("M", [34, 128, 1000, 4640, 18560])
 def test_layernorm_folding_chain(dev, M):
     """(A) producer u1 = R + A1 W1^T + b1 in place over the residual pair, with per-row partial statistics;
     (B) consumer y = LN(u1) W2^T + b2 through gamma-folded weights and the epilogue correction;

@@ -20,7 +20,6 @@ import pytest
 import torch
 
 import kernel_probe as kp
-import long_clip_probe as lp
 from helpers import NoiseTape, TOL
 from oracle import diffusion_oracle as do
 from oracle import kinematics_oracle as ko
@@ -28,7 +27,7 @@ from oracle import pipeline_oracle, posenet_oracle
 from rohm_b200 import _lib, diffusion, synthetic
 from rohm_b200._lib import RohmB200Error
 from rohm_b200.posenet import PoseNet
-from test_gpu_attention import B, D, POISONED, REGIMES, SENTINEL, _qkv, _split_ok
+from test_gpu_attention import B, D, POISONED, REGIMES, SENTINEL, _launch, _split_ok
 
 pytestmark = pytest.mark.gpu
 
@@ -42,37 +41,7 @@ SAMPLED_FROM = 1000  # from this clip length on, the float64 reference covers sa
 @pytest.fixture(scope="module")
 def dev(cuda_device):
     kp.lib()  # a missing probe library fails every test of the module
-    lp.lib()
     return cuda_device
-
-
-def _launch(dev, which, kind, S, dh, regime, seed):
-    """test_gpu_attention's launch (poisoned clips 1 and 3, NaN past B * S, sentinel context) through the long-clip
-    probe -> (rc, hi + lo values of Q|K|V, ctx_hi, ctx_lo, scale)."""
-    H = D // dh
-    q, k, v, scale = _qkv(S, dh, regime, seed)
-    rows = B * S + 37
-    qkv = torch.full((rows, 3 * D), float("nan"))
-    qkv[:B * S] = torch.cat([t.reshape(B * S, D) for t in (q, k, v)], dim=1)
-    for b in POISONED:
-        qkv[b * S:(b + 1) * S] = float("nan")
-    qkv = qkv.to(dev)
-    if kind == F16:
-        hi, lo = kp.split(F16, qkv)
-        planes = torch.stack([hi, lo])  # one buffer, as the engine keeps them
-        planes[:, B * S:] = float("nan")
-        for b in POISONED:
-            planes[:, b * S:(b + 1) * S] = float("nan")
-        qkv_hi, qkv_lo = planes[0], planes[1]
-        value = kp.pair_value(qkv_hi, qkv_lo)
-        cdt = torch.float16
-    else:
-        qkv_hi, qkv_lo, value, cdt = qkv, None, qkv.double(), torch.float32
-    ctx_hi = torch.full((rows, D), SENTINEL, dtype=cdt, device=dev)
-    ctx_lo = torch.full((rows, D), SENTINEL, dtype=cdt, device=dev)
-    rc = lp.attention(qkv_hi, qkv_lo, ctx_hi, ctx_lo, B, S, D, H, scale, kind, which)
-    torch.cuda.synchronize()
-    return rc, value, ctx_hi, ctx_lo, scale
 
 
 def _query_rows(S, seed):
@@ -102,7 +71,7 @@ def _reference_rows(value, S, scale, rows):
 
 def _check_stream(dev, S, regime):
     seed = 1000 * S + DH + REGIMES.index(regime)
-    rc, value, ctx_hi, ctx_lo, scale = _launch(dev, lp.ATTN_WGMMA_STREAM, F16, S, DH, regime, seed)
+    rc, value, ctx_hi, ctx_lo, scale = _launch(dev, kp.ATTN_WGMMA_STREAM, F16, S, DH, regime, seed)
     assert rc == 0, (S, rc)
     assert bool((ctx_hi[B * S:] == SENTINEL).all()) and bool((ctx_lo[B * S:] == SENTINEL).all()), "wrote past B * S"
     got = kp.pair_value(ctx_hi, ctx_lo)[:B * S].reshape(B, S, D)
@@ -126,7 +95,7 @@ def test_streaming_kernel_against_float64(dev, regime):
 
 def test_automatic_choice_on_fp16_pairs_of_head_dim_128(dev):
     """kAttnAuto: the streaming kernel above 160 tokens, the 160-key wgmma kernel at 160 or fewer (bit for bit)."""
-    for S, forced in ((161, lp.ATTN_WGMMA_STREAM), (1000, lp.ATTN_WGMMA_STREAM), (145, kp.ATTN_WGMMA)):
+    for S, forced in ((161, kp.ATTN_WGMMA_STREAM), (1000, kp.ATTN_WGMMA_STREAM), (145, kp.ATTN_WGMMA)):
         outs = []
         for which in (kp.ATTN_AUTO, forced):
             rc, _, hi, lo, _ = _launch(dev, which, F16, S, DH, "flat", 19)
@@ -138,7 +107,7 @@ def test_automatic_choice_on_fp16_pairs_of_head_dim_128(dev):
 def test_streaming_kernel_outside_its_domain_is_refused(dev):
     """TF32 Q|K|V or head dim 64: cudaErrorInvalidValue before any launch, the context buffer untouched."""
     for kind, dh, S in ((TF32, 128, 200), (TF32, 128, 1000), (F16, 64, 200), (F16, 64, 1000)):
-        rc, _, ctx_hi, ctx_lo, _ = _launch(dev, lp.ATTN_WGMMA_STREAM, kind, S, dh, "flat", 5)
+        rc, _, ctx_hi, ctx_lo, _ = _launch(dev, kp.ATTN_WGMMA_STREAM, kind, S, dh, "flat", 5)
         assert rc == kp.CUDA_ERROR_INVALID_VALUE, (kind, dh, S, rc)
         assert bool((ctx_hi == SENTINEL).all()) and bool((ctx_lo == SENTINEL).all())
 

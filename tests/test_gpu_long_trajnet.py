@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 import torch
 
-import group_norm_probe as gp
+import kernel_probe as kp
 from helpers import NoiseTape, TOL
 from oracle import diffusion_oracle as do
 from oracle import glue_oracle as go
@@ -95,7 +95,7 @@ def _gn_run(case, n, reps=1):
     out = torch.full((c["rows"] * c["C"] + extra,), SENTINEL, device=dev)
     hi = torch.full((c["rows"] * c["C"] + extra,), SENTINEL, device=dev, dtype=c["pair_dtype"])
     lo = torch.full_like(hi, SENTINEL)
-    rc = gp.group_norm(c["part"], c["splits"], c["rows"] * c["C"], c["bias"], c["gamma"], c["beta"], c["tp"],
+    rc = kp.group_norm(c["part"], c["splits"], c["rows"] * c["C"], c["bias"], c["gamma"], c["beta"], c["tp"],
                        c["C"] + 4, c["r1"], c["r2"], out, hi, lo, c["C"], c["Tp"], c["TL"], c["B"], n, c["f16"], reps=reps)
     torch.cuda.synchronize()
     assert rc == 0, rc

@@ -6,7 +6,7 @@ Prints the card and its power limit, then
   * per clip length T: B ~ 4640 / (T + 1) clips (about the token count of the benchmark's 32 x 145), the forward graph's
     time (CUDA events over --iters replays), the attention share of one event-timed forward (engine.profile) and the
     attention rate, counting 4 S^2 D flops per clip and layer (S = T + 1);
-  * kernel against kernel through the long-clip test probe (tests/native_long/liblong_clip_probe.so), CUDA events around --reps
+  * kernel against kernel through the kernel test probe (tests/native/libkernel_probe.so), CUDA events around --reps
     back-to-back launches: the SIMT kernel against the streaming wgmma kernel where both run (161 - 212 tokens), and the
     streaming kernel against the 160-key wgmma kernel where that one runs (<= 160 tokens).
 Needs an H100; writes nothing unless --json is given."""
@@ -85,8 +85,7 @@ def clip_lengths(dev, iters):
 
 def kernels(dev, reps):
     import kernel_probe as kp
-    import long_clip_probe as lp
-    ids = {"simt": kp.ATTN_SIMT, "stream": lp.ATTN_WGMMA_STREAM, "wgmma": kp.ATTN_WGMMA}
+    ids = {"simt": kp.ATTN_SIMT, "stream": kp.ATTN_WGMMA_STREAM, "wgmma": kp.ATTN_WGMMA}
     rows = []
     for first, second, lengths in KERNEL_PAIRS:
         for S in lengths:
@@ -99,7 +98,7 @@ def kernels(dev, reps):
             scale = 1.0 / math.sqrt(D // H)
             r = {"S": S, "B": B}
             for name in (first, second):
-                call = lambda n=reps: lp.attention(hi, lo, ctx_hi, ctx_lo, B, S, D, H, scale, kp.KIND_F16, ids[name], reps=n)
+                call = lambda n=reps: kp.attention(hi, lo, ctx_hi, ctx_lo, B, S, D, H, scale, kp.KIND_F16, ids[name], reps=n)
                 assert call(5) == 0, (name, S)
                 torch.cuda.synchronize()
                 r[name + "_us"] = time_ms(call, 1) / reps * 1e3

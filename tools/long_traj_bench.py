@@ -7,7 +7,7 @@ Prints the card and its power limit, then
     time of TrajNet and of TrajNet+TrajControl (CUDA events over --iters replays), and the GroupNorm kernel's share of
     one forward from a separate torch.profiler run with graphs off;
   * the GroupNorm kernel alone at 1 clip x 4992 frames on the widest level (64 channels, 8 groups of 8, one partial plus
-    the time projection) through the GroupNorm test probe (tests/native_groupnorm/libgroup_norm_probe.so), CUDA events
+    the time projection) through the kernel test probe (tests/native/libkernel_probe.so), CUDA events
     around --reps back-to-back launches: one CTA per group (the shared-memory attribute raised), the size the engine chooses,
     and clusters of 8;
   * one 2-round pipeline.run_rounds at 1 clip x 4993 raw frames (TrajNet 4992 frames, 100 steps; PoseNet 4991 frames,
@@ -111,7 +111,7 @@ def clip_lengths(dev, iters):
 
 
 def group_norm_kernel(dev, reps):
-    import group_norm_probe as gp
+    import kernel_probe as kp
     B, G = 1, 8
     Tp = GN_T + 32
     rows = B * Tp
@@ -121,10 +121,10 @@ def group_norm_kernel(dev, reps):
     hi = torch.empty(rows * GN_C, device=dev, dtype=torch.float16)
     lo = torch.empty_like(hi)
     slice_bytes = lambda n: -(-GN_T // n) * (GN_C // G) * 4
-    chosen = gp.group_norm_cluster(GN_T, GN_C, G)
+    chosen = kp.group_norm_cluster(GN_T, GN_C, G)
     res = []
     for label, n in (("one CTA per group", 1), ("chosen", chosen), ("clusters of 8", 8)):
-        call = lambda k=reps: gp.group_norm(part, 1, rows * GN_C, bias, gamma, beta, tp, GN_C, None, None, None, hi, lo,
+        call = lambda k=reps: kp.group_norm(part, 1, rows * GN_C, bias, gamma, beta, tp, GN_C, None, None, None, hi, lo,
                                             GN_C, Tp, GN_T, B, n, 1, reps=k)
         assert call(5) == 0, n
         torch.cuda.synchronize()
