@@ -148,6 +148,14 @@ ROHM_API void rohm_posenet_destroy(rohm_posenet* pn);
  * cond: [B, in_feats, 1, T] contiguous.  Must be called whenever batch['cond'], B or T change. */
 ROHM_API int rohm_posenet_set_cond(rohm_posenet* pn, const float* cond, int B, int T, void* stream);
 
+/* Per-clip lengths for the following set_cond, forward, sample_step and profile calls: clip b of the padded
+ * [B, in_feats, 1, T] tensors has lengths_host[b] real frames, 1 <= lengths_host[b] <= T.  Frames [0, lengths[b]) of the
+ * output equal a forward of that clip alone as a [1, in_feats, 1, lengths[b]] batch, bit for bit; frames past it are zero,
+ * and the input values there are never read.  Inside, the clips' tokens are packed with no padding rows, so a batch of
+ * mixed lengths does no wasted tensor work.  NULL returns to uniform clips of T frames.  Precision f16x2 with head dim 128
+ * only (else ROHM_ERR_INVALID).  Changing the lengths waits for the device to go idle; call set_cond again afterwards. */
+ROHM_API int rohm_posenet_set_lengths(rohm_posenet* pn, const int* lengths_host, int B);
+
 /* PoseNet.forward (posenet.py:75-96).  x_t: [B, in_feats, 1, T]; timesteps: int64 [B] (original, un-respaced);
  * out: [B, in_feats, 1, T] with channels [0, traj_feats) copied from the cond given to set_cond. */
 ROHM_API int rohm_posenet_forward(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* out, int B, int T,
@@ -261,6 +269,12 @@ ROHM_API int rohm_body_from_repr_layout(rohm_body* bd, const float* x, int chann
  * loss_out: optional device float[4] = {sum_abs, count_abs, sum_smpl, count_smpl}. */
 ROHM_API int rohm_skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, int B, int T,
                                    float* grad, float* loss_out, void* stream);
+
+/* rohm_skating_guidance over clips of lengths[b] real frames (device int[B], 1 <= lengths[b] <= T): frames at or past
+ * lengths[b] add nothing to the sums or counts and get a zero gradient, a velocity pair (t, t + 1) counts only when
+ * t + 1 < lengths[b], and their values are never used.  The normalisers stay batch-wide over the real frames. */
+ROHM_API int rohm_skating_guidance_lengths(rohm_body* bd, const float* x0, const float* mean, const float* stdv,
+                                           const int* lengths, int B, int T, float* grad, float* loss_out, void* stream);
 
 /* rohm_skating_guidance in two halves, for clip-sharded runs that reproduce the reference's BATCH-GLOBAL normalisers
  * (posenet.py:230-233, 242-248): _sums computes this shard's {sum_abs, count_abs, sum_smpl, count_smpl} into sums_out (device

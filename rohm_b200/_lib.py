@@ -50,6 +50,7 @@ SIGNATURES = {
     "rohm_posenet_create": (_i, [_p, C.POINTER(PoseNetW), _i, _i, _i, C.POINTER(_p)]),
     "rohm_posenet_destroy": (None, [_p]),
     "rohm_posenet_set_cond": (_i, [_p, _p, _i, _i, _p]),
+    "rohm_posenet_set_lengths": (_i, [_p, C.POINTER(_i), _i]),
     "rohm_posenet_forward": (_i, [_p, _p, _p, _p, _i, _i, _p]),
     "rohm_posenet_sample_step": (_i, [_p, _p, _p, _p, _p, _p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), _i, _i, _p]),
     "rohm_posenet_profile": (_i, [_p, _p, _p, _p, _i, _i, _p, C.POINTER(C.c_float), C.POINTER(C.c_int)]),
@@ -71,6 +72,7 @@ SIGNATURES = {
     "rohm_body_from_repr": (_i, [_p, _p, _p, _p, _i, _i, _p, _i, _p, _p]),
     "rohm_body_from_repr_layout": (_i, [_p, _p, _i, _p, _p, _i, _i, _p, _i, _p, _p]),
     "rohm_skating_guidance": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p]),
+    "rohm_skating_guidance_lengths": (_i, [_p, _p, _p, _p, _p, _i, _i, _p, _p, _p]),
     "rohm_skating_guidance_sums": (_i, [_p, _p, _p, _p, _i, _i, _p, _p]),
     "rohm_skating_guidance_backward": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p]),
     "rohm_projection_guidance": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _i, _p, _p, _p]),

@@ -107,13 +107,20 @@ class BodyKernels:
         joints = joints.reshape(B, T, num_joints, 3)
         return (joints, verts.reshape(B, T, self.V, 3)) if want_vertices else joints
 
-    def skating_guidance(self, x0, mean, std, want_loss=False):
+    def skating_guidance(self, x0, mean, std, want_loss=False, lengths=None):
+        """lengths: optional int32 device tensor [B] of real frames per clip (rohm_skating_guidance_lengths)."""
         B, _, _, T = x0.shape
         grad = torch.empty_like(x0)
         loss = torch.empty(4, device=self.device) if want_loss else None
-        rc = self.lib.rohm_skating_guidance(self.handle, C.c_void_p(x0.data_ptr()), C.c_void_p(mean.data_ptr()),
-                                            C.c_void_p(std.data_ptr()), B, T, C.c_void_p(grad.data_ptr()),
-                                            C.c_void_p(loss.data_ptr() if loss is not None else 0), self._stream())
+        loss_p = C.c_void_p(loss.data_ptr() if loss is not None else 0)
+        if lengths is not None:
+            rc = self.lib.rohm_skating_guidance_lengths(self.handle, C.c_void_p(x0.data_ptr()), C.c_void_p(mean.data_ptr()),
+                                                        C.c_void_p(std.data_ptr()), C.c_void_p(lengths.data_ptr()), B, T,
+                                                        C.c_void_p(grad.data_ptr()), loss_p, self._stream())
+        else:
+            rc = self.lib.rohm_skating_guidance(self.handle, C.c_void_p(x0.data_ptr()), C.c_void_p(mean.data_ptr()),
+                                                C.c_void_p(std.data_ptr()), B, T, C.c_void_p(grad.data_ptr()), loss_p,
+                                                self._stream())
         _lib.check(rc, self.ctx)
         return (grad, loss) if want_loss else grad
 

@@ -586,6 +586,8 @@ struct AttnWgParams {
   __half* ctx_lo;
   int S, D, H;
   float scale;
+  const int* clip_off;  // packed clips (AttnArgs::clip_off / clip_ids), or null
+  const int* clip_ids;
 };
 constexpr int kAwKeys = 160;                 // padded key count = N of the S product
 constexpr int kAwQRows = 64;                 // queries per CTA = M of one wgmma
@@ -601,12 +603,18 @@ __global__ void __launch_bounds__(128, 1) attention_wgmma_kernel(const __grid_co
   uint8_t* const Qb = sm;                   // [plane][chunk]
   uint8_t* const Kb = sm + 4 * kAwQBuf;     // [plane][chunk]
   uint8_t* const Vb = Kb + 4 * kAwKBuf;     // [plane][chunk]
-  const int S = p.S;
-  const int qtiles = (S + kAwQRows - 1) / kAwQRows;
+  const int qtiles = (p.S + kAwQRows - 1) / kAwQRows;
   const int qt = static_cast<int>(blockIdx.x) % qtiles;
   const int bh = static_cast<int>(blockIdx.x) / qtiles;
   const int h = bh % p.H, b = bh / p.H;
-  const int row0 = b * S, q0 = qt * kAwQRows;
+  const int q0 = qt * kAwQRows;
+  int S = p.S, row0 = b * p.S;
+  if (p.clip_off != nullptr) {  // packed clips: the grid's clip b is clip_ids[b]; tiles past a shorter clip have no work
+    const int c = p.clip_ids[b];
+    row0 = p.clip_off[c];
+    S = p.clip_off[c + 1] - row0;
+    if (q0 >= S) return;
+  }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&p.q_hi);
@@ -775,6 +783,8 @@ struct AttnStreamParams {
   __half* ctx_lo;
   int S, D, H;
   float scale;
+  const int* clip_off;  // packed clips (AttnArgs::clip_off / clip_ids), or null
+  const int* clip_ids;
 };
 constexpr int kAsBlock = 64;                  // keys per block = queries per CTA
 constexpr int kAsBuf = kAsBlock * 128;        // bytes of one {plane, 64-wide head-dim chunk} tile
@@ -790,12 +800,19 @@ __global__ void __launch_bounds__(128, 1) attention_wgmma_stream_kernel(const __
   uint8_t* const Qb = sm;                             // [plane][chunk]
   uint8_t* const Kb = sm + kAsTile;                   // [stage][plane][chunk]
   uint8_t* const Vb = Kb + kAsStages * kAsTile;       // [stage][plane][chunk]
-  const int S = p.S;
-  const int nblk = (S + kAsBlock - 1) / kAsBlock;     // key blocks = query tiles
-  const int qt = static_cast<int>(blockIdx.x) % nblk;
-  const int bh = static_cast<int>(blockIdx.x) / nblk;
+  const int qtiles = (p.S + kAsBlock - 1) / kAsBlock;
+  const int qt = static_cast<int>(blockIdx.x) % qtiles;
+  const int bh = static_cast<int>(blockIdx.x) / qtiles;
   const int h = bh % p.H, b = bh / p.H;
-  const int row0 = b * S, q0 = qt * kAsBlock;
+  const int q0 = qt * kAsBlock;
+  int S = p.S, row0 = b * p.S;
+  if (p.clip_off != nullptr) {  // packed clips: the grid's clip b is clip_ids[b]; tiles past a shorter clip have no work
+    const int c = p.clip_ids[b];
+    row0 = p.clip_off[c];
+    S = p.clip_off[c + 1] - row0;
+    if (q0 >= S) return;
+  }
+  const int nblk = (S + kAsBlock - 1) / kAsBlock;     // key blocks of the clip, counted from its first token
   const int kcol = p.D + h * 128, vcol = 2 * p.D + h * 128;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -1047,8 +1064,10 @@ cudaError_t attention_init_attributes(int max_tokens, int dh) {
 }
 
 cudaError_t launch_attention(const AttnArgs& a, int which, const AttnWgmmaMaps* wg, cudaStream_t st, bool pdl) {
-  if (a.B <= 0 || a.S <= 0 || a.H <= 0 || a.D % a.H != 0 || static_cast<int64_t>(a.B) * a.S > a.rows)
+  const bool packed = a.clip_off != nullptr;
+  if (a.B <= 0 || a.S <= 0 || a.H <= 0 || a.D % a.H != 0 || (packed ? a.S > a.rows : static_cast<int64_t>(a.B) * a.S > a.rows))
     return cudaErrorInvalidValue;
+  if (packed && (a.clip_ids == nullptr || which == kAttnAuto)) return cudaErrorInvalidValue;
   const int dh = a.D / a.H;
   if (dh != 64 && dh != 128) return cudaErrorInvalidValue;
   const bool f16 = a.kind == kKindF16;
@@ -1064,6 +1083,7 @@ cudaError_t launch_attention(const AttnArgs& a, int which, const AttnWgmmaMaps* 
     prm.hi = wg->q_hi, prm.lo = wg->q_lo;
     prm.ctx_hi = static_cast<__half*>(a.ctx_hi), prm.ctx_lo = static_cast<__half*>(a.ctx_lo);
     prm.S = S, prm.D = a.D, prm.H = a.H, prm.scale = a.scale;
+    prm.clip_off = a.clip_off, prm.clip_ids = a.clip_ids;
     const int qtiles = (S + kAsBlock - 1) / kAsBlock;
     return launch_chain(attention_wgmma_stream_kernel, dim3(a.B * a.H * qtiles), dim3(128), kAsSmemBytes, st, pdl, prm);
   }
@@ -1073,9 +1093,11 @@ cudaError_t launch_attention(const AttnArgs& a, int which, const AttnWgmmaMaps* 
     prm.q_hi = wg->q_hi, prm.q_lo = wg->q_lo, prm.kv_hi = wg->kv_hi, prm.kv_lo = wg->kv_lo;
     prm.ctx_hi = static_cast<__half*>(a.ctx_hi), prm.ctx_lo = static_cast<__half*>(a.ctx_lo);
     prm.S = S, prm.D = a.D, prm.H = a.H, prm.scale = a.scale;
+    prm.clip_off = a.clip_off, prm.clip_ids = a.clip_ids;
     const int qtiles = (S + kAwQRows - 1) / kAwQRows;
     return launch_chain(attention_wgmma_kernel, dim3(a.B * a.H * qtiles), dim3(128), kAwSmemBytes, st, pdl, prm);
   }
+  if (packed) return cudaErrorInvalidValue;  // packed clips run on the wgmma kernels only
   if (which == kAttnMmaF16) {
     if (!f16 || !mma_ok) return cudaErrorInvalidValue;
     const int nk = (S + 15) / 16;

@@ -40,6 +40,11 @@ struct AttnArgs {
   int B, S, D, H;
   float scale;  // usually 1 / sqrt(D / H)
   int kind;     // GemmKind of the planes
+  // Packed clips (optional, device arrays, wgmma kernels only): clip c holds rows [clip_off[c], clip_off[c + 1]) of the
+  // planes, and the launch runs the B clips listed in clip_ids, S being the most tokens among them.  Null: clip b holds
+  // rows [b S, b S + S).
+  const int* clip_off = nullptr;
+  const int* clip_ids = nullptr;
 };
 
 // Encodes the wgmma kernels' tensor maps over the planes of a.  Returns 0 or a CUresult.
@@ -48,7 +53,8 @@ int attention_wgmma_maps(AttnWgmmaMaps* maps, const AttnArgs& a);
 // Launches one attention.  kAttnAuto picks the kernel the PoseNet engine uses: with `wg` given on fp16 pairs of head
 // dim 128, the wgmma kernel up to 160 tokens and the streaming wgmma kernel above; otherwise the mma.sync kernel of the
 // kind up to 160 tokens, else the SIMT kernel.  A forced kernel that cannot run the launch (kind, head dim, token count,
-// missing maps) is refused with cudaErrorInvalidValue before anything is launched.
+// missing maps) is refused with cudaErrorInvalidValue before anything is launched.  Packed clips need a forced wgmma kernel:
+// each clip runs with the block decomposition it would get alone, on the kernel the caller chose for the listed clips.
 cudaError_t launch_attention(const AttnArgs& a, int which, const AttnWgmmaMaps* wg, cudaStream_t stream, bool pdl);
 
 // Raises the dynamic shared-memory limit of every attention kernel; the SIMT kernel's for clips of up to max_tokens

@@ -484,14 +484,18 @@ __global__ void __launch_bounds__(128) guide_forward_kernel(const float* __restr
   }
 }
 
-// pass 2: foot speeds, masks, loss sums, and dL/dposition directions
+// pass 2: foot speeds, masks, loss sums, and dL/dposition directions.  kMasked: clip b has lengths[b] real frames (device
+// int[B]); a velocity pair counts only inside them, so later frames add nothing and get no direction.
+template <bool kMasked>
 __global__ void __launch_bounds__(128) guide_loss_kernel(const float* __restrict__ x, const float* __restrict__ mean,
-                                                         const float* __restrict__ stdv, int B, int T, GuideWs ws) {
+                                                         const float* __restrict__ stdv, int B, int T, GuideWs ws,
+                                                         const int* __restrict__ lengths) {
   const int64_t f = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const int64_t frames = static_cast<int64_t>(B) * T;
   float lsum[2] = {0.f, 0.f}, lcnt[2] = {0.f, 0.f};
   if (f < frames) {
     const int b = static_cast<int>(f / T), t = static_cast<int>(f % T);
+    const int len = kMasked ? lengths[b] : T;
 #pragma unroll
     for (int path = 0; path < 2; ++path) {
 #pragma unroll
@@ -499,7 +503,7 @@ __global__ void __launch_bounds__(128) guide_loss_kernel(const float* __restrict
         // gradient on p(t) = +m(t-1) vhat(t-1) - m(t) vhat(t), each scaled by fps (d|v|/dp)
         V3 g = {0.f, 0.f, 0.f};
         const float* p0 = ws.foot + ((path * frames + f) * 4 + k) * 3;
-        if (t + 1 < T) {
+        if (t + 1 < len) {
           const float* p1 = p0 + 12;
           const V3 v = {(p1[0] - p0[0]) * 30.0f, (p1[1] - p0[1]) * 30.0f, (p1[2] - p0[2]) * 30.0f};
           const float sp = sqrtf(dot(v, v));
@@ -509,7 +513,7 @@ __global__ void __launch_bounds__(128) guide_loss_kernel(const float* __restrict
             g = g - (30.0f / sp) * v;
           }
         }
-        if (t > 0) {
+        if (t > 0 && (!kMasked || t < len)) {
           const float* pm = p0 - 12;
           const V3 v = {(p0[0] - pm[0]) * 30.0f, (p0[1] - pm[1]) * 30.0f, (p0[2] - pm[2]) * 30.0f};
           const float sp = sqrtf(dot(v, v));
@@ -538,11 +542,12 @@ __global__ void __launch_bounds__(128) guide_loss_kernel(const float* __restrict
 __global__ void __launch_bounds__(128) guide_backward_kernel(const float* __restrict__ x, const float* __restrict__ mean,
                                                              const float* __restrict__ stdv, const float* __restrict__ Jt,
                                                              const float* __restrict__ Jd, int B, int T, GuideWs ws,
-                                                             float* __restrict__ grad) {
+                                                             float* __restrict__ grad, const int* __restrict__ lengths) {
   const int64_t f = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const int64_t frames = static_cast<int64_t>(B) * T;
   if (f >= frames) return;
   const int b = static_cast<int>(f / T), t = static_cast<int>(f % T);
+  if (lengths != nullptr && t >= lengths[b]) return;  // past the clip: the cleared zero gradient
   auto ch = [&](int c) { return ld_ch(x, mean, stdv, b, t, T, c); };
   auto put = [&](int c, float g) { grad[(static_cast<int64_t>(b) * kC + c) * T + t] = g * stdv[c]; };
   const float cnt_abs = ws.sums[1], cnt_smpl = ws.sums[3];
@@ -999,7 +1004,7 @@ extern "C" int rohm_skating_guidance_sums(rohm_body* bd, const float* x0, const 
   ROHM_CUDA(ctx, cudaMemsetAsync(sums_out, 0, 4 * sizeof(float), st));
   const unsigned blocks = static_cast<unsigned>((N + 127) / 128);
   guide_forward_kernel<<<blocks, 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws);
-  guide_loss_kernel<<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws);
+  guide_loss_kernel<false><<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws, nullptr);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }
@@ -1015,30 +1020,43 @@ extern "C" int rohm_skating_guidance_backward(rohm_body* bd, const float* x0, co
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   GuideWs ws{bd->foot, bd->gdir, const_cast<float*>(sums)};
   ROHM_CUDA(ctx, cudaMemsetAsync(grad, 0, sizeof(float) * N * kC, st));
-  guide_backward_kernel<<<static_cast<unsigned>((N + 127) / 128), 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws, grad);
+  guide_backward_kernel<<<static_cast<unsigned>((N + 127) / 128), 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws, grad,
+                                                                               nullptr);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }
 
-extern "C" int rohm_skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, int B, int T,
-                                     float* grad, float* loss_out, void* stream) {
+static int skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, const int* lengths, int B,
+                            int T, float* grad, float* loss_out, void* stream, const char* fn) {
   if (bd == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = bd->ctx;
   rohm::DeviceGuard device_guard__(ctx);
   const int64_t N = static_cast<int64_t>(B) * T;
   if (!x0 || !mean || !stdv || !grad || B <= 0 || T <= 0 || N > bd->max_frames)
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_skating_guidance: bad arguments (B*T=%lld, capacity %lld)",
-                static_cast<long long>(N), static_cast<long long>(bd->max_frames));
+    return fail(ctx, ROHM_ERR_INVALID, "%s: bad arguments (B*T=%lld, capacity %lld)", fn, static_cast<long long>(N),
+                static_cast<long long>(bd->max_frames));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   GuideWs ws{bd->foot, bd->gdir, bd->sums};
   ROHM_CUDA(ctx, cudaMemsetAsync(bd->sums, 0, 4 * sizeof(float), st));
   ROHM_CUDA(ctx, cudaMemsetAsync(grad, 0, sizeof(float) * N * kC, st));
   const unsigned blocks = static_cast<unsigned>((N + 127) / 128);
   guide_forward_kernel<<<blocks, 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws);
-  guide_loss_kernel<<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws);
-  guide_backward_kernel<<<blocks, 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws, grad);
+  if (lengths != nullptr) guide_loss_kernel<true><<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws, lengths);
+  else guide_loss_kernel<false><<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws, nullptr);
+  guide_backward_kernel<<<blocks, 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws, grad, lengths);
   ROHM_CUDA(ctx, cudaGetLastError());
   if (loss_out != nullptr)
     ROHM_CUDA(ctx, cudaMemcpyAsync(loss_out, bd->sums, 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return ROHM_OK;
+}
+
+extern "C" int rohm_skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, int B, int T,
+                                     float* grad, float* loss_out, void* stream) {
+  return skating_guidance(bd, x0, mean, stdv, nullptr, B, T, grad, loss_out, stream, "rohm_skating_guidance");
+}
+
+extern "C" int rohm_skating_guidance_lengths(rohm_body* bd, const float* x0, const float* mean, const float* stdv,
+                                             const int* lengths, int B, int T, float* grad, float* loss_out, void* stream) {
+  if (bd != nullptr && lengths == nullptr) return fail(bd->ctx, ROHM_ERR_INVALID, "rohm_skating_guidance_lengths: null lengths");
+  return skating_guidance(bd, x0, mean, stdv, lengths, B, T, grad, loss_out, stream, "rohm_skating_guidance_lengths");
 }

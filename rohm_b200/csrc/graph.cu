@@ -19,17 +19,19 @@ ForwardGraphs::~ForwardGraphs() {
 }
 
 int ForwardGraphs::run(rohm_ctx* ctx, int B, int T, bool with_step, bool eager, cudaStream_t st,
-                       const std::function<int(cudaStream_t)>& launches, const std::vector<KernelPatch>& patches) {
+                       const std::function<int(cudaStream_t)>& launches, const std::vector<KernelPatch>& patches,
+                       const std::vector<int>& lengths) {
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   ROHM_CUDA(ctx, cudaStreamIsCapturing(st, &cap));
   if (eager || !enabled || cap != cudaStreamCaptureStatusNone) return launches(st);
 
   Entry* g = nullptr;
   for (Entry& e : graphs_)
-    if (e.B == B && e.T == T && e.with_step == with_step) g = &e;
+    if (e.B == B && e.T == T && e.with_step == with_step && e.lengths == lengths) g = &e;
   if (g == nullptr) {
     Entry e;
     e.B = B, e.T = T, e.with_step = with_step;
+    e.lengths = lengths;
     const int rc = capture(ctx, launches, patches, &e);
     if (rc != ROHM_OK) return rc;
     if (graphs_.size() >= kMaxGraphs) graphs_.erase(graphs_.begin());

@@ -60,7 +60,7 @@ class KernelPatch {
   int n_ = 0;
 };
 
-// An engine's captured forwards, keyed by (B, T, with_step); at most kMaxGraphs, the oldest evicted first.
+// An engine's captured forwards, keyed by (B, T, with_step, per-clip lengths); at most kMaxGraphs, the oldest evicted first.
 class ForwardGraphs {
  public:
   static constexpr size_t kMaxGraphs = 8;
@@ -74,9 +74,11 @@ class ForwardGraphs {
   // Issues one forward on `st`.  launches(stream) issues its kernels on `stream`.  That runs directly on `st` when `eager`,
   // when graphs are off, or when the caller is capturing `st`.  Otherwise the graph of (B, T, with_step) is replayed with
   // the arguments of `patches` set; launches() is captured into it on first use.  Every call passes the same kernels in
-  // `patches` for the same key.
+  // `patches` for the same key.  `lengths` (empty: uniform clips) is part of the key: the packed layout it implies sets
+  // grids and row counts that a replay cannot change.
   int run(rohm_ctx* ctx, int B, int T, bool with_step, bool eager, cudaStream_t st,
-          const std::function<int(cudaStream_t)>& launches, const std::vector<KernelPatch>& patches);
+          const std::function<int(cudaStream_t)>& launches, const std::vector<KernelPatch>& patches,
+          const std::vector<int>& lengths = {});
   void clear() { graphs_.clear(); }  // the next run() of every key captures again
 
  private:
@@ -89,6 +91,7 @@ class ForwardGraphs {
   struct Entry {
     int B = 0, T = 0;
     bool with_step = false;
+    std::vector<int> lengths;
     std::unique_ptr<std::remove_pointer_t<cudaGraph_t>, DestroyGraph> graph;  // owns the captured arguments in `params`
     std::unique_ptr<std::remove_pointer_t<cudaGraphExec_t>, DestroyExec> exec;
     std::vector<cudaGraphNode_t> nodes;  // the boundary nodes, in the order of the patches

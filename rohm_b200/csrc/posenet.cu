@@ -2,7 +2,9 @@
 // (reference model/posenet.py:75-96, model/heads.py:112-176; torch nn.TransformerEncoderLayer post-norm, exact GELU).
 //
 // Token-major layout: every activation is a row-major [B*S, width] matrix, S = T + 1 tokens per clip (token 0 is the
-// timestep embedding), clips contiguous.  All linear layers run on the wgmma GEMM (gemm.cu); operands that feed a
+// timestep embedding), clips contiguous.  With per-clip lengths (rohm_posenet_set_lengths) the clips are packed instead:
+// clip b takes lengths[b] + 1 consecutive rows from clip_off[b], with no padding rows, so every GEMM runs over
+// sum(lengths[b] + 1) rows.  Only attention crosses rows; everything else is per row and does not see the layout.  All linear layers run on the wgmma GEMM (gemm.cu); operands that feed a
 // tensor-core product are kept as hi/lo pairs (fp16 halves by default, TF32 in the tf32 modes) written by the
 // producing kernel's epilogue, so no separate conversion pass exists.
 //
@@ -29,9 +31,21 @@ namespace {
 // small kernels
 // ------------------------------------------------------------------------------------------------------------
 
-// [B, C, T] (frames contiguous) -> token rows (b*S + 1 + t) of a [B*S, ld] hi/lo pair.  32x32 smem transpose.
+// First row and frame count of clip b: packed (clip_off[b], clip_off[b + 1] - clip_off[b] - 1) or uniform (b S, T).
+__device__ __forceinline__ void clip_rows(const int* clip_off, int b, int S, int T, int64_t& row0, int& frames) {
+  if (clip_off != nullptr) {
+    row0 = clip_off[b];
+    frames = clip_off[b + 1] - clip_off[b] - 1;
+  } else {
+    row0 = static_cast<int64_t>(b) * S;
+    frames = T;
+  }
+}
+
+// [B, C, T] (frames contiguous) -> token rows (row0(b) + 1 + t) of a [rows, ld] hi/lo pair, t < frames(b) (padded
+// frames are never read).  32x32 smem transpose.
 __global__ void pack_tokens_kernel(const float* __restrict__ x, float* __restrict__ hi, float* __restrict__ lo, int C,
-                                   int T, int S, int ld, int f16) {
+                                   int T, int S, int ld, int f16, const int* __restrict__ clip_off) {
   __shared__ float tile[32][33];
   // programmatic dependent launch: the embedding GEMM behind this kernel may set itself up (barriers, weight tiles)
   // while it runs; as a dependent (a no-op for a plain launch) nothing is read before the previous kernel has completed
@@ -40,16 +54,19 @@ __global__ void pack_tokens_kernel(const float* __restrict__ x, float* __restric
   const int b = blockIdx.z;
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   const int tx = threadIdx.x, ty = threadIdx.y;  // 32 x 8
+  int64_t row0;
+  int len;
+  clip_rows(clip_off, b, S, T, row0, len);
   for (int j = ty; j < 32; j += 8) {
     const int c = c0 + j, t = t0 + tx;
-    tile[j][tx] = (c < C && t < T) ? x[(static_cast<int64_t>(b) * C + c) * T + t] : 0.0f;
+    tile[j][tx] = (c < C && t < len) ? x[(static_cast<int64_t>(b) * C + c) * T + t] : 0.0f;
   }
   __syncthreads();
   for (int j = ty; j < 32; j += 8) {
     const int t = t0 + j, c = c0 + tx;
-    if (t < T && c < C) {
+    if (t < len && c < C) {
       const float v = tile[tx][j];
-      const int64_t o = (static_cast<int64_t>(b) * S + 1 + t) * ld + c;
+      const int64_t o = (row0 + 1 + t) * ld + c;
       if (f16) {
         ptx::split_f16(v, reinterpret_cast<__half*>(hi)[o], reinterpret_cast<__half*>(lo)[o]);
       } else {
@@ -62,18 +79,23 @@ __global__ void pack_tokens_kernel(const float* __restrict__ x, float* __restric
 }
 constexpr size_t kPackTokensX = 0;  // the argument replaced on every replay of a cached forward graph
 
-// Token rows -> [B, C, T]: channels [traj, traj+Cout) from tok[b*S+1+t][c - traj], channels [0, traj) from cond.
+// Token rows -> [B, C, T]: channels [traj, traj+Cout) from tok[row0(b)+1+t][c - traj], channels [0, traj) from cond;
+// frames at or past frames(b) are zero.
 __global__ void unpack_tokens_kernel(const float* __restrict__ tok, const float* __restrict__ cond_traj,
-                                     float* __restrict__ out, int C, int Cout, int traj, int T, int S, int ldt) {
+                                     float* __restrict__ out, int C, int Cout, int traj, int T, int S, int ldt,
+                                     const int* __restrict__ clip_off) {
   __shared__ float tile[32][33];
   ptx::pdl_launch_dependents();
   ptx::pdl_wait_prior_grid();  // the output-head GEMM has completed
   const int b = blockIdx.z;
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;  // c0 indexes the Cout predicted channels
   const int tx = threadIdx.x, ty = threadIdx.y;
+  int64_t row0;
+  int len;
+  clip_rows(clip_off, b, S, T, row0, len);
   for (int j = ty; j < 32; j += 8) {
     const int t = t0 + j, c = c0 + tx;
-    tile[j][tx] = (t < T && c < Cout) ? tok[(static_cast<int64_t>(b) * S + 1 + t) * ldt + c] : 0.0f;
+    tile[j][tx] = (t < len && c < Cout) ? tok[(row0 + 1 + t) * ldt + c] : 0.0f;
   }
   __syncthreads();
   for (int j = ty; j < 32; j += 8) {
@@ -83,21 +105,25 @@ __global__ void unpack_tokens_kernel(const float* __restrict__ tok, const float*
   if (blockIdx.y == 0) {  // given trajectory channels are a verbatim copy of the condition (posenet.py:94-95)
     for (int c = ty; c < traj; c += 8) {
       const int t = t0 + tx;
-      if (t < T) out[(static_cast<int64_t>(b) * C + c) * T + t] = cond_traj[(static_cast<int64_t>(b) * traj + c) * T + t];
+      if (t < T) out[(static_cast<int64_t>(b) * C + c) * T + t] = t < len ? cond_traj[(static_cast<int64_t>(b) * traj + c) * T + t] : 0.0f;
     }
   }
 }
 constexpr size_t kUnpackTokensOut = 2;  // the argument replaced on every replay of a cached forward graph
 
-// rows[b*S + s][:] = pe[s][:]   (positional rows added to every token incl. the timestep token, posenet.py:90-91)
-__global__ void pe_rows_kernel(const float* __restrict__ pe, float* __restrict__ rows, int S, int D, int64_t total4) {
-  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= total4) return;
+// rows[row0(b) + s][:] = pe[s][:] for the frames(b) + 1 tokens of clip b = blockIdx.y (positional rows added to every
+// token incl. the timestep token, posenet.py:90-91)
+__global__ void pe_rows_kernel(const float* __restrict__ pe, float* __restrict__ rows, int T, int S, int D,
+                               const int* __restrict__ clip_off) {
+  int64_t row0;
+  int len;
+  clip_rows(clip_off, blockIdx.y, S, T, row0, len);
   const int d4 = D / 4;
-  const int64_t row = i / d4;
-  const int c = static_cast<int>(i - row * d4);
-  const int s = static_cast<int>(row % S);
-  reinterpret_cast<float4*>(rows)[i] = reinterpret_cast<const float4*>(pe)[static_cast<int64_t>(s) * d4 + c];
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<int64_t>(len + 1) * d4) return;
+  const int s = static_cast<int>(i / d4);
+  const int c = static_cast<int>(i - static_cast<int64_t>(s) * d4);
+  reinterpret_cast<float4*>(rows)[row0 * d4 + i] = reinterpret_cast<const float4*>(pe)[static_cast<int64_t>(s) * d4 + c];
 }
 
 // TimestepEmbedder (heads.py:132-146): e(t) = W2 silu(W0 pe[t] + b0) + b2 depends on the timestep only, so the whole
@@ -105,7 +131,7 @@ __global__ void pe_rows_kernel(const float* __restrict__ pe, float* __restrict__
 // over all pe_len timesteps); per step the token row (b, 0) is a gather.
 __global__ void time_token_gather_kernel(const int64_t* __restrict__ timesteps, const float* __restrict__ table,
                                          int table_rows, float* __restrict__ X, float* __restrict__ Xh,
-                                         float* __restrict__ Xl, int S, int D, int f16) {
+                                         float* __restrict__ Xl, int S, int D, int f16, const int* __restrict__ clip_off) {
   ptx::pdl_launch_dependents();
   ptx::pdl_wait_prior_grid();  // the embedding GEMM (which also writes row (b, 0)) has completed
   const int b = blockIdx.x;
@@ -116,7 +142,7 @@ __global__ void time_token_gather_kernel(const int64_t* __restrict__ timesteps, 
   const bool bad = t < 0 || t >= table_rows;
   t = bad ? 0 : t;
   const float4* src = reinterpret_cast<const float4*>(table + t * D);
-  const int64_t o = static_cast<int64_t>(b) * S * D;
+  const int64_t o = (clip_off != nullptr ? static_cast<int64_t>(clip_off[b]) : static_cast<int64_t>(b) * S) * D;
   const float nan = __int_as_float(0x7fc00000);
   for (int i = threadIdx.x; i < D / 4; i += blockDim.x) {
     const float4 v = bad ? make_float4(nan, nan, nan, nan) : src[i];
@@ -251,6 +277,14 @@ struct rohm_posenet {
   float *Hh = nullptr, *Hl = nullptr, *condpe = nullptr, *OUT = nullptr;
   float* cond_traj = nullptr;  // [B, traj, T] copy of cond[:, :traj] taken by set_cond (output channels [0,traj))
   int cond_B = -1, cond_T = -1;
+  // Per-clip lengths (rohm_posenet_set_lengths); empty: every clip has the call's T frames.  The clips are packed
+  // (clip_off) and attention runs as up to two launches: the clips of at most 160 tokens on the 160-key wgmma kernel,
+  // the longer ones on the streaming kernel, each clip on the kernel its own length picks when it runs alone.
+  std::vector<int> lengths;
+  std::vector<int> cond_lengths;  // the lengths set_cond embedded the condition with
+  int* clip_off = nullptr;        // device [max_batch + 1]: first packed row of every clip, then the packed row count
+  int* clip_ids = nullptr;        // device [max_batch]: the clips of at most 160 tokens, then the longer ones
+  int packed_rows = 0, n_short = 0, short_tokens = 0, long_tokens = 0;
   int launches = 0;
   // CUDA graph of one forward per (B, T): 45 launches become one cudaGraphLaunch; the three nodes that touch caller
   // memory (pack: x_t, time-token gather: timesteps, unpack: out) get their pointers patched before every replay.
@@ -464,6 +498,24 @@ static int run_ln(rohm_posenet* pn, const float* in, const float* res, const flo
 // ROHM_B200_TC_ATTENTION=0) and the streaming wgmma kernel above; else the mma.sync kernel of the operand kind up to 160
 // tokens and the SIMT kernel above.
 static int run_attention(rohm_posenet* pn, int B, int S, cudaStream_t st) {
+  if (!pn->lengths.empty()) {  // packed clips: one launch per kernel that some clip's own length picks
+    const int n_long = B - pn->n_short;
+    for (int k = 0; k < 2; ++k) {
+      AttnArgs a = pn->attn;
+      a.clip_off = pn->clip_off;
+      a.clip_ids = pn->clip_ids + (k == 0 ? 0 : pn->n_short);
+      a.B = k == 0 ? pn->n_short : n_long;
+      a.S = k == 0 ? pn->short_tokens : pn->long_tokens;
+      if (a.B == 0) continue;
+      prof_begin(pn, kCatAttention, st);
+      const cudaError_t e = launch_attention(a, k == 0 ? kAttnWgmma : kAttnWgmmaStream, &pn->attn_wg, st,
+                                             pn->use_pdl && !pn->profiling);
+      prof_end(pn, st);
+      ROHM_CUDA(pn->ctx, e);
+      pn->launches++;
+    }
+    return ROHM_OK;
+  }
   AttnArgs a = pn->attn;
   a.B = B, a.S = S;
   const bool maps = pn->attn_maps && (pn->tc_attention || S > kAttnWgmmaMaxTokens);
@@ -633,6 +685,14 @@ extern "C" int rohm_posenet_create(rohm_ctx* ctx, const rohm_posenet_weights* w,
     }
   }
 
+  pn->clip_off = static_cast<int*>(pn->pool.bytes(static_cast<int64_t>(max_batch + 1) * sizeof(int)));
+  pn->clip_ids = static_cast<int*>(pn->pool.bytes(static_cast<int64_t>(max_batch) * sizeof(int)));
+  if (pn->clip_off == nullptr || pn->clip_ids == nullptr) {
+    const int rc = fail(ctx, ROHM_ERR_CUDA, "clip table alloc failed: %s", cudaGetErrorString(pn->pool.last_error()));
+    delete pn;
+    return rc;
+  }
+
   // GEMM descriptors.  Input embedding: residual = cond embedding + positional rows (set per set_cond).
   TRY(setup_linear(pn, &pn->g_in, pn->Ain_h, pn->Ain_l, R, pn->C, pn->Kin_p, pn->w_in, pn->in_b));
   pn->g_in.residual = pn->condpe, pn->g_in.ldr = D;
@@ -739,6 +799,18 @@ extern "C" void rohm_posenet_destroy(rohm_posenet* pn) { delete pn; }
 
 extern "C" int rohm_posenet_launches_per_forward(const rohm_posenet* pn) { return pn ? pn->launches : 0; }
 
+// The lengths set by rohm_posenet_set_lengths must describe the call's B clips of at most T frames.
+static int check_lengths(rohm_posenet* pn, int B, int T, const char* fn) {
+  if (pn->lengths.empty()) return ROHM_OK;
+  if (static_cast<int>(pn->lengths.size()) != B)
+    return fail(pn->ctx, ROHM_ERR_INVALID, "%s: lengths were set for %d clips, the call has B=%d", fn,
+                static_cast<int>(pn->lengths.size()), B);
+  for (int b = 0; b < B; ++b)
+    if (pn->lengths[b] > T)
+      return fail(pn->ctx, ROHM_ERR_INVALID, "%s: lengths[%d] = %d exceeds T=%d", fn, b, pn->lengths[b], T);
+  return ROHM_OK;
+}
+
 extern "C" int rohm_posenet_set_cond(rohm_posenet* pn, const float* cond, int B, int T, void* stream) {
   if (pn == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = pn->ctx;
@@ -746,21 +818,26 @@ extern "C" int rohm_posenet_set_cond(rohm_posenet* pn, const float* cond, int B,
   if (cond == nullptr || B <= 0 || T <= 0 || B > pn->max_batch || T > pn->max_frames)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_posenet_set_cond: B=%d T=%d outside the created capacity (%d, %d)", B, T,
                 pn->max_batch, pn->max_frames);
+  int rc = check_lengths(pn, B, T, "rohm_posenet_set_cond");
+  if (rc != ROHM_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int S = T + 1, D = pn->D;
-  const int rows = B * S;
-  // A_in <- tokens of cond (row (b,0) stays zero: the buffer was zero-initialised and is never written there)
+  const bool packed = !pn->lengths.empty();
+  const int* off = packed ? pn->clip_off : nullptr;
+  const int rows = packed ? pn->packed_rows : B * S;
+  // A_in <- tokens of cond (row (b,0) is never written: whatever it holds, the embedding GEMM's row (b,0) is overwritten
+  // by the timestep token)
   dim3 grid((T + 31) / 32, (pn->C + 31) / 32, B);
   pack_tokens_kernel<<<grid, dim3(32, 8), 0, st>>>(cond, pn->Ain_h, pn->Ain_l, pn->C, T, S, pn->Kin_p,
-                                                   pn->kind == kKindF16 ? 1 : 0);
+                                                   pn->kind == kKindF16 ? 1 : 0, off);
   ROHM_CUDA(ctx, cudaGetLastError());
-  const int64_t total4 = static_cast<int64_t>(rows) * D / 4;
-  pe_rows_kernel<<<static_cast<unsigned>((total4 + 255) / 256), 256, 0, st>>>(pn->pe, pn->condpe, S, D, total4);
+  const int64_t clip4 = static_cast<int64_t>(S) * D / 4;
+  pe_rows_kernel<<<dim3(static_cast<unsigned>((clip4 + 255) / 256), B), 256, 0, st>>>(pn->pe, pn->condpe, T, S, D, off);
   ROHM_CUDA(ctx, cudaGetLastError());
   // condpe <- cond_embed(cond) + cond_b + pe rows   (in place; rows (b,0) become cond_b + pe[0]: overwritten later
   // by the timestep token, so their value is irrelevant)
   const int saved = pn->launches;
-  int rc = run_gemm(pn, pn->g_cond, pn->w_cond, rows, st);
+  rc = run_gemm(pn, pn->g_cond, pn->w_cond, rows, st);
   pn->launches = saved;
   if (rc != ROHM_OK) return rc;
   if (pn->traj > 0) {
@@ -769,6 +846,50 @@ extern "C" int rohm_posenet_set_cond(rohm_posenet* pn, const float* cond, int B,
                                      B, cudaMemcpyDeviceToDevice, st));
   }
   pn->cond_B = B, pn->cond_T = T;
+  pn->cond_lengths = pn->lengths;
+  return ROHM_OK;
+}
+
+extern "C" int rohm_posenet_set_lengths(rohm_posenet* pn, const int* lengths, int B) {
+  if (pn == nullptr) return ROHM_ERR_INVALID;
+  rohm_ctx* ctx = pn->ctx;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (lengths == nullptr) {
+    pn->lengths.clear();
+    return ROHM_OK;
+  }
+  if (!pn->attn_maps || !pn->tc_attention)
+    return fail(ctx, ROHM_ERR_INVALID,
+                "rohm_posenet_set_lengths: per-clip lengths run on the wgmma attention kernels: precision f16x2 with head "
+                "dim 128 only (the tf32x3 / tf32 precisions, head dim 64 and ROHM_B200_TC_ATTENTION=0 are not supported)");
+  if (B <= 0 || B > pn->max_batch)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_posenet_set_lengths: B=%d outside the created capacity %d", B, pn->max_batch);
+  for (int b = 0; b < B; ++b)
+    if (lengths[b] < 1 || lengths[b] > pn->max_frames)
+      return fail(ctx, ROHM_ERR_INVALID, "rohm_posenet_set_lengths: lengths[%d] = %d outside [1, %d]", b, lengths[b],
+                  pn->max_frames);
+  std::vector<int> v(lengths, lengths + B);
+  if (v == pn->lengths) return ROHM_OK;
+  std::vector<int> off(B + 1), ids;
+  int n_short = 0, short_tokens = 0, long_tokens = 0;
+  off[0] = 0;
+  for (int b = 0; b < B; ++b) off[b + 1] = off[b] + v[b] + 1;
+  for (int pass = 0; pass < 2; ++pass)
+    for (int b = 0; b < B; ++b) {
+      const int S = v[b] + 1;
+      const bool is_short = S <= kAttnWgmmaMaxTokens;
+      if (is_short != (pass == 0)) continue;
+      ids.push_back(b);
+      if (is_short) ++n_short, short_tokens = S > short_tokens ? S : short_tokens;
+      else long_tokens = S > long_tokens ? S : long_tokens;
+    }
+  // a forward still in flight on any stream may be reading the tables being replaced
+  ROHM_CUDA(ctx, cudaDeviceSynchronize());
+  ROHM_CUDA(ctx, cudaMemcpy(pn->clip_off, off.data(), (B + 1) * sizeof(int), cudaMemcpyHostToDevice));
+  ROHM_CUDA(ctx, cudaMemcpy(pn->clip_ids, ids.data(), B * sizeof(int), cudaMemcpyHostToDevice));
+  pn->lengths = std::move(v);
+  pn->packed_rows = off[B];
+  pn->n_short = n_short, pn->short_tokens = short_tokens, pn->long_tokens = long_tokens;
   return ROHM_OK;
 }
 
@@ -778,7 +899,9 @@ static int forward_launches(rohm_posenet* pn, const float* x_t, const int64_t* t
   rohm_ctx* ctx = pn->ctx;
   rohm::DeviceGuard device_guard__(ctx);
   const int S = T + 1, D = pn->D;
-  const int rows = B * S;
+  const bool packed = !pn->lengths.empty();
+  const int* off = packed ? pn->clip_off : nullptr;
+  const int rows = packed ? pn->packed_rows : B * S;
   pn->launches = 0;
   int rc;
 
@@ -786,14 +909,14 @@ static int forward_launches(rohm_posenet* pn, const float* x_t, const int64_t* t
   prof_begin(pn, kCatOther, st);
   const bool pdl = pn->use_pdl && !pn->profiling;
   ROHM_CUDA(ctx, launch_chain(pack_tokens_kernel, grid, dim3(32, 8), 0, st, pdl, x_t, pn->Ain_h, pn->Ain_l, pn->C, T, S, pn->Kin_p,
-                              pn->kind == kKindF16 ? 1 : 0));
+                              pn->kind == kKindF16 ? 1 : 0, off));
   prof_end(pn, st);
   ROHM_CUDA(ctx, cudaGetLastError());
   pn->launches++;
   if ((rc = run_gemm(pn, pn->g_in, pn->w_in, rows, st)) != ROHM_OK) return rc;
   prof_begin(pn, kCatOther, st);
   ROHM_CUDA(ctx, launch_chain(time_token_gather_kernel, dim3(B), dim3(128), 0, st, pdl, timesteps, pn->time_table, pn->pe_len,
-                              pn->X, pn->Xh, pn->Xl, S, D, pn->kind == kKindF16 ? 1 : 0));
+                              pn->X, pn->Xh, pn->Xl, S, D, pn->kind == kKindF16 ? 1 : 0, off));
   prof_end(pn, st);
   ROHM_CUDA(ctx, cudaGetLastError());
   pn->launches++;
@@ -812,7 +935,7 @@ static int forward_launches(rohm_posenet* pn, const float* x_t, const int64_t* t
   dim3 grid_o((T + 31) / 32, (pn->Cout + 31) / 32, B);
   prof_begin(pn, kCatOther, st);
   ROHM_CUDA(ctx, launch_chain(unpack_tokens_kernel, grid_o, dim3(32, 8), 0, st, pdl, pn->OUT, pn->cond_traj, out, pn->C, pn->Cout,
-                              pn->traj, T, S, pn->Cout));
+                              pn->traj, T, S, pn->Cout, off));
   prof_end(pn, st);
   ROHM_CUDA(ctx, cudaGetLastError());
   pn->launches++;
@@ -861,6 +984,8 @@ static int forward_or_step(rohm_posenet* pn, const float* x_t, const int64_t* ti
   if (B != pn->cond_B || T != pn->cond_T)
     return fail(ctx, ROHM_ERR_STATE, "rohm_posenet_forward: B=%d T=%d but set_cond was called with B=%d T=%d", B, T,
                 pn->cond_B, pn->cond_T);
+  if (pn->lengths != pn->cond_lengths)
+    return fail(ctx, ROHM_ERR_STATE, "rohm_posenet_forward: the clip lengths differ from those set_cond was called with");
   auto launches = [&](cudaStream_t st) {
     const int rc = forward_launches(pn, x_t, timesteps, out, B, T, st);
     if (rc != ROHM_OK || step == nullptr) return rc;
@@ -871,7 +996,8 @@ static int forward_or_step(rohm_posenet* pn, const float* x_t, const int64_t* ti
                                       {time_token_gather_kernel, arg<kTimeTokenTimesteps>(timesteps)},
                                       {unpack_tokens_kernel, arg<kUnpackTokensOut>(out)}};
   if (step != nullptr) patches.push_back(ddpm_step_patch(*step));
-  return pn->graphs.run(ctx, B, T, step != nullptr, pn->profiling, static_cast<cudaStream_t>(stream), launches, patches);
+  return pn->graphs.run(ctx, B, T, step != nullptr, pn->profiling, static_cast<cudaStream_t>(stream), launches, patches,
+                        pn->lengths);
 }
 
 extern "C" int rohm_posenet_forward(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* out, int B,

@@ -255,7 +255,7 @@ class _GaussianDiffusion:
         x = x if (x.is_contiguous() and x.dtype == th.float32) else x.contiguous().float()
         batch['x_t'] = x
         ts = model.map_timesteps(t) if isinstance(model, _WrappedModel) else t
-        e = prep(batch['cond'])
+        e = prep(batch['cond'], inner.clip_lengths(batch, x.shape))
         x0, nxt = e.sample_step(x, ts.to(th.int64).contiguous(), self._coef_row(t, step_index))
         return {"sample": nxt, "pred_xstart": x0, "x_t": x}
 
@@ -360,11 +360,14 @@ class _GaussianDiffusion:
         return {"sample": sample, "pred_xstart": x0, "x_t": x}
 
     # ------------------------------------------------------------------ loops
-    def _begin_loop(self, model, grad_type=None):
+    def _begin_loop(self, model, grad_type=None, batch=None, shape=None):
         """Once per sampling loop, before any step: drop the denoiser's cached step-invariant condition embedding (a
         condition tensor can never outlive the loop it was embedded for) and reject what cannot run BEFORE a thousand
-        denoiser steps are spent (the reference would fail, or silently do nothing, at the first guided step)."""
+        denoiser steps are spent (the reference would fail, or silently do nothing, at the first guided step), per-clip
+        lengths included."""
         inner = model.model if isinstance(model, _WrappedModel) else model
+        if batch is not None and batch.get('lengths') is not None and hasattr(inner, "clip_lengths"):
+            inner.clip_lengths(batch, shape, grad_type=grad_type)
         inv = getattr(inner, "invalidate_cond", None)
         if inv is not None:
             inv()
@@ -419,7 +422,7 @@ class _GaussianDiffusion:
         if device is None:
             device = next(model.parameters()).device
         assert isinstance(shape, (tuple, list))
-        self._begin_loop(model, grad_type if cond_fn_with_grad else None)
+        self._begin_loop(model, grad_type if cond_fn_with_grad else None, batch, shape)
         img = noise if noise is not None else self._randn(*shape, device=device)
         if skip_timesteps and init_image is None:
             init_image = th.zeros_like(img)
@@ -535,6 +538,9 @@ class GaussianDiffusionPoseNet(_GaussianDiffusion):
                     const_noise=False, cur_epoch=0, timestep_respacing='', compute_loss=True, smplx_model=None, epoch=0):
         """The call the drivers make (test_amass_full.py:376, test_posenet.py:178): full sampling loop, then the
         optional loss dict.  Returns (loss_dict | None, model_output)."""
+        if compute_loss and batch.get('lengths') is not None:
+            raise RohmB200Error("eval_losses: the loss dictionary over clips with batch['lengths'] is out of scope (it "
+                                "would average over padded frames); pass compute_loss=False and score each clip's frames")
         model_output = self._sample_for_eval(model, batch, shape, progress, clip_denoised, cond_fn_with_grad,
                                              timestep_respacing, grad_type=grad_type, early_stop=early_stop)
         inner = model.model if isinstance(model, _WrappedModel) else model

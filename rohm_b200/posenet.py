@@ -84,9 +84,12 @@ class PoseNetEngine:
         if os.environ.get("ROHM_B200_GRAPH", "1") == "0":
             self.lib.rohm_posenet_set_option(handle, 0, 0)
         # the condition whose step-invariant embedding the engine currently holds: a STRONG reference (so the caching
-        # allocator cannot hand its address to a different tensor while it is cached) plus its version counter
+        # allocator cannot hand its address to a different tensor while it is cached), its version counter and the
+        # per-clip lengths it was embedded with
         self.cond_ref = None
         self.cond_version = -1
+        self.cond_lengths = None
+        self.lengths = None  # what rohm_posenet_set_lengths last received (None: uniform clips)
         from . import ops
         self.op_key = ops.register_engine(self)
 
@@ -106,6 +109,15 @@ class PoseNetEngine:
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def set_lengths(self, lengths):
+        """Per-clip lengths (a tuple of ints) for the following set_cond / forward / sample_step / profile, or None."""
+        if lengths == self.lengths:
+            return
+        arr = None if lengths is None else (C.c_int * len(lengths))(*lengths)
+        rc = self.lib.rohm_posenet_set_lengths(self.handle, arr, 0 if lengths is None else len(lengths))
+        _lib.check(rc, self.ctx)
+        self.lengths = lengths
 
     def set_cond(self, cond):
         B, _, _, T = cond.shape
@@ -278,23 +290,71 @@ class PoseNet(nn.Module):
             self._engine_fingerprint = self._fingerprint()
         return e
 
-    def prepare_cond(self, cond):
-        """Runs the step-invariant part of the forward for this condition tensor if it is new or was modified."""
+    def prepare_cond(self, cond, lengths=None):
+        """Runs the step-invariant part of the forward for this condition tensor if it is new or was modified, or if the
+        per-clip lengths (a tuple from clip_lengths, or None) differ from those it was embedded with."""
         if cond.device.type != "cuda":
             raise RohmB200Error("PoseNet: batch tensors must live on a CUDA device (no CPU path)")
         B, Cc, _, T = cond.shape
         e = self.engine(B, T, cond.device)
         # Same tensor OBJECT, unmodified since it was embedded -> reuse.  Identity (not data_ptr): a freed condition's
         # address and version count can be handed to the next batch's tensor by the caching allocator.
-        if e.cond_ref is not cond or e.cond_version != cond._version:
+        if e.cond_ref is not cond or e.cond_version != cond._version or e.cond_lengths != lengths:
             fp = self._fingerprint()  # parameters are re-checked once per new condition, not per step
             if fp != self._engine_fingerprint:
                 self._engine = None
                 e = self.engine(B, T, cond.device)
             c = cond if (cond.is_contiguous() and cond.dtype == torch.float32) else cond.contiguous().float()
+            e.set_lengths(lengths)
             e.set_cond(c)
-            e.cond_ref, e.cond_version = cond, cond._version
+            e.cond_ref, e.cond_version, e.cond_lengths = cond, cond._version, lengths
         return e
+
+    def clip_lengths(self, batch, shape=None, grad_type=None):
+        """batch['lengths'] checked against the padded [B, C, 1, T] batch (`shape`, else batch['cond'] / batch['x_t']) and
+        this configuration, as a tuple of ints; None when the key is absent.  Raises RohmB200Error before anything runs on
+        the device.  grad_type: the sampling loop's guidance, refused where lengths are not supported."""
+        lengths = batch.get('lengths') if isinstance(batch, dict) else None
+        if lengths is None:
+            return None
+        if shape is None:
+            shape = (batch['cond'] if 'cond' in batch else batch['x_t']).shape
+        B, T = int(shape[0]), int(shape[-1])
+        cache = getattr(self, "_lengths_cache", None)
+        if cache is not None and cache[0] is lengths and cache[1] == lengths._version and cache[2] == (B, T):
+            values = cache[3]
+        else:
+            if (not isinstance(lengths, torch.Tensor) or lengths.is_floating_point() or lengths.is_complex() or
+                    lengths.dtype == torch.bool or tuple(lengths.shape) != (B,)):
+                raise RohmB200Error(f"PoseNet: batch['lengths'] must be an integer tensor of shape [{B}], got "
+                                    f"{getattr(lengths, 'dtype', type(lengths))} {tuple(getattr(lengths, 'shape', ()))}")
+            values = tuple(int(v) for v in lengths.tolist())
+            bad = [(b, v) for b, v in enumerate(values) if not 1 <= v <= T]
+            if bad:
+                raise RohmB200Error(f"PoseNet: batch['lengths'] must lie in [1, T={T}]; lengths[{bad[0][0]}] = {bad[0][1]}")
+            self._lengths_cache = (lengths, lengths._version, (B, T), values)
+        out_of_scope = None
+        prec = self.precision if self.precision is not None else _precision_from_env()
+        if prec != _lib.PRECISION_F16X2:
+            out_of_scope = "the tf32x3 / tf32 precisions"
+        elif self.latent_dim // self.num_heads != 128:
+            out_of_scope = f"head dim {self.latent_dim // self.num_heads}"
+        elif grad_type == 'prox':
+            out_of_scope = "grad_type='prox' (2-D projection guidance)"
+        elif grad_type is not None and getattr(self, "guidance_sum_reducer", None) is not None:
+            out_of_scope = "parallel.global_guidance (the exact-global sharded skating normaliser)"
+        if out_of_scope is not None:
+            raise RohmB200Error(f"PoseNet: batch['lengths'] with {out_of_scope} is out of scope; per-clip lengths run "
+                                "with precision f16x2, head dim 128 and the skating guidance only")
+        return values
+
+    def _lengths_on(self, values, device):
+        """The per-clip lengths as an int32 device tensor (cached for the guided steps of one loop)."""
+        cache = getattr(self, "_lengths_dev", None)
+        if cache is None or cache[0] != values or cache[1] != device:
+            cache = (values, device, torch.tensor(values, dtype=torch.int32, device=device))
+            self._lengths_dev = cache
+        return cache[2]
 
     def invalidate_cond(self):
         """Forget the cached step-invariant condition embedding (the samplers call this at the start of every loop,
@@ -324,8 +384,12 @@ class PoseNet(nn.Module):
             raise RohmB200Error("guide_skating_with_smpl: implemented for the 294-channel representation with the "
                                 "22-channel trajectory block (the configuration RoHM ships)")
         B, _, _, T = x.shape
+        lengths = self.clip_lengths(batch, x.shape, grad_type='amass')
         mean, std = self._norm_stats(x.device)
         k = kernels_for(self.smplx_model, x.device, B * T, with_vertices=False)
+        if lengths is not None:
+            # frames past a clip's length add nothing; the normalisers stay batch-wide over the real frames
+            return k.skating_guidance(x, mean, std, lengths=self._lengths_on(lengths, x.device))
         reducer = getattr(self, "guidance_sum_reducer", None)
         if reducer is not None:
             # clip-sharded run reproducing the unsharded batch: the loss normalisers are batch-wide counts (reference
@@ -363,6 +427,7 @@ class PoseNet(nn.Module):
             raise RohmB200Error("guide_2d_projection_with_smpl: implemented for the 294-channel representation with the "
                                 "22-channel trajectory block (the configuration RoHM ships)")
         B, _, _, T = x.shape
+        self.clip_lengths(batch, x.shape, grad_type='prox')  # per-clip lengths are refused here
         dev = x.device
         mean, std = self._norm_stats(dev)
         f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()
@@ -383,7 +448,9 @@ class PoseNet(nn.Module):
     # ---------------------------------------------------------------- forward
     def forward(self, batch, timesteps):
         """batch['x_t'], batch['cond']: [bs, body_feat_dim, 1, T]; timesteps: [bs] int -> [bs, body_feat_dim, 1, T]
-        (channels [0, traj_feat_dim) are batch['cond'][:, :traj_feat_dim], the rest is the denoised pose)."""
+        (channels [0, traj_feat_dim) are batch['cond'][:, :traj_feat_dim], the rest is the denoised pose).
+        batch['lengths'] (optional, integer [bs], 1 <= lengths[b] <= T): clip b has lengths[b] real frames; those come out
+        bit-identical to running the clip alone, later frames come out zero and their inputs are never read."""
         x_t, cond = batch['x_t'], batch['cond']
         if x_t.dim() != 4 or x_t.shape[2] != 1 or x_t.shape != cond.shape or x_t.shape[1] != self.input_feats:
             raise RohmB200Error(f"PoseNet: expected x_t/cond of shape [B, {self.input_feats}, 1, T], got "
@@ -396,7 +463,8 @@ class PoseNet(nn.Module):
             # T frames + the timestep token take T + 1 rows of the table; the reference's pe[:T + 1] add fails there too
             raise RohmB200Error(f"PoseNet: a clip of {x_t.shape[3]} frames needs {x_t.shape[3] + 1} rows of the positional "
                                 f"table sequence_pos_encoder.pe, which has {pe_rows} (at most {pe_rows - 1} frames)")
-        e = self.prepare_cond(cond)
+        lengths = self.clip_lengths(batch, x_t.shape)
+        e = self.prepare_cond(cond, lengths)
         x = x_t if (x_t.is_contiguous() and x_t.dtype == torch.float32) else x_t.contiguous().float()
         ts = timesteps.to(device=x.device, dtype=torch.int64).contiguous()
         return e.forward(x, ts)
