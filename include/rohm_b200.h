@@ -206,6 +206,16 @@ ROHM_API void rohm_trajnet_destroy(rohm_trajnet* tn);
  * [B, frames, control_cond_dim] or NULL for the vanilla network.  Call whenever batch['cond'] / ['control_cond'] change. */
 ROHM_API int rohm_trajnet_set_cond(rohm_trajnet* tn, const float* cond, const float* control_cond, int B, void* stream);
 
+/* Per-clip lengths for the following set_cond, forward and sample_step calls: clip b of the padded [B, frames, *] tensors
+ * has lengths_host[b] real frames, a multiple of 16 with 16 <= lengths_host[b] <= frames.  Inside, the clips are packed
+ * with no padding rows past each clip's own 32 (so a batch of mixed lengths does no wasted tensor work).  Frames
+ * [0, lengths[b]) of the output depend on that clip alone: bit-identical to the clip as a one-clip padded batch through
+ * the same engine, and equal to the clip at its own length up to summation order (another engine may choose other
+ * split-K ranges).  Frames past it are zero, and the input values there are never read.  NULL returns to uniform clips.
+ * Changing the lengths waits for the device to go idle; call set_cond again afterwards.  ROHM_ERR_INVALID for B outside
+ * the created capacity or a bad length. */
+ROHM_API int rohm_trajnet_set_lengths(rohm_trajnet* tn, const int* lengths_host, int B);
+
 /* TrajNet.forward (trajnet.py:177-275).  x_t: [B, frames, traj_feat_dim]; time: int64 [B]; out: same shape as x_t. */
 ROHM_API int rohm_trajnet_forward(rohm_trajnet* tn, const float* x_t, const int64_t* time, float* out, int B,
                                   void* stream);

@@ -60,6 +60,7 @@ SIGNATURES = {
                                  _i, _i, _i, C.POINTER(_p)]),
     "rohm_trajnet_destroy": (None, [_p]),
     "rohm_trajnet_set_cond": (_i, [_p, _p, _p, _i, _p]),
+    "rohm_trajnet_set_lengths": (_i, [_p, C.POINTER(_i), _i]),
     "rohm_trajnet_forward": (_i, [_p, _p, _p, _p, _i, _p]),
     "rohm_trajnet_sample_step": (_i, [_p, _p, _p, _p, _p, _p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), _i, _p]),
     "rohm_trajnet_set_option": (_i, [_p, _i, _i]),

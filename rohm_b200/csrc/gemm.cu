@@ -15,7 +15,7 @@ namespace {
 // Warp roles.  Warpgroup 0: TMA producer (one lane).  Warpgroups 1, 2 (warps 4-11): wgmma, 64 tile rows each.
 // EPI 0, 1, 3 (the lean variants the PoseNet forward runs): warpgroup 3 (warps 12-15) is a dedicated epilogue, one tile row
 // per thread, so the MMA warpgroups go straight on to the next tile's K loop while it runs (512 threads).
-// EPI 2 (TrajNet: split-K, activations, padded clips) and EPI 4 (skinning, ~168 registers per epilogue thread): the MMA
+// EPI 2 / 5 (TrajNet: split-K, activations, padded or packed clips) and EPI 4 (skinning, ~168 registers per epilogue thread): the MMA
 // warpgroups run the epilogue themselves, after the tile's MMAs (384 threads) -- these epilogues do not fit the register
 // budget of an epilogue warpgroup next to two MMA warpgroups.
 constexpr int kFirstMmaWarp = 4;
@@ -199,7 +199,9 @@ __device__ __forceinline__ void stage_pair_chunk(const float (&v)[32], uint8_t* 
 // while those MMAs run, waits on acc_full, and arrives on acc_empty once it has read the tile.
 template <int BLOCK_N, int PASSES, int EPI, int KIND>
 __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const __grid_constant__ GemmParams p) {
-  constexpr bool LEAN = EPI != 2;  // EPI: 0 bias / stores, 1 + exact GELU, 2 everything (TrajNet), 3 LayerNorm-folding producer, 4 skinning
+  // EPI: 0 bias / stores, 1 + exact GELU, 2 everything (TrajNet), 3 LayerNorm-folding producer, 4 skinning, 5 = 2 with the
+  // pad rows given by GemmParams::row_mask (TrajNet on packed clips; a separate instance keeps 2's code as it is)
+  constexpr bool LEAN = EPI != 2 && EPI != 5;
   constexpr bool EPI_ROLE = epi_role(EPI);  // a dedicated epilogue warpgroup (see kFirstMmaWarp)
   constexpr int kElemK = gemm_block_k(KIND);  // K elements per pipeline stage (TMA coordinates are in elements)
   using Cfg = TileCfg<BLOCK_N, PASSES, EPI_ROLE>;
@@ -238,7 +240,7 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
   for (int s = 0; s < p.num_segs; ++s) total_iters += p.seg_kblocks[s];
   // Split-K (GemmParams::k_splits, masked variant only): work item w = tile * S + split; split s runs the K
   // iterations [s * per_split, min(total_iters, (s + 1) * per_split)).  S == 1 everywhere else: one item per tile.
-  const int S = (EPI == 2 && p.k_splits > 1) ? p.k_splits : 1;
+  const int S = (!LEAN && p.k_splits > 1) ? p.k_splits : 1;
   const int per_split = (total_iters + S - 1) / S;
   const int num_work = num_tiles * S;
 
@@ -606,13 +608,14 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
     for (int wi = blockIdx.x; EPI != 4 && epi_warp && wi < num_work; wi += gridDim.x, ++tcount) {
       const int tile_idx = wi / S;
       // split-K: the partial tile of split s goes to output rows m + s * split_row_stride
-      const int split_rows = (wi - tile_idx * S) * (EPI == 2 ? p.split_row_stride : 0);
+      const int split_rows = (wi - tile_idx * S) * (!LEAN ? p.split_row_stride : 0);
       const int m0 = (tile_idx / tiles_n) * kGemmBlockM;
       const int n0 = (tile_idx % tiles_n) * BLOCK_N;
       const int m = m0 + q * 32 + lane;
       const bool row_ok = m < e.M;
       bool row_real = true;
-      if (!LEAN && e.clip_rows > 0) row_real = (m % e.clip_rows) < e.clip_valid;
+      if constexpr (EPI == 5) row_real = row_ok && __ldg(p.row_mask + m) != 0;
+      else if (!LEAN && e.clip_rows > 0) row_real = (m % e.clip_rows) < e.clip_valid;
       const int64_t orow = static_cast<int64_t>(m) * e.out_row_mul + e.out_row_add + split_rows;
       const float bias_row = (e.bias != nullptr && e.bias_per_row && row_ok) ? __ldg(e.bias + m) : 0.0f;
 
@@ -923,7 +926,8 @@ __global__ void __launch_bounds__(kernel_threads(EPI), 1) gemm_tile_kernel(const
             if (mr < e.M) {
               if (use_res) {
                 bool real = true;
-                if (!LEAN && e.clip_rows > 0) real = (mr % e.clip_rows) < e.clip_valid;
+                if constexpr (EPI == 5) real = __ldg(p.row_mask + mr) != 0;
+                else if (!LEAN && e.clip_rows > 0) real = (mr % e.clip_rows) < e.clip_valid;
                 if (real) w.x += res[rr].x, w.y += res[rr].y, w.z += res[rr].z, w.w += res[rr].w;
               }
               const int64_t orr = static_cast<int64_t>(mr) * e.out_row_mul + e.out_row_add + split_rows;
@@ -1040,6 +1044,9 @@ static cudaError_t set_attr() {
   e = cudaFuncSetAttribute(gemm_tile_kernel<BLOCK_N, PASSES, 2, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            TileCfg<BLOCK_N, PASSES, false>::kSmemBytes);
   if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(gemm_tile_kernel<BLOCK_N, PASSES, 5, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           TileCfg<BLOCK_N, PASSES, false>::kSmemBytes);
+  if (e != cudaSuccess) return e;
   if constexpr (BLOCK_N == 128 && PASSES == 3 && KIND == kKindF16)
     e = cudaFuncSetAttribute(gemm_tile_kernel<BLOCK_N, PASSES, 3, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRoleSmem);
   return e;
@@ -1049,13 +1056,15 @@ template <int BLOCK_N, int PASSES, int KIND>
 cudaError_t launch_cfg(const GemmParams& p, int m_rows, int n_cols, cudaStream_t stream, bool pdl) {
   using Cfg = TileCfg<BLOCK_N, PASSES, false>;  // the 384-thread variants (EPI 2, 4)
   const bool plain = p.clip_rows == 0;
-  const int epi = (plain && p.act == kActNone) ? 0 : (plain && p.act == kActGelu) ? 1 : 2;
-  auto kern = epi == 0 ? gemm_tile_kernel<BLOCK_N, PASSES, 0, KIND>
+  const int epi = (plain && p.act == kActNone) ? 0 : (plain && p.act == kActGelu) ? 1 : p.row_mask != nullptr ? 5 : 2;
+  auto kern = epi == 0   ? gemm_tile_kernel<BLOCK_N, PASSES, 0, KIND>
               : epi == 1 ? gemm_tile_kernel<BLOCK_N, PASSES, 1, KIND>
-                         : gemm_tile_kernel<BLOCK_N, PASSES, 2, KIND>;
+              : epi == 2 ? gemm_tile_kernel<BLOCK_N, PASSES, 2, KIND>
+                         : gemm_tile_kernel<BLOCK_N, PASSES, 5, KIND>;
   int threads = kernel_threads(epi);
   int smem_bytes = epi_role(epi) ? TileCfg<BLOCK_N, PASSES, true>::kSmemBytes : Cfg::kSmemBytes;
   if (p.a_stats != nullptr && (!plain || p.a_corr == nullptr)) return cudaErrorInvalidValue;
+  if (p.row_mask != nullptr && plain) return cudaErrorInvalidValue;  // the mask is read by the masked variant only
   if (p.stats_out != nullptr) {
     // LayerNorm-folding producer: the output pair overwrites the residual pair tile by tile (st_hi / st_lo both ways), rows are
     // four 128-column tiles wide, and the column tile of a CTA must not change between its tiles (per-column vectors)

@@ -84,6 +84,9 @@ struct alignas(64) GemmParams {
   // are real frames; the others are written as zeros so that they act as conv padding for the next layer.
   int clip_rows;  // 0 = disabled
   int clip_valid;
+  // Packed-clip layouts (TrajNet with per-clip lengths): row m is a real frame iff row_mask[m] != 0, in place of the
+  // clip_rows / clip_valid rule (which must still be set: it selects the masked variant).  nullptr = that rule.
+  const unsigned char* row_mask;
   // TMA-store epilogue (gemm_enable_tma_store): 32 x 32 output chunks go registers -> swizzled shared-memory tile ->
   // cp.async.bulk.tensor store.  Eligible launches: no residual, identity output row map (not the transposed-conv
   // phases), and either only `out` (fp32) or only an fp16 out_hi/out_lo pair.  Chunks on a ragged M or N edge still take

@@ -11,21 +11,23 @@ namespace cg = cooperative_groups;
 namespace rohm {
 namespace {
 
-// One cluster of n CTAs per (clip, group); CTA `rank` owns rows [rank * ceil(T / n), ...) of the group's T real rows.
+// One cluster of n CTAs per (clip, group); CTA `rank` owns rows [rank * ceil(T / n), ...) of the group's T real rows (with
+// clip_off: of the clip's own real rows, fewer than T for a short clip, in the slices sized for T).
 // kCluster = false is the n = 1 instantiation (a plain launch): with n and rank compile-time constants it is the one-CTA
-// kernel without any cluster code.
+// kernel without any cluster code.  kPacked = false is the uniform-clip code (clip b at b * Tp, T real rows); kPacked = true
+// reads clip b's first row and real-row count from clip_off.
 // y = bias + the `splits` fp32 partials (added in split order: deterministic; an un-split convolution passes its output as the
 // one partial) is formed once into shared memory while each CTA sums its slice in double; the CTAs' (s1, s2) are then added
 // in rank order by every CTA through distributed shared memory, so all hold bit-identical statistics (n = 1: the CTA's own
 // sums, nothing added).  Pad rows are written as zeros, spread over the cluster.
-template <bool kCluster>
+template <bool kCluster, bool kPacked>
 __global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restrict__ part, int splits, int64_t split_stride,
                                                             const float* __restrict__ bias, const float* __restrict__ gamma,
                                                             const float* __restrict__ beta, const float* __restrict__ tp,
                                                             int tp_stride, const float* __restrict__ r1,
                                                             const float* __restrict__ r2, float* __restrict__ out,
                                                             float* __restrict__ out_hi, float* __restrict__ out_lo, int C, int Tp,
-                                                            int T, int groups, int f16) {
+                                                            int T, int groups, int f16, const int* __restrict__ clip_off) {
   extern __shared__ float4 gn_vals[];  // ceil(T / n) * (C / groups) / 4
   __shared__ double red[2][8];         // per-warp sums; then [0][0], [1][0]: this CTA's (s1, s2), read by the whole cluster
   ptx::pdl_launch_dependents();
@@ -36,11 +38,14 @@ __global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restr
   const unsigned bg = blockIdx.x / static_cast<unsigned>(n);  // unsigned, as blockIdx.x: n = 1 is the one-CTA code
   const int b = bg / groups, g = bg - b * groups;
   const int gs = C / groups, gs4 = gs / 4;
-  const int rows = (T + n - 1) / n;
-  const int t0 = rank * rows;                     // past T in trailing CTAs of a short group: their slice is empty
-  const int n4 = (min(T, t0 + rows) - t0) * gs4;  // <= 0 for an empty slice
+  // packed clips: clip b takes rows [clip_off[b], clip_off[b + 1]), the last Tp - T of them pad rows
+  int Tc = T;
+  int64_t clip0 = static_cast<int64_t>(b) * Tp;
+  if constexpr (kPacked) clip0 = clip_off[b], Tc = clip_off[b + 1] - clip_off[b] - (Tp - T);
+  const int rows = (Tc + n - 1) / n;
+  const int t0 = rank * rows;                      // past Tc in trailing CTAs of a short group: their slice is empty
+  const int n4 = (min(Tc, t0 + rows) - t0) * gs4;  // <= 0 for an empty slice
   const int c4 = C / 4;
-  const int64_t clip0 = static_cast<int64_t>(b) * Tp;
   const int64_t row0 = clip0 + t0;
   double s1 = 0.0, s2 = 0.0;
   for (int i = threadIdx.x; i < n4; i += blockDim.x) {
@@ -86,7 +91,7 @@ __global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restr
     // at the end of the kernel)
     cluster.barrier_arrive();
   }
-  const double cnt = static_cast<double>(gs) * static_cast<double>(T);
+  const double cnt = static_cast<double>(gs) * static_cast<double>(Tc);
   const double mean = s1 / cnt;
   double var = s2 / cnt - mean * mean;
   var = var < 0.0 ? 0.0 : var;
@@ -121,7 +126,7 @@ __global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restr
   const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
   // pad rows: the next convolution's zero padding
   for (int i = rank * blockDim.x + threadIdx.x; i < (Tp - T) * gs4; i += n * blockDim.x) {
-    const int t = T + i / gs4;
+    const int t = Tc + i / gs4;
     const int c = g * gs + (i % gs4) * 4;
     store_act4(out, out_hi, out_lo, (clip0 + t) * c4 + c / 4, zero, f16);
   }
@@ -136,8 +141,8 @@ size_t gn_slice_bytes(int T, int C, int groups, int n) {
 
 cudaError_t gn_smem_budgets(size_t* default_budget, size_t* max_budget) {
   cudaFuncAttributes single{}, cluster{};
-  cudaError_t e = cudaFuncGetAttributes(&single, gn_mish_split_kernel<false>);
-  if (e == cudaSuccess) e = cudaFuncGetAttributes(&cluster, gn_mish_split_kernel<true>);
+  cudaError_t e = cudaFuncGetAttributes(&single, gn_mish_split_kernel<false, false>);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&cluster, gn_mish_split_kernel<true, false>);
   if (e != cudaSuccess) return e;
   int dev = 0, optin = 0;
   if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
@@ -155,7 +160,8 @@ int gn_pick_cluster(int T, int C, int groups, size_t budget) {
 }
 
 cudaError_t gn_reserve_smem(size_t bytes) {
-  for (auto kern : {gn_mish_split_kernel<false>, gn_mish_split_kernel<true>}) {
+  for (auto kern : {gn_mish_split_kernel<false, false>, gn_mish_split_kernel<true, false>, gn_mish_split_kernel<false, true>,
+                    gn_mish_split_kernel<true, true>}) {
     cudaFuncAttributes fa{};
     cudaError_t e = cudaFuncGetAttributes(&fa, kern);
     if (e == cudaSuccess && bytes > static_cast<size_t>(fa.maxDynamicSharedSizeBytes))
@@ -165,12 +171,14 @@ cudaError_t gn_reserve_smem(size_t bytes) {
   return cudaSuccess;
 }
 
-cudaError_t launch_gn_mish(const GnArgs& a, int B, int n, cudaStream_t st, bool pdl) {
+cudaError_t launch_gn_mish(const GnArgs& a, int B, int n, cudaStream_t st, bool pdl, const int* clip_off) {
   if (n < 1 || n > kGnMaxCluster || a.groups <= 0 || a.C % (4 * a.groups) != 0) return cudaErrorInvalidValue;
-  return launch_chain(n == 1 ? gn_mish_split_kernel<false> : gn_mish_split_kernel<true>, dim3(static_cast<unsigned>(B * a.groups * n)), dim3(256),
+  auto kern = clip_off != nullptr ? (n == 1 ? gn_mish_split_kernel<false, true> : gn_mish_split_kernel<true, true>)
+                                     : (n == 1 ? gn_mish_split_kernel<false, false> : gn_mish_split_kernel<true, false>);
+  return launch_chain(kern, dim3(static_cast<unsigned>(B * a.groups * n)), dim3(256),
                       gn_slice_bytes(a.T, a.C, a.groups, n), st, ChainAttrs(pdl, static_cast<unsigned>(n)), a.part,
                       a.splits, a.split_stride, a.bias, a.gamma, a.beta, a.tp, a.tp_stride, a.r1, a.r2, a.out, a.out_hi,
-                      a.out_lo, a.C, a.Tp, a.T, a.groups, a.f16);
+                      a.out_lo, a.C, a.Tp, a.T, a.groups, a.f16, clip_off);
 }
 
 }  // namespace rohm

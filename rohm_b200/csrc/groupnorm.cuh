@@ -72,7 +72,9 @@ cudaError_t gn_smem_budgets(size_t* default_budget, size_t* max_budget);
 int gn_pick_cluster(int T, int C, int groups, size_t budget);
 // Raises the kernel's dynamic shared-memory limit on the current device to at least `bytes` (never lowers it).
 cudaError_t gn_reserve_smem(size_t bytes);
-// Launches B x groups clusters of n CTAs (256 threads each), with programmatic dependent launch when pdl.
-cudaError_t launch_gn_mish(const GnArgs& a, int B, int n, cudaStream_t st, bool pdl);
+// Launches B x groups clusters of n CTAs (256 threads each), with programmatic dependent launch when pdl.  clip_off (device
+// int[B + 1], or nullptr for clips at b * Tp): packed clips, clip b at rows [clip_off[b], clip_off[b + 1]) with its Tp - T
+// pad rows last, so clip_off[b + 1] - clip_off[b] - (Tp - T) <= T real rows; statistics over those rows only.
+cudaError_t launch_gn_mish(const GnArgs& a, int B, int n, cudaStream_t st, bool pdl, const int* clip_off = nullptr);
 
 }  // namespace rohm

@@ -2,7 +2,12 @@
 // (reference model/trajnet.py:10-75 ControlNet.forward, :177-275 TrajNet.forward; blocks model/heads.py:20-106).
 //
 // Layout: every activation is a channels-last matrix [B * Tp_L, C] per pyramid level L (T_L = T / 2^L real frames
-// per clip followed by Tp_L - T_L >= 2 all-zero rows, Tp_L = (T + 32) / 2^L).  In that layout
+// per clip followed by Tp_L - T_L >= 2 all-zero rows, Tp_L = (T + 32) / 2^L).  With per-clip lengths
+// (rohm_trajnet_set_lengths) the clips are packed instead: clip b takes (lengths[b] + 32) / 2^L rows from
+// off_L[b] = sum_{c<b} (lengths[c] + 32) / 2^L = off_0[b] / 2^L (exact: every lengths[c] + 32 is a multiple of 16), its
+// lengths[b] / 2^L real frames first, and every GEMM runs over off_L[B] rows.  Stride-2 reads and the transposed
+// convolution's interleaved stores still map clip b onto clip b, and every clip keeps >= 2 zero rows at every level.  In
+// either layout
 //   * Conv1d(k, pad k/2)        = k shifted reads of the same matrix: the zero rows between clips ARE the padding,
 //   * channel concat [x, skip]  = two K-segments of one GEMM,
 //   * Downsample (k3, stride 2) = the same with a row-stride-2 TMA descriptor,
@@ -29,17 +34,36 @@
 namespace rohm {
 namespace {
 
+// Real frames of packed clip b: its rows less the Tp - T pad rows every clip ends with.
+__device__ __forceinline__ int packed_frames(const int* clip_off, int b, int T, int Tp) {
+  return clip_off[b + 1] - clip_off[b] - (Tp - T);
+}
+
 // [B, T, C] channels-last API tensor -> padded-clip hi/lo rows (b * Tp + t), pitch ld.  Pad rows stay zero.
+// kPacked (clip_off: level-0 offsets of packed clips): `total` covers B x Tp x C instead, and every row of clip b is
+// written, its real frames from x and its pad rows as zeros; frames of x past the clip are never read.  Each of these
+// boundary kernels has a uniform-clip instance of its own, which runs the code it ran before packed clips existed.
+template <bool kPacked>
 __global__ void pack_rows_kernel(const float* __restrict__ x, float* __restrict__ hi, float* __restrict__ lo, int T,
-                                 int Tp, int C, int ld, int64_t total, int f16) {
+                                 int Tp, int C, int ld, int64_t total, int f16, const int* __restrict__ clip_off) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int c = static_cast<int>(i % C);
   const int64_t bt = i / C;
-  const int t = static_cast<int>(bt % T);
-  const int64_t b = bt / T;
-  const float v = x[i];
-  const int64_t o = (b * Tp + t) * ld + c;
+  float v;
+  int64_t o;
+  if constexpr (!kPacked) {
+    const int t = static_cast<int>(bt % T);
+    const int64_t b = bt / T;
+    v = x[i];
+    o = (b * Tp + t) * ld + c;
+  } else {
+    const int t = static_cast<int>(bt % Tp);
+    const int b = static_cast<int>(bt / Tp);
+    if (t >= clip_off[b + 1] - clip_off[b]) return;
+    v = t < packed_frames(clip_off, b, T, Tp) ? x[(static_cast<int64_t>(b) * T + t) * C + c] : 0.0f;
+    o = (static_cast<int64_t>(clip_off[b]) + t) * ld + c;
+  }
   if (f16) {
     ptx::split_f16(v, reinterpret_cast<__half*>(hi)[o], reinterpret_cast<__half*>(lo)[o]);
   } else {
@@ -111,11 +135,14 @@ __global__ void __launch_bounds__(256) trajnet_time_kernel(const int64_t* __rest
 constexpr size_t kTrajnetTimeT = 0;  // the argument replaced on every replay of a cached forward graph
 
 // Split-K convolution without a GroupNorm behind it (the stride-2 downsampling convolutions): out = bias + the partials (in
-// split order) on real rows, 0 on pad rows.  4 channels per thread over the [B * Tp, C] output.
+// split order) on real rows, 0 on pad rows.  4 channels per thread over the [B * Tp, C] output.  kPacked: row r is real iff
+// row_mask[r] != 0.
+template <bool kPacked>
 __global__ void __launch_bounds__(256) sum_split_kernel(const float* __restrict__ part, int splits, int64_t split_stride,
                                                         const float* __restrict__ bias, float* __restrict__ out,
                                                         float* __restrict__ out_hi, float* __restrict__ out_lo, int C, int Tp,
-                                                        int T, int64_t total4, int f16) {
+                                                        int T, int64_t total4, int f16,
+                                                        const unsigned char* __restrict__ row_mask) {
   ptx::pdl_launch_dependents();
   ptx::pdl_wait_prior_grid();
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -123,9 +150,9 @@ __global__ void __launch_bounds__(256) sum_split_kernel(const float* __restrict_
   const int c4 = C / 4;
   const int64_t row = i / c4;
   const int c = static_cast<int>(i - row * c4) * 4;
-  const int t = static_cast<int>(row % Tp);
+  const bool real = kPacked ? row_mask[row] != 0 : static_cast<int>(row % Tp) < T;
   float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (t < T) {
+  if (real) {
     float4 a[kMaxSplitsDev];
 #pragma unroll
     for (int sp = 0; sp < kMaxSplitsDev; ++sp)
@@ -138,16 +165,21 @@ __global__ void __launch_bounds__(256) sum_split_kernel(const float* __restrict_
   store_act4(out, out_hi, out_lo, i, v, f16);
 }
 
-// padded-clip rows [B * Tp, ld] -> compact [B, T, C]
+// padded-clip rows [B * Tp, ld] -> compact [B, T, C]; kPacked (clip_off: packed clips): frames past a clip are zero
+template <bool kPacked>
 __global__ void unpack_rows_kernel(const float* __restrict__ x, float* __restrict__ out, int T, int Tp, int C, int ld,
-                                   int64_t total) {
+                                   int64_t total, const int* __restrict__ clip_off) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int c = static_cast<int>(i % C);
   const int64_t bt = i / C;
   const int t = static_cast<int>(bt % T);
   const int64_t b = bt / T;
-  out[i] = x[(b * Tp + t) * ld + c];
+  if constexpr (!kPacked)
+    out[i] = x[(b * Tp + t) * ld + c];
+  else
+    out[i] = t < packed_frames(clip_off, static_cast<int>(b), T, Tp) ? x[(static_cast<int64_t>(clip_off[b]) + t) * ld + c]
+                                                                      : 0.0f;
 }
 constexpr size_t kUnpackRowsOut = 1;  // the argument replaced on every replay of a cached forward graph
 
@@ -281,7 +313,15 @@ struct rohm_trajnet {
   size_t ev_next = 0;
   int cond_B = -1;
   int launches = 0;
-  ForwardGraphs graphs;  // CUDA graph of one forward per batch size
+  ForwardGraphs graphs;  // CUDA graph of one forward per batch size and lengths
+  // Per-clip lengths (rohm_trajnet_set_lengths); empty: every clip has T frames at b * Tp[L].  Packed clips: clip_off[L]
+  // (device int[max_batch + 1]) holds every clip's first row at level L, then the row count packed_rows[L]; row_mask[L]
+  // (device, one byte per row) marks the real frames for the GEMM epilogue and sum_split_kernel.
+  std::vector<int> lengths;
+  std::vector<int> cond_lengths;  // the lengths set_cond embedded the condition with
+  int* clip_off[kLevels] = {};
+  unsigned char* row_mask[kLevels] = {};
+  int packed_rows[kLevels] = {};
   bool use_pdl = true;  // ROHM_B200_PDL / rohm_trajnet_set_option(1): programmatic dependent launch along the conv / GroupNorm chains
   size_t gn_budget = 0;    // gn_mish_split_kernel's default dynamic shared-memory budget per CTA
   size_t gn_smem_max = 0;  // the largest slice of any of its launches
@@ -543,17 +583,20 @@ int make_rtb(rohm_trajnet* tn, Rtb& r, const std::string& p, std::vector<const A
 }
 
 int run_conv(rohm_trajnet* tn, Conv& cv, int B, cudaStream_t st) {
-  const int rows = B * tn->Tp[cv.level_out];
+  const bool packed = !tn->lengths.empty();
+  const int rows = packed ? tn->packed_rows[cv.level_out] : B * tn->Tp[cv.level_out];
+  const unsigned char* mask = packed ? tn->row_mask[cv.level_out] : nullptr;
   cv.g.M = rows;
+  cv.g.row_mask = mask;
   ROHM_CUDA(tn->ctx, launch_gemm(cv.g, rows, cv.w.N, cv.w.block_n, tn->passes, st, tn->use_pdl, tn->kind));
   tn->launches++;
   if (cv.sum_after) {
     const int C = cv.w.N;
     const int64_t total4 = static_cast<int64_t>(rows) * C / 4;
-    ROHM_CUDA(tn->ctx, launch_chain(sum_split_kernel, dim3(static_cast<unsigned>((total4 + 255) / 256)), dim3(256), 0, st,
+    ROHM_CUDA(tn->ctx, launch_chain(packed ? sum_split_kernel<true> : sum_split_kernel<false>, dim3(static_cast<unsigned>((total4 + 255) / 256)), dim3(256), 0, st,
                                     tn->use_pdl, cv.partial, cv.splits, cv.split_rows * C, cv.bias, cv.out.f32, cv.out.hi,
                                     cv.out.lo, C, tn->Tp[cv.level_out], tn->Tl[cv.level_out], total4,
-                                    tn->kind == kKindF16 ? 1 : 0));
+                                    tn->kind == kKindF16 ? 1 : 0, mask));
     tn->launches++;
   }
   return ROHM_OK;
@@ -566,7 +609,8 @@ int run_gn(rohm_trajnet* tn, const Conv& cv, const GroupNorm& gn, int B, const f
   const int C = cv.w.N, level = cv.level_out;
   const GnArgs a{cv.partial, cv.splits, cv.split_rows * C, cv.bias, gn.gamma, gn.beta, tp, tn->tp_total, r1, r2,
                  out.f32, out.hi, out.lo, C, tn->Tp[level], tn->Tl[level], kGroups, tn->kind == kKindF16 ? 1 : 0};
-  ROHM_CUDA(tn->ctx, launch_gn_mish(a, B, cv.gn_cluster, st, tn->use_pdl));
+  ROHM_CUDA(tn->ctx, launch_gn_mish(a, B, cv.gn_cluster, st, tn->use_pdl,
+                                    tn->lengths.empty() ? nullptr : tn->clip_off[level]));
   tn->launches++;
   return ROHM_OK;
 }
@@ -662,6 +706,11 @@ extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* cons
   }
   if (const char* env = getenv("ROHM_B200_TRAJ_PARALLEL")) tn->parallel = env[0] != '0';
   if (const char* env = getenv("ROHM_B200_TRAJ_SPLITK")) tn->use_splitk = env[0] != '0';
+  for (int l = 0; l < kLevels; ++l) {
+    tn->clip_off[l] = static_cast<int*>(tn->pool.bytes(static_cast<int64_t>(max_batch + 1) * sizeof(int)));
+    tn->row_mask[l] = static_cast<unsigned char*>(tn->pool.bytes(rows_of(tn, l)));
+    if (!tn->clip_off[l] || !tn->row_mask[l]) return fail(ctx, ROHM_ERR_CUDA, "clip table alloc failed");
+  }
   if (tn->use_splitk) {
     for (int br = 0; br < 2; ++br) {
       tn->scratchSplit[br] = tn->pool.floats(kMaxSplits * max_padded);
@@ -798,22 +847,27 @@ extern "C" void rohm_trajnet_destroy(rohm_trajnet* tn) { delete tn; }
 extern "C" int rohm_trajnet_launches_per_forward(const rohm_trajnet* tn) { return tn ? tn->launches : 0; }
 
 static int trajnet_pack(rohm_trajnet* tn, const float* x, const Act& a, int B, cudaStream_t st) {
-  const int64_t total = static_cast<int64_t>(B) * tn->T * a.C;
-  pack_rows_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(x, a.hi, a.lo, tn->T, tn->Tp[0], a.C, a.ld,
-                                                                             total, tn->kind == kKindF16 ? 1 : 0);
+  const bool packed = !tn->lengths.empty();
+  const int64_t total = static_cast<int64_t>(B) * (packed ? tn->Tp[0] : tn->T) * a.C;
+  (packed ? pack_rows_kernel<true> : pack_rows_kernel<false>)<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
+      x, a.hi, a.lo, tn->T, tn->Tp[0], a.C, a.ld, total, tn->kind == kKindF16 ? 1 : 0, packed ? tn->clip_off[0] : nullptr);
   ROHM_CUDA(tn->ctx, cudaGetLastError());
   tn->launches++;
   return ROHM_OK;
 }
 
 // Step-invariant part: the condition pyramid (and control_zero_conv_0).  cond: [B, T, cond_dim];
-// control_cond: [B, T, control_cond_dim] or NULL for the vanilla network.
+// control_cond: [B, T, control_cond_dim] or NULL for the vanilla network.  Packed clips (rohm_trajnet_set_lengths) read only
+// each clip's real frames.
 extern "C" int rohm_trajnet_set_cond(rohm_trajnet* tn, const float* cond, const float* control_cond, int B, void* stream) {
   if (tn == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = tn->ctx;
   rohm::DeviceGuard device_guard__(ctx);
   if (cond == nullptr || B <= 0 || B > tn->max_batch || (tn->control && control_cond == nullptr))
     return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_set_cond: bad arguments (B=%d, capacity %d)", B, tn->max_batch);
+  if (!tn->lengths.empty() && static_cast<int>(tn->lengths.size()) != B)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_set_cond: lengths were set for %d clips, the call has B=%d",
+                static_cast<int>(tn->lengths.size()), B);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int saved = tn->launches;
   TRY(trajnet_pack(tn, cond, tn->cin, B, st));
@@ -827,6 +881,54 @@ extern "C" int rohm_trajnet_set_cond(rohm_trajnet* tn, const float* cond, const 
   }
   tn->launches = saved;
   tn->cond_B = B;
+  tn->cond_lengths = tn->lengths;
+  return ROHM_OK;
+}
+
+extern "C" int rohm_trajnet_set_lengths(rohm_trajnet* tn, const int* lengths, int B) {
+  if (tn == nullptr) return ROHM_ERR_INVALID;
+  rohm_ctx* ctx = tn->ctx;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (lengths == nullptr) {
+    if (tn->lengths.empty()) return ROHM_OK;
+    // the uniform layout's pad rows of the packed inputs must be zero again (packing writes real frames there), and a
+    // forward still in flight may be reading them
+    ROHM_CUDA(ctx, cudaDeviceSynchronize());
+    for (const Act* a : {&tn->xin, &tn->cin, &tn->kin}) {
+      if (a->hi == nullptr) continue;
+      const size_t n = static_cast<size_t>(rows_of(tn, 0)) * a->ld * sizeof(float);
+      ROHM_CUDA(ctx, cudaMemset(a->hi, 0, n));
+      ROHM_CUDA(ctx, cudaMemset(a->lo, 0, n));
+    }
+    tn->lengths.clear();
+    return ROHM_OK;
+  }
+  if (B <= 0 || B > tn->max_batch)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_set_lengths: B=%d outside the created capacity %d", B, tn->max_batch);
+  for (int b = 0; b < B; ++b)
+    if (lengths[b] < 16 || lengths[b] > tn->T || lengths[b] % 16 != 0)
+      return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_set_lengths: lengths[%d] = %d must be a multiple of 16 in [16, %d]",
+                  b, lengths[b], tn->T);
+  std::vector<int> v(lengths, lengths + B);
+  if (v == tn->lengths) return ROHM_OK;
+  std::vector<int> off[kLevels];
+  std::vector<unsigned char> mask[kLevels];
+  for (int l = 0; l < kLevels; ++l) {
+    off[l].assign(B + 1, 0);
+    for (int b = 0; b < B; ++b) {
+      const int rows = (v[b] + 32) >> l, real = v[b] >> l;
+      off[l][b + 1] = off[l][b] + rows;
+      for (int t = 0; t < rows; ++t) mask[l].push_back(t < real ? 1 : 0);
+    }
+  }
+  // a forward still in flight on any stream may be reading the tables being replaced
+  ROHM_CUDA(ctx, cudaDeviceSynchronize());
+  for (int l = 0; l < kLevels; ++l) {
+    ROHM_CUDA(ctx, cudaMemcpy(tn->clip_off[l], off[l].data(), (B + 1) * sizeof(int), cudaMemcpyHostToDevice));
+    ROHM_CUDA(ctx, cudaMemcpy(tn->row_mask[l], mask[l].data(), mask[l].size(), cudaMemcpyHostToDevice));
+    tn->packed_rows[l] = off[l][B];
+  }
+  tn->lengths = std::move(v);
   return ROHM_OK;
 }
 
@@ -883,7 +985,9 @@ static int trajnet_forward_launches(rohm_trajnet* tn, const float* x_t, const in
   TRY(run_conv(tn, tn->final_o, B, st));
   const Act& o = tn->final_o.out;
   const int64_t total = static_cast<int64_t>(B) * tn->T * o.C;
-  unpack_rows_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(o.f32, out, tn->T, tn->Tp[0], o.C, o.ld, total);
+  const bool packed = !tn->lengths.empty();
+  (packed ? unpack_rows_kernel<true> : unpack_rows_kernel<false>)<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
+      o.f32, out, tn->T, tn->Tp[0], o.C, o.ld, total, packed ? tn->clip_off[0] : nullptr);
   ROHM_CUDA(ctx, cudaGetLastError());
   tn->launches++;
   return ROHM_OK;
@@ -898,17 +1002,22 @@ static int trajnet_forward_or_step(rohm_trajnet* tn, const float* x_t, const int
   if (x_t == nullptr || time == nullptr || out == nullptr) return fail(ctx, ROHM_ERR_INVALID, "rohm_trajnet_forward: null pointer");
   if (B != tn->cond_B)
     return fail(ctx, ROHM_ERR_STATE, "rohm_trajnet_forward: B=%d but set_cond was called with B=%d", B, tn->cond_B);
+  if (tn->lengths != tn->cond_lengths)
+    return fail(ctx, ROHM_ERR_STATE, "rohm_trajnet_forward: the clip lengths differ from those set_cond was called with");
   auto launches = [&](cudaStream_t st) {
     const int rc = trajnet_forward_launches(tn, x_t, time, out, B, st);
     if (rc != ROHM_OK || step == nullptr) return rc;
     tn->launches++;
     return launch_ddpm_step(ctx, *step, st, tn->use_pdl);
   };
-  std::vector<KernelPatch> patches = {{pack_rows_kernel, arg<kPackRowsX>(x_t)},
+  const bool packed = !tn->lengths.empty();
+  std::vector<KernelPatch> patches = {{packed ? pack_rows_kernel<true> : pack_rows_kernel<false>, arg<kPackRowsX>(x_t)},
                                       {trajnet_time_kernel, arg<kTrajnetTimeT>(time)},
-                                      {unpack_rows_kernel, arg<kUnpackRowsOut>(out)}};
+                                      {packed ? unpack_rows_kernel<true> : unpack_rows_kernel<false>,
+                                       arg<kUnpackRowsOut>(out)}};
   if (step != nullptr) patches.push_back(ddpm_step_patch(*step));
-  return tn->graphs.run(ctx, B, tn->T, step != nullptr, false, static_cast<cudaStream_t>(stream), launches, patches);
+  return tn->graphs.run(ctx, B, tn->T, step != nullptr, false, static_cast<cudaStream_t>(stream), launches, patches,
+                        tn->lengths);
 }
 
 // TrajNet.forward (trajnet.py:177-275).  x_t: [B, T, traj_dim]; time: int64 [B]; out: [B, T, traj_dim].

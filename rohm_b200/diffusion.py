@@ -489,7 +489,7 @@ class _GaussianDiffusion:
         if device is None:
             device = next(model.parameters()).device
         assert isinstance(shape, (tuple, list))
-        self._begin_loop(model)
+        self._begin_loop(model, batch=batch, shape=shape)
         img = noise if noise is not None else self._randn(*shape, device=device)
         if skip_timesteps and init_image is None:
             init_image = th.zeros_like(img)
@@ -529,6 +529,12 @@ class _GaussianDiffusion:
                                   cond_fn_with_grad=cond_fn_with_grad, **kw)
 
 
+def _refuse_losses_with_lengths(batch, compute_loss):
+    if compute_loss and batch.get('lengths') is not None:
+        raise RohmB200Error("eval_losses: the loss dictionary over clips with batch['lengths'] is out of scope (it "
+                            "would average over padded frames); pass compute_loss=False and score each clip's frames")
+
+
 class GaussianDiffusionPoseNet(_GaussianDiffusion):
     _POSENET = True
 
@@ -538,9 +544,7 @@ class GaussianDiffusionPoseNet(_GaussianDiffusion):
                     const_noise=False, cur_epoch=0, timestep_respacing='', compute_loss=True, smplx_model=None, epoch=0):
         """The call the drivers make (test_amass_full.py:376, test_posenet.py:178): full sampling loop, then the
         optional loss dict.  Returns (loss_dict | None, model_output)."""
-        if compute_loss and batch.get('lengths') is not None:
-            raise RohmB200Error("eval_losses: the loss dictionary over clips with batch['lengths'] is out of scope (it "
-                                "would average over padded frames); pass compute_loss=False and score each clip's frames")
+        _refuse_losses_with_lengths(batch, compute_loss)
         model_output = self._sample_for_eval(model, batch, shape, progress, clip_denoised, cond_fn_with_grad,
                                              timestep_respacing, grad_type=grad_type, early_stop=early_stop)
         inner = model.model if isinstance(model, _WrappedModel) else model
@@ -573,6 +577,7 @@ class GaussianDiffusionTrajNet(_GaussianDiffusion):
                     cond_fn_with_grad=False, cond_grad_weight=1.0, dump_steps=None, const_noise=False, cur_epoch=0,
                     timestep_respacing='', compute_loss=True, smplx_model=None):
         """test_amass_full.py:245/259, test_trajnet.py:154.  Returns (loss_dict | None, model_output)."""
+        _refuse_losses_with_lengths(batch, compute_loss)
         model_output = self._sample_for_eval(model, batch, shape, progress, clip_denoised, cond_fn_with_grad,
                                              timestep_respacing)
         inner = model.model if isinstance(model, _WrappedModel) else model

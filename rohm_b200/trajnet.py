@@ -138,8 +138,19 @@ class TrajNet(nn.Module):
         from .eval_losses import trajnet_losses
         return trajnet_losses(self, batch, model_output, smplx_model)
 
+    def clip_lengths(self, batch, shape=None, grad_type=None):
+        """batch['lengths'] checked against the padded [B, T, traj_dim] batch (`shape`, else batch['x_t'] / batch['cond']),
+        as a tuple of ints; None when the key is absent.  Raises RohmB200Error before anything runs on the device.
+        grad_type: accepted for the sampling loops' call; TrajNet has no guidance."""
+        from .trajnet_engine import clip_lengths
+        if shape is None and isinstance(batch, dict):
+            shape = (batch['x_t'] if 'x_t' in batch else batch['cond']).shape
+        return clip_lengths(batch, shape)
+
     def forward(self, batch, time):
         """batch['x_t'], batch['cond']: [bs, T, traj_dim]; batch['control_cond']: [bs, T, 272] when trajcontrol;
-        time: [bs] int -> [bs, T, traj_dim] (reconstructed trajectory representation at timestep 0)."""
+        time: [bs] int -> [bs, T, traj_dim] (reconstructed trajectory representation at timestep 0).
+        batch['lengths'] (optional, integer [bs], multiples of 16 with 16 <= lengths[b] <= T): clip b has lengths[b] real
+        frames; those depend on that clip alone, later frames come out zero and their inputs are never read."""
         from .trajnet_engine import run_forward
         return run_forward(self, batch, time)

@@ -37,6 +37,8 @@ class TrajNetEngine:
         self.cond_ref, self.cond_version = None, -1
         self.control_ref, self.control_version = None, -1
         self.cond_B = -1
+        self.cond_lengths = None  # the per-clip lengths the pyramid was embedded with
+        self.lengths = None  # what rohm_trajnet_set_lengths last received (None: uniform clips)
         from . import ops
         self.op_key = ops.register_engine(self)
         del sd
@@ -57,6 +59,15 @@ class TrajNetEngine:
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def set_lengths(self, lengths):
+        """Per-clip lengths (a tuple of ints) for the following set_cond / forward / sample_step, or None."""
+        if lengths == self.lengths:
+            return
+        arr = None if lengths is None else (C.c_int * len(lengths))(*lengths)
+        rc = self.lib.rohm_trajnet_set_lengths(self.handle, arr, 0 if lengths is None else len(lengths))
+        _lib.check(rc, self.ctx)
+        self.lengths = lengths
 
     def set_cond(self, cond, control_cond):
         rc = self.lib.rohm_trajnet_set_cond(self.handle, C.c_void_p(cond.data_ptr()),
@@ -139,16 +150,37 @@ def prepare(module, batch, time):
     control = batch.get('control_cond') if module.trajcontrol else None
     if module.trajcontrol and (control is None or tuple(control.shape) != (B, T, module.control_cond_dim)):
         raise RohmB200Error(f"TrajNet(trajcontrol=True): batch['control_cond'] must be [B, T, {module.control_cond_dim}]")
+    lengths = clip_lengths(batch, x_t.shape) if batch.get('lengths') is not None else None
     e = get_engine(module, B, T, x_t.device)
     # object identity + version (never data_ptr: freed addresses are recycled by the caching allocator)
     same = (e.cond_ref is cond and e.cond_version == cond._version and e.cond_B == B and e.control_ref is control and
-            (control is None or e.control_version == control._version))
+            (control is None or e.control_version == control._version) and e.cond_lengths == lengths)
     if not same:
         if _fingerprint(module) != module._engine_fingerprint:  # parameters changed since the weights were packed
             module._engine = None
             e = get_engine(module, B, T, x_t.device)
+        e.set_lengths(lengths)
         e.set_cond(_f32c(cond), _f32c(control) if control is not None else None)
-        e.cond_ref, e.cond_version, e.cond_B = cond, cond._version, B
+        e.cond_ref, e.cond_version, e.cond_B, e.cond_lengths = cond, cond._version, B, lengths
         e.control_ref, e.control_version = control, (control._version if control is not None else -1)
     ts = time.to(device=x_t.device, dtype=torch.int64).contiguous()
     return e, _f32c(x_t), ts
+
+
+def clip_lengths(batch, shape):
+    """batch['lengths'] checked against the padded [B, T, *] batch `shape`, as a tuple of ints; None when the key is absent.
+    Raises RohmB200Error before anything runs on the device."""
+    lengths = batch.get('lengths') if isinstance(batch, dict) else None
+    if lengths is None:
+        return None
+    B, T = int(shape[0]), int(shape[1])
+    if (not isinstance(lengths, torch.Tensor) or lengths.is_floating_point() or lengths.is_complex() or
+            lengths.dtype == torch.bool or tuple(lengths.shape) != (B,)):
+        raise RohmB200Error(f"TrajNet: batch['lengths'] must be an integer tensor of shape [{B}], got "
+                            f"{getattr(lengths, 'dtype', type(lengths))} {tuple(getattr(lengths, 'shape', ()))}")
+    values = tuple(int(v) for v in lengths.tolist())
+    bad = [(b, v) for b, v in enumerate(values) if not (16 <= v <= T and v % 16 == 0)]
+    if bad:
+        raise RohmB200Error(f"TrajNet: batch['lengths'] must be multiples of 16 in [16, T={T}] (four stride-2 stages); "
+                            f"lengths[{bad[0][0]}] = {bad[0][1]}")
+    return values
