@@ -274,6 +274,21 @@ ROHM_API int rohm_body_from_repr_layout(rohm_body* bd, const float* x, int chann
                                         const float* stdv, int B, int T, float* joints, int num_joints, float* vertices,
                                         void* stream);
 
+/* Clips of different lengths inside padded tensors.  The *_lengths entry points below take the clips' frame counts as device
+ * arrays: lengths (int[B], in the frame count of the tensor that call works on) and, where frames are packed, clip_off
+ * (int[B+1], the exclusive prefix sum of lengths) with total_frames = clip_off[B] known to the host.  Packed means frame t of
+ * clip b is row clip_off[b] + t.  Frames past a clip are never read, whatever they hold; where an output keeps its padded
+ * shape its frames past a clip are written as zeros. */
+
+/* rohm_body_from_repr_layout over clips of lengths[b] <= T frames (lengths[b] = clip_off[b+1] - clip_off[b]) of the padded
+ * x: joints [total_frames, num_joints, 3] and optionally vertices [total_frames, V, 3] (pitched as rohm_body_forward's),
+ * packed.  FK and the blend GEMM + skinning run over total_frames rows, and total_frames (not B*T) is what has to fit the
+ * handle's capacity.  Each frame equals the same frame of the padded call bit for bit. */
+ROHM_API int rohm_body_from_repr_lengths(rohm_body* bd, const float* x, int channels_last, const float* mean,
+                                         const float* stdv, int B, int T, const int* lengths, const int* clip_off,
+                                         int64_t total_frames, float* joints, int num_joints, float* vertices,
+                                         void* stream);
+
 /* PoseNet.guide_skating_with_smpl(compute_grad='x_0'): grad [B,294,1,T] = d(-(loss_smpl + loss_abs))/d x0 with the
  * channels [0,22) and the 4 contact channels zero.  Analytic VJP (no autograd); all-zero if nothing skates.
  * loss_out: optional device float[4] = {sum_abs, count_abs, sum_smpl, count_smpl}. */
@@ -320,6 +335,16 @@ ROHM_API int rohm_traj_glue(rohm_body* bd, const float* traj_out, int traj_dim, 
                             const float* traj_mean, const float* traj_std, const float* pose_mean, const float* pose_std,
                             int B, int T, float* composite_out, float* traj_full_out, void* stream);
 
+/* rohm_traj_glue over clips of 2 <= lengths[b] <= T trajectory frames: composite_out [B,T,294] and traj_full_out [B,T-1,22]
+ * keep their padded shapes, rows lengths[b] .. T-1 (composite) and lengths[b]-1 .. T-2 (traj_full) are zeros.  FK runs over
+ * the total_frames packed frames; the first-NaN search and repair of the root quaternion and the velocity pairs stay inside
+ * the clip (the repair of frame 0 takes frame lengths[b]-1).  A clip's rows equal rohm_traj_glue on the clip alone with
+ * T = lengths[b], bit for bit. */
+ROHM_API int rohm_traj_glue_lengths(rohm_body* bd, const float* traj_out, int traj_dim, const float* repr_clean,
+                                    const float* traj_mean, const float* traj_std, const float* pose_mean,
+                                    const float* pose_std, int B, int T, const int* lengths, const int* clip_off,
+                                    int64_t total_frames, float* composite_out, float* traj_full_out, void* stream);
+
 /* The last stage of rohm_traj_glue on its own: get_repr_smplx's trajectory block (motion_representation.py:187-282) from
  * joints [B,T,22,3], global-orient axis-angles [B*T,3] and translations [B*T,3] -> traj_full_out [B,T-1,22], z-scored with
  * mean/stdv (the first 22 entries are read).  2 <= T <= 8192, as rohm_traj_glue. */
@@ -327,10 +352,22 @@ ROHM_API int rohm_traj_repr_from_joints(rohm_ctx* ctx, const float* joints, cons
                                         const float* transl, const float* mean, const float* stdv, int B, int T,
                                         float* traj_full_out, void* stream);
 
+/* The last stage of rohm_traj_glue_lengths on its own: joints [total_frames,22,3], global_orient_aa / transl
+ * [total_frames,3] packed -> traj_full_out [B,T-1,22] (padded, zeros from row lengths[b]-1). */
+ROHM_API int rohm_traj_repr_from_joints_lengths(rohm_ctx* ctx, const float* joints, const float* global_orient_aa,
+                                                const float* transl, const float* mean, const float* stdv, int B, int T,
+                                                const int* lengths, const int* clip_off, float* traj_full_out,
+                                                void* stream);
+
 /* test_amass_full.py:256-258: control_cond [B,T,cond_feats] from the PoseNet output pose_out [B,traj_feats+cond_feats,1,Tp]
  * (frames [0,Tp) copied, frames [Tp,T) repeat frame Tp-1). */
 ROHM_API int rohm_pose_to_control_cond(rohm_ctx* ctx, const float* pose_out, int B, int Tp, int T, int traj_feats,
                                        int cond_feats, float* control_cond, void* stream);
+
+/* rohm_pose_to_control_cond over clips of 1 <= lengths[b] <= Tp pose frames (T > Tp): control frames [0, lengths[b]) are
+ * the clip's pose frames, frame lengths[b] repeats the clip's own last pose frame, later frames are zeros. */
+ROHM_API int rohm_pose_to_control_cond_lengths(rohm_ctx* ctx, const float* pose_out, int B, int Tp, int T, int traj_feats,
+                                               int cond_feats, const int* lengths, float* control_cond, void* stream);
 
 /* test_amass_full.py:320-370: PoseNet condition cond_out [B,294,1,Tp] = src (channel-major [B,294,1,src_T] or channels-last
  * [B,src_T,294]) with channels [0,22) replaced by traj_full [B,Tp,22] (NULL keeps src) and channels >= 22 zeroed where
@@ -340,6 +377,12 @@ ROHM_API int rohm_build_pose_cond(rohm_ctx* ctx, const float* src, int src_chann
                                   const unsigned char* chan_keep, const int* frame_lo, const int* frame_hi,
                                   int zero_contact, int B, int Tp, float* cond_out, void* stream);
 
+/* rohm_build_pose_cond over clips of 1 <= lengths[b] <= Tp frames: frames past a clip are zeros in every channel. */
+ROHM_API int rohm_build_pose_cond_lengths(rohm_ctx* ctx, const float* src, int src_channel_major, int src_T,
+                                          const float* traj_full, const unsigned char* chan_keep, const int* frame_lo,
+                                          const int* frame_hi, int zero_contact, int B, int Tp, const int* lengths,
+                                          float* cond_out, void* stream);
+
 /* rot6d_to_rotmat (quaternion.py:482-501) and rotation_matrix_to_angle_axis (konia_transform.py:317-340 -> :350-444 ->
  * :561-631) on n 6-D rotations: aa [n,3] and/or rotmat [n,9] (row-major), either may be NULL. */
 ROHM_API int rohm_rot6d_to_aa(rohm_ctx* ctx, const float* rot6d, int64_t n, float* aa, float* rotmat, void* stream);
@@ -348,6 +391,13 @@ ROHM_API int rohm_rot6d_to_aa(rohm_ctx* ctx, const float* rot6d, int64_t n, floa
  * representation in either layout -> joints [B,T,22,3]. */
 ROHM_API int rohm_joints_from_traj(rohm_ctx* ctx, const float* x, int channels_last, const float* mean, const float* stdv,
                                    int B, int T, int relative, float* joints, void* stream);
+
+/* rohm_joints_from_traj over clips of 1 <= lengths[b] <= T frames of the padded x -> packed joints [total_frames,22,3].  The
+ * absolute mode has no dependence between frames and runs one thread per packed frame; the relative mode keeps one thread
+ * per clip and stops at lengths[b]. */
+ROHM_API int rohm_joints_from_traj_lengths(rohm_ctx* ctx, const float* x, int channels_last, const float* mean,
+                                           const float* stdv, int B, int T, const int* lengths, const int* clip_off,
+                                           int64_t total_frames, int relative, float* joints, void* stream);
 
 #ifdef __cplusplus
 }

@@ -72,17 +72,23 @@ SIGNATURES = {
     "rohm_body_forward": (_i, [_p, _p, _p, _p, _p, _i64, _p, _i, _p, _p]),
     "rohm_body_from_repr": (_i, [_p, _p, _p, _p, _i, _i, _p, _i, _p, _p]),
     "rohm_body_from_repr_layout": (_i, [_p, _p, _i, _p, _p, _i, _i, _p, _i, _p, _p]),
+    "rohm_body_from_repr_lengths": (_i, [_p, _p, _i, _p, _p, _i, _i, _p, _p, _i64, _p, _i, _p, _p]),
     "rohm_skating_guidance": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p]),
     "rohm_skating_guidance_lengths": (_i, [_p, _p, _p, _p, _p, _i, _i, _p, _p, _p]),
     "rohm_skating_guidance_sums": (_i, [_p, _p, _p, _p, _i, _i, _p, _p]),
     "rohm_skating_guidance_backward": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p]),
     "rohm_projection_guidance": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _i, _p, _p, _p]),
     "rohm_traj_glue": (_i, [_p, _p, _i, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p]),
+    "rohm_traj_glue_lengths": (_i, [_p, _p, _i, _p, _p, _p, _p, _p, _i, _i, _p, _p, _i64, _p, _p, _p]),
     "rohm_traj_repr_from_joints": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p]),
+    "rohm_traj_repr_from_joints_lengths": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p]),
     "rohm_pose_to_control_cond": (_i, [_p, _p, _i, _i, _i, _i, _i, _p, _p]),
+    "rohm_pose_to_control_cond_lengths": (_i, [_p, _p, _i, _i, _i, _i, _i, _p, _p, _p]),
     "rohm_build_pose_cond": (_i, [_p, _p, _i, _i, _p, _p, _p, _p, _i, _i, _i, _p, _p]),
+    "rohm_build_pose_cond_lengths": (_i, [_p, _p, _i, _i, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p]),
     "rohm_rot6d_to_aa": (_i, [_p, _p, _i64, _p, _p, _p]),
     "rohm_joints_from_traj": (_i, [_p, _p, _i, _p, _p, _i, _i, _i, _p, _p]),
+    "rohm_joints_from_traj_lengths": (_i, [_p, _p, _i, _p, _p, _i, _i, _p, _p, _i64, _i, _p, _p]),
 }
 
 _lock = threading.Lock()

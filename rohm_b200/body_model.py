@@ -90,13 +90,27 @@ class BodyKernels:
         _lib.check(rc, self.ctx)
         return joints, verts
 
-    def from_repr(self, x, mean, std, want_vertices, num_joints=22, channels_last=False):
+    def from_repr(self, x, mean, std, want_vertices, num_joints=22, channels_last=False, lengths=None):
         """x: normalised [B, 294, 1, T] (or [B, T, 294] with channels_last) -> joints [B, T, num_joints, 3]
-        (+ vertices [B, T, V, 3])."""
+        (+ vertices [B, T, V, 3]).  lengths (int32 device [B], see glue.device_lengths): only the clips' own frames are
+        computed -> packed joints [sum of lengths, num_joints, 3] (+ vertices [sum of lengths, V, 3]), each frame equal to
+        the same frame of the padded call; the sum of lengths, not B * T, has to fit the handle's capacity."""
         if channels_last:
             B, T, _ = x.shape
         else:
             B, _, _, T = x.shape
+        if lengths is not None:
+            from .glue import clip_layout
+            clip_off, total = clip_layout(lengths, B, T, "from_repr")
+            joints = torch.empty(total, num_joints, 3, device=self.device)
+            verts = self._vertex_buffer(total) if want_vertices else None
+            rc = self.lib.rohm_body_from_repr_lengths(
+                self.handle, C.c_void_p(x.data_ptr()), int(bool(channels_last)), C.c_void_p(mean.data_ptr()),
+                C.c_void_p(std.data_ptr()), B, T, C.c_void_p(lengths.data_ptr()), C.c_void_p(clip_off.data_ptr()), total,
+                C.c_void_p(joints.data_ptr()), num_joints, C.c_void_p(verts.data_ptr() if verts is not None else 0),
+                self._stream())
+            _lib.check(rc, self.ctx)
+            return (joints, verts) if want_vertices else joints
         joints = torch.empty(B * T, num_joints, 3, device=self.device)
         verts = self._vertex_buffer(B * T) if want_vertices else None
         rc = self.lib.rohm_body_from_repr_layout(self.handle, C.c_void_p(x.data_ptr()), int(bool(channels_last)),
@@ -156,11 +170,21 @@ class BodyKernels:
         _lib.check(rc, self.ctx)
         return (grad, loss) if want_loss else grad
 
-    def traj_glue(self, traj_out, repr_clean, traj_mean, traj_std, pose_mean, pose_std):
-        """test_amass_full.py:268-311 on the device: -> (composite [B,T,294], traj_full [B,T-1,22])."""
+    def traj_glue(self, traj_out, repr_clean, traj_mean, traj_std, pose_mean, pose_std, lengths=None):
+        """test_amass_full.py:268-311 on the device: -> (composite [B,T,294], traj_full [B,T-1,22]).  lengths: (int32 device
+        [B], clip_off int32 device [B+1], their sum) for clips of different lengths (rohm_traj_glue_lengths)."""
         B, T, D = traj_out.shape
         composite = torch.empty(B, T, 294, device=self.device)
         traj_full = torch.empty(B, T - 1, 22, device=self.device)
+        if lengths is not None:
+            lens, clip_off, total = lengths
+            rc = self.lib.rohm_traj_glue_lengths(
+                self.handle, C.c_void_p(traj_out.data_ptr()), D, C.c_void_p(repr_clean.data_ptr()),
+                C.c_void_p(traj_mean.data_ptr()), C.c_void_p(traj_std.data_ptr()), C.c_void_p(pose_mean.data_ptr()),
+                C.c_void_p(pose_std.data_ptr()), B, T, C.c_void_p(lens.data_ptr()), C.c_void_p(clip_off.data_ptr()), total,
+                C.c_void_p(composite.data_ptr()), C.c_void_p(traj_full.data_ptr()), self._stream())
+            _lib.check(rc, self.ctx)
+            return composite, traj_full
         rc = self.lib.rohm_traj_glue(self.handle, C.c_void_p(traj_out.data_ptr()), D, C.c_void_p(repr_clean.data_ptr()),
                                      C.c_void_p(traj_mean.data_ptr()), C.c_void_p(traj_std.data_ptr()),
                                      C.c_void_p(pose_mean.data_ptr()), C.c_void_p(pose_std.data_ptr()), B, T,

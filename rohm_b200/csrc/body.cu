@@ -352,17 +352,23 @@ constexpr int kChAngle = 0, kChRootPos = 2, kChHeight = 6, kChRot6d = 7, kChTran
               kChBodyPose = 154, kChBetas = 280, kChContact = 290;
 
 // element (b, c, t) of x lives at x[b * sb + c * sc + t * st]: channel-major [B,294,1,T] (sb = 294 T, sc = T, st = 1,
-// PoseNet tensors) or channels-last [B,T,294] (sb = 294 T, sc = 1, st = 294: TrajNet-side / driver tensors)
+// PoseNet tensors) or channels-last [B,T,294] (sb = 294 T, sc = 1, st = 294: TrajNet-side / driver tensors).
+// kLengths: clip b has clip_off[b + 1] - clip_off[b] <= T frames; only those are gathered, packed: frame t of clip b
+// becomes row f = clip_off[b] + t of go / bp / betas / transl (`total` rows), and frames past a clip are never read.
+template <bool kLengths>
 __global__ void repr_to_smplx_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int64_t st,
                                      const float* __restrict__ mean,
                                      const float* __restrict__ stdv, int B, int T, float* __restrict__ go,
-                                     float* __restrict__ bp, float* __restrict__ betas, float* __restrict__ transl) {
+                                     float* __restrict__ bp, float* __restrict__ betas, float* __restrict__ transl,
+                                     const int* __restrict__ clip_off, int64_t total) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const int64_t frames = static_cast<int64_t>(B) * T;
+  const int64_t frames = kLengths ? total : static_cast<int64_t>(B) * T;
   if (i >= frames * kBodyJ) return;
   const int j = static_cast<int>(i % kBodyJ);
   const int64_t f = i / kBodyJ;
-  const int b = static_cast<int>(f / T), t = static_cast<int>(f % T);
+  const int b = kLengths ? clip_of_frame(clip_off, B, static_cast<int>(f)) : static_cast<int>(f / T);
+  const int t = kLengths ? static_cast<int>(f) - clip_off[b] : static_cast<int>(f % T);
+  if (kLengths && (t >= clip_off[b + 1] - clip_off[b] || t >= T)) return;
   auto ch = [&](int c) { return x[b * sb + c * sc + t * st] * stdv[c] + mean[c]; };
   const int c0 = (j == 0) ? kChRot6d : kChBodyPose + (j - 1) * 6;
   float r6[6];
@@ -974,10 +980,32 @@ extern "C" int rohm_body_from_repr_layout(rohm_body* bd, const float* x, int cha
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t total = N * kBodyJ;
   const int64_t sb = static_cast<int64_t>(kC) * T, sc = channels_last ? 1 : T, stt = channels_last ? kC : 1;
-  repr_to_smplx_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(x, sb, sc, stt, mean, stdv, B, T, bd->go,
-                                                                                 bd->bp, bd->betas, bd->transl);
+  repr_to_smplx_kernel<false><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
+      x, sb, sc, stt, mean, stdv, B, T, bd->go, bd->bp, bd->betas, bd->transl, nullptr, 0);
   ROHM_CUDA(ctx, cudaGetLastError());
   return rohm_body_forward(bd, bd->go, bd->bp, bd->betas, bd->transl, N, joints, num_joints, vertices, stream);
+}
+
+// The same over clips of different lengths inside the padded x: only the clips' own frames are gathered, so FK and the
+// blend GEMM + skinning run over total_frames rows and write packed joints / vertices.
+extern "C" int rohm_body_from_repr_lengths(rohm_body* bd, const float* x, int channels_last, const float* mean,
+                                           const float* stdv, int B, int T, const int* lengths, const int* clip_off,
+                                           int64_t total_frames, float* joints, int num_joints, float* vertices,
+                                           void* stream) {
+  if (bd == nullptr) return ROHM_ERR_INVALID;
+  rohm_ctx* ctx = bd->ctx;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (!x || !mean || !stdv || !lengths || !clip_off || B <= 0 || T <= 0 || total_frames < B ||
+      total_frames > static_cast<int64_t>(B) * T || total_frames > INT32_MAX || total_frames > bd->max_frames)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_body_from_repr_lengths: bad arguments (B=%d T=%d, %lld frames in the clips, "
+                "capacity %lld)", B, T, static_cast<long long>(total_frames), static_cast<long long>(bd->max_frames));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t total = total_frames * kBodyJ;
+  const int64_t sb = static_cast<int64_t>(kC) * T, sc = channels_last ? 1 : T, stt = channels_last ? kC : 1;
+  repr_to_smplx_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
+      x, sb, sc, stt, mean, stdv, B, T, bd->go, bd->bp, bd->betas, bd->transl, clip_off, total_frames);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return rohm_body_forward(bd, bd->go, bd->bp, bd->betas, bd->transl, total_frames, joints, num_joints, vertices, stream);
 }
 
 // guide_skating_with_smpl (posenet.py:196-257): grad [B, 294, 1, T] = d(-(loss_smpl + loss_abs))/dx0 with the

@@ -10,6 +10,7 @@
 //   rohm_joints_from_traj       motion_representation.py:285-371 recover_from_repr_smpl 'joint_abs_traj' / 'joint_rel_traj'
 //   rohm_projection_guidance    model/posenet.py:260-317 guide_2d_projection_with_smpl, analytic VJP instead of autograd
 #include <cmath>
+#include <cstdint>
 
 #include <cooperative_groups.h>
 
@@ -37,11 +38,20 @@ __device__ __forceinline__ int traj_channel(int k, int traj_dim) {
   return k == 0 ? 0 : (k <= 2 ? k + 1 : (k == 3 ? 6 : (k <= 9 ? k + 3 : k + 6)));
 }
 
-// composite[b,t,:] = clean[b,t,:] with the trajectory channels replaced by the TrajNet output (both normalised)
+// composite[b,t,:] = clean[b,t,:] with the trajectory channels replaced by the TrajNet output (both normalised).
+// kLengths: rows are [B, T] and clip b has lengths[b] frames; rows past a clip are written as zeros, their sources not read.
+template <bool kLengths>
 __global__ void compose_repr_kernel(const float* __restrict__ traj, int traj_dim, const float* __restrict__ clean,
-                                    float* __restrict__ out, int64_t rows) {
+                                    float* __restrict__ out, int64_t rows, const int* __restrict__ lengths, int T) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= rows * kC) return;
+  if constexpr (kLengths) {
+    const int64_t row = i / kC;
+    if (row % T >= lengths[row / T]) {
+      out[i] = 0.0f;
+      return;
+    }
+  }
   out[i] = clean[i];
   const int c = static_cast<int>(i % kC);
   const int64_t r = i / kC;
@@ -87,9 +97,15 @@ constexpr int kReprMaxCluster = 8;       // CTAs per clip: clips of up to 8192 f
 // clip-wide first NaN frame (rank 0's first_nan) and the quaternions of frames in other CTAs are reached through
 // distributed shared memory.  joints: [B, T, 22, 3]; go: [B*T, 3] axis-angle global orient; transl: [B*T, 3]; out:
 // [B, T-1, 22] z-scored with the PoseNet dataset statistics.
+// kLengths: clip b has len = lengths[b] <= T frames and joints / go / transl hold the clips packed, clip b's frames from row
+// clip_off[b].  The cluster shape still follows T (it is a property of the launch), so a CTA whose frames all lie past its
+// clip computes nothing but takes part in every cluster barrier.  The NaN search, the wrap-around source of the repair and
+// the velocity pairs stop at len; out keeps its padded [B, T-1, 22] shape, rows len-1 .. T-2 are written as zeros.
+template <bool kLengths>
 __global__ void traj_full_repr_kernel(const float* __restrict__ joints, const float* __restrict__ go,
                                       const float* __restrict__ transl, const float* __restrict__ mean,
-                                      const float* __restrict__ stdv, int T, float* __restrict__ out) {
+                                      const float* __restrict__ stdv, int T, float* __restrict__ out,
+                                      const int* __restrict__ lengths, const int* __restrict__ clip_off) {
   extern __shared__ float sm[];
   cg::cluster_group cluster = cg::this_cluster();
   const int ncta = static_cast<int>(cluster.num_blocks()), rank = static_cast<int>(cluster.block_rank());
@@ -102,10 +118,13 @@ __global__ void traj_full_repr_kernel(const float* __restrict__ joints, const fl
   auto sync = [&] { ncta > 1 ? cluster.sync() : __syncthreads(); };
   const int b = blockIdx.x / ncta;
   const int t = rank * rows + threadIdx.x;
-  const bool mine = threadIdx.x < rows && t < T;  // this thread's frame exists and belongs to this CTA
-  if (rank == 0 && threadIdx.x == 0) first_nan = T;
+  const int len = kLengths ? lengths[b] : T;  // frames of this clip
+  // row of the clip's frame 0 in joints / go / transl
+  auto row0 = [&] { return kLengths ? static_cast<int64_t>(clip_off[b]) : static_cast<int64_t>(b) * T; };
+  const bool mine = threadIdx.x < rows && t < len;  // this thread's frame exists and belongs to this CTA
+  if (rank == 0 && threadIdx.x == 0) first_nan = len;
   sync();
-  const float* P = joints + (static_cast<int64_t>(b) * T + (mine ? t : 0)) * kBodyJ * 3;
+  const float* P = joints + (row0() + (mine ? t : 0)) * kBodyJ * 3;
   auto J = [&](const float* base, int j) { return V3{base[j * 3], base[j * 3 + 1], base[j * 3 + 2]}; };
   if (mine) {
     // forward direction from hips (2 = right, 1 = left) and shoulders (17 = right, 16 = left)
@@ -125,17 +144,17 @@ __global__ void traj_full_repr_kernel(const float* __restrict__ joints, const fl
   if (rank == 0 && threadIdx.x == 0) {
     // "several frames have nan values": the reference repairs the FIRST one only, with its predecessor
     // (frame -1 = the last frame when the first frame is the bad one), then pins frame 0 to the identity
-    if (first_nan < T) {
-      const int dst = first_nan, src = first_nan > 0 ? first_nan - 1 : T - 1;
+    if (first_nan < len) {
+      const int dst = first_nan, src = first_nan > 0 ? first_nan - 1 : len - 1;
       peer(qw, dst / rows)[dst % rows] = peer(qw, src / rows)[src % rows];
       peer(qz, dst / rows)[dst % rows] = peer(qz, src / rows)[src % rows];
     }
     qw[0] = 1.0f, qz[0] = 0.0f;
   }
   sync();
-  if (mine && t < T - 1) {
+  if (mine && t < len - 1) {
     const float* P1 = P + kBodyJ * 3;
-    const int64_t f = static_cast<int64_t>(b) * T + t;
+    const int64_t f = row0() + t;
     float o[kTrajFull];
     // frame t + 1 is the next CTA's first when t is this CTA's last
     const int u = threadIdx.x + 1 < rows ? threadIdx.x + 1 : 0, ur = threadIdx.x + 1 < rows ? rank : rank + 1;
@@ -178,31 +197,41 @@ __global__ void traj_full_repr_kernel(const float* __restrict__ joints, const fl
     float* dst = out + (static_cast<int64_t>(b) * (T - 1) + t) * kTrajFull;
 #pragma unroll
     for (int c = 0; c < kTrajFull; ++c) dst[c] = (o[c] - mean[c]) / stdv[c];
+  } else if (kLengths && threadIdx.x < rows && t < T - 1) {
+    float* dst = out + (static_cast<int64_t>(b) * (T - 1) + t) * kTrajFull;
+#pragma unroll
+    for (int c = 0; c < kTrajFull; ++c) dst[c] = 0.0f;
   }
   if (ncta > 1) cluster.sync();  // peers may still read this CTA's quaternions
 }
 
-// B clusters of ceil(T / 1024) CTAs; T <= kReprFramesPerCta * kReprMaxCluster (checked by the callers)
+// B clusters of ceil(T / 1024) CTAs; T <= kReprFramesPerCta * kReprMaxCluster (checked by the callers).  lengths / clip_off
+// (device int[B] / int[B + 1]) select the instance for packed clips of different lengths.
 cudaError_t launch_traj_full_repr(const float* joints, const float* go, const float* transl, const float* mean,
-                                  const float* stdv, int B, int T, float* out, cudaStream_t st) {
+                                  const float* stdv, int B, int T, float* out, cudaStream_t st,
+                                  const int* lengths = nullptr, const int* clip_off = nullptr) {
   const int n = (T + kReprFramesPerCta - 1) / kReprFramesPerCta;
   const int rows = (T + n - 1) / n;
-  return launch_chain(traj_full_repr_kernel, dim3(static_cast<unsigned>(B * n)), dim3((rows + 31) / 32 * 32),
-                      2 * rows * sizeof(float), st, ChainAttrs(false, static_cast<unsigned>(n)), joints, go, transl, mean,
-                      stdv, T, out);
+  return launch_chain(lengths != nullptr ? traj_full_repr_kernel<true> : traj_full_repr_kernel<false>,
+                      dim3(static_cast<unsigned>(B * n)), dim3((rows + 31) / 32 * 32), 2 * rows * sizeof(float), st,
+                      ChainAttrs(false, static_cast<unsigned>(n)), joints, go, transl, mean, stdv, T, out, lengths, clip_off);
 }
 
 // control_cond[b, t, :] = pose_out[b, 22 + c, 0, min(t, Tp-1)]   (Tp = T-1 frames of PoseNet output; last frame repeated)
+// kLengths: clip b has lengths[b] <= Tp pose frames; its own last pose frame is the one repeated (into control frame
+// lengths[b]), later control frames are zero and pose_out is not read past the clip.
+template <bool kLengths>
 __global__ void pose_to_control_kernel(const float* __restrict__ pose_out, int Tp, int T, int traj, int ncond,
-                                       float* __restrict__ control) {
+                                       float* __restrict__ control, const int* __restrict__ lengths) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   const int tx = threadIdx.x, ty = threadIdx.y;
   for (int j = ty; j < 32; j += 8) {
     const int c = c0 + j, t = t0 + tx;
-    const int ts = t < Tp ? t : Tp - 1;
-    tile[j][tx] = (c < ncond && t < T) ? pose_out[(static_cast<int64_t>(b) * (traj + ncond) + traj + c) * Tp + ts] : 0.0f;
+    const int len = kLengths ? lengths[b] : Tp;  // pose frames of this clip; control frames [0, len] are real
+    const int ts = t < len ? t : len - 1;
+    tile[j][tx] = (c < ncond && t < (kLengths ? len + 1 : T)) ? pose_out[(static_cast<int64_t>(b) * (traj + ncond) + traj + c) * Tp + ts] : 0.0f;
   }
   __syncthreads();
   for (int j = ty; j < 32; j += 8) {
@@ -211,25 +240,29 @@ __global__ void pose_to_control_kernel(const float* __restrict__ pose_out, int T
   }
 }
 
-// PoseNet condition [B, 294, 1, Tp] from a source in either layout, the trajectory block and the occlusion masks
+// PoseNet condition [B, 294, 1, Tp] from a source in either layout, the trajectory block and the occlusion masks.
+// kLengths: clip b has lengths[b] <= Tp frames; later frames are written as zeros, src and traj_full are not read there.
+template <bool kLengths>
 __global__ void build_pose_cond_kernel(const float* __restrict__ src, int src_channel_major, int src_T,
                                        const float* __restrict__ traj_full, const unsigned char* __restrict__ chan_keep,
                                        const int* __restrict__ frame_lo, const int* __restrict__ frame_hi,
-                                       int zero_contact, int Tp, float* __restrict__ out) {
+                                       int zero_contact, int Tp, float* __restrict__ out,
+                                       const int* __restrict__ lengths) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   const int tx = threadIdx.x, ty = threadIdx.y;
+  const int len = kLengths ? lengths[b] : Tp;  // frames of this clip
   // load tile[c][t]
   if (src_channel_major) {
     for (int j = ty; j < 32; j += 8) {
       const int c = c0 + j, t = t0 + tx;
-      tile[j][tx] = (c < kC && t < Tp) ? src[(static_cast<int64_t>(b) * kC + c) * src_T + t] : 0.0f;
+      tile[j][tx] = (c < kC && t < len) ? src[(static_cast<int64_t>(b) * kC + c) * src_T + t] : 0.0f;
     }
   } else {
     for (int j = ty; j < 32; j += 8) {
       const int t = t0 + j, c = c0 + tx;
-      tile[tx][j] = (c < kC && t < Tp) ? src[(static_cast<int64_t>(b) * src_T + t) * kC + c] : 0.0f;
+      tile[tx][j] = (c < kC && t < len) ? src[(static_cast<int64_t>(b) * src_T + t) * kC + c] : 0.0f;
     }
   }
   __syncthreads();
@@ -238,7 +271,9 @@ __global__ void build_pose_cond_kernel(const float* __restrict__ src, int src_ch
     const int c = c0 + j, t = t0 + tx;
     if (c >= kC || t >= Tp) continue;
     float v = tile[j][tx];
-    if (c < kTrajFull) {
+    if (kLengths && t >= len) {
+      v = 0.0f;
+    } else if (c < kTrajFull) {
       if (traj_full != nullptr) v = traj_full[(static_cast<int64_t>(b) * Tp + t) * kTrajFull + c];
     } else {
       const bool masked = (chan_keep != nullptr && chan_keep[c] == 0) || (t >= lo && t < hi) ||
@@ -271,14 +306,23 @@ __global__ void rot6d_to_aa_kernel(const float* __restrict__ r6, int64_t n, floa
 // recover_from_repr_smpl, 'joint_abs_traj' (mode 0) and 'joint_rel_traj' (mode 1): one thread per clip walks the frames
 // (the relative mode is two running sums over time; the absolute mode has no dependency but shares the code).
 // x element (b, c, t) at x[b*sb + c*sc + t*st], normalised; joints [B, T, 22, 3].
+// kLengths: clip b has lengths[b] <= T frames and joints holds the clips packed ([sum of lengths, 22, 3], clip b from row
+// clip_off[b]).  The absolute mode runs one thread per packed frame (total of them), the relative mode keeps one thread
+// per clip and stops at the clip's length.
+template <bool kLengths>
 __global__ void joints_from_traj_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int64_t st,
                                         const float* __restrict__ mean, const float* __restrict__ stdv, int B, int T,
-                                        int mode, float* __restrict__ joints) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
+                                        int mode, float* __restrict__ joints, const int* __restrict__ lengths,
+                                        const int* __restrict__ clip_off, int total) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;  // clip, or packed frame (kLengths, absolute mode)
+  if (i >= (kLengths && mode == 0 ? total : B)) return;
+  const int b = kLengths && mode == 0 ? clip_of_frame(clip_off, B, i) : i;
+  const int t_begin = kLengths && mode == 0 ? i - clip_off[b] : 0;
+  const int t_end = kLengths ? (mode == 0 ? t_begin + 1 : lengths[b]) : T;
+  if (kLengths && t_begin >= lengths[b]) return;
   float ang = 0.0f;            // running root angle (rel)
   float px = 0.0f, py = 0.0f;  // running root position (rel)
-  for (int t = 0; t < T; ++t) {
+  for (int t = t_begin; t < t_end; ++t) {
     auto ch = [&](int c, int tt) { return x[b * sb + c * sc + tt * st] * stdv[c] + mean[c]; };
     float a, rx, ry;
     const float rz = ch(kChHeight, t);
@@ -302,7 +346,7 @@ __global__ void joints_from_traj_kernel(const float* __restrict__ x, int64_t sb,
     }
     float sn, cs;
     sincosf(a, &sn, &cs);
-    float* o = joints + (static_cast<int64_t>(b) * T + t) * kBodyJ * 3;
+    float* o = joints + (kLengths ? static_cast<int64_t>(clip_off[b]) + t : static_cast<int64_t>(b) * T + t) * kBodyJ * 3;
     o[0] = rx, o[1] = ry, o[2] = rz;
     for (int j = 1; j < kBodyJ; ++j) {
       const V3 v = {ch(kChLocalPos + j * 3, t), ch(kChLocalPos + j * 3 + 1, t), ch(kChLocalPos + j * 3 + 2, t)};
@@ -472,12 +516,43 @@ extern "C" int rohm_traj_glue(rohm_body* bd, const float* traj_out, int traj_dim
                 "per clip)", T, kReprFramesPerCta * kReprMaxCluster, kReprMaxCluster, kReprFramesPerCta);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t total = N * kC;
-  compose_repr_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(traj_out, traj_dim, repr_clean,
-                                                                                composite_out, N);
+  compose_repr_kernel<false><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(traj_out, traj_dim, repr_clean,
+                                                                                       composite_out, N, nullptr, T);
   ROHM_CUDA(ctx, cudaGetLastError());
   int rc = rohm_body_from_repr_layout(bd, composite_out, 1, traj_mean, traj_std, B, T, bd->jwork, kBodyJ, nullptr, stream);
   if (rc != ROHM_OK) return rc;
   ROHM_CUDA(ctx, launch_traj_full_repr(bd->jwork, bd->go, bd->transl, pose_mean, pose_std, B, T, traj_full_out, st));
+  return ROHM_OK;
+}
+
+extern "C" int rohm_traj_glue_lengths(rohm_body* bd, const float* traj_out, int traj_dim, const float* repr_clean,
+                                      const float* traj_mean, const float* traj_std, const float* pose_mean,
+                                      const float* pose_std, int B, int T, const int* lengths, const int* clip_off,
+                                      int64_t total_frames, float* composite_out, float* traj_full_out, void* stream) {
+  if (bd == nullptr) return ROHM_ERR_INVALID;
+  rohm_ctx* ctx = bd->ctx;
+  rohm::DeviceGuard device_guard__(ctx);
+  const int64_t N = static_cast<int64_t>(B) * T;
+  if (!traj_out || !repr_clean || !traj_mean || !traj_std || !pose_mean || !pose_std || !composite_out || !traj_full_out ||
+      !lengths || !clip_off || B <= 0 || T < 2 || total_frames < 2 * static_cast<int64_t>(B) || total_frames > N ||
+      total_frames > bd->max_frames || (traj_dim != 13 && (traj_dim < 1 || traj_dim > kTrajFull)))
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_glue_lengths: bad arguments (B=%d T=%d traj_dim=%d, %lld frames in the "
+                "clips, capacity %lld frames)", B, T, traj_dim, static_cast<long long>(total_frames),
+                static_cast<long long>(bd->max_frames));
+  if (T > kReprFramesPerCta * kReprMaxCluster)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_glue_lengths: T=%d frames exceeds %d (one cluster of at most %d CTAs of %d "
+                "frames per clip)", T, kReprFramesPerCta * kReprMaxCluster, kReprMaxCluster, kReprFramesPerCta);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t total = N * kC;
+  compose_repr_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(traj_out, traj_dim, repr_clean,
+                                                                                      composite_out, N, lengths, T);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  // FK over the clips' own frames only: packed joints in jwork, packed global orientations / translations in the handle
+  int rc = rohm_body_from_repr_lengths(bd, composite_out, 1, traj_mean, traj_std, B, T, lengths, clip_off, total_frames,
+                                       bd->jwork, kBodyJ, nullptr, stream);
+  if (rc != ROHM_OK) return rc;
+  ROHM_CUDA(ctx, launch_traj_full_repr(bd->jwork, bd->go, bd->transl, pose_mean, pose_std, B, T, traj_full_out, st, lengths,
+                                       clip_off));
   return ROHM_OK;
 }
 
@@ -496,6 +571,22 @@ extern "C" int rohm_traj_repr_from_joints(rohm_ctx* ctx, const float* joints, co
   return ROHM_OK;
 }
 
+extern "C" int rohm_traj_repr_from_joints_lengths(rohm_ctx* ctx, const float* joints, const float* global_orient_aa,
+                                                  const float* transl, const float* mean, const float* stdv, int B, int T,
+                                                  const int* lengths, const int* clip_off, float* traj_full_out,
+                                                  void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (!joints || !global_orient_aa || !transl || !mean || !stdv || !traj_full_out || !lengths || !clip_off || B <= 0 || T < 2)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_repr_from_joints_lengths: bad arguments");
+  if (T > kReprFramesPerCta * kReprMaxCluster)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_repr_from_joints_lengths: T=%d frames exceeds %d (one cluster of at most "
+                "%d CTAs of %d frames per clip)", T, kReprFramesPerCta * kReprMaxCluster, kReprMaxCluster, kReprFramesPerCta);
+  ROHM_CUDA(ctx, launch_traj_full_repr(joints, global_orient_aa, transl, mean, stdv, B, T, traj_full_out,
+                                       static_cast<cudaStream_t>(stream), lengths, clip_off));
+  return ROHM_OK;
+}
+
 extern "C" int rohm_pose_to_control_cond(rohm_ctx* ctx, const float* pose_out, int B, int Tp, int T, int traj_feats,
                                          int cond_feats, float* control_cond, void* stream) {
   if (ctx == nullptr) return ROHM_ERR_INVALID;
@@ -503,8 +594,21 @@ extern "C" int rohm_pose_to_control_cond(rohm_ctx* ctx, const float* pose_out, i
   if (!pose_out || !control_cond || B <= 0 || Tp <= 0 || T < Tp || traj_feats < 0 || cond_feats <= 0 || B > 65535)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_pose_to_control_cond: bad arguments");
   dim3 grid((T + 31) / 32, (cond_feats + 31) / 32, B);
-  pose_to_control_kernel<<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(pose_out, Tp, T, traj_feats,
-                                                                                    cond_feats, control_cond);
+  pose_to_control_kernel<false><<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
+      pose_out, Tp, T, traj_feats, cond_feats, control_cond, nullptr);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return ROHM_OK;
+}
+
+extern "C" int rohm_pose_to_control_cond_lengths(rohm_ctx* ctx, const float* pose_out, int B, int Tp, int T, int traj_feats,
+                                                 int cond_feats, const int* lengths, float* control_cond, void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (!pose_out || !control_cond || !lengths || B <= 0 || Tp <= 0 || T <= Tp || traj_feats < 0 || cond_feats <= 0 || B > 65535)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_pose_to_control_cond_lengths: bad arguments");
+  dim3 grid((T + 31) / 32, (cond_feats + 31) / 32, B);
+  pose_to_control_kernel<true><<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
+      pose_out, Tp, T, traj_feats, cond_feats, control_cond, lengths);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }
@@ -517,8 +621,24 @@ extern "C" int rohm_build_pose_cond(rohm_ctx* ctx, const float* src, int src_cha
   if (!src || !cond_out || B <= 0 || Tp <= 0 || src_T < Tp || B > 65535 || ((frame_lo == nullptr) != (frame_hi == nullptr)))
     return fail(ctx, ROHM_ERR_INVALID, "rohm_build_pose_cond: bad arguments");
   dim3 grid((Tp + 31) / 32, (kC + 31) / 32, B);
-  build_pose_cond_kernel<<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
-      src, src_channel_major, src_T, traj_full, chan_keep, frame_lo, frame_hi, zero_contact, Tp, cond_out);
+  build_pose_cond_kernel<false><<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
+      src, src_channel_major, src_T, traj_full, chan_keep, frame_lo, frame_hi, zero_contact, Tp, cond_out, nullptr);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return ROHM_OK;
+}
+
+extern "C" int rohm_build_pose_cond_lengths(rohm_ctx* ctx, const float* src, int src_channel_major, int src_T,
+                                            const float* traj_full, const unsigned char* chan_keep, const int* frame_lo,
+                                            const int* frame_hi, int zero_contact, int B, int Tp, const int* lengths,
+                                            float* cond_out, void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (!src || !cond_out || !lengths || B <= 0 || Tp <= 0 || src_T < Tp || B > 65535 ||
+      ((frame_lo == nullptr) != (frame_hi == nullptr)))
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_build_pose_cond_lengths: bad arguments");
+  dim3 grid((Tp + 31) / 32, (kC + 31) / 32, B);
+  build_pose_cond_kernel<true><<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
+      src, src_channel_major, src_T, traj_full, chan_keep, frame_lo, frame_hi, zero_contact, Tp, cond_out, lengths);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }
@@ -542,8 +662,27 @@ extern "C" int rohm_joints_from_traj(rohm_ctx* ctx, const float* x, int channels
   if (!x || !mean || !stdv || !joints || B <= 0 || T <= 0)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_joints_from_traj: bad arguments");
   const int64_t sb = static_cast<int64_t>(kC) * T, sc = channels_last ? 1 : T, stt = channels_last ? kC : 1;
-  joints_from_traj_kernel<<<(B + 31) / 32, 32, 0, static_cast<cudaStream_t>(stream)>>>(x, sb, sc, stt, mean, stdv, B, T,
-                                                                                     relative ? 1 : 0, joints);
+  joints_from_traj_kernel<false><<<(B + 31) / 32, 32, 0, static_cast<cudaStream_t>(stream)>>>(
+      x, sb, sc, stt, mean, stdv, B, T, relative ? 1 : 0, joints, nullptr, nullptr, 0);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return ROHM_OK;
+}
+
+extern "C" int rohm_joints_from_traj_lengths(rohm_ctx* ctx, const float* x, int channels_last, const float* mean,
+                                             const float* stdv, int B, int T, const int* lengths, const int* clip_off,
+                                             int64_t total_frames, int relative, float* joints, void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (!x || !mean || !stdv || !joints || !lengths || !clip_off || B <= 0 || T <= 0 || total_frames < B ||
+      total_frames > static_cast<int64_t>(B) * T || total_frames > INT32_MAX)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_joints_from_traj_lengths: bad arguments");
+  const int64_t sb = static_cast<int64_t>(kC) * T, sc = channels_last ? 1 : T, stt = channels_last ? kC : 1;
+  // absolute mode: frames are independent, one thread per packed frame; relative mode: one thread per clip
+  const int64_t threads = relative ? B : total_frames;
+  const int block = relative ? 32 : 128;
+  joints_from_traj_kernel<true><<<static_cast<unsigned>((threads + block - 1) / block), block, 0,
+                                  static_cast<cudaStream_t>(stream)>>>(
+      x, sb, sc, stt, mean, stdv, B, T, relative ? 1 : 0, joints, lengths, clip_off, static_cast<int>(total_frames));
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }

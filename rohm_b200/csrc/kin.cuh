@@ -99,5 +99,19 @@ __device__ __forceinline__ M3 rodrigues(V3 r) {
 }
 
 
+// Packed frame f of a batch of clips with different lengths -> its clip b: clip_off (int[B + 1], the exclusive prefix sum of
+// the clips' lengths) has clip_off[b] <= f < clip_off[b + 1].  A binary search per thread (log2 B reads of a table every
+// thread of the launch shares, L1-resident) instead of a frame -> clip map, which would cost a scan launch and a 4-byte read
+// per frame for tables of a handful of clips.
+__device__ __forceinline__ int clip_of_frame(const int* __restrict__ clip_off, int B, int f) {
+  int lo = 0, hi = B;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (clip_off[mid] <= f) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
 }  // namespace kin
 }  // namespace rohm

@@ -59,9 +59,11 @@ def _unit(device):
 
 
 def recover_from_repr_smpl(data_dict, recover_mode='joint_abs_traj', smplx_model=None, return_verts=False,
-                           return_full_joints=False):
+                           return_full_joints=False, lengths=None):
     """joints [bs, T, 22, 3] (and vertices [bs, T, V, 3] with return_verts) from the motion representation:
-    'joint_abs_traj' / 'joint_rel_traj' (joint-based, quaternion path) or 'smplx_params' (6-D -> axis-angle -> SMPL-X)."""
+    'joint_abs_traj' / 'joint_rel_traj' (joint-based, quaternion path) or 'smplx_params' (6-D -> axis-angle -> SMPL-X).
+    lengths (int32 device [bs], see glue.device_lengths): clip b has lengths[b] <= T frames; only those are computed and
+    the results are packed: joints [sum of lengths, 22, 3], vertices [sum of lengths, V, 3]."""
     if recover_mode not in ('joint_abs_traj', 'joint_rel_traj', 'smplx_params'):
         raise RohmB200Error(f"recover_from_repr_smpl: recover_mode {recover_mode!r} is not one of 'joint_abs_traj', "
                             "'joint_rel_traj', 'smplx_params'")
@@ -70,15 +72,23 @@ def recover_from_repr_smpl(data_dict, recover_mode='joint_abs_traj', smplx_model
         raise RohmB200Error("recover_from_repr_smpl: tensors must live on a CUDA device (no CPU path)")
     mean, std = _unit(row.device)
     B, T = row.shape[0], row.shape[1]
+    if lengths is not None and len(lead) != 2:
+        raise RohmB200Error("recover_from_repr_smpl: lengths go with [bs, T, d] entries")
     if recover_mode != 'smplx_params':
-        j = glue.joints_from_traj_repr(row, mean, std, relative=(recover_mode == 'joint_rel_traj'), channels_last=True)
-        return j.reshape(lead + (22, 3))
+        j = glue.joints_from_traj_repr(row, mean, std, relative=(recover_mode == 'joint_rel_traj'), channels_last=True,
+                                       lengths=lengths)
+        return j if lengths is not None else j.reshape(lead + (22, 3))
     if return_full_joints:
         raise RohmB200Error("recover_from_repr_smpl(return_full_joints=True): the 72 landmark joints beyond the 55 "
                             "kinematic ones are not evaluated by the CUDA body kernels (no inference driver asks for them)")
     if smplx_model is None:
         raise RohmB200Error("recover_from_repr_smpl('smplx_params') needs smplx_model")
     from .body_model import kernels_for
+    if lengths is not None:
+        _, total = glue.clip_layout(lengths, B, T, "recover_from_repr_smpl")
+        k = kernels_for(smplx_model, row.device, total, with_vertices=bool(return_verts))
+        return k.from_repr(row, mean, std, want_vertices=bool(return_verts), num_joints=22, channels_last=True,
+                           lengths=lengths)
     k = kernels_for(smplx_model, row.device, B * T, with_vertices=bool(return_verts))
     res = k.from_repr(row, mean, std, want_vertices=bool(return_verts), num_joints=22, channels_last=True)
     if return_verts:
