@@ -80,6 +80,23 @@ ROHM_API int rohm_ddpm_step_philox(rohm_ctx* ctx, const float* x0, const float* 
                                    int64_t coef_clip_stride, uint64_t seed, uint64_t offset, uint64_t* offset_increment,
                                    void* stream);
 
+/* Per-clip noise streams.  out: a padded batch of B clips of C channels and T frames, [B][C][T] (channels_last = 0, PoseNet
+ * [B, C, 1, T]) or [B][T][C] (channels_last = 1, TrajNet [B, T, C]); clip b has lengths_host[b] real frames (1..T; NULL:
+ * T).  streams: device uint64 [B][2], clip b's (seed, offset) at draw 0.  Clip b's real frames receive exactly what
+ * torch.randn(S_b, generator=g_b) returns for a CUDA generator in state (seed_b, offset_b + draw * inc_b), S_b being
+ * [1, C, 1, n_b] or [1, n_b, C]; its padded frames receive 0.  offset_increments (host uint64 [B], optional) receives inc_b,
+ * what torch advances that generator's offset by for this draw.  At most 256 clips. */
+ROHM_API int rohm_randn_clips(rohm_ctx* ctx, float* out, int B, int C, int T, int channels_last, const int* lengths_host,
+                              const uint64_t* streams, uint64_t draw, uint64_t* offset_increments, void* stream);
+
+/* rohm_ddpm_step with noise = rohm_randn_clips(same arguments) drawn inside the kernel: bit-identical to rohm_ddpm_step on
+ * that noise tensor, and 0 in every clip's padded frames.  coef: device float[8] (coef_clip_stride = 0) or [B][8]
+ * (coef_clip_stride = 8). */
+ROHM_API int rohm_ddpm_step_philox_clips(rohm_ctx* ctx, const float* x0, const float* x_t, const float* grad0,
+                                         const float* grad1, int n_grads, float* out, int B, int C, int T, int channels_last,
+                                         const int* lengths_host, const float* coef, int64_t coef_clip_stride,
+                                         const uint64_t* streams, uint64_t draw, uint64_t* offset_increments, void* stream);
+
 /* q_sample :192-210:  out = sqrt_ac*x_start + sqrt_1m_ac*noise. */
 ROHM_API int rohm_q_sample(rohm_ctx* ctx, const float* x_start, const float* noise, float* out, int64_t n, float sqrt_ac,
                   float sqrt_one_minus_ac, void* stream);
@@ -169,6 +186,13 @@ ROHM_API int rohm_posenet_sample_step(rohm_posenet* pn, const float* x_t, const 
                                       float* x_next, const float* coef_row, uint64_t seed, uint64_t offset,
                                       uint64_t* offset_increment, int B, int T, void* stream);
 
+/* rohm_posenet_sample_step with per-clip noise streams: the update is rohm_ddpm_step_philox_clips over the engine's current
+ * lengths (rohm_posenet_set_lengths), so clip b's frames past its length come out 0 in x_next.  streams: device
+ * uint64 [B][2]; draw: this step's draw index; offset_increments: host uint64 [B] (optional), see rohm_randn_clips. */
+ROHM_API int rohm_posenet_sample_step_clips(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* x0_out,
+                                            float* x_next, const float* coef_row, const uint64_t* streams, uint64_t draw,
+                                            uint64_t* offset_increments, int B, int T, void* stream);
+
 /* Same as rohm_posenet_forward but with CUDA events recorded on `stream` around every kernel launch; synchronises the
  * stream and returns, per category {0: tensor-core GEMM, 1: attention, 2: LayerNorm, 3: pack/unpack/time-token}, the
  * summed device milliseconds (host float[4]) and the number of launches (host int[4]).  For bench.py's roofline. */
@@ -226,6 +250,11 @@ ROHM_API int rohm_trajnet_forward(rohm_trajnet* tn, const float* x_t, const int6
 ROHM_API int rohm_trajnet_sample_step(rohm_trajnet* tn, const float* x_t, const int64_t* time, float* x0_out, float* x_next,
                                       const float* coef_row, uint64_t seed, uint64_t offset, uint64_t* offset_increment, int B,
                                       void* stream);
+/* rohm_trajnet_sample_step with per-clip noise streams over the engine's current lengths; arguments as
+ * rohm_posenet_sample_step_clips. */
+ROHM_API int rohm_trajnet_sample_step_clips(rohm_trajnet* tn, const float* x_t, const int64_t* time, float* x0_out,
+                                            float* x_next, const float* coef_row, const uint64_t* streams, uint64_t draw,
+                                            uint64_t* offset_increments, int B, void* stream);
 ROHM_API int rohm_trajnet_set_option(rohm_trajnet* tn, int option, int value); /* 0: CUDA-graph replay, 1: programmatic dependent launch (both default 1) */
 ROHM_API int rohm_trajnet_launches_per_forward(const rohm_trajnet* tn);
 

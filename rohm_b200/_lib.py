@@ -45,6 +45,9 @@ SIGNATURES = {
     "rohm_ddpm_step": (_i, [_p, _p, _p, _p, _p, _p, _i, _p, _i64, _i64, _p, _i64, _p]),
     "rohm_ddpm_step_philox": (_i, [_p, _p, _p, _p, _p, _i, _p, _i64, _i64, _p, _i64, C.c_uint64, C.c_uint64,
                                     C.POINTER(C.c_uint64), _p]),
+    "rohm_randn_clips": (_i, [_p, _p, _i, _i, _i, _i, C.POINTER(_i), _p, C.c_uint64, C.POINTER(C.c_uint64), _p]),
+    "rohm_ddpm_step_philox_clips": (_i, [_p, _p, _p, _p, _p, _i, _p, _i, _i, _i, _i, C.POINTER(_i), _p, _i64, _p,
+                                          C.c_uint64, C.POINTER(C.c_uint64), _p]),
     "rohm_q_sample": (_i, [_p, _p, _p, _p, _i64, _f, _f, _p]),
     "rohm_ddim_step": (_i, [_p, _p, _p, _p, _p, _i64, _f, _f, _f, _f, _f, _p]),
     "rohm_posenet_create": (_i, [_p, C.POINTER(PoseNetW), _i, _i, _i, C.POINTER(_p)]),
@@ -53,7 +56,8 @@ SIGNATURES = {
     "rohm_posenet_set_lengths": (_i, [_p, C.POINTER(_i), _i]),
     "rohm_posenet_forward": (_i, [_p, _p, _p, _p, _i, _i, _p]),
     "rohm_posenet_sample_step": (_i, [_p, _p, _p, _p, _p, _p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), _i, _i, _p]),
-    "rohm_posenet_profile": (_i, [_p, _p, _p, _p, _i, _i, _p, C.POINTER(C.c_float), C.POINTER(C.c_int)]),
+    "rohm_posenet_sample_step_clips": (_i, [_p, _p, _p, _p, _p, _p, _p, C.c_uint64, C.POINTER(C.c_uint64), _i, _i, _p]),
+    "rohm_posenet_profile":(_i, [_p, _p, _p, _p, _i, _i, _p, C.POINTER(C.c_float), C.POINTER(C.c_int)]),
     "rohm_posenet_set_option": (_i, [_p, _i, _i]),
     "rohm_posenet_launches_per_forward": (_i, [_p]),
     "rohm_trajnet_create": (_i, [_p, _i, C.POINTER(C.c_char_p), C.POINTER(_p), C.POINTER(_i64), _i, _i, _i, _i, _i, _i,
@@ -63,7 +67,8 @@ SIGNATURES = {
     "rohm_trajnet_set_lengths": (_i, [_p, C.POINTER(_i), _i]),
     "rohm_trajnet_forward": (_i, [_p, _p, _p, _p, _i, _p]),
     "rohm_trajnet_sample_step": (_i, [_p, _p, _p, _p, _p, _p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), _i, _p]),
-    "rohm_trajnet_set_option": (_i, [_p, _i, _i]),
+    "rohm_trajnet_sample_step_clips": (_i, [_p, _p, _p, _p, _p, _p, _p, C.c_uint64, C.POINTER(C.c_uint64), _i, _p]),
+    "rohm_trajnet_set_option":(_i, [_p, _i, _i]),
     "rohm_trajnet_launches_per_forward": (_i, [_p]),
     "rohm_body_create": (_i, [_p, _p, _p, _i, _p, _p, _p, C.POINTER(C.c_int), _i, _i64, _i, _i, C.POINTER(_p)]),
     "rohm_body_destroy": (None, [_p]),

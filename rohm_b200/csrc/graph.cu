@@ -18,7 +18,7 @@ ForwardGraphs::~ForwardGraphs() {
   if (capture_stream_) cudaStreamDestroy(capture_stream_);
 }
 
-int ForwardGraphs::run(rohm_ctx* ctx, int B, int T, bool with_step, bool eager, cudaStream_t st,
+int ForwardGraphs::run(rohm_ctx* ctx, int B, int T, StepKind step, bool eager, cudaStream_t st,
                        const std::function<int(cudaStream_t)>& launches, const std::vector<KernelPatch>& patches,
                        const std::vector<int>& lengths) {
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -27,10 +27,10 @@ int ForwardGraphs::run(rohm_ctx* ctx, int B, int T, bool with_step, bool eager, 
 
   Entry* g = nullptr;
   for (Entry& e : graphs_)
-    if (e.B == B && e.T == T && e.with_step == with_step && e.lengths == lengths) g = &e;
+    if (e.B == B && e.T == T && e.step == step && e.lengths == lengths) g = &e;
   if (g == nullptr) {
     Entry e;
-    e.B = B, e.T = T, e.with_step = with_step;
+    e.B = B, e.T = T, e.step = step;
     e.lengths = lengths;
     const int rc = capture(ctx, launches, patches, &e);
     if (rc != ROHM_OK) return rc;

@@ -60,7 +60,11 @@ class KernelPatch {
   int n_ = 0;
 };
 
-// An engine's captured forwards, keyed by (B, T, with_step, per-clip lengths); at most kMaxGraphs, the oldest evicted first.
+// What a forward graph appends to the forward: nothing, the single-stream update (DdpmStep) or the per-clip one
+// (DdpmClipStep).  Part of the graph key, since the two updates are different kernels.
+enum StepKind : int { kNoStep = 0, kStepSingleStream = 1, kStepPerClip = 2 };
+
+// An engine's captured forwards, keyed by (B, T, step kind, per-clip lengths); at most kMaxGraphs, the oldest evicted first.
 class ForwardGraphs {
  public:
   static constexpr size_t kMaxGraphs = 8;
@@ -72,11 +76,11 @@ class ForwardGraphs {
   ~ForwardGraphs();
 
   // Issues one forward on `st`.  launches(stream) issues its kernels on `stream`.  That runs directly on `st` when `eager`,
-  // when graphs are off, or when the caller is capturing `st`.  Otherwise the graph of (B, T, with_step) is replayed with
+  // when graphs are off, or when the caller is capturing `st`.  Otherwise the graph of (B, T, step) is replayed with
   // the arguments of `patches` set; launches() is captured into it on first use.  Every call passes the same kernels in
   // `patches` for the same key.  `lengths` (empty: uniform clips) is part of the key: the packed layout it implies sets
   // grids and row counts that a replay cannot change.
-  int run(rohm_ctx* ctx, int B, int T, bool with_step, bool eager, cudaStream_t st,
+  int run(rohm_ctx* ctx, int B, int T, StepKind step, bool eager, cudaStream_t st,
           const std::function<int(cudaStream_t)>& launches, const std::vector<KernelPatch>& patches,
           const std::vector<int>& lengths = {});
   void clear() { graphs_.clear(); }  // the next run() of every key captures again
@@ -90,7 +94,7 @@ class ForwardGraphs {
   };
   struct Entry {
     int B = 0, T = 0;
-    bool with_step = false;
+    StepKind step = kNoStep;
     std::vector<int> lengths;
     std::unique_ptr<std::remove_pointer_t<cudaGraph_t>, DestroyGraph> graph;  // owns the captured arguments in `params`
     std::unique_ptr<std::remove_pointer_t<cudaGraphExec_t>, DestroyExec> exec;
@@ -122,5 +126,35 @@ int ddpm_step_plan(rohm_ctx* ctx, DdpmStep* s, uint64_t* offset_increment);
 int launch_ddpm_step(rohm_ctx* ctx, const DdpmStep& s, cudaStream_t st, bool pdl);
 // The update node's per-call arguments in a replayed graph.
 KernelPatch ddpm_step_patch(const DdpmStep& s);
+
+// Per-clip noise streams.  Clip b of a padded batch draws its noise from its own Philox stream, exactly as
+// torch.randn(S_b, generator=g_b) draws it for the shape S_b the clip has alone: [1, C, 1, n_b] channel-major (PoseNet,
+// padded layout [B][C][T]) or [1, n_b, C] channels-last (TrajNet, padded layout [B][T][C]).  Clip b uses the launch
+// geometry torch's normal_ kernel picks for C * n_b elements; the launch concatenates the clips' grids, and blk[] (a prefix
+// sum of the per-clip block counts) tells each block its clip.  Padded frames get zero.
+constexpr int kMaxStreamClips = 256;  // keeps ClipPlan, a kernel parameter, within the 4 KB parameter space
+struct ClipPlan {
+  int B, C, T;
+  int channels_last;                 // 0: [B][C][T], 1: [B][T][C]
+  int blk[kMaxStreamClips + 1];      // clip b owns blocks [blk[b], blk[b + 1]); blk[B] = the grid
+  int n[kMaxStreamClips];            // real frames of clip b
+};
+// Fills *p for B clips of C channels padded to T frames; lengths (host, NULL: all T).  incs (host [B], optional): what
+// clip b's generator offset advances by per draw, as torch would advance it for the clip alone.
+int clip_plan(rohm_ctx* ctx, int B, int C, int T, bool channels_last, const int* lengths, ClipPlan* p, uint64_t* incs);
+
+// The per-clip form of DdpmStep (rohm_posenet_sample_step_clips, rohm_trajnet_sample_step_clips).  streams: device
+// uint64 [B][2] of (seed, offset at draw 0); draw k of clip b starts at offset + k * incs[b].
+struct DdpmClipStep {
+  const float* x0;
+  const float* x_t;
+  float* x_next;
+  const float* coef_row;  // one row for every clip
+  const unsigned long long* streams;
+  unsigned long long draw;
+  ClipPlan plan;
+};
+int launch_ddpm_clip_step(rohm_ctx* ctx, const DdpmClipStep& s, cudaStream_t st, bool pdl);
+KernelPatch ddpm_clip_step_patch(const DdpmClipStep& s);
 
 }  // namespace rohm

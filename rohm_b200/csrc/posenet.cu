@@ -973,9 +973,10 @@ extern "C" int rohm_posenet_profile(rohm_posenet* pn, const float* x_t, const in
   return ROHM_OK;
 }
 
-// One forward, with the ancestral update appended when `step` is given (rohm_posenet_sample_step).
+// One forward, with the ancestral update appended when `step` (rohm_posenet_sample_step) or `clip_step`
+// (rohm_posenet_sample_step_clips) is given.
 static int forward_or_step(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* out, int B, int T,
-                           void* stream, const DdpmStep* step) {
+                           void* stream, const DdpmStep* step, const DdpmClipStep* clip_step = nullptr) {
   if (pn == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = pn->ctx;
   rohm::DeviceGuard device_guard__(ctx);
@@ -988,16 +989,18 @@ static int forward_or_step(rohm_posenet* pn, const float* x_t, const int64_t* ti
     return fail(ctx, ROHM_ERR_STATE, "rohm_posenet_forward: the clip lengths differ from those set_cond was called with");
   auto launches = [&](cudaStream_t st) {
     const int rc = forward_launches(pn, x_t, timesteps, out, B, T, st);
-    if (rc != ROHM_OK || step == nullptr) return rc;
+    if (rc != ROHM_OK || (step == nullptr && clip_step == nullptr)) return rc;
     pn->launches++;
+    if (clip_step != nullptr) return launch_ddpm_clip_step(ctx, *clip_step, st, pn->use_pdl && !pn->profiling);
     return launch_ddpm_step(ctx, *step, st, pn->use_pdl && !pn->profiling);
   };
   std::vector<KernelPatch> patches = {{pack_tokens_kernel, arg<kPackTokensX>(x_t)},
                                       {time_token_gather_kernel, arg<kTimeTokenTimesteps>(timesteps)},
                                       {unpack_tokens_kernel, arg<kUnpackTokensOut>(out)}};
   if (step != nullptr) patches.push_back(ddpm_step_patch(*step));
-  return pn->graphs.run(ctx, B, T, step != nullptr, pn->profiling, static_cast<cudaStream_t>(stream), launches, patches,
-                        pn->lengths);
+  if (clip_step != nullptr) patches.push_back(ddpm_clip_step_patch(*clip_step));
+  const StepKind kind = clip_step != nullptr ? kStepPerClip : step != nullptr ? kStepSingleStream : kNoStep;
+  return pn->graphs.run(ctx, B, T, kind, pn->profiling, static_cast<cudaStream_t>(stream), launches, patches, pn->lengths);
 }
 
 extern "C" int rohm_posenet_forward(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* out, int B,
@@ -1016,6 +1019,22 @@ extern "C" int rohm_posenet_sample_step(rohm_posenet* pn, const float* x_t, cons
   const int rc = ddpm_step_plan(pn->ctx, &step, offset_increment);
   if (rc != ROHM_OK) return rc;
   return forward_or_step(pn, x_t, timesteps, x0_out, B, T, stream, &step);
+}
+
+extern "C" int rohm_posenet_sample_step_clips(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* x0_out,
+                                              float* x_next, const float* coef_row, const uint64_t* streams, uint64_t draw,
+                                              uint64_t* offset_increments, int B, int T, void* stream) {
+  if (pn == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(pn->ctx);
+  if (x_next == nullptr || coef_row == nullptr || streams == nullptr)
+    return fail(pn->ctx, ROHM_ERR_INVALID, "rohm_posenet_sample_step_clips: null pointer");
+  int rc = check_lengths(pn, B, T, "rohm_posenet_sample_step_clips");
+  if (rc != ROHM_OK) return rc;
+  DdpmClipStep step{x0_out, x_t, x_next, coef_row, reinterpret_cast<const unsigned long long*>(streams), draw, {}};
+  rc = clip_plan(pn->ctx, B, pn->C, T, false, pn->lengths.empty() ? nullptr : pn->lengths.data(), &step.plan,
+                 offset_increments);
+  if (rc != ROHM_OK) return rc;
+  return forward_or_step(pn, x_t, timesteps, x0_out, B, T, stream, nullptr, &step);
 }
 
 extern "C" int rohm_posenet_set_option(rohm_posenet* pn, int option, int value) {

@@ -4,6 +4,9 @@
 // (diffusion/gaussian_diffusion_posenet.py:212-234, 426-434, 461-479, 192-210, 696-715).
 #include <curand_kernel.h>
 
+#include <algorithm>
+#include <cstdint>
+
 #include "graph.cuh"
 
 namespace rohm {
@@ -119,6 +122,77 @@ __global__ void __launch_bounds__(kThreads) ddpm_step_philox_kernel(const float*
 // The arguments of ddpm_step_philox_kernel that change from step to step in a replayed graph (ddpm_step_patch)
 constexpr size_t kStepX0 = 0, kStepXt = 1, kStepOut = 5, kStepCoef = 8, kStepSeed = 10, kStepOffset = 11;
 
+// Per-clip noise streams (graph.cuh ClipPlan).  Block blockIdx.x belongs to the clip b with blk[b] <= blockIdx.x <
+// blk[b + 1]; its threads are virtual threads vidx of torch's normal_ grid for that clip alone (G_b = 256 * its block count),
+// so thread vidx draws curand_normal4 on Philox4_32_10(seed_b, subsequence = vidx, offset_b + draw * inc_b) and owns the
+// clip-alone elements li = vidx + G_b * j, mapped to padded positions (c, t): li = c * n_b + t channel-major, li = t * C + c
+// channels-last.  The same threads then write zeros to the clip's padded frames.  kUpdate: the value written is the DDPM
+// update of ddpm_step_kernel with that noise (0-2 gradient terms, coefficient row shared or per clip); else the noise itself.
+template <bool kUpdate>
+__global__ void __launch_bounds__(kThreads) clip_noise_kernel(const float* __restrict__ x0, const float* x_t,
+                                                              const float* __restrict__ g0, const float* __restrict__ g1,
+                                                              int n_grads, float* out, const float* __restrict__ coef,
+                                                              int64_t coef_stride,
+                                                              const unsigned long long* __restrict__ streams,
+                                                              unsigned long long draw, const __grid_constant__ ClipPlan plan) {
+  const int bx = static_cast<int>(blockIdx.x);
+  int b = 0, hi = plan.B;  // plan.blk[b] <= bx < plan.blk[hi]
+  while (hi - b > 1) {
+    const int mid = (b + hi) >> 1;
+    if (plan.blk[mid] <= bx) b = mid;
+    else hi = mid;
+  }
+  const int n = plan.n[b], C = plan.C, T = plan.T;
+  const int64_t G = static_cast<int64_t>(plan.blk[b + 1] - plan.blk[b]) * kThreads;
+  const int64_t vidx = static_cast<int64_t>(bx - plan.blk[b]) * kThreads + threadIdx.x;
+  const int64_t numel = static_cast<int64_t>(C) * n;
+  const int iters = static_cast<int>((numel - 1) / (G * 4) + 1);
+  // as the programmatic dependent of the denoiser's last kernel: memory, the stream table included, is read after it completes
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  curandStatePhilox4_32_10_t state;
+  curand_init(streams[2 * b], static_cast<unsigned long long>(vidx), streams[2 * b + 1] + draw * 4ull * iters, &state);
+  float c1 = 0.f, c2 = 0.f, sigma = 0.f, gs0 = 0.f, gs1 = 0.f;
+  if (kUpdate) {
+    const float* cf = coef + b * coef_stride;
+    c1 = cf[0], c2 = cf[1], sigma = cf[2], gs0 = cf[3], gs1 = cf[4];
+  }
+  const int64_t base = static_cast<int64_t>(b) * C * T;
+  for (int k = 0; k < iters; ++k) {
+    const float4 nz = curand_normal4(&state);
+    const float z[4] = {nz.x, nz.y, nz.z, nz.w};
+#pragma unroll
+    for (int ii = 0; ii < 4; ++ii) {
+      const int64_t li = vidx + G * (4 * k + ii);
+      if (li < numel) {
+        int64_t idx;
+        if (plan.channels_last) {
+          idx = base + li;  // t * C + c is also the offset inside the padded clip
+        } else {
+          const unsigned l = static_cast<unsigned>(li), c = l / static_cast<unsigned>(n);
+          idx = base + static_cast<int64_t>(c) * T + (l - c * static_cast<unsigned>(n));
+        }
+        if (kUpdate)
+          out[idx] = ddpm_one(x0[idx], x_t[idx], z[ii], n_grads > 0 ? g0[idx] : 0.f, n_grads > 1 ? g1[idx] : 0.f, n_grads, c1,
+                              c2, sigma, gs0, gs1);
+        else
+          out[idx] = z[ii];
+      }
+    }
+  }
+  const int pad = T - n;
+  const int64_t npad = static_cast<int64_t>(C) * pad;
+  for (int64_t j = vidx; j < npad; j += G) {
+    if (plan.channels_last) {
+      out[base + static_cast<int64_t>(n) * C + j] = 0.f;
+    } else {
+      const int64_t c = j / pad;
+      out[base + c * T + n + (j - c * pad)] = 0.f;
+    }
+  }
+}
+// The arguments of clip_noise_kernel<true> that change from step to step in a replayed graph (ddpm_clip_step_patch)
+constexpr size_t kClipX0 = 0, kClipXt = 1, kClipOut = 5, kClipCoef = 6, kClipStreams = 8, kClipDraw = 9;
+
 int grid_for(const rohm_ctx* ctx, int64_t work_items) {
   const int sms = ctx->sm_count > 0 ? ctx->sm_count : 132;
   int64_t blocks = (work_items + kThreads - 1) / kThreads;
@@ -223,7 +297,72 @@ KernelPatch ddpm_step_patch(const DdpmStep& s) {
   return {ddpm_step_philox_kernel, arg<kStepX0>(s.x0),         arg<kStepXt>(s.x_t),       arg<kStepOut>(s.x_next),
           arg<kStepCoef>(s.coef_row), arg<kStepSeed>(s.seed), arg<kStepOffset>(s.offset)};
 }
+
+int clip_plan(rohm_ctx* ctx, int B, int C, int T, bool channels_last, const int* lengths, ClipPlan* p, uint64_t* incs) {
+  if (B < 1 || B > kMaxStreamClips || C < 1 || T < 1)
+    return fail(ctx, ROHM_ERR_INVALID, "per-clip noise streams: B=%d (at most %d), C=%d, T=%d", B, kMaxStreamClips, C, T);
+  // torch's normal_ grid (ATen calc_execution_policy, as torch_normal_policy): min(ceil(numel / 256), SMs * blocks per SM)
+  int threads_per_sm = 0;
+  ROHM_CUDA(ctx, cudaDeviceGetAttribute(&threads_per_sm, cudaDevAttrMaxThreadsPerMultiProcessor, ctx->device));
+  const int64_t cap = static_cast<int64_t>(ctx->sm_count) * (threads_per_sm / 256);
+  p->B = B, p->C = C, p->T = T, p->channels_last = channels_last ? 1 : 0;
+  p->blk[0] = 0;
+  for (int b = 0; b < B; ++b) {
+    const int n = lengths != nullptr ? lengths[b] : T;
+    if (n < 1 || n > T) return fail(ctx, ROHM_ERR_INVALID, "per-clip noise streams: lengths[%d] = %d outside [1, %d]", b, n, T);
+    const int64_t numel = static_cast<int64_t>(C) * n;
+    const int64_t grid = std::min((numel + kThreads - 1) / kThreads, cap);
+    if (p->blk[b] + grid > INT32_MAX) return fail(ctx, ROHM_ERR_INVALID, "per-clip noise streams: grid too large");
+    p->n[b] = n;
+    p->blk[b + 1] = p->blk[b] + static_cast<int>(grid);
+    if (incs != nullptr) incs[b] = 4ull * static_cast<uint64_t>((numel - 1) / (grid * kThreads * 4) + 1);
+  }
+  return ROHM_OK;
+}
+int launch_ddpm_clip_step(rohm_ctx* ctx, const DdpmClipStep& s, cudaStream_t st, bool pdl) {
+  ROHM_CUDA(ctx, launch_chain(clip_noise_kernel<true>, dim3(static_cast<unsigned>(s.plan.blk[s.plan.B])), dim3(kThreads), 0,
+                              st, pdl, s.x0, s.x_t, nullptr, nullptr, 0, s.x_next, s.coef_row, 0, s.streams, s.draw, s.plan));
+  return ROHM_OK;
+}
+KernelPatch ddpm_clip_step_patch(const DdpmClipStep& s) {
+  return {clip_noise_kernel<true>,      arg<kClipX0>(s.x0),           arg<kClipXt>(s.x_t),   arg<kClipOut>(s.x_next),
+          arg<kClipCoef>(s.coef_row), arg<kClipStreams>(s.streams), arg<kClipDraw>(s.draw)};
+}
 }  // namespace rohm
+
+extern "C" int rohm_randn_clips(rohm_ctx* ctx, float* out, int B, int C, int T, int channels_last, const int* lengths,
+                                const uint64_t* streams, uint64_t draw, uint64_t* offset_increments, void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (out == nullptr || streams == nullptr) return fail(ctx, ROHM_ERR_INVALID, "rohm_randn_clips: null pointer");
+  ClipPlan plan;
+  const int rc = clip_plan(ctx, B, C, T, channels_last != 0, lengths, &plan, offset_increments);
+  if (rc != ROHM_OK) return rc;
+  clip_noise_kernel<false><<<static_cast<unsigned>(plan.blk[B]), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      nullptr, nullptr, nullptr, nullptr, 0, out, nullptr, 0, reinterpret_cast<const unsigned long long*>(streams), draw, plan);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return ROHM_OK;
+}
+
+extern "C" int rohm_ddpm_step_philox_clips(rohm_ctx* ctx, const float* x0, const float* x_t, const float* grad0,
+                                           const float* grad1, int n_grads, float* out, int B, int C, int T,
+                                           int channels_last, const int* lengths, const float* coef,
+                                           int64_t coef_clip_stride, const uint64_t* streams, uint64_t draw,
+                                           uint64_t* offset_increments, void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (x0 == nullptr || x_t == nullptr || out == nullptr || coef == nullptr || streams == nullptr || n_grads < 0 ||
+      n_grads > 2 || (n_grads > 0 && grad0 == nullptr) || (n_grads > 1 && grad1 == nullptr) || coef_clip_stride < 0)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_ddpm_step_philox_clips: bad arguments");
+  ClipPlan plan;
+  const int rc = clip_plan(ctx, B, C, T, channels_last != 0, lengths, &plan, offset_increments);
+  if (rc != ROHM_OK) return rc;
+  clip_noise_kernel<true><<<static_cast<unsigned>(plan.blk[B]), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      x0, x_t, grad0, grad1, n_grads, out, coef, coef_clip_stride, reinterpret_cast<const unsigned long long*>(streams), draw,
+      plan);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return ROHM_OK;
+}
 
 extern "C" int rohm_q_sample(rohm_ctx* ctx, const float* x_start, const float* noise, float* out, int64_t n,
                              float sqrt_ac, float sqrt_one_minus_ac, void* stream) {

@@ -993,9 +993,10 @@ static int trajnet_forward_launches(rohm_trajnet* tn, const float* x_t, const in
   return ROHM_OK;
 }
 
-// One forward, with the ancestral update appended when `step` is given (rohm_trajnet_sample_step).
+// One forward, with the ancestral update appended when `step` (rohm_trajnet_sample_step) or `clip_step`
+// (rohm_trajnet_sample_step_clips) is given.
 static int trajnet_forward_or_step(rohm_trajnet* tn, const float* x_t, const int64_t* time, float* out, int B, void* stream,
-                                   const DdpmStep* step) {
+                                   const DdpmStep* step, const DdpmClipStep* clip_step = nullptr) {
   if (tn == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = tn->ctx;
   rohm::DeviceGuard device_guard__(ctx);
@@ -1006,8 +1007,9 @@ static int trajnet_forward_or_step(rohm_trajnet* tn, const float* x_t, const int
     return fail(ctx, ROHM_ERR_STATE, "rohm_trajnet_forward: the clip lengths differ from those set_cond was called with");
   auto launches = [&](cudaStream_t st) {
     const int rc = trajnet_forward_launches(tn, x_t, time, out, B, st);
-    if (rc != ROHM_OK || step == nullptr) return rc;
+    if (rc != ROHM_OK || (step == nullptr && clip_step == nullptr)) return rc;
     tn->launches++;
+    if (clip_step != nullptr) return launch_ddpm_clip_step(ctx, *clip_step, st, tn->use_pdl);
     return launch_ddpm_step(ctx, *step, st, tn->use_pdl);
   };
   const bool packed = !tn->lengths.empty();
@@ -1016,8 +1018,9 @@ static int trajnet_forward_or_step(rohm_trajnet* tn, const float* x_t, const int
                                       {packed ? unpack_rows_kernel<true> : unpack_rows_kernel<false>,
                                        arg<kUnpackRowsOut>(out)}};
   if (step != nullptr) patches.push_back(ddpm_step_patch(*step));
-  return tn->graphs.run(ctx, B, tn->T, step != nullptr, false, static_cast<cudaStream_t>(stream), launches, patches,
-                        tn->lengths);
+  if (clip_step != nullptr) patches.push_back(ddpm_clip_step_patch(*clip_step));
+  const StepKind kind = clip_step != nullptr ? kStepPerClip : step != nullptr ? kStepSingleStream : kNoStep;
+  return tn->graphs.run(ctx, B, tn->T, kind, false, static_cast<cudaStream_t>(stream), launches, patches, tn->lengths);
 }
 
 // TrajNet.forward (trajnet.py:177-275).  x_t: [B, T, traj_dim]; time: int64 [B]; out: [B, T, traj_dim].
@@ -1039,6 +1042,24 @@ extern "C" int rohm_trajnet_sample_step(rohm_trajnet* tn, const float* x_t, cons
   const int rc = ddpm_step_plan(tn->ctx, &step, offset_increment);
   if (rc != ROHM_OK) return rc;
   return trajnet_forward_or_step(tn, x_t, time, x0_out, B, stream, &step);
+}
+
+// The same step with per-clip noise streams (rohm_randn_clips); see rohm_posenet_sample_step_clips.
+extern "C" int rohm_trajnet_sample_step_clips(rohm_trajnet* tn, const float* x_t, const int64_t* time, float* x0_out,
+                                              float* x_next, const float* coef_row, const uint64_t* streams, uint64_t draw,
+                                              uint64_t* offset_increments, int B, void* stream) {
+  if (tn == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(tn->ctx);
+  if (x_next == nullptr || coef_row == nullptr || streams == nullptr)
+    return fail(tn->ctx, ROHM_ERR_INVALID, "rohm_trajnet_sample_step_clips: null pointer");
+  if (!tn->lengths.empty() && static_cast<int>(tn->lengths.size()) != B)
+    return fail(tn->ctx, ROHM_ERR_INVALID, "rohm_trajnet_sample_step_clips: lengths were set for %d clips, the call has B=%d",
+                static_cast<int>(tn->lengths.size()), B);
+  DdpmClipStep step{x0_out, x_t, x_next, coef_row, reinterpret_cast<const unsigned long long*>(streams), draw, {}};
+  const int rc = clip_plan(tn->ctx, B, tn->traj_dim, tn->T, true, tn->lengths.empty() ? nullptr : tn->lengths.data(),
+                           &step.plan, offset_increments);
+  if (rc != ROHM_OK) return rc;
+  return trajnet_forward_or_step(tn, x_t, time, x0_out, B, stream, nullptr, &step);
 }
 
 extern "C" int rohm_trajnet_set_option(rohm_trajnet* tn, int option, int value) {

@@ -13,7 +13,9 @@ method names, keyword arguments and return values.  What differs is where the wo
 * the per-step ``t`` tensors and the respacing map live on the device for the whole loop (no per-step H2D).
 
 Noise is drawn with ``torch.randn`` / ``torch.randn_like`` in exactly the reference's order (once for x_T, then once per
-step including t == 0), so with the same seed on the same device the random stream is identical.
+step including t == 0), so with the same seed on the same device the random stream is identical.  With
+``batch['generators']`` (one CUDA generator per clip, rohm_b200.noise_streams) the same draws come from each clip's own
+generator instead, as the clip alone would draw them.
 """
 import enum
 from copy import deepcopy
@@ -87,6 +89,8 @@ class _GaussianDiffusion:
         # RNG entry points (kept as attributes so tests can inject a recorded noise stream)
         self._randn = th.randn
         self._randn_like = th.randn_like
+        # (batch['generators'] list, NoiseStreams) of the sampling loop in progress, if it draws from per-clip streams
+        self._loop_streams = None
 
     # ------------------------------------------------------------------ device-side tables
     def _dev(self, device):
@@ -236,6 +240,40 @@ class _GaussianDiffusion:
         stream, see ops.ddpm_step_philox); an injected noise source (tests, sharded parity noise) keeps the explicit tensor."""
         return self._randn_like is th.randn_like and x.is_cuda and _FUSED_STEP
 
+    # ------------------------------------------------------------------ per-clip noise streams (batch['generators'])
+    def _channels_last(self):
+        return not self._POSENET  # PoseNet batches are [B, C, 1, T], TrajNet batches [B, T, C]
+
+    def _draw_lengths(self, model, batch, shape):
+        """The per-clip lengths the draws of a [B, ...] batch follow (the denoiser's check of batch['lengths']), or None."""
+        if batch.get('lengths') is None:
+            return None
+        inner = model.model if isinstance(model, _WrappedModel) else model
+        if self._POSENET:
+            return inner.clip_lengths(batch, shape)
+        from .trajnet_engine import clip_lengths
+        return clip_lengths(batch, shape)
+
+    def _open_streams(self, batch, shape, device, const_noise=False):
+        """NoiseStreams of batch['generators'] after the validator's checks, or None without the key."""
+        from .noise_streams import NoiseStreams, check_generators
+        gens = check_generators(batch, shape[0], device, diffusion=self, const_noise=const_noise)
+        return None if gens is None else NoiseStreams(gens, device)
+
+    def _step_streams(self, batch, x, const_noise=False):
+        """(streams, owned) of one step: the loop's streams when the step runs inside a loop over this batch's generators,
+        else streams opened for this call alone (owned: the caller closes them, writing the offsets back)."""
+        if not isinstance(batch, dict) or batch.get('generators') is None:
+            return None, False
+        ls = self._loop_streams
+        if ls is not None and ls[0] is batch['generators']:
+            return ls[1], False
+        return self._open_streams(batch, x.shape, x.device, const_noise), True
+
+    def _randn_clips(self, model, batch, x, streams):
+        return ops.randn_clips(streams, x.shape, self._channels_last(), self._draw_lengths(model, batch, x.shape),
+                               device=x.device)
+
     def _coef_row(self, t, step_index):
         """The step's coefficient row: a view of the per-device table when the (batch-uniform) step index is known to the
         host, else a gather by the per-clip indices."""
@@ -243,8 +281,9 @@ class _GaussianDiffusion:
             return self._dev(t.device)["coef"][int(step_index)]
         return self._coef_for(t)
 
-    def _fused_posenet_step(self, model, batch, x, t, step_index, model_kwargs):
-        """PoseNet, unguided step, noise from torch's generator, no model kwargs: forward + update as ONE graph launch."""
+    def _fused_posenet_step(self, model, batch, x, t, step_index, model_kwargs, streams=None):
+        """PoseNet, unguided step, noise from torch's generator (or the per-clip streams), no model kwargs: forward + update
+        as ONE graph launch."""
         if not (self._POSENET and step_index is not None and not model_kwargs and self._noise_in_kernel(x)):
             return None
         model = self._wrap_model(model)  # respaced schedules: step index -> original timestep
@@ -256,10 +295,10 @@ class _GaussianDiffusion:
         batch['x_t'] = x
         ts = model.map_timesteps(t) if isinstance(model, _WrappedModel) else t
         e = prep(batch['cond'], inner.clip_lengths(batch, x.shape))
-        x0, nxt = e.sample_step(x, ts.to(th.int64).contiguous(), self._coef_row(t, step_index))
+        x0, nxt = e.sample_step(x, ts.to(th.int64).contiguous(), self._coef_row(t, step_index), streams=streams)
         return {"sample": nxt, "pred_xstart": x0, "x_t": x}
 
-    def _fused_trajnet_step(self, model, batch, x, t, step_index, model_kwargs):
+    def _fused_trajnet_step(self, model, batch, x, t, step_index, model_kwargs, streams=None):
         """TrajNet, step without cond_fn, noise from torch's generator, no model kwargs: forward + update as ONE graph launch
         (rohm_trajnet_sample_step); the same arithmetic and the same noise as the separate launches below."""
         if self._POSENET or step_index is None or model_kwargs or not self._noise_in_kernel(x):
@@ -274,23 +313,38 @@ class _GaussianDiffusion:
         ts = model.map_timesteps(t) if isinstance(model, _WrappedModel) else t
         e, xc, tsc = prepare(inner, batch, ts)
         batch['x_t'] = xc
-        x0, nxt = e.sample_step(xc, tsc, self._coef_row(t, step_index))
+        x0, nxt = e.sample_step(xc, tsc, self._coef_row(t, step_index), streams=streams)
         return {"sample": nxt, "pred_xstart": x0, "x_t": xc}
 
     def p_sample(self, model, batch, x, t, clip_denoised=True, denoised_fn=None, cond_fn=None, model_kwargs=None,
                  const_noise=False, _step_index=None):
         """x_{t-1} = coef1[t] x0 + coef2[t] x_t + (t != 0) exp(0.5 logvar[t]) noise, x0 = model(batch | x_t, t).
-        Returns {'sample', 'pred_xstart', 'x_t'}."""
+        Returns {'sample', 'pred_xstart', 'x_t'}.  With batch['generators'] clip b's noise comes from generators[b]
+        (rohm_b200.noise_streams)."""
+        streams, owned = self._step_streams(batch, x, const_noise)
+        try:
+            return self._p_sample(model, batch, x, t, cond_fn, model_kwargs, const_noise, _step_index, streams)
+        finally:
+            if owned:
+                streams.close()
+
+    def _p_sample(self, model, batch, x, t, cond_fn, model_kwargs, const_noise, _step_index, streams):
         if cond_fn is None and not const_noise:
-            fused = self._fused_posenet_step(model, batch, x, t, _step_index, model_kwargs)
+            fused = self._fused_posenet_step(model, batch, x, t, _step_index, model_kwargs, streams)
             if fused is None:
-                fused = self._fused_trajnet_step(model, batch, x, t, _step_index, model_kwargs)
+                fused = self._fused_trajnet_step(model, batch, x, t, _step_index, model_kwargs, streams)
             if fused is not None:
                 return fused
         x, x0 = self._denoise(model, batch, x, t, model_kwargs)
         if cond_fn is None and not const_noise and self._noise_in_kernel(x):
-            return {"sample": ops.ddpm_step_philox(x0, x, self._coef_row(t, _step_index)), "pred_xstart": x0, "x_t": x}
-        noise = self._randn_like(x)
+            coef = self._coef_row(t, _step_index)
+            if streams is not None:
+                sample = ops.ddpm_step_philox_clips(x0, x, coef, streams, self._channels_last(),
+                                                    self._draw_lengths(model, batch, x.shape))
+            else:
+                sample = ops.ddpm_step_philox(x0, x, coef)
+            return {"sample": sample, "pred_xstart": x0, "x_t": x}
+        noise = self._randn_like(x) if streams is None else self._randn_clips(model, batch, x, streams)
         if const_noise:
             noise = noise[[0]].repeat(x.shape[0], *([1] * (x.dim() - 1)))
         coef = self._coef_row(t, _step_index)
@@ -313,19 +367,31 @@ class _GaussianDiffusion:
     def p_sample_with_grad(self, model, batch, x, t, clip_denoised=True, denoised_fn=None, cond_fn=None, grad_type=None,
                            model_kwargs=None, const_noise=False, _step_index=None):
         """PoseNet: p_sample plus the hard-coded test-time guidance schedule; TrajNet: identical to p_sample without
-        const_noise / cond_fn (the reference's TrajNet variant contains no guidance)."""
+        const_noise / cond_fn (the reference's TrajNet variant contains no guidance).  batch['generators']: as p_sample."""
+        streams, owned = self._step_streams(batch, x, const_noise)
+        try:
+            return self._p_sample_with_grad(model, batch, x, t, cond_fn, grad_type, model_kwargs, const_noise, _step_index,
+                                            streams)
+        finally:
+            if owned:
+                streams.close()
+
+    def _p_sample_with_grad(self, model, batch, x, t, cond_fn, grad_type, model_kwargs, const_noise, _step_index, streams):
         step = None if _step_index is None else int(_step_index)
         guided_now = (self._POSENET and grad_type in _GUIDANCE and
                       (step is None or any(step <= last for _, _, last in _GUIDANCE[grad_type])))
         if not guided_now:
-            fused = self._fused_posenet_step(model, batch, x, t, _step_index, model_kwargs)
+            fused = self._fused_posenet_step(model, batch, x, t, _step_index, model_kwargs, streams)
             if fused is None and cond_fn is None and not const_noise:
-                fused = self._fused_trajnet_step(model, batch, x, t, _step_index, model_kwargs)
+                fused = self._fused_trajnet_step(model, batch, x, t, _step_index, model_kwargs, streams)
             if fused is not None:
                 return fused
         x, x0 = self._denoise(model, batch, x, t, model_kwargs)
         in_kernel = self._noise_in_kernel(x)
-        noise = None if in_kernel else self._randn_like(x)
+        if in_kernel:
+            noise = None
+        else:
+            noise = self._randn_like(x) if streams is None else self._randn_clips(model, batch, x, streams)
         coef = self._coef_row(t, _step_index)
         if coef.dim() == 1:
             coef = coef.unsqueeze(0).expand(x.shape[0], -1)  # guidance scales are written per clip below
@@ -353,21 +419,32 @@ class _GaussianDiffusion:
         elif grad_type is not None and self._POSENET:
             pass  # unknown grad_type: the reference silently applies no guidance
         coef = coef.contiguous()
-        if in_kernel:
+        if in_kernel and streams is not None:
+            sample = ops.ddpm_step_philox_clips(x0, x, coef, streams, self._channels_last(),
+                                                self._draw_lengths(model, batch, x.shape), grads=tuple(grads))
+        elif in_kernel:
             sample = ops.ddpm_step_philox(x0, x, coef, grads=tuple(grads))
         else:
             sample = ops.ddpm_step(x0, x, noise, coef, grads=tuple(grads))
         return {"sample": sample, "pred_xstart": x0, "x_t": x}
 
     # ------------------------------------------------------------------ loops
-    def _begin_loop(self, model, grad_type=None, batch=None, shape=None):
+    def _begin_loop(self, model, grad_type=None, batch=None, shape=None, device=None, const_noise=False):
         """Once per sampling loop, before any step: drop the denoiser's cached step-invariant condition embedding (a
         condition tensor can never outlive the loop it was embedded for) and reject what cannot run BEFORE a thousand
         denoiser steps are spent (the reference would fail, or silently do nothing, at the first guided step), per-clip
-        lengths included."""
+        lengths and generators included.  Returns the loop's NoiseStreams with batch['generators'] (the caller closes
+        them when the loop ends), else None."""
         inner = model.model if isinstance(model, _WrappedModel) else model
         if batch is not None and batch.get('lengths') is not None and hasattr(inner, "clip_lengths"):
             inner.clip_lengths(batch, shape, grad_type=grad_type)
+        streams = None
+        if batch is not None and batch.get('generators') is not None:
+            if batch.get('lengths') is not None and not self._POSENET:
+                from .trajnet_engine import clip_lengths
+                clip_lengths(batch, shape)
+            from .noise_streams import check_generators
+            check_generators(batch, shape[0], device, diffusion=self, const_noise=const_noise)
         inv = getattr(inner, "invalidate_cond", None)
         if inv is not None:
             inv()
@@ -380,6 +457,28 @@ class _GaussianDiffusion:
         pe = getattr(getattr(inner, "sequence_pos_encoder", None), "pe", None)
         if tmap is not None and pe is not None and len(tmap) and max(tmap) >= pe.shape[0]:
             raise RohmB200Error(f"timestep {max(tmap)} exceeds the positional table ({pe.shape[0]} rows) that embeds it")
+        if batch is not None and batch.get('generators') is not None:
+            streams = self._open_streams(batch, shape, device, const_noise)
+        if streams is not None:
+            self._loop_streams = (batch['generators'], streams)
+        return streams
+
+    def _end_loop(self, streams):
+        """When a loop returns or its generator is closed: writes the generators' offsets back."""
+        if streams is None:
+            return
+        if self._loop_streams is not None and self._loop_streams[1] is streams:
+            self._loop_streams = None
+        streams.close()
+
+    def _initial_noise(self, model, batch, shape, device, noise, streams):
+        """x_T: the caller's `noise`, else per-clip streams, else the global generator."""
+        if noise is not None:
+            return noise
+        if streams is not None:
+            return ops.randn_clips(streams, shape, self._channels_last(), self._draw_lengths(model, batch, shape),
+                                   device=device)
+        return self._randn(*shape, device=device)
 
     def p_sample_loop(self, model, batch, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
                       model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
@@ -422,46 +521,57 @@ class _GaussianDiffusion:
         if device is None:
             device = next(model.parameters()).device
         assert isinstance(shape, (tuple, list))
-        self._begin_loop(model, grad_type if cond_fn_with_grad else None, batch, shape)
-        img = noise if noise is not None else self._randn(*shape, device=device)
-        if skip_timesteps and init_image is None:
-            init_image = th.zeros_like(img)
-        indices = list(range(self.num_timesteps - skip_timesteps))[::-1]
-        t_rows = self._t_rows(shape[0], device)
-        if init_image is not None:
-            img = self.q_sample(init_image, t_rows[indices[0]], img)
-        if early_stop:
-            indices = indices[0:980]
-        if progress:
-            from tqdm.auto import tqdm
-            indices = tqdm(indices)
-        for i in indices:
-            t = t_rows[i]
-            with th.no_grad():
-                if cond_fn_with_grad:
-                    if self._POSENET:
-                        out = self.p_sample_with_grad(model, batch, img, t, clip_denoised=clip_denoised,
-                                                      denoised_fn=denoised_fn, cond_fn=cond_fn, grad_type=grad_type,
-                                                      model_kwargs=model_kwargs, const_noise=const_noise, _step_index=i)
+        streams = self._begin_loop(model, grad_type if cond_fn_with_grad else None, batch, shape, device, const_noise)
+        try:
+            img = self._initial_noise(model, batch, shape, device, noise, streams)
+            if skip_timesteps and init_image is None:
+                init_image = th.zeros_like(img)
+            indices = list(range(self.num_timesteps - skip_timesteps))[::-1]
+            t_rows = self._t_rows(shape[0], device)
+            if init_image is not None:
+                img = self.q_sample(init_image, t_rows[indices[0]], img)
+            if early_stop:
+                indices = indices[0:980]
+            if progress:
+                from tqdm.auto import tqdm
+                indices = tqdm(indices)
+            for i in indices:
+                t = t_rows[i]
+                with th.no_grad():
+                    if cond_fn_with_grad:
+                        if self._POSENET:
+                            out = self.p_sample_with_grad(model, batch, img, t, clip_denoised=clip_denoised,
+                                                          denoised_fn=denoised_fn, cond_fn=cond_fn, grad_type=grad_type,
+                                                          model_kwargs=model_kwargs, const_noise=const_noise,
+                                                          _step_index=i)
+                        else:
+                            out = self.p_sample_with_grad(model, batch, img, t, clip_denoised=clip_denoised,
+                                                          denoised_fn=denoised_fn, cond_fn=cond_fn,
+                                                          model_kwargs=model_kwargs, const_noise=const_noise,
+                                                          _step_index=i)
                     else:
-                        out = self.p_sample_with_grad(model, batch, img, t, clip_denoised=clip_denoised,
-                                                      denoised_fn=denoised_fn, cond_fn=cond_fn,
-                                                      model_kwargs=model_kwargs, const_noise=const_noise, _step_index=i)
-                else:
-                    out = self.p_sample(model, batch, img, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
-                                        cond_fn=cond_fn, model_kwargs=model_kwargs, const_noise=const_noise, _step_index=i)
-                yield out
-                img = out["sample"]
+                        out = self.p_sample(model, batch, img, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
+                                            cond_fn=cond_fn, model_kwargs=model_kwargs, const_noise=const_noise,
+                                            _step_index=i)
+                    yield out
+                    img = out["sample"]
+        finally:
+            self._end_loop(streams)
 
     # ------------------------------------------------------------------ DDIM
     # The reference's ddim_* methods cannot run (they call p_mean_variance without `batch`, and eval_losses never
     # reaches them -- SURVEY.md D4).  These implement the update those methods spell out, with `batch` threaded.
     def ddim_sample(self, model, batch, x, t, clip_denoised=True, denoised_fn=None, cond_fn=None, model_kwargs=None,
                     eta=0.0, _step_index=None):
-        x, x0 = self._denoise(model, batch, x, t, model_kwargs)
         if cond_fn is not None:
             raise NotImplementedError("cond_fn with DDIM sampling (condition_score) is not on the supported path")
-        noise = self._randn_like(x)
+        streams, owned = self._step_streams(batch, x)
+        try:
+            x, x0 = self._denoise(model, batch, x, t, model_kwargs)
+            noise = self._randn_like(x) if streams is None else self._randn_clips(model, batch, x, streams)
+        finally:
+            if owned:
+                streams.close()
         step = int(t[0]) if _step_index is None else _step_index
         sample = ops.ddim_step(x0, x, noise, schedule.ddim_coefs(self.__dict__, step, eta))
         return {"sample": sample, "pred_xstart": x0}
@@ -489,24 +599,27 @@ class _GaussianDiffusion:
         if device is None:
             device = next(model.parameters()).device
         assert isinstance(shape, (tuple, list))
-        self._begin_loop(model, batch=batch, shape=shape)
-        img = noise if noise is not None else self._randn(*shape, device=device)
-        if skip_timesteps and init_image is None:
-            init_image = th.zeros_like(img)
-        indices = list(range(self.num_timesteps - skip_timesteps))[::-1]
-        t_rows = self._t_rows(shape[0], device)
-        if init_image is not None:
-            img = self.q_sample(init_image, t_rows[indices[0]], img)
-        if progress:
-            from tqdm.auto import tqdm
-            indices = tqdm(indices)
-        for i in indices:
-            with th.no_grad():
-                out = self.ddim_sample(model, batch, img, t_rows[i], clip_denoised=clip_denoised,
-                                       denoised_fn=denoised_fn, cond_fn=cond_fn, model_kwargs=model_kwargs, eta=eta,
-                                       _step_index=i)
-                yield out
-                img = out["sample"]
+        streams = self._begin_loop(model, batch=batch, shape=shape, device=device)
+        try:
+            img = self._initial_noise(model, batch, shape, device, noise, streams)
+            if skip_timesteps and init_image is None:
+                init_image = th.zeros_like(img)
+            indices = list(range(self.num_timesteps - skip_timesteps))[::-1]
+            t_rows = self._t_rows(shape[0], device)
+            if init_image is not None:
+                img = self.q_sample(init_image, t_rows[indices[0]], img)
+            if progress:
+                from tqdm.auto import tqdm
+                indices = tqdm(indices)
+            for i in indices:
+                with th.no_grad():
+                    out = self.ddim_sample(model, batch, img, t_rows[i], clip_denoised=clip_denoised,
+                                           denoised_fn=denoised_fn, cond_fn=cond_fn, model_kwargs=model_kwargs, eta=eta,
+                                           _step_index=i)
+                    yield out
+                    img = out["sample"]
+        finally:
+            self._end_loop(streams)
 
     # ------------------------------------------------------------------ entry points used by the drivers
     def training_losses(self, *a, **k):

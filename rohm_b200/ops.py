@@ -101,6 +101,68 @@ def ddpm_step_philox(x0, x_t, coef, grads=(), out=None):
     return out
 
 
+def _clip_layout(shape, channels_last):
+    """(B, C, T) of a padded PoseNet [B, C, 1, T] (channels_last=False) or TrajNet [B, T, C] (channels_last=True) batch."""
+    if channels_last:
+        if len(shape) != 3:
+            raise RohmB200Error(f"per-clip noise: a channels-last batch is [B, T, C], got {tuple(shape)}")
+        return int(shape[0]), int(shape[2]), int(shape[1])
+    if len(shape) != 4 or shape[2] != 1:
+        raise RohmB200Error(f"per-clip noise: a channel-major batch is [B, C, 1, T], got {tuple(shape)}")
+    return int(shape[0]), int(shape[1]), int(shape[3])
+
+
+def randn_clips(streams, shape, channels_last, lengths=None, device=None):
+    """A padded batch of `shape` whose clip b holds torch.randn(S_b, generator=streams.generators[b]) in its real frames
+    (lengths[b], or all T) and zero past them (rohm_randn_clips).  streams: noise_streams.NoiseStreams."""
+    B, Cc, T = _clip_layout(shape, channels_last)
+    if B != len(streams):
+        raise RohmB200Error(f"randn_clips: {len(streams)} streams for a batch of {B} clips")
+    dev = streams.table.device if device is None else torch.device(device)
+    out = torch.empty(tuple(shape), device=dev, dtype=torch.float32)
+    draw = streams.next_draw((Cc, T, bool(channels_last), lengths))
+    lib, c = _lib.load(), _lib.ctx(out.device.index)
+    rc = lib.rohm_randn_clips(c, _ptr(out), B, Cc, T, int(bool(channels_last)), streams.lengths_c(lengths),
+                              _ptr(streams.table), draw, streams.incs, _stream(out.device))
+    _lib.check(rc, c)
+    return out
+
+
+def ddpm_step_philox_clips(x0, x_t, coef, streams, channels_last, lengths=None, grads=(), out=None):
+    """ddpm_step with noise = randn_clips(streams, x_t.shape, channels_last, lengths) drawn inside the kernel (same bits),
+    and zero in every clip's padded frames."""
+    for n, t in (("x0", x0), ("x_t", x_t), ("coef", coef)):
+        _require_cuda(n, t)
+    if x0.shape != x_t.shape:
+        raise RohmB200Error("ddpm_step_philox_clips: x0 and x_t must have the same shape")
+    for g in grads:
+        _require_cuda("grad", g)
+        if g.shape != x0.shape:
+            raise RohmB200Error("ddpm_step_philox_clips: grad shape mismatch")
+    B, Cc, T = _clip_layout(x0.shape, channels_last)
+    if B != len(streams):
+        raise RohmB200Error(f"ddpm_step_philox_clips: {len(streams)} streams for a batch of {B} clips")
+    if coef.dim() == 1:
+        stride = 0
+        if coef.numel() < _lib.DDPM_COEFS:
+            raise RohmB200Error("ddpm_step_philox_clips: coef row must hold 8 floats")
+    else:
+        if coef.shape != (B, _lib.DDPM_COEFS):
+            raise RohmB200Error(f"ddpm_step_philox_clips: per-clip coef must be [{B}, 8]")
+        stride = _lib.DDPM_COEFS
+    if out is None:
+        out = torch.empty_like(x0)
+    draw = streams.next_draw((Cc, T, bool(channels_last), lengths))
+    lib, c = _lib.load(), _lib.ctx(x0.device.index)
+    g0 = grads[0] if len(grads) > 0 else None
+    g1 = grads[1] if len(grads) > 1 else None
+    rc = lib.rohm_ddpm_step_philox_clips(c, _ptr(x0), _ptr(x_t), _ptr(g0), _ptr(g1), len(grads), _ptr(out), B, Cc, T,
+                                         int(bool(channels_last)), streams.lengths_c(lengths), _ptr(coef), stride,
+                                         _ptr(streams.table), draw, streams.incs, _stream(x0.device))
+    _lib.check(rc, c)
+    return out
+
+
 def q_sample(x_start, noise, sqrt_ac, sqrt_one_minus_ac):
     _require_cuda("x_start", x_start)
     _require_cuda("noise", noise)

@@ -83,13 +83,24 @@ def global_guidance(model, group=None, enable=True):
     return model
 
 
+def shard_generators(generators, rank, world):
+    """This rank's slice of the global batch's per-clip generators (batch['generators']), by shard_bounds."""
+    lo, hi = shard_bounds(len(generators), rank, world)
+    return list(generators[lo:hi])
+
+
 def sample_sharded(diffusion, model, batch, shape, parity_noise=True, group=None, **eval_kwargs):
-    """eval_losses on this rank's shard + the final all-gather.  `batch` and `shape` describe the GLOBAL batch."""
+    """eval_losses on this rank's shard + the final all-gather.  `batch` and `shape` describe the GLOBAL batch.
+    With batch['generators'] (one CUDA generator per clip, rohm_b200.noise_streams) each rank gets its slice of the list
+    and draws only its own clips' noise; no ShardedNoise is installed, so the fused step graph stays on."""
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     n = int(shape[0])
     local = shard_batch(batch, rank, world, n)
     lo, hi = shard_bounds(n, rank, world)
     lshape = [hi - lo] + list(shape[1:])
+    if batch.get('generators') is not None:
+        local['generators'] = shard_generators(batch['generators'], rank, world)
+        parity_noise = False  # each clip's noise comes from its own generator, wherever it runs
     if parity_noise:
         ShardedNoise(n, rank, world).install(diffusion)
     try:

@@ -51,10 +51,20 @@ def run_rounds(args, model_posenet, model_trajnet, model_trajnet_control, diffus
     a clip's result depends on its batch-mates.  mask_scheme='full' draws one uniform per clip as without lengths and
     places the window inside the clip: start = floor(u * (lengths[b] - 2)), end = min(start + 30, lengths[b] - 1).
     Refused with lengths: grad_type='prox', and infill_traj when its window [65, 65 + int(traj_mask_ratio * 145)) does not
-    lie inside every clip."""
+    lie inside every clip.
+
+    test_batch_traj['generators'] (optional, B distinct CUDA torch.Generator objects, rohm_b200.noise_streams): recording
+    b's noise comes from generators[b] in every TrajNet, TrajControl and PoseNet loop of every round;
+    test_batch_pose['generators'] is set to the same list.  Without guidance a recording's result then depends on the
+    recording and its generator only, whatever batch or position it has.  mask_scheme='full' still makes the driver's one
+    CPU uniform draw per batch (from torch's global CPU generator) to place its windows."""
     dev = test_batch_traj['cond'].device
     tfd = traj_dataset.traj_feat_dim
     pose_feat_dim = traj_dataset.pose_feat_dim
+    if test_batch_traj.get('generators') is not None:
+        from .noise_streams import check_generators
+        check_generators(test_batch_traj, test_batch_traj['cond'].shape[0], dev)
+        test_batch_pose['generators'] = test_batch_traj['generators']
     mask_traj = start = end = None
     len_t = len_p = lens = None  # int32 device lengths in trajectory / pose frames, and the ints
     if test_batch_traj.get('lengths') is not None:

@@ -86,11 +86,22 @@ class TrajNetEngine:
         _lib.check(rc, self.ctx)
         return out
 
-    def sample_step(self, x_t, time, coef_row):
+    def sample_step(self, x_t, time, coef_row, streams=None):
         """One whole ancestral step as one graph launch (rohm_trajnet_sample_step): -> (pred_xstart, x_{t-1}); the noise is
-        what torch.randn_like(x_t) would have drawn (torch's CUDA generator is advanced accordingly)."""
+        what torch.randn_like(x_t) would have drawn (torch's CUDA generator is advanced accordingly).  streams
+        (noise_streams.NoiseStreams): clip b's noise comes from its own generator instead (rohm_trajnet_sample_step_clips),
+        over the engine's current lengths, and x_{t-1} is zero past each clip."""
         from .ops import cuda_generator_state
         x0, nxt = torch.empty_like(x_t), torch.empty_like(x_t)
+        if streams is not None:
+            draw = streams.next_draw((x_t.shape[2], x_t.shape[1], True, self.lengths))
+            rc = self.lib.rohm_trajnet_sample_step_clips(self.handle, C.c_void_p(x_t.data_ptr()), C.c_void_p(time.data_ptr()),
+                                                         C.c_void_p(x0.data_ptr()), C.c_void_p(nxt.data_ptr()),
+                                                         C.c_void_p(coef_row.data_ptr()),
+                                                         C.c_void_p(streams.table.data_ptr()), draw, streams.incs,
+                                                         x_t.shape[0], self._stream())
+            _lib.check(rc, self.ctx)
+            return x0, nxt
         gen, seed, offset = cuda_generator_state(x_t.device)
         inc = C.c_uint64(0)
         rc = self.lib.rohm_trajnet_sample_step(self.handle, C.c_void_p(x_t.data_ptr()), C.c_void_p(time.data_ptr()),
