@@ -278,7 +278,7 @@ ROHM_API void rohm_body_destroy(rohm_body* bd);
  * more than 16 bones).  Introspection only. */
 ROHM_API int rohm_body_uses_fused_lbs(const rohm_body* bd);
 
-/* Row pitch, in floats, of the `vertices` buffers handed to rohm_body_forward / rohm_body_from_repr[_layout] from now on:
+/* Row pitch, in floats, of the `vertices` buffers handed to rohm_body_forward / rohm_body_from_repr from now on:
  * frame n's vertices start at vertices + n * pitch.  0 (the default) = dense [N, V, 3] as smplx returns them
  * (reference: body_model output `.vertices`, test_amass_full.py:392-428).  A pitch that is a multiple of 4 floats (>= 3 V;
  * 16-byte-aligned buffer) lets the fused launch write the vertices with TMA bulk stores instead of 4-byte stores (3 V =
@@ -292,43 +292,31 @@ ROHM_API int rohm_body_forward(rohm_body* bd, const float* global_orient, const 
                                const float* transl, int64_t N, float* joints, int num_joints, float* vertices,
                                void* stream);
 
-/* recover_from_repr_smpl(recover_mode='smplx_params') on a normalised representation x [B,294,1,T] with the dataset's
- * mean/std [294]: denormalise, rot6d -> rotmat -> axis-angle (kornia route), then rohm_body_forward. */
-ROHM_API int rohm_body_from_repr(rohm_body* bd, const float* x, const float* mean, const float* stdv, int B, int T,
-                                 float* joints, int num_joints, float* vertices, void* stream);
+/* Clips of different lengths inside padded tensors.  The entry points below that take `lengths` read the clips' frame
+ * counts from device arrays: lengths (int[B], in the frame count of the tensor that call works on) and, where frames are
+ * packed, clip_off (int[B+1], the exclusive prefix sum of lengths) with total_frames = clip_off[B] known to the host.  Packed
+ * means frame t of clip b is row clip_off[b] + t.  Frames past a clip are never read, whatever they hold; where an output
+ * keeps its padded shape its frames past a clip are written as zeros.  lengths = NULL means uniform clips of T frames; then
+ * clip_off must be NULL and total_frames 0, anything else returns ROHM_ERR_INVALID. */
 
-/* The same with an explicit layout: channels_last = 0 -> x is [B,294,1,T] (PoseNet tensors); 1 -> x is [B,T,294] (the
- * drivers' tensors, test_amass_full.py:279-293, 386-428). */
-ROHM_API int rohm_body_from_repr_layout(rohm_body* bd, const float* x, int channels_last, const float* mean,
-                                        const float* stdv, int B, int T, float* joints, int num_joints, float* vertices,
-                                        void* stream);
-
-/* Clips of different lengths inside padded tensors.  The *_lengths entry points below take the clips' frame counts as device
- * arrays: lengths (int[B], in the frame count of the tensor that call works on) and, where frames are packed, clip_off
- * (int[B+1], the exclusive prefix sum of lengths) with total_frames = clip_off[B] known to the host.  Packed means frame t of
- * clip b is row clip_off[b] + t.  Frames past a clip are never read, whatever they hold; where an output keeps its padded
- * shape its frames past a clip are written as zeros. */
-
-/* rohm_body_from_repr_layout over clips of lengths[b] <= T frames (lengths[b] = clip_off[b+1] - clip_off[b]) of the padded
- * x: joints [total_frames, num_joints, 3] and optionally vertices [total_frames, V, 3] (pitched as rohm_body_forward's),
- * packed.  FK and the blend GEMM + skinning run over total_frames rows, and total_frames (not B*T) is what has to fit the
- * handle's capacity.  Each frame equals the same frame of the padded call bit for bit. */
-ROHM_API int rohm_body_from_repr_lengths(rohm_body* bd, const float* x, int channels_last, const float* mean,
-                                         const float* stdv, int B, int T, const int* lengths, const int* clip_off,
-                                         int64_t total_frames, float* joints, int num_joints, float* vertices,
-                                         void* stream);
+/* recover_from_repr_smpl(recover_mode='smplx_params') on a normalised representation x with the dataset's mean/std [294]:
+ * denormalise, rot6d -> rotmat -> axis-angle (kornia route), then rohm_body_forward.  channels_last = 0 -> x is
+ * [B,294,1,T] (PoseNet tensors); 1 -> x is [B,T,294] (the drivers' tensors, test_amass_full.py:279-293, 386-428).
+ * Uniform clips: joints [B*T, num_joints, 3] and optionally vertices [B*T, V, 3].  With lengths (1 <= lengths[b] <= T):
+ * the clips' own frames only, packed: joints [total_frames, num_joints, 3] and optionally vertices [total_frames, V, 3]; FK
+ * and the blend GEMM + skinning run over total_frames rows, and total_frames (not B*T) is what has to fit the handle's
+ * capacity.  Each frame equals the same frame of the uniform call bit for bit.  Vertices are pitched as rohm_body_forward's. */
+ROHM_API int rohm_body_from_repr(rohm_body* bd, const float* x, int channels_last, const float* mean, const float* stdv,
+                                 int B, int T, const int* lengths, const int* clip_off, int64_t total_frames, float* joints,
+                                 int num_joints, float* vertices, void* stream);
 
 /* PoseNet.guide_skating_with_smpl(compute_grad='x_0'): grad [B,294,1,T] = d(-(loss_smpl + loss_abs))/d x0 with the
  * channels [0,22) and the 4 contact channels zero.  Analytic VJP (no autograd); all-zero if nothing skates.
- * loss_out: optional device float[4] = {sum_abs, count_abs, sum_smpl, count_smpl}. */
-ROHM_API int rohm_skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, int B, int T,
-                                   float* grad, float* loss_out, void* stream);
-
-/* rohm_skating_guidance over clips of lengths[b] real frames (device int[B], 1 <= lengths[b] <= T): frames at or past
- * lengths[b] add nothing to the sums or counts and get a zero gradient, a velocity pair (t, t + 1) counts only when
- * t + 1 < lengths[b], and their values are never used.  The normalisers stay batch-wide over the real frames. */
-ROHM_API int rohm_skating_guidance_lengths(rohm_body* bd, const float* x0, const float* mean, const float* stdv,
-                                           const int* lengths, int B, int T, float* grad, float* loss_out, void* stream);
+ * loss_out: optional device float[4] = {sum_abs, count_abs, sum_smpl, count_smpl}.  With lengths (1 <= lengths[b] <= T):
+ * frames at or past lengths[b] add nothing to the sums or counts and get a zero gradient, a velocity pair (t, t + 1) counts
+ * only when t + 1 < lengths[b], and their values are never used.  The normalisers stay batch-wide over the real frames. */
+ROHM_API int rohm_skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, const int* lengths,
+                                   int B, int T, float* grad, float* loss_out, void* stream);
 
 /* rohm_skating_guidance in two halves, for clip-sharded runs that reproduce the reference's BATCH-GLOBAL normalisers
  * (posenet.py:230-233, 242-248): _sums computes this shard's {sum_abs, count_abs, sum_smpl, count_smpl} into sums_out (device
@@ -359,74 +347,52 @@ ROHM_API int rohm_projection_guidance(rohm_body* bd, const float* x0, const floa
  * (z-scored with the trajectory dataset's mean/std) -> SMPL-X joints (rot6d -> axis-angle -> FK) -> get_repr_smplx
  * (data_loaders/motion_representation.py:187-282: forward direction, root quaternion incl. the first-NaN repair, velocities,
  * global-orient 6-D / angular velocity, translation) -> traj_full_out [B,T-1,22], z-scored with the pose dataset's stats.
- * 2 <= T <= 8192 (one cluster of at most 8 CTAs of 1024 frames per clip). */
+ * 2 <= T <= 8192 (one cluster of at most 8 CTAs of 1024 frames per clip).  With lengths (2 <= lengths[b] <= T trajectory
+ * frames): composite_out and traj_full_out keep their padded shapes, rows lengths[b] .. T-1 (composite) and
+ * lengths[b]-1 .. T-2 (traj_full) are zeros.  FK runs over the total_frames packed frames; the first-NaN search and repair of
+ * the root quaternion and the velocity pairs stay inside the clip (the repair of frame 0 takes frame lengths[b]-1).  A
+ * clip's rows equal the uniform call on the clip alone with T = lengths[b], bit for bit. */
 ROHM_API int rohm_traj_glue(rohm_body* bd, const float* traj_out, int traj_dim, const float* repr_clean,
                             const float* traj_mean, const float* traj_std, const float* pose_mean, const float* pose_std,
-                            int B, int T, float* composite_out, float* traj_full_out, void* stream);
-
-/* rohm_traj_glue over clips of 2 <= lengths[b] <= T trajectory frames: composite_out [B,T,294] and traj_full_out [B,T-1,22]
- * keep their padded shapes, rows lengths[b] .. T-1 (composite) and lengths[b]-1 .. T-2 (traj_full) are zeros.  FK runs over
- * the total_frames packed frames; the first-NaN search and repair of the root quaternion and the velocity pairs stay inside
- * the clip (the repair of frame 0 takes frame lengths[b]-1).  A clip's rows equal rohm_traj_glue on the clip alone with
- * T = lengths[b], bit for bit. */
-ROHM_API int rohm_traj_glue_lengths(rohm_body* bd, const float* traj_out, int traj_dim, const float* repr_clean,
-                                    const float* traj_mean, const float* traj_std, const float* pose_mean,
-                                    const float* pose_std, int B, int T, const int* lengths, const int* clip_off,
-                                    int64_t total_frames, float* composite_out, float* traj_full_out, void* stream);
+                            int B, int T, const int* lengths, const int* clip_off, int64_t total_frames,
+                            float* composite_out, float* traj_full_out, void* stream);
 
 /* The last stage of rohm_traj_glue on its own: get_repr_smplx's trajectory block (motion_representation.py:187-282) from
  * joints [B,T,22,3], global-orient axis-angles [B*T,3] and translations [B*T,3] -> traj_full_out [B,T-1,22], z-scored with
- * mean/stdv (the first 22 entries are read).  2 <= T <= 8192, as rohm_traj_glue. */
+ * mean/stdv (the first 22 entries are read).  2 <= T <= 8192, as rohm_traj_glue.  With lengths (2 <= lengths[b] <= T):
+ * joints [total_frames,22,3] and global_orient_aa / transl [total_frames,3] hold the clips packed, and traj_full_out keeps
+ * its padded shape with zeros from row lengths[b]-1. */
 ROHM_API int rohm_traj_repr_from_joints(rohm_ctx* ctx, const float* joints, const float* global_orient_aa,
                                         const float* transl, const float* mean, const float* stdv, int B, int T,
-                                        float* traj_full_out, void* stream);
-
-/* The last stage of rohm_traj_glue_lengths on its own: joints [total_frames,22,3], global_orient_aa / transl
- * [total_frames,3] packed -> traj_full_out [B,T-1,22] (padded, zeros from row lengths[b]-1). */
-ROHM_API int rohm_traj_repr_from_joints_lengths(rohm_ctx* ctx, const float* joints, const float* global_orient_aa,
-                                                const float* transl, const float* mean, const float* stdv, int B, int T,
-                                                const int* lengths, const int* clip_off, float* traj_full_out,
-                                                void* stream);
+                                        const int* lengths, const int* clip_off, float* traj_full_out, void* stream);
 
 /* test_amass_full.py:256-258: control_cond [B,T,cond_feats] from the PoseNet output pose_out [B,traj_feats+cond_feats,1,Tp]
- * (frames [0,Tp) copied, frames [Tp,T) repeat frame Tp-1). */
+ * (frames [0,Tp) copied, frames [Tp,T) repeat frame Tp-1).  With lengths (1 <= lengths[b] <= Tp pose frames, and then
+ * T > Tp): control frames [0, lengths[b]) are the clip's pose frames, frame lengths[b] repeats the clip's own last pose
+ * frame, later frames are zeros. */
 ROHM_API int rohm_pose_to_control_cond(rohm_ctx* ctx, const float* pose_out, int B, int Tp, int T, int traj_feats,
-                                       int cond_feats, float* control_cond, void* stream);
-
-/* rohm_pose_to_control_cond over clips of 1 <= lengths[b] <= Tp pose frames (T > Tp): control frames [0, lengths[b]) are
- * the clip's pose frames, frame lengths[b] repeats the clip's own last pose frame, later frames are zeros. */
-ROHM_API int rohm_pose_to_control_cond_lengths(rohm_ctx* ctx, const float* pose_out, int B, int Tp, int T, int traj_feats,
-                                               int cond_feats, const int* lengths, float* control_cond, void* stream);
+                                       int cond_feats, const int* lengths, float* control_cond, void* stream);
 
 /* test_amass_full.py:320-370: PoseNet condition cond_out [B,294,1,Tp] = src (channel-major [B,294,1,src_T] or channels-last
  * [B,src_T,294]) with channels [0,22) replaced by traj_full [B,Tp,22] (NULL keeps src) and channels >= 22 zeroed where
  * chan_keep[c] == 0 (294 bytes, NULL = keep all: the 'lower' / 'upper' joint masks), where frame_lo[b] <= t < frame_hi[b]
- * (int [B], NULL = none: the 'full' scheme) and, with zero_contact, in the 4 contact channels. */
+ * (int [B], NULL = none: the 'full' scheme) and, with zero_contact, in the 4 contact channels.  With lengths
+ * (1 <= lengths[b] <= Tp): frames past a clip are zeros in every channel. */
 ROHM_API int rohm_build_pose_cond(rohm_ctx* ctx, const float* src, int src_channel_major, int src_T, const float* traj_full,
                                   const unsigned char* chan_keep, const int* frame_lo, const int* frame_hi,
-                                  int zero_contact, int B, int Tp, float* cond_out, void* stream);
-
-/* rohm_build_pose_cond over clips of 1 <= lengths[b] <= Tp frames: frames past a clip are zeros in every channel. */
-ROHM_API int rohm_build_pose_cond_lengths(rohm_ctx* ctx, const float* src, int src_channel_major, int src_T,
-                                          const float* traj_full, const unsigned char* chan_keep, const int* frame_lo,
-                                          const int* frame_hi, int zero_contact, int B, int Tp, const int* lengths,
-                                          float* cond_out, void* stream);
+                                  int zero_contact, int B, int Tp, const int* lengths, float* cond_out, void* stream);
 
 /* rot6d_to_rotmat (quaternion.py:482-501) and rotation_matrix_to_angle_axis (konia_transform.py:317-340 -> :350-444 ->
  * :561-631) on n 6-D rotations: aa [n,3] and/or rotmat [n,9] (row-major), either may be NULL. */
 ROHM_API int rohm_rot6d_to_aa(rohm_ctx* ctx, const float* rot6d, int64_t n, float* aa, float* rotmat, void* stream);
 
 /* recover_from_repr_smpl(recover_mode='joint_abs_traj' | 'joint_rel_traj') (motion_representation.py:285-371) on a z-scored
- * representation in either layout -> joints [B,T,22,3]. */
+ * representation in either layout -> joints [B,T,22,3].  With lengths (1 <= lengths[b] <= T): packed joints
+ * [total_frames,22,3] of the clips' own frames.  The absolute mode then has no dependence between frames and runs one thread
+ * per packed frame; the relative mode keeps one thread per clip and stops at lengths[b]. */
 ROHM_API int rohm_joints_from_traj(rohm_ctx* ctx, const float* x, int channels_last, const float* mean, const float* stdv,
-                                   int B, int T, int relative, float* joints, void* stream);
-
-/* rohm_joints_from_traj over clips of 1 <= lengths[b] <= T frames of the padded x -> packed joints [total_frames,22,3].  The
- * absolute mode has no dependence between frames and runs one thread per packed frame; the relative mode keeps one thread
- * per clip and stops at lengths[b]. */
-ROHM_API int rohm_joints_from_traj_lengths(rohm_ctx* ctx, const float* x, int channels_last, const float* mean,
-                                           const float* stdv, int B, int T, const int* lengths, const int* clip_off,
-                                           int64_t total_frames, int relative, float* joints, void* stream);
+                                   int B, int T, const int* lengths, const int* clip_off, int64_t total_frames,
+                                   int relative, float* joints, void* stream);
 
 #ifdef __cplusplus
 }

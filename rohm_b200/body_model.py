@@ -16,6 +16,10 @@ from . import _lib, synthetic
 from ._lib import RohmB200Error
 
 
+def _p(t):
+    return C.c_void_p(t.data_ptr() if t is not None else 0)
+
+
 class BodyOutput:
     """Mirror of smplx's output object: the attributes RoHM reads (``joints``, ``vertices``)."""
 
@@ -99,42 +103,29 @@ class BodyKernels:
             B, T, _ = x.shape
         else:
             B, _, _, T = x.shape
+        clip_off, total = None, 0
         if lengths is not None:
             from .glue import clip_layout
             clip_off, total = clip_layout(lengths, B, T, "from_repr")
-            joints = torch.empty(total, num_joints, 3, device=self.device)
-            verts = self._vertex_buffer(total) if want_vertices else None
-            rc = self.lib.rohm_body_from_repr_lengths(
-                self.handle, C.c_void_p(x.data_ptr()), int(bool(channels_last)), C.c_void_p(mean.data_ptr()),
-                C.c_void_p(std.data_ptr()), B, T, C.c_void_p(lengths.data_ptr()), C.c_void_p(clip_off.data_ptr()), total,
-                C.c_void_p(joints.data_ptr()), num_joints, C.c_void_p(verts.data_ptr() if verts is not None else 0),
-                self._stream())
-            _lib.check(rc, self.ctx)
-            return (joints, verts) if want_vertices else joints
-        joints = torch.empty(B * T, num_joints, 3, device=self.device)
-        verts = self._vertex_buffer(B * T) if want_vertices else None
-        rc = self.lib.rohm_body_from_repr_layout(self.handle, C.c_void_p(x.data_ptr()), int(bool(channels_last)),
-                                                 C.c_void_p(mean.data_ptr()), C.c_void_p(std.data_ptr()), B, T,
-                                                 C.c_void_p(joints.data_ptr()), num_joints,
-                                                 C.c_void_p(verts.data_ptr() if verts is not None else 0), self._stream())
+        frames = B * T if lengths is None else total
+        joints = torch.empty(frames, num_joints, 3, device=self.device)
+        verts = self._vertex_buffer(frames) if want_vertices else None
+        rc = self.lib.rohm_body_from_repr(self.handle, _p(x), int(bool(channels_last)), _p(mean), _p(std), B, T,
+                                          _p(lengths), _p(clip_off), total, _p(joints), num_joints, _p(verts),
+                                          self._stream())
         _lib.check(rc, self.ctx)
+        if lengths is not None:
+            return (joints, verts) if want_vertices else joints
         joints = joints.reshape(B, T, num_joints, 3)
         return (joints, verts.reshape(B, T, self.V, 3)) if want_vertices else joints
 
     def skating_guidance(self, x0, mean, std, want_loss=False, lengths=None):
-        """lengths: optional int32 device tensor [B] of real frames per clip (rohm_skating_guidance_lengths)."""
+        """lengths: optional int32 device tensor [B] of real frames per clip (None: every clip has T frames)."""
         B, _, _, T = x0.shape
         grad = torch.empty_like(x0)
         loss = torch.empty(4, device=self.device) if want_loss else None
-        loss_p = C.c_void_p(loss.data_ptr() if loss is not None else 0)
-        if lengths is not None:
-            rc = self.lib.rohm_skating_guidance_lengths(self.handle, C.c_void_p(x0.data_ptr()), C.c_void_p(mean.data_ptr()),
-                                                        C.c_void_p(std.data_ptr()), C.c_void_p(lengths.data_ptr()), B, T,
-                                                        C.c_void_p(grad.data_ptr()), loss_p, self._stream())
-        else:
-            rc = self.lib.rohm_skating_guidance(self.handle, C.c_void_p(x0.data_ptr()), C.c_void_p(mean.data_ptr()),
-                                                C.c_void_p(std.data_ptr()), B, T, C.c_void_p(grad.data_ptr()), loss_p,
-                                                self._stream())
+        rc = self.lib.rohm_skating_guidance(self.handle, _p(x0), _p(mean), _p(std), _p(lengths), B, T, _p(grad),
+                                            _p(loss), self._stream())
         _lib.check(rc, self.ctx)
         return (grad, loss) if want_loss else grad
 
@@ -172,23 +163,14 @@ class BodyKernels:
 
     def traj_glue(self, traj_out, repr_clean, traj_mean, traj_std, pose_mean, pose_std, lengths=None):
         """test_amass_full.py:268-311 on the device: -> (composite [B,T,294], traj_full [B,T-1,22]).  lengths: (int32 device
-        [B], clip_off int32 device [B+1], their sum) for clips of different lengths (rohm_traj_glue_lengths)."""
+        [B], clip_off int32 device [B+1], their sum) for clips of different lengths, None for clips of T frames."""
         B, T, D = traj_out.shape
         composite = torch.empty(B, T, 294, device=self.device)
         traj_full = torch.empty(B, T - 1, 22, device=self.device)
-        if lengths is not None:
-            lens, clip_off, total = lengths
-            rc = self.lib.rohm_traj_glue_lengths(
-                self.handle, C.c_void_p(traj_out.data_ptr()), D, C.c_void_p(repr_clean.data_ptr()),
-                C.c_void_p(traj_mean.data_ptr()), C.c_void_p(traj_std.data_ptr()), C.c_void_p(pose_mean.data_ptr()),
-                C.c_void_p(pose_std.data_ptr()), B, T, C.c_void_p(lens.data_ptr()), C.c_void_p(clip_off.data_ptr()), total,
-                C.c_void_p(composite.data_ptr()), C.c_void_p(traj_full.data_ptr()), self._stream())
-            _lib.check(rc, self.ctx)
-            return composite, traj_full
-        rc = self.lib.rohm_traj_glue(self.handle, C.c_void_p(traj_out.data_ptr()), D, C.c_void_p(repr_clean.data_ptr()),
-                                     C.c_void_p(traj_mean.data_ptr()), C.c_void_p(traj_std.data_ptr()),
-                                     C.c_void_p(pose_mean.data_ptr()), C.c_void_p(pose_std.data_ptr()), B, T,
-                                     C.c_void_p(composite.data_ptr()), C.c_void_p(traj_full.data_ptr()), self._stream())
+        lens, clip_off, total = lengths if lengths is not None else (None, None, 0)
+        rc = self.lib.rohm_traj_glue(self.handle, _p(traj_out), D, _p(repr_clean), _p(traj_mean), _p(traj_std),
+                                     _p(pose_mean), _p(pose_std), B, T, _p(lens), _p(clip_off), total, _p(composite),
+                                     _p(traj_full), self._stream())
         _lib.check(rc, self.ctx)
         return composite, traj_full
 

@@ -960,52 +960,31 @@ extern "C" int rohm_body_forward(rohm_body* bd, const float* global_orient, cons
   return ROHM_OK;
 }
 
-// recover_from_repr_smpl(recover_mode='smplx_params') on a normalised representation x [B, 294, 1, T]:
-// joints [B*T, num_joints, 3] and optionally vertices [B*T, V, 3].
-extern "C" int rohm_body_from_repr(rohm_body* bd, const float* x, const float* mean, const float* stdv, int B, int T,
+// recover_from_repr_smpl(recover_mode='smplx_params') on a normalised representation x ([B, 294, 1, T] or, channels_last,
+// [B, T, 294]): joints [B*T, num_joints, 3] and optionally vertices [B*T, V, 3].  With lengths only the clips' own frames are
+// gathered, so FK and the blend GEMM + skinning run over total_frames rows and write packed joints / vertices.
+extern "C" int rohm_body_from_repr(rohm_body* bd, const float* x, int channels_last, const float* mean, const float* stdv,
+                                   int B, int T, const int* lengths, const int* clip_off, int64_t total_frames,
                                    float* joints, int num_joints, float* vertices, void* stream) {
-  return rohm_body_from_repr_layout(bd, x, 0, mean, stdv, B, T, joints, num_joints, vertices, stream);
-}
-
-extern "C" int rohm_body_from_repr_layout(rohm_body* bd, const float* x, int channels_last, const float* mean,
-                                          const float* stdv, int B, int T, float* joints, int num_joints,
-                                          float* vertices, void* stream) {
   if (bd == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = bd->ctx;
   rohm::DeviceGuard device_guard__(ctx);
+  const bool ragged = lengths != nullptr;
   const int64_t N = static_cast<int64_t>(B) * T;
-  if (!x || !mean || !stdv || B <= 0 || T <= 0 || N > bd->max_frames)
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_body_from_repr: bad arguments (B*T=%lld, capacity %lld)",
-                static_cast<long long>(N), static_cast<long long>(bd->max_frames));
+  const int64_t frames = ragged ? total_frames : N;  // rows FK runs over
+  if (!x || !mean || !stdv || B <= 0 || T <= 0 || frames > bd->max_frames ||
+      (ragged ? (!clip_off || total_frames < B || total_frames > N || total_frames > INT32_MAX)
+              : (clip_off != nullptr || total_frames != 0)))
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_body_from_repr: bad arguments (B=%d T=%d, %lld frames in the clips, "
+                "capacity %lld)", B, T, static_cast<long long>(frames), static_cast<long long>(bd->max_frames));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int64_t total = N * kBodyJ;
+  const int64_t total = frames * kBodyJ;
   const int64_t sb = static_cast<int64_t>(kC) * T, sc = channels_last ? 1 : T, stt = channels_last ? kC : 1;
-  repr_to_smplx_kernel<false><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-      x, sb, sc, stt, mean, stdv, B, T, bd->go, bd->bp, bd->betas, bd->transl, nullptr, 0);
+  const auto kernel = ragged ? repr_to_smplx_kernel<true> : repr_to_smplx_kernel<false>;
+  kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(x, sb, sc, stt, mean, stdv, B, T, bd->go, bd->bp,
+                                                                     bd->betas, bd->transl, clip_off, total_frames);
   ROHM_CUDA(ctx, cudaGetLastError());
-  return rohm_body_forward(bd, bd->go, bd->bp, bd->betas, bd->transl, N, joints, num_joints, vertices, stream);
-}
-
-// The same over clips of different lengths inside the padded x: only the clips' own frames are gathered, so FK and the
-// blend GEMM + skinning run over total_frames rows and write packed joints / vertices.
-extern "C" int rohm_body_from_repr_lengths(rohm_body* bd, const float* x, int channels_last, const float* mean,
-                                           const float* stdv, int B, int T, const int* lengths, const int* clip_off,
-                                           int64_t total_frames, float* joints, int num_joints, float* vertices,
-                                           void* stream) {
-  if (bd == nullptr) return ROHM_ERR_INVALID;
-  rohm_ctx* ctx = bd->ctx;
-  rohm::DeviceGuard device_guard__(ctx);
-  if (!x || !mean || !stdv || !lengths || !clip_off || B <= 0 || T <= 0 || total_frames < B ||
-      total_frames > static_cast<int64_t>(B) * T || total_frames > INT32_MAX || total_frames > bd->max_frames)
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_body_from_repr_lengths: bad arguments (B=%d T=%d, %lld frames in the clips, "
-                "capacity %lld)", B, T, static_cast<long long>(total_frames), static_cast<long long>(bd->max_frames));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int64_t total = total_frames * kBodyJ;
-  const int64_t sb = static_cast<int64_t>(kC) * T, sc = channels_last ? 1 : T, stt = channels_last ? kC : 1;
-  repr_to_smplx_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-      x, sb, sc, stt, mean, stdv, B, T, bd->go, bd->bp, bd->betas, bd->transl, clip_off, total_frames);
-  ROHM_CUDA(ctx, cudaGetLastError());
-  return rohm_body_forward(bd, bd->go, bd->bp, bd->betas, bd->transl, total_frames, joints, num_joints, vertices, stream);
+  return rohm_body_forward(bd, bd->go, bd->bp, bd->betas, bd->transl, frames, joints, num_joints, vertices, stream);
 }
 
 // guide_skating_with_smpl (posenet.py:196-257): grad [B, 294, 1, T] = d(-(loss_smpl + loss_abs))/dx0 with the
@@ -1054,15 +1033,16 @@ extern "C" int rohm_skating_guidance_backward(rohm_body* bd, const float* x0, co
   return ROHM_OK;
 }
 
-static int skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, const int* lengths, int B,
-                            int T, float* grad, float* loss_out, void* stream, const char* fn) {
+// lengths (device int[B], or nullptr for clips of T frames): frames at or past lengths[b] add nothing and get a zero gradient.
+extern "C" int rohm_skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, const int* lengths,
+                                     int B, int T, float* grad, float* loss_out, void* stream) {
   if (bd == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = bd->ctx;
   rohm::DeviceGuard device_guard__(ctx);
   const int64_t N = static_cast<int64_t>(B) * T;
   if (!x0 || !mean || !stdv || !grad || B <= 0 || T <= 0 || N > bd->max_frames)
-    return fail(ctx, ROHM_ERR_INVALID, "%s: bad arguments (B*T=%lld, capacity %lld)", fn, static_cast<long long>(N),
-                static_cast<long long>(bd->max_frames));
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_skating_guidance: bad arguments (B*T=%lld, capacity %lld)",
+                static_cast<long long>(N), static_cast<long long>(bd->max_frames));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   GuideWs ws{bd->foot, bd->gdir, bd->sums};
   ROHM_CUDA(ctx, cudaMemsetAsync(bd->sums, 0, 4 * sizeof(float), st));
@@ -1076,15 +1056,4 @@ static int skating_guidance(rohm_body* bd, const float* x0, const float* mean, c
   if (loss_out != nullptr)
     ROHM_CUDA(ctx, cudaMemcpyAsync(loss_out, bd->sums, 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return ROHM_OK;
-}
-
-extern "C" int rohm_skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, int B, int T,
-                                     float* grad, float* loss_out, void* stream) {
-  return skating_guidance(bd, x0, mean, stdv, nullptr, B, T, grad, loss_out, stream, "rohm_skating_guidance");
-}
-
-extern "C" int rohm_skating_guidance_lengths(rohm_body* bd, const float* x0, const float* mean, const float* stdv,
-                                             const int* lengths, int B, int T, float* grad, float* loss_out, void* stream) {
-  if (bd != nullptr && lengths == nullptr) return fail(bd->ctx, ROHM_ERR_INVALID, "rohm_skating_guidance_lengths: null lengths");
-  return skating_guidance(bd, x0, mean, stdv, lengths, B, T, grad, loss_out, stream, "rohm_skating_guidance_lengths");
 }

@@ -501,55 +501,34 @@ using namespace rohm;
 
 extern "C" int rohm_traj_glue(rohm_body* bd, const float* traj_out, int traj_dim, const float* repr_clean,
                               const float* traj_mean, const float* traj_std, const float* pose_mean,
-                              const float* pose_std, int B, int T, float* composite_out, float* traj_full_out,
-                              void* stream) {
+                              const float* pose_std, int B, int T, const int* lengths, const int* clip_off,
+                              int64_t total_frames, float* composite_out, float* traj_full_out, void* stream) {
   if (bd == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = bd->ctx;
   rohm::DeviceGuard device_guard__(ctx);
+  const bool ragged = lengths != nullptr;
   const int64_t N = static_cast<int64_t>(B) * T;
+  const int64_t frames = ragged ? total_frames : N;  // frames FK runs over
   if (!traj_out || !repr_clean || !traj_mean || !traj_std || !pose_mean || !pose_std || !composite_out || !traj_full_out ||
-      B <= 0 || T < 2 || N > bd->max_frames || (traj_dim != 13 && (traj_dim < 1 || traj_dim > kTrajFull)))
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_glue: bad arguments (B=%d T=%d traj_dim=%d capacity %lld frames)", B, T,
-                traj_dim, static_cast<long long>(bd->max_frames));
+      B <= 0 || T < 2 || frames > bd->max_frames || (traj_dim != 13 && (traj_dim < 1 || traj_dim > kTrajFull)) ||
+      (ragged ? (!clip_off || total_frames < 2 * static_cast<int64_t>(B) || total_frames > N)
+              : (clip_off != nullptr || total_frames != 0)))
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_glue: bad arguments (B=%d T=%d traj_dim=%d, %lld frames in the clips, "
+                "capacity %lld frames)", B, T, traj_dim, static_cast<long long>(frames),
+                static_cast<long long>(bd->max_frames));
   if (T > kReprFramesPerCta * kReprMaxCluster)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_glue: T=%d frames exceeds %d (one cluster of at most %d CTAs of %d frames "
                 "per clip)", T, kReprFramesPerCta * kReprMaxCluster, kReprMaxCluster, kReprFramesPerCta);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t total = N * kC;
-  compose_repr_kernel<false><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(traj_out, traj_dim, repr_clean,
-                                                                                       composite_out, N, nullptr, T);
+  const auto compose = ragged ? compose_repr_kernel<true> : compose_repr_kernel<false>;
+  compose<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(traj_out, traj_dim, repr_clean, composite_out, N,
+                                                                     lengths, T);
   ROHM_CUDA(ctx, cudaGetLastError());
-  int rc = rohm_body_from_repr_layout(bd, composite_out, 1, traj_mean, traj_std, B, T, bd->jwork, kBodyJ, nullptr, stream);
-  if (rc != ROHM_OK) return rc;
-  ROHM_CUDA(ctx, launch_traj_full_repr(bd->jwork, bd->go, bd->transl, pose_mean, pose_std, B, T, traj_full_out, st));
-  return ROHM_OK;
-}
-
-extern "C" int rohm_traj_glue_lengths(rohm_body* bd, const float* traj_out, int traj_dim, const float* repr_clean,
-                                      const float* traj_mean, const float* traj_std, const float* pose_mean,
-                                      const float* pose_std, int B, int T, const int* lengths, const int* clip_off,
-                                      int64_t total_frames, float* composite_out, float* traj_full_out, void* stream) {
-  if (bd == nullptr) return ROHM_ERR_INVALID;
-  rohm_ctx* ctx = bd->ctx;
-  rohm::DeviceGuard device_guard__(ctx);
-  const int64_t N = static_cast<int64_t>(B) * T;
-  if (!traj_out || !repr_clean || !traj_mean || !traj_std || !pose_mean || !pose_std || !composite_out || !traj_full_out ||
-      !lengths || !clip_off || B <= 0 || T < 2 || total_frames < 2 * static_cast<int64_t>(B) || total_frames > N ||
-      total_frames > bd->max_frames || (traj_dim != 13 && (traj_dim < 1 || traj_dim > kTrajFull)))
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_glue_lengths: bad arguments (B=%d T=%d traj_dim=%d, %lld frames in the "
-                "clips, capacity %lld frames)", B, T, traj_dim, static_cast<long long>(total_frames),
-                static_cast<long long>(bd->max_frames));
-  if (T > kReprFramesPerCta * kReprMaxCluster)
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_glue_lengths: T=%d frames exceeds %d (one cluster of at most %d CTAs of %d "
-                "frames per clip)", T, kReprFramesPerCta * kReprMaxCluster, kReprMaxCluster, kReprFramesPerCta);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int64_t total = N * kC;
-  compose_repr_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(traj_out, traj_dim, repr_clean,
-                                                                                      composite_out, N, lengths, T);
-  ROHM_CUDA(ctx, cudaGetLastError());
-  // FK over the clips' own frames only: packed joints in jwork, packed global orientations / translations in the handle
-  int rc = rohm_body_from_repr_lengths(bd, composite_out, 1, traj_mean, traj_std, B, T, lengths, clip_off, total_frames,
-                                       bd->jwork, kBodyJ, nullptr, stream);
+  // with lengths, FK over the clips' own frames only: packed joints in jwork, packed global orientations / translations in
+  // the handle
+  int rc = rohm_body_from_repr(bd, composite_out, 1, traj_mean, traj_std, B, T, lengths, clip_off, total_frames, bd->jwork,
+                               kBodyJ, nullptr, stream);
   if (rc != ROHM_OK) return rc;
   ROHM_CUDA(ctx, launch_traj_full_repr(bd->jwork, bd->go, bd->transl, pose_mean, pose_std, B, T, traj_full_out, st, lengths,
                                        clip_off));
@@ -558,86 +537,47 @@ extern "C" int rohm_traj_glue_lengths(rohm_body* bd, const float* traj_out, int 
 
 extern "C" int rohm_traj_repr_from_joints(rohm_ctx* ctx, const float* joints, const float* global_orient_aa,
                                           const float* transl, const float* mean, const float* stdv, int B, int T,
-                                          float* traj_full_out, void* stream) {
+                                          const int* lengths, const int* clip_off, float* traj_full_out, void* stream) {
   if (ctx == nullptr) return ROHM_ERR_INVALID;
   rohm::DeviceGuard device_guard__(ctx);
-  if (!joints || !global_orient_aa || !transl || !mean || !stdv || !traj_full_out || B <= 0 || T < 2)
+  if (!joints || !global_orient_aa || !transl || !mean || !stdv || !traj_full_out || B <= 0 || T < 2 ||
+      (lengths == nullptr) != (clip_off == nullptr))
     return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_repr_from_joints: bad arguments");
   if (T > kReprFramesPerCta * kReprMaxCluster)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_repr_from_joints: T=%d frames exceeds %d (one cluster of at most %d CTAs "
                 "of %d frames per clip)", T, kReprFramesPerCta * kReprMaxCluster, kReprMaxCluster, kReprFramesPerCta);
   ROHM_CUDA(ctx, launch_traj_full_repr(joints, global_orient_aa, transl, mean, stdv, B, T, traj_full_out,
-                                       static_cast<cudaStream_t>(stream)));
-  return ROHM_OK;
-}
-
-extern "C" int rohm_traj_repr_from_joints_lengths(rohm_ctx* ctx, const float* joints, const float* global_orient_aa,
-                                                  const float* transl, const float* mean, const float* stdv, int B, int T,
-                                                  const int* lengths, const int* clip_off, float* traj_full_out,
-                                                  void* stream) {
-  if (ctx == nullptr) return ROHM_ERR_INVALID;
-  rohm::DeviceGuard device_guard__(ctx);
-  if (!joints || !global_orient_aa || !transl || !mean || !stdv || !traj_full_out || !lengths || !clip_off || B <= 0 || T < 2)
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_repr_from_joints_lengths: bad arguments");
-  if (T > kReprFramesPerCta * kReprMaxCluster)
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_traj_repr_from_joints_lengths: T=%d frames exceeds %d (one cluster of at most "
-                "%d CTAs of %d frames per clip)", T, kReprFramesPerCta * kReprMaxCluster, kReprMaxCluster, kReprFramesPerCta);
-  ROHM_CUDA(ctx, launch_traj_full_repr(joints, global_orient_aa, transl, mean, stdv, B, T, traj_full_out,
                                        static_cast<cudaStream_t>(stream), lengths, clip_off));
   return ROHM_OK;
 }
 
+// With lengths the clips' control frames end one past their pose frames, so T must exceed Tp.
 extern "C" int rohm_pose_to_control_cond(rohm_ctx* ctx, const float* pose_out, int B, int Tp, int T, int traj_feats,
-                                         int cond_feats, float* control_cond, void* stream) {
+                                         int cond_feats, const int* lengths, float* control_cond, void* stream) {
   if (ctx == nullptr) return ROHM_ERR_INVALID;
   rohm::DeviceGuard device_guard__(ctx);
-  if (!pose_out || !control_cond || B <= 0 || Tp <= 0 || T < Tp || traj_feats < 0 || cond_feats <= 0 || B > 65535)
+  if (!pose_out || !control_cond || B <= 0 || Tp <= 0 || (lengths != nullptr ? T <= Tp : T < Tp) || traj_feats < 0 ||
+      cond_feats <= 0 || B > 65535)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_pose_to_control_cond: bad arguments");
   dim3 grid((T + 31) / 32, (cond_feats + 31) / 32, B);
-  pose_to_control_kernel<false><<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
-      pose_out, Tp, T, traj_feats, cond_feats, control_cond, nullptr);
-  ROHM_CUDA(ctx, cudaGetLastError());
-  return ROHM_OK;
-}
-
-extern "C" int rohm_pose_to_control_cond_lengths(rohm_ctx* ctx, const float* pose_out, int B, int Tp, int T, int traj_feats,
-                                                 int cond_feats, const int* lengths, float* control_cond, void* stream) {
-  if (ctx == nullptr) return ROHM_ERR_INVALID;
-  rohm::DeviceGuard device_guard__(ctx);
-  if (!pose_out || !control_cond || !lengths || B <= 0 || Tp <= 0 || T <= Tp || traj_feats < 0 || cond_feats <= 0 || B > 65535)
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_pose_to_control_cond_lengths: bad arguments");
-  dim3 grid((T + 31) / 32, (cond_feats + 31) / 32, B);
-  pose_to_control_kernel<true><<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
-      pose_out, Tp, T, traj_feats, cond_feats, control_cond, lengths);
+  const auto kernel = lengths != nullptr ? pose_to_control_kernel<true> : pose_to_control_kernel<false>;
+  kernel<<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(pose_out, Tp, T, traj_feats, cond_feats, control_cond,
+                                                                      lengths);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }
 
 extern "C" int rohm_build_pose_cond(rohm_ctx* ctx, const float* src, int src_channel_major, int src_T,
                                     const float* traj_full, const unsigned char* chan_keep, const int* frame_lo,
-                                    const int* frame_hi, int zero_contact, int B, int Tp, float* cond_out, void* stream) {
+                                    const int* frame_hi, int zero_contact, int B, int Tp, const int* lengths,
+                                    float* cond_out, void* stream) {
   if (ctx == nullptr) return ROHM_ERR_INVALID;
   rohm::DeviceGuard device_guard__(ctx);
   if (!src || !cond_out || B <= 0 || Tp <= 0 || src_T < Tp || B > 65535 || ((frame_lo == nullptr) != (frame_hi == nullptr)))
     return fail(ctx, ROHM_ERR_INVALID, "rohm_build_pose_cond: bad arguments");
   dim3 grid((Tp + 31) / 32, (kC + 31) / 32, B);
-  build_pose_cond_kernel<false><<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
-      src, src_channel_major, src_T, traj_full, chan_keep, frame_lo, frame_hi, zero_contact, Tp, cond_out, nullptr);
-  ROHM_CUDA(ctx, cudaGetLastError());
-  return ROHM_OK;
-}
-
-extern "C" int rohm_build_pose_cond_lengths(rohm_ctx* ctx, const float* src, int src_channel_major, int src_T,
-                                            const float* traj_full, const unsigned char* chan_keep, const int* frame_lo,
-                                            const int* frame_hi, int zero_contact, int B, int Tp, const int* lengths,
-                                            float* cond_out, void* stream) {
-  if (ctx == nullptr) return ROHM_ERR_INVALID;
-  rohm::DeviceGuard device_guard__(ctx);
-  if (!src || !cond_out || !lengths || B <= 0 || Tp <= 0 || src_T < Tp || B > 65535 ||
-      ((frame_lo == nullptr) != (frame_hi == nullptr)))
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_build_pose_cond_lengths: bad arguments");
-  dim3 grid((Tp + 31) / 32, (kC + 31) / 32, B);
-  build_pose_cond_kernel<true><<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
+  const auto kernel = lengths != nullptr ? build_pose_cond_kernel<true> : build_pose_cond_kernel<false>;
+  kernel<<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
       src, src_channel_major, src_T, traj_full, chan_keep, frame_lo, frame_hi, zero_contact, Tp, cond_out, lengths);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
@@ -655,33 +595,23 @@ extern "C" int rohm_rot6d_to_aa(rohm_ctx* ctx, const float* rot6d, int64_t n, fl
   return ROHM_OK;
 }
 
+// With lengths the absolute mode runs one thread per packed frame (frames are independent); otherwise one thread per clip.
 extern "C" int rohm_joints_from_traj(rohm_ctx* ctx, const float* x, int channels_last, const float* mean,
-                                     const float* stdv, int B, int T, int relative, float* joints, void* stream) {
+                                     const float* stdv, int B, int T, const int* lengths, const int* clip_off,
+                                     int64_t total_frames, int relative, float* joints, void* stream) {
   if (ctx == nullptr) return ROHM_ERR_INVALID;
   rohm::DeviceGuard device_guard__(ctx);
-  if (!x || !mean || !stdv || !joints || B <= 0 || T <= 0)
+  const bool ragged = lengths != nullptr;
+  if (!x || !mean || !stdv || !joints || B <= 0 || T <= 0 ||
+      (ragged ? (!clip_off || total_frames < B || total_frames > static_cast<int64_t>(B) * T || total_frames > INT32_MAX)
+              : (clip_off != nullptr || total_frames != 0)))
     return fail(ctx, ROHM_ERR_INVALID, "rohm_joints_from_traj: bad arguments");
   const int64_t sb = static_cast<int64_t>(kC) * T, sc = channels_last ? 1 : T, stt = channels_last ? kC : 1;
-  joints_from_traj_kernel<false><<<(B + 31) / 32, 32, 0, static_cast<cudaStream_t>(stream)>>>(
-      x, sb, sc, stt, mean, stdv, B, T, relative ? 1 : 0, joints, nullptr, nullptr, 0);
-  ROHM_CUDA(ctx, cudaGetLastError());
-  return ROHM_OK;
-}
-
-extern "C" int rohm_joints_from_traj_lengths(rohm_ctx* ctx, const float* x, int channels_last, const float* mean,
-                                             const float* stdv, int B, int T, const int* lengths, const int* clip_off,
-                                             int64_t total_frames, int relative, float* joints, void* stream) {
-  if (ctx == nullptr) return ROHM_ERR_INVALID;
-  rohm::DeviceGuard device_guard__(ctx);
-  if (!x || !mean || !stdv || !joints || !lengths || !clip_off || B <= 0 || T <= 0 || total_frames < B ||
-      total_frames > static_cast<int64_t>(B) * T || total_frames > INT32_MAX)
-    return fail(ctx, ROHM_ERR_INVALID, "rohm_joints_from_traj_lengths: bad arguments");
-  const int64_t sb = static_cast<int64_t>(kC) * T, sc = channels_last ? 1 : T, stt = channels_last ? kC : 1;
-  // absolute mode: frames are independent, one thread per packed frame; relative mode: one thread per clip
-  const int64_t threads = relative ? B : total_frames;
-  const int block = relative ? 32 : 128;
-  joints_from_traj_kernel<true><<<static_cast<unsigned>((threads + block - 1) / block), block, 0,
-                                  static_cast<cudaStream_t>(stream)>>>(
+  const bool per_frame = ragged && !relative;
+  const int64_t threads = per_frame ? total_frames : B;
+  const int block = per_frame ? 128 : 32;
+  const auto kernel = ragged ? joints_from_traj_kernel<true> : joints_from_traj_kernel<false>;
+  kernel<<<static_cast<unsigned>((threads + block - 1) / block), block, 0, static_cast<cudaStream_t>(stream)>>>(
       x, sb, sc, stt, mean, stdv, B, T, relative ? 1 : 0, joints, lengths, clip_off, static_cast<int>(total_frames));
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;

@@ -4,7 +4,7 @@ model/trajnet.py:278-400 key for key.
 
 This runs ONCE after a sampling loop, on [B, T, .] tensors of a few hundred KB: it is not part of the denoising hot path
 (SURVEY.md 8a), so the reductions are plain device-side torch ops; every joint / rotation recovery inside goes through the
-CUDA entry points (rohm_joints_from_traj, rohm_body_from_repr_layout, rohm_rot6d_to_aa).
+CUDA entry points (rohm_joints_from_traj, rohm_body_from_repr, rohm_rot6d_to_aa).
 """
 import torch
 

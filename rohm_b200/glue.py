@@ -111,20 +111,17 @@ def traj_repr_from_joints(joints, global_orient_aa, transl, mean, std, lengths=N
     ...]); the output keeps the padded shape [B,T-1,22] with zeros from row lengths[b] - 1."""
     joints, go, tr = _f32c(joints, "joints"), _f32c(global_orient_aa, "global_orient_aa"), _f32c(transl, "transl")
     lib, ctx = _lib.load(), _lib.ctx(joints.device.index)
+    clip_off = None
     if lengths is not None:
         B, T = int(lengths.shape[0]), int(frames)
         clip_off, total = clip_layout(lengths, B, T, "traj_repr_from_joints", least=2)
         if joints.shape[0] != total or go.numel() != total * 3 or tr.numel() != total * 3:
             raise RohmB200Error(f"traj_repr_from_joints: with lengths the inputs hold the {total} packed frames of the clips")
-        out = torch.empty(B, T - 1, TRAJ_FULL_DIM, device=joints.device)
-        rc = lib.rohm_traj_repr_from_joints_lengths(ctx, _p(joints), _p(go), _p(tr), _p(mean), _p(std), B, T, _p(lengths),
-                                                    _p(clip_off), _p(out), _stream(joints.device))
-        _lib.check(rc, ctx)
-        return out
-    B, T = joints.shape[0], joints.shape[1]
+    else:
+        B, T = joints.shape[0], joints.shape[1]
     out = torch.empty(B, T - 1, TRAJ_FULL_DIM, device=joints.device)
-    rc = lib.rohm_traj_repr_from_joints(ctx, _p(joints), _p(go), _p(tr), _p(mean), _p(std), B, T, _p(out),
-                                        _stream(joints.device))
+    rc = lib.rohm_traj_repr_from_joints(ctx, _p(joints), _p(go), _p(tr), _p(mean), _p(std), B, T, _p(lengths), _p(clip_off),
+                                        _p(out), _stream(joints.device))
     _lib.check(rc, ctx)
     return out
 
@@ -139,11 +136,8 @@ def pose_to_control_cond(pose_out, T, pose_feat_dim=272, lengths=None):
     lib, ctx = _lib.load(), _lib.ctx(pose_out.device.index)
     if lengths is not None:
         clip_layout(lengths, B, Tp, "pose_to_control_cond")
-        rc = lib.rohm_pose_to_control_cond_lengths(ctx, _p(pose_out), B, Tp, T, Cc - pose_feat_dim, pose_feat_dim,
-                                                   _p(lengths), _p(out), _stream(pose_out.device))
-    else:
-        rc = lib.rohm_pose_to_control_cond(ctx, _p(pose_out), B, Tp, T, Cc - pose_feat_dim, pose_feat_dim, _p(out),
-                                           _stream(pose_out.device))
+    rc = lib.rohm_pose_to_control_cond(ctx, _p(pose_out), B, Tp, T, Cc - pose_feat_dim, pose_feat_dim, _p(lengths), _p(out),
+                                       _stream(pose_out.device))
     _lib.check(rc, ctx)
     return out
 
@@ -197,11 +191,8 @@ def build_pose_cond(src, traj_full=None, chan_keep=None, frame_lo=None, frame_hi
     lib, ctx = _lib.load(), _lib.ctx(dev.index)
     if lengths is not None:
         clip_layout(lengths, B, Tp, "build_pose_cond")
-        rc = lib.rohm_build_pose_cond_lengths(ctx, _p(src), channel_major, Ts, _p(traj_full), _p(keep_t), _p(lo_t), _p(hi_t),
-                                              int(bool(zero_contact)), B, Tp, _p(lengths), _p(out), _stream(dev))
-    else:
-        rc = lib.rohm_build_pose_cond(ctx, _p(src), channel_major, Ts, _p(traj_full), _p(keep_t), _p(lo_t), _p(hi_t),
-                                      int(bool(zero_contact)), B, Tp, _p(out), _stream(dev))
+    rc = lib.rohm_build_pose_cond(ctx, _p(src), channel_major, Ts, _p(traj_full), _p(keep_t), _p(lo_t), _p(hi_t),
+                                  int(bool(zero_contact)), B, Tp, _p(lengths), _p(out), _stream(dev))
     _lib.check(rc, ctx)
     return out
 
@@ -229,15 +220,13 @@ def joints_from_traj_repr(x, mean, std, relative=False, channels_last=True, leng
     else:
         B, _, _, T = x.shape
     lib, ctx = _lib.load(), _lib.ctx(x.device.index)
+    clip_off, total = None, 0
     if lengths is not None:
         clip_off, total = clip_layout(lengths, B, T, "joints_from_traj_repr")
         out = torch.empty(total, 22, 3, device=x.device)
-        rc = lib.rohm_joints_from_traj_lengths(ctx, _p(x), int(bool(channels_last)), _p(mean), _p(std), B, T, _p(lengths),
-                                               _p(clip_off), total, int(bool(relative)), _p(out), _stream(x.device))
-        _lib.check(rc, ctx)
-        return out
-    out = torch.empty(B, T, 22, 3, device=x.device)
-    rc = lib.rohm_joints_from_traj(ctx, _p(x), int(bool(channels_last)), _p(mean), _p(std), B, T, int(bool(relative)),
-                                   _p(out), _stream(x.device))
+    else:
+        out = torch.empty(B, T, 22, 3, device=x.device)
+    rc = lib.rohm_joints_from_traj(ctx, _p(x), int(bool(channels_last)), _p(mean), _p(std), B, T, _p(lengths), _p(clip_off),
+                                   total, int(bool(relative)), _p(out), _stream(x.device))
     _lib.check(rc, ctx)
     return out

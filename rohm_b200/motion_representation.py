@@ -3,7 +3,7 @@ data_loaders/motion_representation.py (:332-398) that the inference drivers call
 (test_amass_full.py:292, 406, 416-418, 428; test_posenet.py / test_trajnet.py through compute_losses_with_smpl).
 
 Same signature, same dict-of-tensors input (de-normalised [..., T, d] slices of the 294-channel row, keyed by REPR_LIST),
-same outputs; the arithmetic runs in librohm_b200.so (rohm_joints_from_traj, rohm_body_from_repr_layout).
+same outputs; the arithmetic runs in librohm_b200.so (rohm_joints_from_traj, rohm_body_from_repr).
 """
 import torch
 

@@ -37,13 +37,14 @@ class Gemm(C.Structure):
                 ("out_row_add", C.c_int), ("clip_rows", C.c_int), ("clip_valid", C.c_int), ("a_stats", C.c_void_p),
                 ("a_corr", C.c_void_p), ("res_stats", C.c_void_p), ("res_gamma", C.c_void_p), ("res_beta", C.c_void_p),
                 ("stats_out", C.c_void_p), ("ln_eps", C.c_float), ("k_splits", C.c_int), ("split_row_stride", C.c_int),
-                ("want_tma_store", C.c_int), ("store_rows", C.c_int64), ("pdl", C.c_int), ("tma_store", C.c_int)]
+                ("want_tma_store", C.c_int), ("store_rows", C.c_int64), ("pdl", C.c_int), ("tma_store", C.c_int),
+                ("row_mask", C.c_void_p)]
 
 
 class Attn(C.Structure):
     _fields_ = [("qkv_hi", C.c_void_p), ("qkv_lo", C.c_void_p), ("rows", C.c_int64), ("ctx_hi", C.c_void_p),
                 ("ctx_lo", C.c_void_p), ("B", C.c_int), ("S", C.c_int), ("D", C.c_int), ("H", C.c_int), ("scale", C.c_float),
-                ("kind", C.c_int), ("which", C.c_int), ("pdl", C.c_int)]
+                ("kind", C.c_int), ("which", C.c_int), ("pdl", C.c_int), ("clip_off", C.c_void_p), ("clip_ids", C.c_void_p)]
 
 
 class GnArgs(C.Structure):  # rohm_b200/csrc/groupnorm.cuh GnArgs
@@ -68,7 +69,7 @@ def lib():
         _lib.probe_split.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float]
         _lib.probe_f16_weight_scale.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_float)]
         _lib.probe_attention.argtypes = [C.POINTER(Attn), C.c_int]
-        _lib.probe_group_norm.argtypes = [C.POINTER(GnArgs), C.c_int, C.c_int, C.c_int]
+        _lib.probe_group_norm.argtypes = [C.POINTER(GnArgs), C.c_int, C.c_int, C.c_int, C.c_void_p]
         _lib.probe_group_norm_cluster.argtypes = [C.c_int, C.c_int, C.c_int]
     return _lib
 
@@ -145,8 +146,9 @@ def gemm(kind, w, segs, M, N, *, passes=3, m_rows=None, out=None, ldo=None, out_
          bias=None, residual=None, ldr=None, act=ACT_NONE, out_row_mul=1, out_row_add=0, clip_rows=0, clip_valid=0,
          tma_store=False, store_rows=None, k_splits=0, split_row_stride=0,
          a_stats=None, a_corr=None, res_stats=None, res_gamma=None, res_beta=None, stats_out=None, ln_eps=1e-5,
-         pdl=False, n_cols=None, reps=1):
-    """launch_gemm, `reps` times; returns (rc, the filled Gemm struct).  segs: list of Seg."""
+         pdl=False, n_cols=None, row_mask=None, reps=1):
+    """launch_gemm, `reps` times; returns (rc, the filled Gemm struct).  segs: list of Seg.  row_mask: uint8 device tensor
+    [M] of packed clips' real rows (the others are stored as zeros; it needs clip_rows / clip_valid set) or None."""
     g = Gemm()
     g.kind, g.passes, g.block_n = kind, passes, w.block_n
     g.m_rows = M if m_rows is None else m_rows
@@ -171,24 +173,30 @@ def gemm(kind, w, segs, M, N, *, passes=3, m_rows=None, out=None, ldo=None, out_
     g.want_tma_store = int(tma_store)
     g.store_rows = store_rows if store_rows is not None else M
     g.pdl = int(pdl)
+    g.row_mask = _ptr(row_mask)
     rc = lib().probe_gemm(C.byref(g), reps)
     return rc, g
 
 
-def attention(qkv_hi, qkv_lo, ctx_hi, ctx_lo, B, S, D, H, scale, kind, which, pdl=False, reps=1):
-    """launch_attention for clips of any length, `reps` times; returns 0 or the error code."""
-    a = Attn(_ptr(qkv_hi), _ptr(qkv_lo), qkv_hi.shape[0], _ptr(ctx_hi), _ptr(ctx_lo), B, S, D, H, scale, kind, which, int(pdl))
+def attention(qkv_hi, qkv_lo, ctx_hi, ctx_lo, B, S, D, H, scale, kind, which, pdl=False, reps=1, clip_off=None,
+              clip_ids=None):
+    """launch_attention for clips of any length, `reps` times; returns 0 or the error code.  Packed clips (int32 device
+    tensors, fp16 pairs of head dim 128, wgmma kernels): clip c holds rows [clip_off[c], clip_off[c + 1]) and the launch
+    runs the B clips listed in clip_ids, S being their most tokens."""
+    a = Attn(_ptr(qkv_hi), _ptr(qkv_lo), qkv_hi.shape[0], _ptr(ctx_hi), _ptr(ctx_lo), B, S, D, H, scale, kind, which, int(pdl),
+             _ptr(clip_off), _ptr(clip_ids))
     return lib().probe_attention(C.byref(a), reps)
 
 
 def group_norm(part, splits, split_stride, bias, gamma, beta, tp, tp_stride, r1, r2, out, out_hi, out_lo, C_, Tp, T, B, n,
-               f16, groups=8, reps=1):
+               f16, groups=8, reps=1, clip_off=None):
     """gn_mish_split_kernel over B clips with clusters of n CTAs per (clip, group), `reps` times (tensors or None);
-    returns 0 or the CUDA error code."""
+    returns 0 or the CUDA error code.  clip_off (int32 device tensor [B + 1]): packed clips, clip b at rows
+    [clip_off[b], clip_off[b + 1]) with T real rows at most (the engine's level rows Tp and real rows T per clip)."""
     p = _ptr
     a = GnArgs(p(part), splits, split_stride, p(bias), p(gamma), p(beta), p(tp), tp_stride, p(r1), p(r2), p(out), p(out_hi),
                p(out_lo), C_, Tp, T, groups, int(f16))
-    return lib().probe_group_norm(C.byref(a), B, n, reps)
+    return lib().probe_group_norm(C.byref(a), B, n, reps, p(clip_off))
 
 
 def group_norm_cluster(T, C_, groups=8):

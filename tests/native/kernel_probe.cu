@@ -73,6 +73,7 @@ struct ProbeGemm {
   int pdl;
   // set by probe_gemm: what the library decided
   int tma_store;
+  const unsigned char* row_mask;  // packed clips: rows with row_mask[m] == 0 are stored as zeros (NULL: none)
 };
 
 int probe_gemm(ProbeGemm* g, int reps) {
@@ -99,7 +100,7 @@ int probe_gemm(ProbeGemm* g, int reps) {
   p.act = g->act;
   p.M = g->M, p.N = g->N;
   p.out_row_mul = g->out_row_mul, p.out_row_add = g->out_row_add;
-  p.clip_rows = g->clip_rows, p.clip_valid = g->clip_valid;
+  p.clip_rows = g->clip_rows, p.clip_valid = g->clip_valid, p.row_mask = g->row_mask;
   p.a_stats = reinterpret_cast<const float2*>(g->a_stats), p.a_corr = g->a_corr;
   p.res_stats = reinterpret_cast<const float2*>(g->res_stats), p.res_gamma = g->res_gamma, p.res_beta = g->res_beta;
   p.stats_out = reinterpret_cast<float2*>(g->stats_out), p.ln_eps = g->ln_eps;
@@ -131,6 +132,10 @@ struct ProbeAttn {
   int kind;
   int which;  // AttnKernel
   int pdl;
+  // Packed clips (NULL: B uniform clips of S tokens): clip c holds rows [clip_off[c], clip_off[c + 1]) and the launch runs
+  // the B clips listed in clip_ids, S being the most tokens among them.  fp16 pairs of head dim 128, wgmma kernels only.
+  const int* clip_off;
+  const int* clip_ids;
 };
 
 // Clips of any length: the shared-memory limits of every attention kernel are raised for S tokens (the SIMT kernel's is
@@ -142,14 +147,17 @@ int probe_attention(const ProbeAttn* q, int reps) {
   a.ctx_hi = q->ctx_hi, a.ctx_lo = q->ctx_lo;
   a.B = q->B, a.S = q->S, a.D = q->D, a.H = q->H;
   a.scale = q->scale, a.kind = q->kind;
-  if (q->H <= 0 || q->D % q->H != 0 || reps < 1) return static_cast<int>(cudaErrorInvalidValue);
+  a.clip_off = q->clip_off, a.clip_ids = q->clip_ids;
+  const bool packed = q->clip_off != nullptr;
+  if (q->H <= 0 || q->D % q->H != 0 || reps < 1 || (packed && (q->kind != kKindF16 || q->D / q->H != 128)))
+    return static_cast<int>(cudaErrorInvalidValue);
   const int dh = q->D / q->H;
   const cudaError_t e = attention_init_attributes(q->S, dh);
   if (e != cudaSuccess) return static_cast<int>(e);
   AttnWgmmaMaps maps;
   const AttnWgmmaMaps* wg = nullptr;
-  if (q->kind == kKindF16 && dh == 128 &&
-      (q->which == kAttnWgmma || q->which == kAttnWgmmaStream || q->which == kAttnAuto)) {
+  if (packed || (q->kind == kKindF16 && dh == 128 &&
+                 (q->which == kAttnWgmma || q->which == kAttnWgmmaStream || q->which == kAttnAuto))) {
     const int rc = attention_wgmma_maps(&maps, a);
     if (rc != 0) return -rc;
     wg = &maps;
@@ -158,12 +166,13 @@ int probe_attention(const ProbeAttn* q, int reps) {
 }
 
 // GroupNorm + Mish over B clips with clusters of n CTAs per (clip, group), the kernel's shared-memory limit raised to the
-// slice first (so n = 1 also runs groups above the default 48 KB).
-int probe_group_norm(const GnArgs* a, int B, int n, int reps) {
+// slice first (so n = 1 also runs groups above the default 48 KB).  clip_off (device int[B + 1], NULL: clips at b * Tp):
+// packed clips, as launch_gn_mish takes them.
+int probe_group_norm(const GnArgs* a, int B, int n, int reps, const int* clip_off) {
   if (reps < 1 || B < 1) return static_cast<int>(cudaErrorInvalidValue);
   const cudaError_t e = gn_reserve_smem(gn_slice_bytes(a->T, a->C, a->groups, n));
   if (e != cudaSuccess) return static_cast<int>(e);
-  return repeat(reps, [&] { return launch_gn_mish(*a, B, n, nullptr, false); });
+  return repeat(reps, [&] { return launch_gn_mish(*a, B, n, nullptr, false, clip_off); });
 }
 
 // The cluster size rohm_trajnet_create chooses for a (clip, group) of T rows of C / groups channels; 0 on error.

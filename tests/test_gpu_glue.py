@@ -58,7 +58,7 @@ def test_rotation_chain_edge_cases_through_the_kernel(cuda_device):
 
 def test_rotation_chain_edge_cases_through_body_from_repr(body, cuda_device):
     """The same edge rotations as the global orientation / body pose of a representation row, through
-    rohm_body_from_repr_layout, against the oracle's SMPL-X joints."""
+    rohm_body_from_repr, against the oracle's SMPL-X joints."""
     bm, model = body
     g = golden("kinematics.npz")
     r6 = torch.from_numpy(g["rot6d_in"])
@@ -165,7 +165,7 @@ def test_joint_recovery_modes_match_reference(body, cuda_device):
 
 
 def test_from_repr_with_vertices_both_layouts(body, cuda_device):
-    """rohm_body_from_repr(_layout) with vertices, channel-major and channels-last inputs."""
+    """rohm_body_from_repr with vertices, channel-major and channels-last inputs."""
     bm, model = body
     ds = synthetic.make_dataset('pose', seed=3, realistic_std=True)
     x = synthetic.plausible_motion(2, 9, 17, ds)

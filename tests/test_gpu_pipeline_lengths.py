@@ -1,6 +1,6 @@
 """The TrajNet -> PoseNet rounds and the reconstruction on batches of recordings with different lengths
-(test_batch_traj['lengths']): every glue kernel's lengths instance against the existing entry point on the clip cut to its
-own length (bit for bit) and against the glue oracle, the NaN repair inside a clip, the compacted body path, run_rounds
+(test_batch_traj['lengths']): every glue entry point with lengths against the same entry point without them on the clip cut
+to its own length (bit for bit) and against the glue oracle, the NaN repair inside a clip, the compacted body path, run_rounds
 clip by clip against the clip alone, the skating-guided rounds with poisoned padding, the flag variants with
 reconstruct_outputs / result_dict, and the refusals."""
 import ctypes
@@ -22,22 +22,28 @@ from rohm_b200.motion_representation import recover_from_repr_smpl, split_repr
 
 gpu = pytest.mark.gpu
 
-NEW_SYMBOLS = ("rohm_traj_glue_lengths", "rohm_traj_repr_from_joints_lengths", "rohm_pose_to_control_cond_lengths",
-               "rohm_build_pose_cond_lengths", "rohm_body_from_repr_lengths", "rohm_joints_from_traj_lengths")
+# operations whose C entry point takes the optional per-clip lengths (NULL = uniform clips)
+LENGTHS_OPS = ("body_from_repr", "skating_guidance", "traj_glue", "traj_repr_from_joints", "pose_to_control_cond",
+               "build_pose_cond", "joints_from_traj")
 SEL13 = [0, 2, 3, 6] + list(range(7, 13)) + list(range(16, 19))
 SMALL, LONG = (144, 16, 80, 48), (2064, 1040, 16)  # LONG: clusters of 3 CTAs; a clip ending inside CTA 1; one inside CTA 0
 
 
-def test_c_abi_exports_the_lengths_entry_points():
-    """include/rohm_b200.h <-> the ctypes signature table <-> librohm_b200.so for the entry points of this file."""
+def test_c_abi_has_one_entry_point_per_lengths_operation():
+    """include/rohm_b200.h <-> the ctypes signature table <-> librohm_b200.so: each operation of this file is one entry point
+    that takes the lengths as an argument, with no uniform / lengths / layout twins beside it."""
     header = open(os.path.join(ROOT, "include", "rohm_b200.h")).read()
     declared = set(re.findall(r"ROHM_API\s+[\w\s\*]+?\b(rohm_\w+)\s*\(", header))
     if not os.path.exists(_lib.LIB_PATH):
         import __graft_entry__
         __graft_entry__.build()
     lib = ctypes.CDLL(_lib.LIB_PATH)
-    for name in NEW_SYMBOLS:
+    for op in LENGTHS_OPS:
+        name = f"rohm_{op}"
         assert name in declared and name in _lib.SIGNATURES and hasattr(lib, name), name
+    for name in (f"rohm_{op}_{twin}" for op in LENGTHS_OPS for twin in ("lengths", "layout")):
+        assert name not in declared and name not in _lib.SIGNATURES and not hasattr(lib, name), name
+    assert lib.rohm_version() >= 101
 
 
 def _bits(t):

@@ -8,7 +8,6 @@ import pytest
 import torch
 
 import kernel_probe as kp
-import packed_attention_probe as pap
 from oracle import masked_skating_oracle
 from rohm_b200 import _lib, diffusion, synthetic
 from rohm_b200._lib import RohmB200Error
@@ -242,7 +241,7 @@ def test_packed_attention_kernels_against_float64(cuda_device):
     float64 bounds of the uniform-clip tests, bit-identical to the same clip launched alone, no NaN from the poisoned clip
     in any other, and nothing written outside the listed clips."""
     dev = cuda_device
-    pap.lib()
+    kp.lib()
     tokens = SHORT[:3] + LONG[:2] + SHORT[3:] + LONG[2:]
     tokens.insert(UNLISTED_CLIP, 100)
     off, qkv_hi, qkv_lo = _packed(dev, tokens, 3)
@@ -257,8 +256,8 @@ def test_packed_attention_kernels_against_float64(cuda_device):
     long_ = [c for c in listed if tokens[c] > 160][::-1]
     for ids, which in ((short, kp.ATTN_WGMMA), (long_, kp.ATTN_WGMMA_STREAM)):
         S = max(tokens[c] for c in ids)
-        rc = pap.attention_packed(qkv_hi, qkv_lo, ctx_hi, ctx_lo, clip_off, torch.tensor(ids, dtype=torch.int32, device=dev),
-                                 S, D, H, scale, which)
+        rc = kp.attention(qkv_hi, qkv_lo, ctx_hi, ctx_lo, len(ids), S, D, H, scale, kp.KIND_F16, which, clip_off=clip_off,
+                          clip_ids=torch.tensor(ids, dtype=torch.int32, device=dev))
         assert rc == 0, (which, rc)
     torch.cuda.synchronize()
     u0, u1 = off[UNLISTED_CLIP], off[UNLISTED_CLIP + 1]

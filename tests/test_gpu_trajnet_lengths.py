@@ -7,7 +7,6 @@ import pytest
 import torch
 
 import kernel_probe as kp
-import trajnet_packed_probe as tpp
 from helpers import TOL
 from oracle import trajnet_oracle
 from rohm_b200 import _lib, diffusion, synthetic
@@ -273,8 +272,8 @@ def test_packed_group_norm_matches_float64(cuda_device, C, div):
             out = torch.full((nrows * C + extra,), SENTINEL, device=cuda_device)
             hi = torch.full((nrows * C + extra,), SENTINEL, device=cuda_device, dtype=pair_dtype)
             lo = torch.full_like(hi, SENTINEL)
-            rc = tpp.group_norm_packed(part_, splits, part_.shape[1], bias, gamma, beta, tp_, C + 4, r1_, r2_, out, hi, lo,
-                                       C, Tp, TL, torch.tensor(clip_off, dtype=torch.int32, device=cuda_device), n, f16)
+            rc = kp.group_norm(part_, splits, part_.shape[1], bias, gamma, beta, tp_, C + 4, r1_, r2_, out, hi, lo, C, Tp, TL, nb,
+                               n, f16, clip_off=torch.tensor(clip_off, dtype=torch.int32, device=cuda_device))
             torch.cuda.synchronize()
             assert rc == 0, rc
             for buf in (out, hi, lo):
@@ -311,7 +310,8 @@ def test_gemm_row_mask(cuda_device, tma):
     outs = []
     for rm in (None, mask):
         out = torch.full((M + 8, N), SENTINEL, device=cuda_device)
-        rc, g = tpp.gemm_row_mask(A, W, M, N, out, bias, kp.ACT_MISH, M, M, rm, tma_store=tma)
+        rc, g = kp.gemm(kind, W, [A.seg(W.kblocks[0])], M, N, out=out, bias=bias, act=kp.ACT_MISH, clip_rows=M, clip_valid=M,
+                        row_mask=rm, tma_store=tma)
         torch.cuda.synchronize()
         assert rc == 0, rc
         assert g.tma_store == int(tma), "the bulk-store epilogue was not taken as asked"

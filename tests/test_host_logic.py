@@ -134,18 +134,25 @@ def test_no_cpu_fallback():
 
 
 def test_c_abi_library_exports_every_declared_symbol():
-    """include/rohm_b200.h <-> librohm_b200.so <-> the ctypes signature table (no compute calls here)."""
+    """include/rohm_b200.h <-> librohm_b200.so <-> the ctypes signature table (no compute calls here): the same names, and
+    each declaration's parameter count equal to its argtypes count (a list one pointer short would pass every argument
+    after it in the wrong place)."""
     header = open(os.path.join(ROOT, "include", "rohm_b200.h")).read()
-    declared = set(re.findall(r"ROHM_API\s+[\w\s\*]+?\b(rohm_\w+)\s*\(", header))
+    params = dict(re.findall(r"ROHM_API\s+[\w\s\*]+?\b(rohm_\w+)\s*\(([^)]*)\)", header))
+    declared = set(params)
     assert declared, "no declarations parsed"
     assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
+    for name, plist in params.items():
+        plist = " ".join(plist.split())
+        count = 0 if plist in ("", "void") else plist.count(",") + 1
+        assert count == len(_lib.SIGNATURES[name][1]), (name, count, len(_lib.SIGNATURES[name][1]))
     if not os.path.exists(_lib.LIB_PATH):
         import __graft_entry__
         __graft_entry__.build()
     lib = ctypes.CDLL(_lib.LIB_PATH)
     for name in declared:
         assert hasattr(lib, name), name
-    assert lib.rohm_version() >= 100
+    assert lib.rohm_version() >= 101
 
 
 def test_precision_modes_env_and_header_agree(monkeypatch):
