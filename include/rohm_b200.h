@@ -314,9 +314,13 @@ ROHM_API int rohm_body_from_repr(rohm_body* bd, const float* x, int channels_las
  * channels [0,22) and the 4 contact channels zero.  Analytic VJP (no autograd); all-zero if nothing skates.
  * loss_out: optional device float[4] = {sum_abs, count_abs, sum_smpl, count_smpl}.  With lengths (1 <= lengths[b] <= T):
  * frames at or past lengths[b] add nothing to the sums or counts and get a zero gradient, a velocity pair (t, t + 1) counts
- * only when t + 1 < lengths[b], and their values are never used.  The normalisers stay batch-wide over the real frames. */
+ * only when t + 1 < lengths[b], and their values are never used.  per_clip = 0: the normalisers are batch-wide over the
+ * real frames (the reference on the whole batch).  per_clip = 1: clip b is normalised by its own counts, so its gradient
+ * equals this call on clip b alone ([1,294,1,n_b], n_b = lengths[b] or T, per_clip = 0) bit for bit, and loss_out is
+ * device float[B][4], the four sums per clip.  The counts are exact; the speed sums in loss_out depend on the order of
+ * the device's additions and may differ in the last bits between calls. */
 ROHM_API int rohm_skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, const int* lengths,
-                                   int B, int T, float* grad, float* loss_out, void* stream);
+                                   int B, int T, int per_clip, float* grad, float* loss_out, void* stream);
 
 /* rohm_skating_guidance in two halves, for clip-sharded runs that reproduce the reference's BATCH-GLOBAL normalisers
  * (posenet.py:230-233, 242-248): _sums computes this shard's {sum_abs, count_abs, sum_smpl, count_smpl} into sums_out (device
@@ -332,11 +336,16 @@ ROHM_API int rohm_skating_guidance_backward(rohm_body* bd, const float* x0, cons
  * |perspective_projection(camera <- scene <- canonical joints) - keypoints| * confidence; channels [0,22) and the 4 contact
  * channels zero.  cam_affine [B,12]: rows of the 3x4 map canonical -> camera coordinates per clip
  * (inv(cam_R) (inv(transf_matrix) p - cam_t)); focal, center [B,2]; keypoints_2d [B, kp_frames >= T, 22, 3] = (u, v, conf).
- * Analytic VJP through the 22-joint kinematic tree (no autograd).  loss_out: optional device float = the un-normalised sum. */
-ROHM_API int rohm_projection_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, int B, int T,
-                                      const float* cam_affine, const float* focal, const float* center,
-                                      const float* keypoints_2d, int kp_frames, float* grad, float* loss_out,
-                                      void* stream);
+ * Analytic VJP through the 22-joint kinematic tree (no autograd).  per_clip = 0: the mean runs over the whole batch and
+ * loss_out (optional) is device float[1], the un-normalised sum.  per_clip = 1: the mean of clip b runs over its own
+ * n_b frames (n_b = lengths[b] or T), so its gradient equals this call on clip b alone ([1,294,1,n_b], per_clip = 0) bit for
+ * bit, and loss_out is device float[B], the un-normalised sum per clip.  lengths (1 <= lengths[b] <= T) is accepted only
+ * with per_clip = 1, else ROHM_ERR_INVALID: x0 and keypoints_2d are not read at or past lengths[b] and the gradient there
+ * is zero. */
+ROHM_API int rohm_projection_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv,
+                                      const int* lengths, int B, int T, int per_clip, const float* cam_affine,
+                                      const float* focal, const float* center, const float* keypoints_2d, int kp_frames,
+                                      float* grad, float* loss_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Either side of the sampling loops: the drivers' inter-round glue and representation recovery, on the device

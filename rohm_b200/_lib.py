@@ -76,10 +76,10 @@ SIGNATURES = {
     "rohm_body_set_vertex_pitch": (_i, [_p, _i64]),
     "rohm_body_forward": (_i, [_p, _p, _p, _p, _p, _i64, _p, _i, _p, _p]),
     "rohm_body_from_repr": (_i, [_p, _p, _i, _p, _p, _i, _i, _p, _p, _i64, _p, _i, _p, _p]),
-    "rohm_skating_guidance": (_i, [_p, _p, _p, _p, _p, _i, _i, _p, _p, _p]),
+    "rohm_skating_guidance": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p]),
     "rohm_skating_guidance_sums": (_i, [_p, _p, _p, _p, _i, _i, _p, _p]),
     "rohm_skating_guidance_backward": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p]),
-    "rohm_projection_guidance": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _i, _p, _p, _p]),
+    "rohm_projection_guidance": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _i, _p, _p, _p]),
     "rohm_traj_glue": (_i, [_p, _p, _i, _p, _p, _p, _p, _p, _i, _i, _p, _p, _i64, _p, _p, _p]),
     "rohm_traj_repr_from_joints": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p]),
     "rohm_pose_to_control_cond": (_i, [_p, _p, _i, _i, _i, _i, _i, _p, _p, _p]),

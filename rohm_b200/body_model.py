@@ -119,13 +119,16 @@ class BodyKernels:
         joints = joints.reshape(B, T, num_joints, 3)
         return (joints, verts.reshape(B, T, self.V, 3)) if want_vertices else joints
 
-    def skating_guidance(self, x0, mean, std, want_loss=False, lengths=None):
-        """lengths: optional int32 device tensor [B] of real frames per clip (None: every clip has T frames)."""
+    def skating_guidance(self, x0, mean, std, want_loss=False, lengths=None, per_clip=False):
+        """lengths: optional int32 device tensor [B] of real frames per clip (None: every clip has T frames).
+        per_clip: normalise each clip by its own counts, so clip b's gradient equals the call on clip b alone; the loss
+        is then [B, 4] (the four sums per clip) instead of [4].  Its speed sums may differ in the last bits between calls
+        (the order of the device's additions); the counts are exact."""
         B, _, _, T = x0.shape
         grad = torch.empty_like(x0)
-        loss = torch.empty(4, device=self.device) if want_loss else None
-        rc = self.lib.rohm_skating_guidance(self.handle, _p(x0), _p(mean), _p(std), _p(lengths), B, T, _p(grad),
-                                            _p(loss), self._stream())
+        loss = (torch.empty(B, 4, device=self.device) if per_clip else torch.empty(4, device=self.device)) if want_loss else None
+        rc = self.lib.rohm_skating_guidance(self.handle, _p(x0), _p(mean), _p(std), _p(lengths), B, T, int(bool(per_clip)),
+                                            _p(grad), _p(loss), self._stream())
         _lib.check(rc, self.ctx)
         return (grad, loss) if want_loss else grad
 
@@ -147,17 +150,24 @@ class BodyKernels:
         _lib.check(rc, self.ctx)
         return grad
 
-    def projection_guidance(self, x0, mean, std, cam_affine, focal, center, keypoints_2d, want_loss=False):
+    def projection_guidance(self, x0, mean, std, cam_affine, focal, center, keypoints_2d, want_loss=False, lengths=None,
+                            per_clip=False):
         """d(-loss_2d)/dx0 of guide_2d_projection_with_smpl (reference posenet.py:260-317): x0 [B,294,1,T] normalised,
-        cam_affine [B,3,4] canonical -> camera, focal / center [B,2], keypoints_2d [B,>=T,22,3]."""
+        cam_affine [B,3,4] canonical -> camera, focal / center [B,2], keypoints_2d [B,>=T,22,3].  per_clip: the mean of
+        clip b runs over its own frames, so its gradient equals the call on clip b alone; the loss is then [B] instead of
+        [1].  lengths (optional int32 device tensor [B], per_clip only): frames at or past lengths[b] are not read and get
+        a zero gradient."""
         B, _, _, T = x0.shape
+        if lengths is not None and not per_clip:
+            raise RohmB200Error("projection_guidance: lengths need per_clip=True (a batch-wide mean over clips of different "
+                                "lengths is not defined)")
         grad = torch.empty_like(x0)
-        loss = torch.empty(1, device=self.device) if want_loss else None
+        loss = torch.empty(B if per_clip else 1, device=self.device) if want_loss else None
         rc = self.lib.rohm_projection_guidance(
-            self.handle, C.c_void_p(x0.data_ptr()), C.c_void_p(mean.data_ptr()), C.c_void_p(std.data_ptr()), B, T,
-            C.c_void_p(cam_affine.data_ptr()), C.c_void_p(focal.data_ptr()), C.c_void_p(center.data_ptr()),
-            C.c_void_p(keypoints_2d.data_ptr()), int(keypoints_2d.shape[1]), C.c_void_p(grad.data_ptr()),
-            C.c_void_p(loss.data_ptr() if loss is not None else 0), self._stream())
+            self.handle, C.c_void_p(x0.data_ptr()), C.c_void_p(mean.data_ptr()), C.c_void_p(std.data_ptr()), _p(lengths),
+            B, T, int(bool(per_clip)), C.c_void_p(cam_affine.data_ptr()), C.c_void_p(focal.data_ptr()),
+            C.c_void_p(center.data_ptr()), C.c_void_p(keypoints_2d.data_ptr()), int(keypoints_2d.shape[1]),
+            C.c_void_p(grad.data_ptr()), C.c_void_p(loss.data_ptr() if loss is not None else 0), self._stream())
         _lib.check(rc, self.ctx)
         return (grad, loss) if want_loss else grad
 

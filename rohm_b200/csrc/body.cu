@@ -407,7 +407,7 @@ __device__ __forceinline__ void leg_forward(const M3& R0, const M3* R, const V3*
 struct GuideWs {
   float* foot;   // [2 paths][B*T][4][3] foot joint positions (path 0: abs traj, 1: SMPL-X)
   float* gdir;   // [2][B*T][4][3] dL/dposition before the 1/count normalisation
-  float* sums;   // [4]: sum_abs, cnt_abs, sum_smpl, cnt_smpl
+  float* sums;   // [4]: sum_abs, cnt_abs, sum_smpl, cnt_smpl; per-clip normalisers: [B][4], the same four per clip
 };
 
 __device__ __forceinline__ float ld_ch(const float* x, const float* mean, const float* stdv, int b, int t, int T, int c) {
@@ -491,8 +491,10 @@ __global__ void __launch_bounds__(128) guide_forward_kernel(const float* __restr
 }
 
 // pass 2: foot speeds, masks, loss sums, and dL/dposition directions.  kMasked: clip b has lengths[b] real frames (device
-// int[B]); a velocity pair counts only inside them, so later frames add nothing and get no direction.
-template <bool kMasked>
+// int[B]); a velocity pair counts only inside them, so later frames add nothing and get no direction.  kPerClip: the sums
+// go to clip b's row of ws.sums [B][4].  The counts are integer-valued floats below 2^24, so they come out exact whatever
+// order the atomics land in; the speed sums do depend on that order.
+template <bool kMasked, bool kPerClip>
 __global__ void __launch_bounds__(128) guide_loss_kernel(const float* __restrict__ x, const float* __restrict__ mean,
                                                          const float* __restrict__ stdv, int B, int T, GuideWs ws,
                                                          const int* __restrict__ lengths) {
@@ -531,6 +533,28 @@ __global__ void __launch_bounds__(128) guide_loss_kernel(const float* __restrict
       }
     }
   }
+  if constexpr (kPerClip) {
+    // a warp whose frames all lie in one clip adds its warp totals; a warp that straddles clips adds per thread
+    const unsigned lane = threadIdx.x & 31u;
+    const int b = f < frames ? static_cast<int>(f / T) : -1;
+    const int b0 = __shfl_sync(0xffffffffu, b, 0);
+    float v[4] = {lsum[0], lcnt[0], lsum[1], lcnt[1]};
+    if (__all_sync(0xffffffffu, b == b0 || b < 0)) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
+      if (lane == 0 && b0 >= 0)
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          if (v[q] != 0.0f) atomicAdd(ws.sums + static_cast<int64_t>(b0) * 4 + q, v[q]);
+    } else if (b >= 0) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        if (v[q] != 0.0f) atomicAdd(ws.sums + static_cast<int64_t>(b) * 4 + q, v[q]);
+    }
+    return;
+  }
   // block reduction of the four scalars, then one atomic each
   __shared__ float red[4][128];
   red[0][threadIdx.x] = lsum[0], red[1][threadIdx.x] = lcnt[0], red[2][threadIdx.x] = lsum[1], red[3][threadIdx.x] = lcnt[1];
@@ -544,7 +568,9 @@ __global__ void __launch_bounds__(128) guide_loss_kernel(const float* __restrict
 }
 
 // pass 3: VJP to the normalised representation; grad = d(-(loss_smpl + loss_abs))/dx0, channels [0,traj) and the
-// contact channels are zero (the output buffer was cleared; only the channels with a non-zero gradient are written)
+// contact channels are zero (the output buffer was cleared; only the channels with a non-zero gradient are written).
+// kPerClip: clip b is scaled by its own counts, row b of ws.sums [B][4].
+template <bool kPerClip>
 __global__ void __launch_bounds__(128) guide_backward_kernel(const float* __restrict__ x, const float* __restrict__ mean,
                                                              const float* __restrict__ stdv, const float* __restrict__ Jt,
                                                              const float* __restrict__ Jd, int B, int T, GuideWs ws,
@@ -556,7 +582,8 @@ __global__ void __launch_bounds__(128) guide_backward_kernel(const float* __rest
   if (lengths != nullptr && t >= lengths[b]) return;  // past the clip: the cleared zero gradient
   auto ch = [&](int c) { return ld_ch(x, mean, stdv, b, t, T, c); };
   auto put = [&](int c, float g) { grad[(static_cast<int64_t>(b) * kC + c) * T + t] = g * stdv[c]; };
-  const float cnt_abs = ws.sums[1], cnt_smpl = ws.sums[3];
+  const float* sums = kPerClip ? ws.sums + static_cast<int64_t>(b) * 4 : ws.sums;
+  const float cnt_abs = sums[1], cnt_smpl = sums[3];
   const float sc_abs = cnt_abs != 0.0f ? -1.0f / cnt_abs : 0.0f;   // loss enters as -(loss)
   const float sc_smpl = cnt_smpl != 0.0f ? -1.0f / cnt_smpl : 0.0f;
   // ---- abs path: p = Rz(-2a) lp + ...;  dL/dlp = Rz(-2a)^T g ----
@@ -695,11 +722,12 @@ extern "C" int rohm_body_create(rohm_ctx* ctx, const float* v_template, const fl
   bd->foot = bd->pool.floats(2 * F * 12);
   bd->gdir = bd->pool.floats(2 * F * 12);
   bd->sums = bd->pool.floats(16);
-  bd->go = bd->pool.floats(F * 3), bd->bp = bd->pool.floats(F * 63), bd->betas = bd->pool.floats(F * kBetas);
+  bd->clip_sums = bd->pool.floats(F * 4);
+  bd->go =bd->pool.floats(F * 3), bd->bp = bd->pool.floats(F * 63), bd->betas = bd->pool.floats(F * kBetas);
   bd->transl = bd->pool.floats(F * 3);
   bd->jwork = bd->pool.floats(F * kBodyJ * 3), bd->gwork = bd->pool.floats(F * kBodyJ * 3);
   bd->parents_dev = static_cast<int*>(bd->pool.bytes(sizeof(int) * kJ));
-  bool ok = bd->Jt && bd->Jd && bd->foot && bd->gdir && bd->sums && bd->go && bd->bp && bd->betas && bd->transl &&
+  bool ok = bd->Jt && bd->Jd && bd->foot && bd->gdir && bd->sums && bd->clip_sums && bd->go && bd->bp && bd->betas && bd->transl &&
             bd->jwork && bd->gwork && bd->parents_dev;
   if (ok) ok = cudaMemcpy(bd->parents_dev, parents_host, sizeof(int) * kJ, cudaMemcpyHostToDevice) == cudaSuccess;
   if (ok && with_vertices) {
@@ -1011,7 +1039,7 @@ extern "C" int rohm_skating_guidance_sums(rohm_body* bd, const float* x0, const 
   ROHM_CUDA(ctx, cudaMemsetAsync(sums_out, 0, 4 * sizeof(float), st));
   const unsigned blocks = static_cast<unsigned>((N + 127) / 128);
   guide_forward_kernel<<<blocks, 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws);
-  guide_loss_kernel<false><<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws, nullptr);
+  guide_loss_kernel<false, false><<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws, nullptr);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }
@@ -1027,15 +1055,16 @@ extern "C" int rohm_skating_guidance_backward(rohm_body* bd, const float* x0, co
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   GuideWs ws{bd->foot, bd->gdir, const_cast<float*>(sums)};
   ROHM_CUDA(ctx, cudaMemsetAsync(grad, 0, sizeof(float) * N * kC, st));
-  guide_backward_kernel<<<static_cast<unsigned>((N + 127) / 128), 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws, grad,
-                                                                               nullptr);
+  guide_backward_kernel<false><<<static_cast<unsigned>((N + 127) / 128), 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws,
+                                                                                      grad, nullptr);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }
 
 // lengths (device int[B], or nullptr for clips of T frames): frames at or past lengths[b] add nothing and get a zero gradient.
+// per_clip: each clip is normalised by its own counts (sums [B][4] in the handle, B <= B*T fits its capacity).
 extern "C" int rohm_skating_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, const int* lengths,
-                                     int B, int T, float* grad, float* loss_out, void* stream) {
+                                     int B, int T, int per_clip, float* grad, float* loss_out, void* stream) {
   if (bd == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = bd->ctx;
   rohm::DeviceGuard device_guard__(ctx);
@@ -1044,16 +1073,20 @@ extern "C" int rohm_skating_guidance(rohm_body* bd, const float* x0, const float
     return fail(ctx, ROHM_ERR_INVALID, "rohm_skating_guidance: bad arguments (B*T=%lld, capacity %lld)",
                 static_cast<long long>(N), static_cast<long long>(bd->max_frames));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  GuideWs ws{bd->foot, bd->gdir, bd->sums};
-  ROHM_CUDA(ctx, cudaMemsetAsync(bd->sums, 0, 4 * sizeof(float), st));
+  const bool clip = per_clip != 0;
+  const int64_t nsums = clip ? static_cast<int64_t>(B) * 4 : 4;
+  GuideWs ws{bd->foot, bd->gdir, clip ? bd->clip_sums : bd->sums};
+  ROHM_CUDA(ctx, cudaMemsetAsync(ws.sums, 0, nsums * sizeof(float), st));
   ROHM_CUDA(ctx, cudaMemsetAsync(grad, 0, sizeof(float) * N * kC, st));
   const unsigned blocks = static_cast<unsigned>((N + 127) / 128);
   guide_forward_kernel<<<blocks, 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws);
-  if (lengths != nullptr) guide_loss_kernel<true><<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws, lengths);
-  else guide_loss_kernel<false><<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws, nullptr);
-  guide_backward_kernel<<<blocks, 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws, grad, lengths);
+  const auto loss = lengths != nullptr ? (clip ? guide_loss_kernel<true, true> : guide_loss_kernel<true, false>)
+                                       : (clip ? guide_loss_kernel<false, true> : guide_loss_kernel<false, false>);
+  loss<<<blocks, 128, 0, st>>>(x0, mean, stdv, B, T, ws, lengths);
+  const auto backward = clip ? guide_backward_kernel<true> : guide_backward_kernel<false>;
+  backward<<<blocks, 128, 0, st>>>(x0, mean, stdv, bd->Jt, bd->Jd, B, T, ws, grad, lengths);
   ROHM_CUDA(ctx, cudaGetLastError());
   if (loss_out != nullptr)
-    ROHM_CUDA(ctx, cudaMemcpyAsync(loss_out, bd->sums, 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    ROHM_CUDA(ctx, cudaMemcpyAsync(loss_out, ws.sums, nsums * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return ROHM_OK;
 }

@@ -21,6 +21,7 @@ struct rohm_body {
   float *go = nullptr, *bp = nullptr, *betas = nullptr, *transl = nullptr, *A = nullptr, *feat_h = nullptr,
         *feat_l = nullptr, *vposed = nullptr;
   float *foot = nullptr, *gdir = nullptr, *sums = nullptr;
+  float* clip_sums = nullptr;      // [max_frames][4] per-clip skating sums (per-clip normalisers; at most one clip per frame)
   int* parents_dev = nullptr;      // [55] kinematic tree on the device (glue.cu kernels; body.cu keeps a __constant__ copy)
   float* jwork = nullptr;          // [max_frames, 22, 3] scratch joints (glue)
   float* gwork = nullptr;          // [max_frames, 22, 3] scratch joint gradients (2-D guidance)

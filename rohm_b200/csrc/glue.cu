@@ -382,15 +382,23 @@ struct ProjParams {
   int kpT;
   int B, T;
   float* grad;           // [B, 294, 1, T]
-  float* loss_sum;       // optional scalar accumulator (sum of |.|*conf over the selected joints)
+  float* loss_sum;       // optional accumulator (sum of |.|*conf over the selected joints): [1], per-clip normalisers [B]
+  const int* lengths;    // [B] real frames per clip (kLengths instance only)
 };
 
+// kPerClip: the mean runs over clip b's own n_b frames (n_b = lengths[b] with kLengths, else T), so clip b's gradient is
+// that of the clip run as a one-clip batch of n_b frames.  kLengths (with kPerClip only): frames at or past lengths[b] are
+// never read and keep the cleared zero gradient.
+template <bool kPerClip, bool kLengths>
 __global__ void __launch_bounds__(64) projection_guidance_kernel(const ProjParams p) {
+  static_assert(kPerClip || !kLengths, "a lengths instance normalises per clip");
   const int64_t f = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const int64_t frames = static_cast<int64_t>(p.B) * p.T;
   if (f >= frames) return;
   const int b = static_cast<int>(f / p.T), t = static_cast<int>(f % p.T);
   const int T = p.T;
+  const int n = kLengths ? p.lengths[b] : T;
+  if (kLengths && t >= n) return;
   auto ch = [&](int c) { return p.x[(static_cast<int64_t>(b) * kC + c) * T + t] * p.stdv[c] + p.mean[c]; };
   auto put = [&](int c, float g) { p.grad[(static_cast<int64_t>(b) * kC + c) * T + t] = g * p.stdv[c]; };
   float be[kBetas], gbe[kBetas];
@@ -439,7 +447,9 @@ __global__ void __launch_bounds__(64) projection_guidance_kernel(const ProjParam
   for (int j = 0; j < kBodyJ; ++j) gp[j] = {0.f, 0.f, 0.f};
   const float* cm = p.cam + static_cast<int64_t>(b) * 12;
   const float fx = p.focal[b * 2], fy = p.focal[b * 2 + 1], cx = p.center[b * 2], cy = p.center[b * 2 + 1];
-  const float scale = -1.0f / (static_cast<float>(p.B) * static_cast<float>(p.T) * 10.0f * 2.0f);  // d(-mean)/d term
+  // d(-mean)/d term; per clip the same expression with B = 1 and T = n_b
+  const float scale = kPerClip ? -1.0f / (static_cast<float>(1) * static_cast<float>(n) * 10.0f * 2.0f)
+                               : -1.0f / (static_cast<float>(p.B) * static_cast<float>(p.T) * 10.0f * 2.0f);
   const int sel[10] = {16, 18, 20, 17, 19, 21, 4, 5, 7, 8};
   float lsum = 0.0f;
 #pragma unroll
@@ -461,7 +471,7 @@ __global__ void __launch_bounds__(64) projection_guidance_kernel(const ProjParam
     gp[j] = {cm[0] * gX + cm[4] * gY + cm[8] * gZ, cm[1] * gX + cm[5] * gY + cm[9] * gZ,
              cm[2] * gX + cm[6] * gY + cm[10] * gZ};
   }
-  if (p.loss_sum != nullptr && lsum != 0.0f) atomicAdd(p.loss_sum, lsum);
+  if (p.loss_sum != nullptr && lsum != 0.0f) atomicAdd(kPerClip ? p.loss_sum + b : p.loss_sum, lsum);
   // reverse sweep
   M3 GW[kBodyJ];
 #pragma unroll
@@ -617,10 +627,12 @@ extern "C" int rohm_joints_from_traj(rohm_ctx* ctx, const float* x, int channels
   return ROHM_OK;
 }
 
-extern "C" int rohm_projection_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv, int B, int T,
-                                        const float* cam_affine, const float* focal, const float* center,
-                                        const float* keypoints_2d, int kp_frames, float* grad, float* loss_out,
-                                        void* stream) {
+// Lengths are defined for per-clip normalisers only: a batch-wide mean over clips of different lengths is not what a
+// one-clip reference run computes for any of them.
+extern "C" int rohm_projection_guidance(rohm_body* bd, const float* x0, const float* mean, const float* stdv,
+                                        const int* lengths, int B, int T, int per_clip, const float* cam_affine,
+                                        const float* focal, const float* center, const float* keypoints_2d, int kp_frames,
+                                        float* grad, float* loss_out, void* stream) {
   if (bd == nullptr) return ROHM_ERR_INVALID;
   rohm_ctx* ctx = bd->ctx;
   rohm::DeviceGuard device_guard__(ctx);
@@ -628,12 +640,18 @@ extern "C" int rohm_projection_guidance(rohm_body* bd, const float* x0, const fl
   if (!x0 || !mean || !stdv || !cam_affine || !focal || !center || !keypoints_2d || !grad || B <= 0 || T <= 0 ||
       kp_frames < T)
     return fail(ctx, ROHM_ERR_INVALID, "rohm_projection_guidance: bad arguments");
+  if (lengths != nullptr && per_clip == 0)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_projection_guidance: lengths need per-clip normalisers (per_clip = 1)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool clip = per_clip != 0;
   ROHM_CUDA(ctx, cudaMemsetAsync(grad, 0, sizeof(float) * N * kC, st));
-  if (loss_out != nullptr) ROHM_CUDA(ctx, cudaMemsetAsync(loss_out, 0, sizeof(float), st));
+  if (loss_out != nullptr) ROHM_CUDA(ctx, cudaMemsetAsync(loss_out, 0, sizeof(float) * (clip ? B : 1), st));
   ProjParams p{x0, mean, stdv, bd->Jt, bd->Jd, bd->parents_dev, cam_affine, focal, center, keypoints_2d, kp_frames, B, T,
-               grad, loss_out};
-  projection_guidance_kernel<<<static_cast<unsigned>((N + 63) / 64), 64, 0, st>>>(p);
+               grad, loss_out, lengths};
+  const auto kernel = lengths != nullptr ? projection_guidance_kernel<true, true>
+                                         : (clip ? projection_guidance_kernel<true, false>
+                                                 : projection_guidance_kernel<false, false>);
+  kernel<<<static_cast<unsigned>((N + 63) / 64), 64, 0, st>>>(p);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }

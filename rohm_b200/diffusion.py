@@ -436,6 +436,8 @@ class _GaussianDiffusion:
         lengths and generators included.  Returns the loop's NoiseStreams with batch['generators'] (the caller closes
         them when the loop ends), else None."""
         inner = model.model if isinstance(model, _WrappedModel) else model
+        if grad_type is not None and self._POSENET and hasattr(inner, "guidance_per_clip"):
+            inner.guidance_per_clip()  # a bad guidance_normaliser, or 'clip' with global_guidance
         if batch is not None and batch.get('lengths') is not None and hasattr(inner, "clip_lengths"):
             inner.clip_lengths(batch, shape, grad_type=grad_type)
         streams = None

@@ -74,11 +74,16 @@ def global_guidance(model, group=None, enable=True):
     """Guidance normalisers of a clip-sharded run.  Default contract (enable=False): each shard equals the reference run on
     that sub-batch.  enable=True: the skating loss is normalised by the batch-wide counts as in an unsharded reference run --
     one 4-float all-reduce per guided step (the only intra-step collective of the path; <= 51 of 1000 steps), which makes the
-    gathered result reproduce the single-GPU run on the whole batch."""
+    gathered result reproduce the single-GPU run on the whole batch.  Refused for a model in guidance_normaliser='clip'
+    mode: each clip is then normalised by its own counts, which needs no collective."""
     if not enable:
         if hasattr(model, "guidance_sum_reducer"):
             del model.guidance_sum_reducer
         return model
+    if getattr(model, "guidance_normaliser", "batch") == "clip":
+        from ._lib import RohmB200Error
+        raise RohmB200Error("global_guidance: the model normalises its guidance per clip (guidance_normaliser='clip'), "
+                            "which needs no collective and contradicts the batch-wide normaliser")
     model.guidance_sum_reducer = lambda sums: dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=group)
     return model
 

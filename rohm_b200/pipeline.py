@@ -48,7 +48,8 @@ def run_rounds(args, model_posenet, model_trajnet, model_trajnet_control, diffus
     never reaches a real frame.  Without guidance (cond_fn_with_grad=False, or steps before it starts) clip b equals the
     clip run as a one-clip batch with lengths=[lengths[b]] on the same noise, bit for bit.  The skating guidance
     normalises its loss over the real frames of the WHOLE batch (as the reference does over a batch), so with guidance on
-    a clip's result depends on its batch-mates.  mask_scheme='full' draws one uniform per clip as without lengths and
+    a clip's result depends on its batch-mates -- unless model_posenet.guidance_normaliser = 'clip', which normalises each
+    clip over its own frames, so that guided clips also equal their one-clip runs bit for bit.  mask_scheme='full' draws one uniform per clip as without lengths and
     places the window inside the clip: start = floor(u * (lengths[b] - 2)), end = min(start + 30, lengths[b] - 1).
     Refused with lengths: grad_type='prox', and infill_traj when its window [65, 65 + int(traj_mask_ratio * 145)) does not
     lie inside every clip.
@@ -68,6 +69,10 @@ def run_rounds(args, model_posenet, model_trajnet, model_trajnet_control, diffus
     mask_traj = start = end = None
     len_t = len_p = lens = None  # int32 device lengths in trajectory / pose frames, and the ints
     if test_batch_traj.get('lengths') is not None:
+        if grad_type == 'prox':
+            # these rounds replay the AMASS driver; the PROX/EgoBody driver's rounds are not implemented here
+            raise RohmB200Error("run_rounds: grad_type='prox' with test_batch_traj['lengths'] is out of scope (the rounds "
+                                "replay the AMASS driver)")
         lens = model_trajnet.clip_lengths(test_batch_traj, test_batch_traj['cond'].shape)
         model_trajnet_control.clip_lengths(test_batch_traj, test_batch_traj['cond'].shape)
         B_, T_ = test_batch_traj['cond'].shape[0], test_batch_traj['cond'].shape[1]

@@ -248,6 +248,9 @@ class PoseNet(nn.Module):
         self.output_process = OutputProcess(self.dataset.pose_feat_dim, self.latent_dim, self.nfeats)
 
         self.precision = None  # None -> ROHM_B200_PRECISION env (default f16x2)
+        # test-time guidance loss normalisers: 'batch' (the reference on the whole batch) or 'clip' (each clip as the
+        # reference on that clip alone); see guidance_per_clip
+        self.guidance_normaliser = 'batch'
         self._engine = None
         self._engine_fingerprint = None
 
@@ -345,19 +348,35 @@ class PoseNet(nn.Module):
                 raise RohmB200Error(f"PoseNet: batch['lengths'] must lie in [1, T={T}]; lengths[{bad[0][0]}] = {bad[0][1]}")
             self._lengths_cache = (lengths, lengths._version, (B, T), values)
         out_of_scope = None
+        per_clip = self.guidance_per_clip() if grad_type is not None else False
         prec = self.precision if self.precision is not None else _precision_from_env()
         if prec != _lib.PRECISION_F16X2:
             out_of_scope = "the tf32x3 / tf32 precisions"
         elif self.latent_dim // self.num_heads != 128:
             out_of_scope = f"head dim {self.latent_dim // self.num_heads}"
-        elif grad_type == 'prox':
+        elif grad_type == 'prox' and not per_clip:
             out_of_scope = "grad_type='prox' (2-D projection guidance)"
         elif grad_type is not None and getattr(self, "guidance_sum_reducer", None) is not None:
             out_of_scope = "parallel.global_guidance (the exact-global sharded skating normaliser)"
         if out_of_scope is not None:
             raise RohmB200Error(f"PoseNet: batch['lengths'] with {out_of_scope} is out of scope; per-clip lengths run "
-                                "with precision f16x2, head dim 128 and the skating guidance only")
+                                "with precision f16x2, head dim 128 and the skating guidance only (both guidance terms "
+                                "with guidance_normaliser='clip')")
         return values
+
+    def guidance_per_clip(self):
+        """Whether the guidance terms are normalised per clip (guidance_normaliser='clip'): clip b's skating and 2-D
+        projection terms are then the reference's on clip b alone, a [1, 294, 1, n_b] batch (n_b = lengths[b] or T), so a
+        guided recording samples the same in any batch.  'batch' (the default) normalises over the whole batch as the
+        reference does.  Raises RohmB200Error, before anything runs on the device, for any other value and for 'clip'
+        together with parallel.global_guidance (whose batch-wide normaliser 'clip' replaces)."""
+        mode = getattr(self, "guidance_normaliser", "batch")
+        if not isinstance(mode, str) or mode not in ("batch", "clip"):
+            raise RohmB200Error(f"PoseNet: guidance_normaliser must be 'batch' or 'clip', got {mode!r}")
+        if mode == "clip" and getattr(self, "guidance_sum_reducer", None) is not None:
+            raise RohmB200Error("PoseNet: guidance_normaliser='clip' with parallel.global_guidance: the per-clip "
+                                "normalisers need no collective and contradict the batch-wide one; disable one of them")
+        return mode == "clip"
 
     def _lengths_on(self, values, device):
         """The per-clip lengths as an int32 device tensor (cached for the guided steps of one loop)."""
@@ -395,9 +414,14 @@ class PoseNet(nn.Module):
             raise RohmB200Error("guide_skating_with_smpl: implemented for the 294-channel representation with the "
                                 "22-channel trajectory block (the configuration RoHM ships)")
         B, _, _, T = x.shape
+        per_clip = self.guidance_per_clip()
         lengths = self.clip_lengths(batch, x.shape, grad_type='amass')
         mean, std = self._norm_stats(x.device)
         k = kernels_for(self.smplx_model, x.device, B * T, with_vertices=False)
+        if per_clip:
+            # each clip normalised by its own counts: clip b's gradient is that of clip b run alone
+            lens = None if lengths is None else self._lengths_on(lengths, x.device)
+            return k.skating_guidance(x, mean, std, lengths=lens, per_clip=True)
         if lengths is not None:
             # frames past a clip's length add nothing; the normalisers stay batch-wide over the real frames
             return k.skating_guidance(x, mean, std, lengths=self._lengths_on(lengths, x.device))
@@ -438,7 +462,8 @@ class PoseNet(nn.Module):
             raise RohmB200Error("guide_2d_projection_with_smpl: implemented for the 294-channel representation with the "
                                 "22-channel trajectory block (the configuration RoHM ships)")
         B, _, _, T = x.shape
-        self.clip_lengths(batch, x.shape, grad_type='prox')  # per-clip lengths are refused here
+        per_clip = self.guidance_per_clip()
+        lengths = self.clip_lengths(batch, x.shape, grad_type='prox')  # per-clip lengths need per-clip normalisers
         dev = x.device
         mean, std = self._norm_stats(dev)
         f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()
@@ -448,7 +473,8 @@ class PoseNet(nn.Module):
                                 f"{tuple(kp.shape)}")
         k = kernels_for(self.smplx_model, dev, B * T, with_vertices=False)
         return k.projection_guidance(x, mean, std, self._camera_affine(batch, dev), f32(batch['focal_length']),
-                                     f32(batch['camera_center']), kp)
+                                     f32(batch['camera_center']), kp, per_clip=per_clip,
+                                     lengths=None if lengths is None else self._lengths_on(lengths, dev))
 
     def compute_losses_with_smpl(self, batch, model_output, smplx_model=None, epoch=0):
         """The evaluation loss dictionary of reference posenet.py:99-193 (what eval_losses returns with its default

@@ -364,6 +364,60 @@ def gen_glue(ref):
     print("glue.npz  proj grad absmax", float(gr.abs().max()), " nan-repair traj finite:", bool(np.isfinite(out["nan_traj22"]).all()))
 
 
+def gen_clip_guidance(ref):
+    """Per-clip guidance normalisers: the reference's guide_skating_with_smpl and guide_2d_projection_with_smpl on each clip
+    of a padded batch run alone, as a one-clip batch of its own frames.  Clip 2 has one frame and clip 3 no foot in
+    contact, so nothing of either skates (the reference returns a 0-dim zero, stored as a zero gradient)."""
+    out = {}
+    ds = synthetic.make_dataset('pose', seed=3, realistic_std=True)
+    lengths = [24, 13, 1, 17]
+    B, T = len(lengths), 24
+    x = synthetic.plausible_motion(B, T, 71, ds)
+    mean, std = torch.from_numpy(ds.Mean), torch.from_numpy(ds.Std)
+    x[3, -4:] = ((0.0 - mean[-4:]) / std[-4:]).reshape(4, 1, 1)  # contact labels 0: no skating pair in clip 3
+    for b, n in enumerate(lengths):
+        x[b, ..., n:] = float("nan")  # never read by a per-clip computation
+    g = torch.Generator().manual_seed(72)
+    cam2world = torch.eye(4)
+    ang = -0.2
+    cam2world[:3, :3] = torch.tensor([[np.cos(ang), 0, np.sin(ang)], [0, 1, 0], [-np.sin(ang), 0, np.cos(ang)]]).float() @ \
+        torch.tensor([[1., 0, 0], [0, 0, 1], [0, -1, 0]])
+    cam2world[:3, 3] = torch.tensor([-0.2, -3.5, 1.1])
+    ds.cam_R, ds.cam_t = cam2world[:3, :3].reshape(3, 3).float(), cam2world[:3, 3].reshape(1, 3).float()
+    tm = torch.eye(4).repeat(B, 1, 1)
+    for b in range(B):
+        a = -0.3 * (b + 1)
+        tm[b, :3, :3] = torch.tensor([[np.cos(a), -np.sin(a), 0], [np.sin(a), np.cos(a), 0], [0, 0, 1]]).float()
+        tm[b, :3, 3] = torch.tensor([0.05 * b, 0.1, -0.02 * b])
+    focal = torch.tensor([[1060.0, 1058.0]]).repeat(B, 1) + torch.arange(B).float()[:, None]
+    center = torch.tensor([[951.0, 536.0]]).repeat(B, 1) - torch.arange(B).float()[:, None]
+    kp = torch.zeros(B, T + 3, 22, 3)
+    kp[..., 0] = 951.0 + 300.0 * torch.randn(B, T + 3, 22, generator=g)
+    kp[..., 1] = 536.0 + 200.0 * torch.randn(B, T + 3, 22, generator=g)
+    kp[..., 2] = (torch.rand(B, T + 3, 22, generator=g) > 0.3).float() * torch.rand(B, T + 3, 22, generator=g)
+    mp, _ = build_ref_posenet(ref, seed=1)
+    mp.dataset, mp.device = ds, 'cpu'
+    skating, proj, proj_loss, skates = np.zeros((B, 294, 1, T), np.float32), np.zeros((B, 294, 1, T), np.float32), [], []
+    for b, n in enumerate(lengths):
+        xb = x[b:b + 1, ..., :n].contiguous()
+        gs = mp.guide_skating_with_smpl({'x_t': xb}, {'pred_xstart': xb}, None, compute_grad='x_0')
+        skates.append(int(gs.dim() > 0))
+        if gs.dim() > 0:
+            skating[b:b + 1, ..., :n] = gs.detach().numpy()
+        batch = {'x_t': xb, 'transf_matrix': tm[b:b + 1].float(), 'focal_length': focal[b:b + 1],
+                 'camera_center': center[b:b + 1], 'keypoints_2d': kp[b:b + 1]}
+        gp = mp.guide_2d_projection_with_smpl(batch, {'pred_xstart': xb}, None, compute_grad='x_0')
+        proj[b:b + 1, ..., :n] = gp.detach().numpy()
+    out["x"], out["lengths"], out["skates"] = x.numpy(), np.array(lengths, np.int64), np.array(skates, np.int64)
+    out["ds_seed"] = np.array(3)
+    out["skating_grad"], out["proj_grad"] = skating, proj
+    out["cam_R"], out["cam_t"] = ds.cam_R.numpy(), ds.cam_t.numpy()
+    out["transf"], out["focal"], out["center"], out["kp"] = tm.numpy(), focal.numpy(), center.numpy(), kp.numpy()
+    np.savez_compressed(os.path.join(OUT, "clip_guidance.npz"), **out)
+    print("clip_guidance.npz  skates per clip", skates, " skating absmax", float(np.abs(skating).max()),
+          " proj absmax", float(np.abs(proj).max()))
+
+
 POSE_RESPACING = "12" + ",0" * 19
 POSE_RECORDED_STEPS = (6, 5, 1, 0)
 
@@ -484,7 +538,8 @@ if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     ref = import_reference()
-    which = sys.argv[1:] or ["schedules", "posenet", "trajnet", "sampling", "kinematics", "glue", "pipeline"]
+    which = sys.argv[1:] or ["schedules", "posenet", "trajnet", "sampling", "kinematics", "glue", "pipeline",
+                             "clip_guidance"]
     for w in which:
         {"schedules": gen_schedules, "posenet": gen_posenet, "trajnet": gen_trajnet, "sampling": gen_sampling,
-         "kinematics": gen_kinematics, "glue": gen_glue, "pipeline": gen_pipeline}[w](ref)
+         "kinematics": gen_kinematics, "glue": gen_glue, "pipeline": gen_pipeline, "clip_guidance": gen_clip_guidance}[w](ref)
