@@ -223,6 +223,16 @@ ROHM_API int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* const*
                                  const int64_t* numels, int time_dim, int cond_dim, int traj_feat_dim, int mid_dim,
                                  int trajcontrol, int control_cond_dim, int max_batch, int frames, int precision,
                                  rohm_trajnet** out);
+/* rohm_trajnet_create for a batch-invariant engine (same arguments).  Every real frame of clip b is then a function of that
+ * clip's inputs, its length, the weights and the precision only: not of B, `frames`, `max_batch`, the clip's position, the
+ * engine serving it, the graph / PDL options or the GPU.  Each convolution's GEMM tile width and split-K ranges are chosen
+ * for a fixed row count per level (64 x (144 + 32) / 2^L, so a 64-clip, 144-frame batch runs the default engine's plan and
+ * bits), and each packed clip's GroupNorm statistics are reduced over the slices the clip has alone.  A clip as a one-clip
+ * batch of its own length, without lengths, gives the same bits as inside any ragged batch. */
+ROHM_API int rohm_trajnet_create_batch_invariant(rohm_ctx* ctx, int n_params, const char* const* names,
+                                                 const float* const* ptrs, const int64_t* numels, int time_dim, int cond_dim,
+                                                 int traj_feat_dim, int mid_dim, int trajcontrol, int control_cond_dim,
+                                                 int max_batch, int frames, int precision, rohm_trajnet** out);
 ROHM_API void rohm_trajnet_destroy(rohm_trajnet* tn);
 
 /* Step-invariant part of TrajNet.forward: the condition pyramid cond_enc1..4 (trajnet.py:192-208) and, with
@@ -235,7 +245,7 @@ ROHM_API int rohm_trajnet_set_cond(rohm_trajnet* tn, const float* cond, const fl
  * with no padding rows past each clip's own 32 (so a batch of mixed lengths does no wasted tensor work).  Frames
  * [0, lengths[b]) of the output depend on that clip alone: bit-identical to the clip as a one-clip padded batch through
  * the same engine, and equal to the clip at its own length up to summation order (another engine may choose other
- * split-K ranges).  Frames past it are zero, and the input values there are never read.  NULL returns to uniform clips.
+ * split-K ranges; in a batch-invariant engine, bit-identical to it).  Frames past it are zero, and the input values there are never read.  NULL returns to uniform clips.
  * Changing the lengths waits for the device to go idle; call set_cond again afterwards.  ROHM_ERR_INVALID for B outside
  * the created capacity or a bad length. */
 ROHM_API int rohm_trajnet_set_lengths(rohm_trajnet* tn, const int* lengths_host, int B);

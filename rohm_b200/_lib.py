@@ -62,6 +62,8 @@ SIGNATURES = {
     "rohm_posenet_launches_per_forward": (_i, [_p]),
     "rohm_trajnet_create": (_i, [_p, _i, C.POINTER(C.c_char_p), C.POINTER(_p), C.POINTER(_i64), _i, _i, _i, _i, _i, _i,
                                  _i, _i, _i, C.POINTER(_p)]),
+    "rohm_trajnet_create_batch_invariant": (_i, [_p, _i, C.POINTER(C.c_char_p), C.POINTER(_p), C.POINTER(_i64), _i, _i,
+                                                 _i, _i, _i, _i, _i, _i, _i, C.POINTER(_p)]),
     "rohm_trajnet_destroy": (None, [_p]),
     "rohm_trajnet_set_cond": (_i, [_p, _p, _p, _i, _p]),
     "rohm_trajnet_set_lengths": (_i, [_p, C.POINTER(_i), _i]),

@@ -20,14 +20,18 @@ namespace {
 // one partial) is formed once into shared memory while each CTA sums its slice in double; the CTAs' (s1, s2) are then added
 // in rank order by every CTA through distributed shared memory, so all hold bit-identical statistics (n = 1: the CTA's own
 // sums, nothing added).  Pad rows are written as zeros, spread over the cluster.
-template <bool kCluster, bool kPacked>
-__global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restrict__ part, int splits, int64_t split_stride,
-                                                            const float* __restrict__ bias, const float* __restrict__ gamma,
-                                                            const float* __restrict__ beta, const float* __restrict__ tp,
-                                                            int tp_stride, const float* __restrict__ r1,
-                                                            const float* __restrict__ r2, float* __restrict__ out,
-                                                            float* __restrict__ out_hi, float* __restrict__ out_lo, int C, int Tp,
-                                                            int T, int groups, int f16, const int* __restrict__ clip_off) {
+// kClipSlices (with kCluster and kPacked: the batch-invariant engines' instance): clip b's statistics are the reduction of
+// v = gn_pick_cluster(Tc, C, groups, kGnClipBudget) slices, the cluster a clip of Tc real rows is launched with alone, whatever
+// the launch's n >= v: CTA r < v sums virtual slice r exactly as rank r of a v-CTA cluster does, the slice sums are added in
+// slice order, and CTAs r >= v hold no rows (they only write pad zeros).  With v = n it is the kPacked instance.
+template <bool kCluster, bool kPacked, bool kClipSlices>
+__device__ __forceinline__ void gn_mish_split(const float* __restrict__ part, int splits, int64_t split_stride,
+                                              const float* __restrict__ bias, const float* __restrict__ gamma,
+                                              const float* __restrict__ beta, const float* __restrict__ tp, int tp_stride,
+                                              const float* __restrict__ r1, const float* __restrict__ r2,
+                                              float* __restrict__ out, float* __restrict__ out_hi, float* __restrict__ out_lo,
+                                              int C, int Tp, int T, int groups, int f16, const int* __restrict__ clip_off) {
+  static_assert(!kClipSlices || (kCluster && kPacked), "virtual slices are a packed-cluster instance");
   extern __shared__ float4 gn_vals[];  // ceil(T / n) * (C / groups) / 4
   __shared__ double red[2][8];         // per-warp sums; then [0][0], [1][0]: this CTA's (s1, s2), read by the whole cluster
   ptx::pdl_launch_dependents();
@@ -42,7 +46,9 @@ __global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restr
   int Tc = T;
   int64_t clip0 = static_cast<int64_t>(b) * Tp;
   if constexpr (kPacked) clip0 = clip_off[b], Tc = clip_off[b + 1] - clip_off[b] - (Tp - T);
-  const int rows = (Tc + n - 1) / n;
+  int slices = n;  // the slices the statistics are reduced over
+  if constexpr (kClipSlices) slices = gn_pick_cluster(Tc, C, groups, kGnClipBudget);
+  const int rows = (Tc + slices - 1) / slices;
   const int t0 = rank * rows;                      // past Tc in trailing CTAs of a short group: their slice is empty
   const int n4 = (min(Tc, t0 + rows) - t0) * gs4;  // <= 0 for an empty slice
   const int c4 = C / 4;
@@ -83,7 +89,7 @@ __global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restr
     if (threadIdx.x == 0) red[0][0] = s1, red[1][0] = s2;
     cluster.sync();   // every CTA's pair is written
     s1 = 0.0, s2 = 0.0;
-    for (int r = 0; r < n; ++r) {
+    for (int r = 0; r < slices; ++r) {
       const double* peer = cluster.map_shared_rank(&red[0][0], r);
       s1 += peer[0], s2 += peer[8];
     }
@@ -133,11 +139,33 @@ __global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restr
   if constexpr (kCluster) cg::this_cluster().barrier_wait();
 }
 
-}  // namespace
-
-size_t gn_slice_bytes(int T, int C, int groups, int n) {
-  return static_cast<size_t>((T + n - 1) / n) * static_cast<size_t>(C / groups) * sizeof(float);
+template <bool kCluster, bool kPacked>
+__global__ void __launch_bounds__(256) gn_mish_split_kernel(const float* __restrict__ part, int splits, int64_t split_stride,
+                                                            const float* __restrict__ bias, const float* __restrict__ gamma,
+                                                            const float* __restrict__ beta, const float* __restrict__ tp,
+                                                            int tp_stride, const float* __restrict__ r1,
+                                                            const float* __restrict__ r2, float* __restrict__ out,
+                                                            float* __restrict__ out_hi, float* __restrict__ out_lo, int C, int Tp,
+                                                            int T, int groups, int f16, const int* __restrict__ clip_off) {
+  gn_mish_split<kCluster, kPacked, false>(part, splits, split_stride, bias, gamma, beta, tp, tp_stride, r1, r2, out, out_hi,
+                                          out_lo, C, Tp, T, groups, f16, clip_off);
 }
+
+// The fifth instance: packed clips in clusters, each clip's statistics over the slices it has alone
+__global__ void __launch_bounds__(256) gn_mish_split_clip_kernel(const float* __restrict__ part, int splits,
+                                                                 int64_t split_stride, const float* __restrict__ bias,
+                                                                 const float* __restrict__ gamma,
+                                                                 const float* __restrict__ beta, const float* __restrict__ tp,
+                                                                 int tp_stride, const float* __restrict__ r1,
+                                                                 const float* __restrict__ r2, float* __restrict__ out,
+                                                                 float* __restrict__ out_hi, float* __restrict__ out_lo, int C,
+                                                                 int Tp, int T, int groups, int f16,
+                                                                 const int* __restrict__ clip_off) {
+  gn_mish_split<true, true, true>(part, splits, split_stride, bias, gamma, beta, tp, tp_stride, r1, r2, out, out_hi, out_lo, C,
+                                  Tp, T, groups, f16, clip_off);
+}
+
+}  // namespace
 
 cudaError_t gn_smem_budgets(size_t* default_budget, size_t* max_budget) {
   cudaFuncAttributes single{}, cluster{};
@@ -153,15 +181,9 @@ cudaError_t gn_smem_budgets(size_t* default_budget, size_t* max_budget) {
   return cudaSuccess;
 }
 
-int gn_pick_cluster(int T, int C, int groups, size_t budget) {
-  for (int n = 1; n <= kGnMaxCluster; n *= 2)
-    if (gn_slice_bytes(T, C, groups, n) <= budget) return n;
-  return kGnMaxCluster;
-}
-
 cudaError_t gn_reserve_smem(size_t bytes) {
   for (auto kern : {gn_mish_split_kernel<false, false>, gn_mish_split_kernel<true, false>, gn_mish_split_kernel<false, true>,
-                    gn_mish_split_kernel<true, true>}) {
+                    gn_mish_split_kernel<true, true>, gn_mish_split_clip_kernel}) {
     cudaFuncAttributes fa{};
     cudaError_t e = cudaFuncGetAttributes(&fa, kern);
     if (e == cudaSuccess && bytes > static_cast<size_t>(fa.maxDynamicSharedSizeBytes))
@@ -179,6 +201,15 @@ cudaError_t launch_gn_mish(const GnArgs& a, int B, int n, cudaStream_t st, bool 
                       gn_slice_bytes(a.T, a.C, a.groups, n), st, ChainAttrs(pdl, static_cast<unsigned>(n)), a.part,
                       a.splits, a.split_stride, a.bias, a.gamma, a.beta, a.tp, a.tp_stride, a.r1, a.r2, a.out, a.out_hi,
                       a.out_lo, a.C, a.Tp, a.T, a.groups, a.f16, clip_off);
+}
+
+cudaError_t launch_gn_mish_clip_slices(const GnArgs& a, int B, int n, size_t smem_bytes, cudaStream_t st, bool pdl,
+                                       const int* clip_off) {
+  if (n < 2 || n > kGnMaxCluster || a.groups <= 0 || a.C % (4 * a.groups) != 0 || clip_off == nullptr)
+    return cudaErrorInvalidValue;
+  return launch_chain(gn_mish_split_clip_kernel, dim3(static_cast<unsigned>(B * a.groups * n)), dim3(256), smem_bytes, st,
+                      ChainAttrs(pdl, static_cast<unsigned>(n)), a.part, a.splits, a.split_stride, a.bias, a.gamma, a.beta,
+                      a.tp, a.tp_stride, a.r1, a.r2, a.out, a.out_hi, a.out_lo, a.C, a.Tp, a.T, a.groups, a.f16, clip_off);
 }
 
 }  // namespace rohm

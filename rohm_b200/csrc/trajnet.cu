@@ -20,6 +20,9 @@
 // (+ time projection, + residual, + TrajControl residual) and emits the hi/lo operand pair of the next convolution.  The
 // step-invariant condition pyramid and control_zero_conv_0 run once per condition (set_cond).  rohm_trajnet_sample_step appends
 // the in-kernel-noise sampler update to the forward graph.
+// Batch-invariant engines (rohm_trajnet_create_batch_invariant) choose every convolution's tile width and K ranges at one
+// canonical row count per level instead of the engine's capacity, and reduce each packed clip's GroupNorm statistics over the
+// slices the clip has alone, so a clip's frames depend on that clip only, not on B, T or max_batch.
 #include <cmath>
 #include <memory>
 #include <new>
@@ -325,6 +328,9 @@ struct rohm_trajnet {
   bool use_pdl = true;  // ROHM_B200_PDL / rohm_trajnet_set_option(1): programmatic dependent launch along the conv / GroupNorm chains
   size_t gn_budget = 0;    // gn_mish_split_kernel's default dynamic shared-memory budget per CTA
   size_t gn_smem_max = 0;  // the largest slice of any of its launches
+  // rohm_trajnet_create_batch_invariant: plans from kInvariantPlanRows, GroupNorm slices from kGnClipBudget and each clip's
+  // own length (launch_gn_mish_clip_slices)
+  bool batch_invariant = false;
   ~rohm_trajnet() {
     for (cudaStream_t q : side)
       if (q) cudaStreamDestroy(q);
@@ -341,6 +347,16 @@ struct rohm_trajnet {
 namespace {
 
 int64_t rows_of(const rohm_trajnet* tn, int level) { return static_cast<int64_t>(tn->max_batch) * tn->Tp[level]; }
+
+// The rows a batch-invariant engine plans its convolutions for at level 0: the trajcontrol benchmark's 64 clips x (144 + 32)
+// rows, so that shape runs the default engine's plan.  Level L plans for kInvariantPlanRows >> L rows.
+constexpr int64_t kInvariantPlanRows = 64 * (144 + 32);
+
+// The row count pick_bn / pick_split plan a convolution at `level` for: the engine's capacity, or in a batch-invariant
+// engine a constant, so that the tile width and the K ranges (hence each output's summation order) depend on the layer alone.
+int64_t plan_rows(const rohm_trajnet* tn, int level) {
+  return tn->batch_invariant ? kInvariantPlanRows >> level : rows_of(tn, level);
+}
 
 int param(rohm_trajnet* tn, const std::string& key, int64_t expect_numel, const float** out) {
   for (int i = 0; i < tn->n_params; ++i) {
@@ -461,11 +477,11 @@ int make_conv(rohm_trajnet* tn, Conv& cv, const std::string& name, const std::st
   const int row_level = (kind == kConv) ? out.level : in_level;
   PackedWeight& pw = cv.w;
   pw.N = Cout, pw.K = Ktot, pw.Kp = Ktot;
-  pw.block_n = pick_bn(Cout, rows_of(tn, row_level));
+  pw.block_n = pick_bn(Cout, plan_rows(tn, row_level));
   const bool can_split = tn->use_splitk && kind == kConv && out.ld == Cout && Cout % 4 == 0;
   if (can_split && ((group_normed && stride == 1 && out.f32 != nullptr && out.hi == nullptr) || (!group_normed && ks > 1))) {
     int bn = pw.block_n;
-    cv.splits = pick_split(Cout, rows_of(tn, out.level), Ktot / kblk, kblk, &bn, group_normed ? 0.0 : 4.0);
+    cv.splits = pick_split(Cout, plan_rows(tn, out.level), Ktot / kblk, kblk, &bn, group_normed ? 0.0 : 4.0);
     if (cv.splits > 1) {
       pw.block_n = bn;
       cv.sum_after = !group_normed;
@@ -532,7 +548,7 @@ int make_conv(rohm_trajnet* tn, Conv& cv, const std::string& name, const std::st
     g.bias = nullptr;
   }
   if (group_normed) {
-    cv.gn_cluster = gn_pick_cluster(tn->Tl[row_level], Cout, kGroups, tn->gn_budget);
+    cv.gn_cluster = gn_pick_cluster(tn->Tl[row_level], Cout, kGroups, tn->batch_invariant ? kGnClipBudget : tn->gn_budget);
     tn->gn_smem_max = std::max(tn->gn_smem_max, gn_slice_bytes(tn->Tl[row_level], Cout, kGroups, cv.gn_cluster));
   }
   // fp32-only or fp16-pair-only outputs with the identity row map leave through TMA bulk stores (the transposed-conv phases
@@ -609,8 +625,18 @@ int run_gn(rohm_trajnet* tn, const Conv& cv, const GroupNorm& gn, int B, const f
   const int C = cv.w.N, level = cv.level_out;
   const GnArgs a{cv.partial, cv.splits, cv.split_rows * C, cv.bias, gn.gamma, gn.beta, tp, tn->tp_total, r1, r2,
                  out.f32, out.hi, out.lo, C, tn->Tp[level], tn->Tl[level], kGroups, tn->kind == kKindF16 ? 1 : 0};
-  ROHM_CUDA(tn->ctx, launch_gn_mish(a, B, cv.gn_cluster, st, tn->use_pdl,
-                                    tn->lengths.empty() ? nullptr : tn->clip_off[level]));
+  if (tn->batch_invariant && !tn->lengths.empty() && cv.gn_cluster > 1) {
+    // each packed clip over the slices it has alone (uniform clips have them already: v = n)
+    size_t smem = 0;
+    for (int len : tn->lengths) {
+      const int Tc = len >> level;
+      smem = std::max(smem, gn_slice_bytes(Tc, C, kGroups, gn_pick_cluster(Tc, C, kGroups, kGnClipBudget)));
+    }
+    ROHM_CUDA(tn->ctx, launch_gn_mish_clip_slices(a, B, cv.gn_cluster, smem, st, tn->use_pdl, tn->clip_off[level]));
+  } else {
+    ROHM_CUDA(tn->ctx, launch_gn_mish(a, B, cv.gn_cluster, st, tn->use_pdl,
+                                      tn->lengths.empty() ? nullptr : tn->clip_off[level]));
+  }
   tn->launches++;
   return ROHM_OK;
 }
@@ -644,12 +670,9 @@ int run_rtb(rohm_trajnet* tn, Rtb& r, int B, cudaStream_t st, cudaStream_t side)
   return run_gn(tn, r.c2, r.gn[1], B, nullptr, r.residual, r.extra, r.out, st);
 }
 
-}  // namespace
-
-extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* const* names, const float* const* ptrs,
-                                   const int64_t* numels, int time_dim, int cond_dim, int traj_feat_dim, int mid_dim,
-                                   int trajcontrol, int control_cond_dim, int max_batch, int frames, int precision,
-                                   rohm_trajnet** out) {
+int trajnet_create(rohm_ctx* ctx, int n_params, const char* const* names, const float* const* ptrs, const int64_t* numels,
+                   int time_dim, int cond_dim, int traj_feat_dim, int mid_dim, int trajcontrol, int control_cond_dim,
+                   int max_batch, int frames, int precision, bool batch_invariant, rohm_trajnet** out) {
   if (ctx == nullptr) return ROHM_ERR_INVALID;
   rohm::DeviceGuard device_guard__(ctx);
   if (names == nullptr || ptrs == nullptr || numels == nullptr || out == nullptr || max_batch <= 0)
@@ -685,6 +708,7 @@ extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* cons
   tn->kind = precision == ROHM_PRECISION_F16X2 ? kKindF16 : kKindTf32;
   tn->max_batch = max_batch, tn->T = frames;
   tn->gn_budget = gn_budget;
+  tn->batch_invariant = batch_invariant;
   for (int l = 0; l < kLevels; ++l) tn->Tl[l] = frames >> l, tn->Tp[l] = (frames + 32) >> l;
   tn->n_params = n_params, tn->names = names, tn->ptrs = ptrs, tn->numels = numels;
   const int m = mid_dim, td = time_dim;
@@ -840,6 +864,25 @@ extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* cons
     return fail(ctx, ROHM_ERR_CUDA, "weight packing / time table build failed: %s", cudaGetErrorString(err));
   *out = owner.release();
   return ROHM_OK;
+}
+
+}  // namespace
+
+extern "C" int rohm_trajnet_create(rohm_ctx* ctx, int n_params, const char* const* names, const float* const* ptrs,
+                                   const int64_t* numels, int time_dim, int cond_dim, int traj_feat_dim, int mid_dim,
+                                   int trajcontrol, int control_cond_dim, int max_batch, int frames, int precision,
+                                   rohm_trajnet** out) {
+  return trajnet_create(ctx, n_params, names, ptrs, numels, time_dim, cond_dim, traj_feat_dim, mid_dim, trajcontrol,
+                        control_cond_dim, max_batch, frames, precision, false, out);
+}
+
+extern "C" int rohm_trajnet_create_batch_invariant(rohm_ctx* ctx, int n_params, const char* const* names,
+                                                   const float* const* ptrs, const int64_t* numels, int time_dim,
+                                                   int cond_dim, int traj_feat_dim, int mid_dim, int trajcontrol,
+                                                   int control_cond_dim, int max_batch, int frames, int precision,
+                                                   rohm_trajnet** out) {
+  return trajnet_create(ctx, n_params, names, ptrs, numels, time_dim, cond_dim, traj_feat_dim, mid_dim, trajcontrol,
+                        control_cond_dim, max_batch, frames, precision, true, out);
 }
 
 extern "C" void rohm_trajnet_destroy(rohm_trajnet* tn) { delete tn; }

@@ -438,6 +438,9 @@ class _GaussianDiffusion:
         inner = model.model if isinstance(model, _WrappedModel) else model
         if grad_type is not None and self._POSENET and hasattr(inner, "guidance_per_clip"):
             inner.guidance_per_clip()  # a bad guidance_normaliser, or 'clip' with global_guidance
+        if not self._POSENET and hasattr(inner, "batch_invariant"):
+            from .trajnet_engine import batch_invariant
+            batch_invariant(inner)  # a non-bool TrajNet.batch_invariant
         if batch is not None and batch.get('lengths') is not None and hasattr(inner, "clip_lengths"):
             inner.clip_lengths(batch, shape, grad_type=grad_type)
         streams = None

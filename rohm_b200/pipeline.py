@@ -49,7 +49,9 @@ def run_rounds(args, model_posenet, model_trajnet, model_trajnet_control, diffus
     clip run as a one-clip batch with lengths=[lengths[b]] on the same noise, bit for bit.  The skating guidance
     normalises its loss over the real frames of the WHOLE batch (as the reference does over a batch), so with guidance on
     a clip's result depends on its batch-mates -- unless model_posenet.guidance_normaliser = 'clip', which normalises each
-    clip over its own frames, so that guided clips also equal their one-clip runs bit for bit.  mask_scheme='full' draws one uniform per clip as without lengths and
+    clip over its own frames, so that guided clips also equal their one-clip runs bit for bit.  Those one-clip runs go through
+    the same TrajNet engines; with batch_invariant = True on model_trajnet and model_trajnet_control they may be at the clip's
+    own length in fresh engines, and still give the same bits.  mask_scheme='full' draws one uniform per clip as without lengths and
     places the window inside the clip: start = floor(u * (lengths[b] - 2)), end = min(start + 30, lengths[b] - 1).
     Refused with lengths: grad_type='prox', and infill_traj when its window [65, 65 + int(traj_mask_ratio * 145)) does not
     lie inside every clip.

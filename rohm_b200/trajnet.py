@@ -113,6 +113,10 @@ class TrajNet(nn.Module):
         self.cond_downsample4 = Downsample1d(m)  # present in checkpoints, never evaluated (reference :174)
 
         self.precision = None
+        # True: the engine is created batch-invariant (rohm_trajnet_create_batch_invariant), so every real frame of a clip
+        # depends on that clip alone, whatever B, padded T, position, engine or GPU.  A plain attribute: not in the state
+        # dict, kept by .to() and load_state_dict.
+        self.batch_invariant = False
         self._engine = None
         self._engine_fingerprint = None
 

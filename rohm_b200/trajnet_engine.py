@@ -11,11 +11,12 @@ from .posenet import _precision_from_env
 
 
 class TrajNetEngine:
-    def __init__(self, module, device, max_batch, frames, precision):
+    def __init__(self, module, device, max_batch, frames, precision, batch_invariant=False):
         self.lib = _lib.load()
         self.ctx = _lib.ctx(device.index)
         self.device = device
         self.max_batch, self.frames, self.precision = max_batch, frames, precision
+        self.batch_invariant = batch_invariant
         sd = {k: v.detach().to(device=device, dtype=torch.float32).contiguous() for k, v in module.state_dict().items()
               if v.is_floating_point()}
         n = len(sd)
@@ -24,9 +25,10 @@ class TrajNetEngine:
         numels = (C.c_int64 * n)(*[v.numel() for v in sd.values()])
         handle = C.c_void_p()
         with torch.cuda.device(device):
-            rc = self.lib.rohm_trajnet_create(self.ctx, n, names, ptrs, numels, module.time_dim, module.cond_dim,
-                                              module.traj_feat_dim, module.mid_dim, int(module.trajcontrol),
-                                              module.control_cond_dim, max_batch, frames, precision, C.byref(handle))
+            create = self.lib.rohm_trajnet_create_batch_invariant if batch_invariant else self.lib.rohm_trajnet_create
+            rc = create(self.ctx, n, names, ptrs, numels, module.time_dim, module.cond_dim, module.traj_feat_dim,
+                        module.mid_dim, int(module.trajcontrol), module.control_cond_dim, max_batch, frames, precision,
+                        C.byref(handle))
         _lib.check(rc, self.ctx)
         self.handle = handle
         if os.environ.get("ROHM_B200_PDL", "1") == "0":
@@ -130,14 +132,24 @@ def get_engine(module, B, T, device):
         raise RohmB200Error("TrajNet: the CUDA engine implements the inference path (model.eval()); training is out of "
                             "scope")
     prec = module.precision if module.precision is not None else _precision_from_env()
+    inv = batch_invariant(module)
     e = module._engine
-    if e is None or e.device != device or B > e.max_batch or T != e.frames or e.precision != prec:
+    if e is None or e.device != device or B > e.max_batch or T != e.frames or e.precision != prec or \
+            e.batch_invariant != inv:
         mb = max(B, e.max_batch if (e is not None and e.device == device and e.frames == T) else 0)
         module._engine = None
-        e = TrajNetEngine(module, device, mb, T, prec)
+        e = TrajNetEngine(module, device, mb, T, prec, inv)
         module._engine = e
         module._engine_fingerprint = _fingerprint(module)
     return e
+
+
+def batch_invariant(module):
+    """module.batch_invariant, checked: a bool (absent on modules built before the attribute existed: False)."""
+    v = getattr(module, 'batch_invariant', False)
+    if not isinstance(v, bool):
+        raise RohmB200Error(f"TrajNet: batch_invariant must be True or False, got {v!r}")
+    return v
 
 
 def run_forward(module, batch, time):
