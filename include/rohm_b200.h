@@ -413,6 +413,35 @@ ROHM_API int rohm_joints_from_traj(rohm_ctx* ctx, const float* x, int channels_l
                                    int B, int T, const int* lengths, const int* clip_off, int64_t total_frames,
                                    int relative, float* joints, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Sliding windows over whole recordings (dataloader_video.py:160-183, dataloader_amass.py:105-131 and :319-341)
+ * ---------------------------------------------------------------------------------------------------------- */
+
+/* R recordings packed frame after frame (recording r holds rows rec_off[r] .. rec_off[r+1]-1 of global_orient [.,3],
+ * transl [.,3], betas [.,10], body_pose [.,63] axis-angle and the 22-joint world positions joints [.,22,3], z up) ->
+ * windows of clip_len frames (3..160) with stride clip_len - overlap (overlap 0..2): window k of a recording starts at
+ * k * (clip_len - overlap) and is cut while it ends inside the recording, so a recording shorter than clip_len gives none.
+ * rec_off_host (host) and rec_off (device) hold the same R + 1 offsets.  *n_windows (host) receives the window count W; if
+ * W > max_windows nothing is launched and ROHM_ERR_INVALID is returned.  Outputs, W rows each: win_rec / win_start (int32:
+ * recording and first frame), transf [W,4,4] (cano_seq_smplx's transf_matrix, world -> canonical), repr_traj / repr_pose
+ * [W, clip_len-1, 294]: get_repr_smplx of the canonical window (motion_representation.py:47-110, :187-282;
+ * update_globalRT_for_smplx with delta_T = pelvis - transl) z-scored with traj_mean / traj_std and pose_mean / pose_std
+ * [294].  Frames outside every window are never read. */
+ROHM_API int rohm_window_encode(rohm_ctx* ctx, const float* global_orient, const float* transl, const float* betas,
+                                const float* body_pose, const float* joints, const int* rec_off_host, const int* rec_off,
+                                int R, int clip_len, int overlap, const float* traj_mean, const float* traj_std,
+                                const float* pose_mean, const float* pose_std, int max_windows, int* n_windows,
+                                int* win_rec, int* win_start, float* transf, float* repr_traj, float* repr_pose,
+                                void* stream);
+
+/* The inverse: joints [W*(clip_len-2),22,3] (each window's clip_len-2 pose frames in its canonical frame, as
+ * reconstruct_outputs returns them) -> world [total_frames,22,3] packed by recording (rec_off, device int[R+1]), pose frame t
+ * of window w at row rec_off[win_rec[w]] + win_start[w] + t, mapped by the inverse of transf[w] (eval_prox_egobody.py:177-182).
+ * covered [total_frames] (bytes) is 1 on those rows; every other row of both outputs is 0. */
+ROHM_API int rohm_window_to_world(rohm_ctx* ctx, const float* joints, const int* win_rec, const int* win_start,
+                                  const float* transf, int W, int clip_len, const int* rec_off, int64_t total_frames,
+                                  float* world, unsigned char* covered, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -16,6 +16,7 @@
 
 #include "body_internal.h"
 #include "kin.cuh"
+#include "repr.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -66,29 +67,6 @@ __global__ void compose_repr_kernel(const float* __restrict__ traj, int traj_dim
   if (k >= 0) out[i] = traj[r * traj_dim + k];
 }
 
-// scipy Rotation.from_rotvec(r).as_matrix() (rotvec -> unit quaternion -> matrix), fp32
-__device__ __forceinline__ M3 rotvec_to_mat(V3 r) {
-  const float a2 = dot(r, r);
-  const float a = sqrtf(a2);
-  float sc, qw;
-  if (a <= 1e-3f) {
-    sc = 0.5f - a2 / 48.0f + a2 * a2 / 3840.0f;
-    qw = cosf(0.5f * a);
-  } else {
-    float sn;
-    sincosf(0.5f * a, &sn, &qw);
-    sc = sn / a;
-  }
-  const float x = sc * r.x, y = sc * r.y, z = sc * r.z, w = qw;
-  const float x2 = x * x, y2 = y * y, z2 = z * z, w2 = w * w;
-  const float xy = x * y, zw = z * w, xz = x * z, yw = y * w, yz = y * z, xw = x * w;
-  M3 R;
-  R.c0 = {x2 - y2 - z2 + w2, 2.0f * (xy + zw), 2.0f * (xz - yw)};
-  R.c1 = {2.0f * (xy - zw), -x2 + y2 - z2 + w2, 2.0f * (yz + xw)};
-  R.c2 = {2.0f * (xz + yw), 2.0f * (yz - xw), -x2 - y2 + z2 + w2};
-  return R;
-}
-
 constexpr int kReprFramesPerCta = 1024;  // frames (threads) per CTA of traj_full_repr_kernel
 constexpr int kReprMaxCluster = 8;       // CTAs per clip: clips of up to 8192 frames
 
@@ -127,16 +105,8 @@ __global__ void traj_full_repr_kernel(const float* __restrict__ joints, const fl
   const float* P = joints + (row0() + (mine ? t : 0)) * kBodyJ * 3;
   auto J = [&](const float* base, int j) { return V3{base[j * 3], base[j * 3 + 1], base[j * 3 + 2]}; };
   if (mine) {
-    // forward direction from hips (2 = right, 1 = left) and shoulders (17 = right, 16 = left)
-    V3 across = (J(P, 1) - J(P, 2)) + (J(P, 17) - J(P, 16));
-    across = (1.0f / sqrtf(dot(across, across))) * across;
-    V3 fwd = {-across.y, across.x, 0.0f};  // cross((0,0,1), across)
-    fwd = (1.0f / sqrtf(dot(fwd, fwd))) * fwd;
-    // qbetween(fwd, (0,1,0)): v = fwd x target = (-f.z, 0, f.x), w = |f||t| + f.t
-    const float vx = -fwd.z, vz = fwd.x;
-    const float w = sqrtf(dot(fwd, fwd) * 1.0f) + fwd.y;
-    const float n = sqrtf(w * w + vx * vx + vz * vz);
-    const float q0 = w / n, q1 = vx / n, q3 = vz / n;
+    float q0, q1, q3;
+    repr::heading_quat(J(P, 1), J(P, 2), J(P, 17), J(P, 16), q0, q1, q3);
     qw[threadIdx.x] = q0, qz[threadIdx.x] = q3;
     if (isnan(q0) || isnan(q1) || isnan(q3)) atomicMin(peer(&first_nan, 0), t);
   }
@@ -159,41 +129,10 @@ __global__ void traj_full_repr_kernel(const float* __restrict__ joints, const fl
     // frame t + 1 is the next CTA's first when t is this CTA's last
     const int u = threadIdx.x + 1 < rows ? threadIdx.x + 1 : 0, ur = threadIdx.x + 1 < rows ? rank : rank + 1;
     const float w0 = qw[threadIdx.x], z0 = qz[threadIdx.x], w1 = peer(qw, ur)[u], z1 = peer(qz, ur)[u];
-    o[kChAngle] = atan2f(z0, w0);
-    // q[t+1] * conj(q[t]) for rotations about z
-    o[kChAngleVel] = atan2f(w0 * z1 - z0 * w1, w1 * w0 + z1 * z0);
-    const V3 r0 = J(P, 0), r1 = J(P1, 0);
-    o[kChRootPos] = r0.x, o[kChRootPos + 1] = r0.y;
-    {
-      // qrot(q[t+1], r1 - r0), qvec = (0, 0, z1)
-      const V3 v = r1 - r0;
-      const V3 qv = {0.0f, 0.0f, z1};
-      const V3 uv = cross(qv, v);
-      const V3 uuv = cross(qv, uv);
-      o[kChRootVel] = v.x + 2.0f * (w1 * uv.x + uuv.x);
-      o[kChRootVel + 1] = v.y + 2.0f * (w1 * uv.y + uuv.y);
-    }
-    o[kChHeight] = r0.z;
-    const M3 R0 = rotvec_to_mat({go[f * 3], go[f * 3 + 1], go[f * 3 + 2]});
-    const M3 R1 = rotvec_to_mat({go[(f + 1) * 3], go[(f + 1) * 3 + 1], go[(f + 1) * 3 + 2]});
-    // rot6d = R[:, :2] row-major
-    o[kChRot6d] = R0.c0.x, o[kChRot6d + 1] = R0.c1.x, o[kChRot6d + 2] = R0.c0.y, o[kChRot6d + 3] = R0.c1.y;
-    o[kChRot6d + 4] = R0.c0.z, o[kChRot6d + 5] = R0.c1.z;
-    {
-      // estimate_angular_velocity_np: w_mat = dR R^T; entries (i,j) = sum_k dR[i][k] R[j][k]
-      const M3 dR = {R1.c0 - R0.c0, R1.c1 - R0.c1, R1.c2 - R0.c2};
-      auto rowd = [&](int i) { return i == 0 ? V3{dR.c0.x, dR.c1.x, dR.c2.x} : (i == 1 ? V3{dR.c0.y, dR.c1.y, dR.c2.y} : V3{dR.c0.z, dR.c1.z, dR.c2.z}); };
-      auto rowr = [&](int i) { return i == 0 ? V3{R0.c0.x, R0.c1.x, R0.c2.x} : (i == 1 ? V3{R0.c0.y, R0.c1.y, R0.c2.y} : V3{R0.c0.z, R0.c1.z, R0.c2.z}); };
-      auto wm = [&](int i, int j) { return dot(rowd(i), rowr(j)); };
-      o[13] = (-wm(1, 2) + wm(2, 1)) / 2.0f;
-      o[14] = (wm(0, 2) - wm(2, 0)) / 2.0f;
-      o[15] = (-wm(0, 1) + wm(1, 0)) / 2.0f;
-    }
-    for (int k = 0; k < 3; ++k) {
-      const float a = transl[f * 3 + k], c = transl[(f + 1) * 3 + k];
-      o[kChTrans + k] = a;
-      o[19 + k] = c - a;
-    }
+    auto root = [&](int k) { return J(k == 0 ? P : P1, 0); };
+    auto rot = [&](int k) { return repr::rotvec_to_mat({go[(f + k) * 3], go[(f + k) * 3 + 1], go[(f + k) * 3 + 2]}); };
+    auto tr = [&](int k, int c) { return transl[(f + k) * 3 + c]; };
+    repr::traj_channels(o, w0, z0, w1, z1, root, rot, tr);
     float* dst = out + (static_cast<int64_t>(b) * (T - 1) + t) * kTrajFull;
 #pragma unroll
     for (int c = 0; c < kTrajFull; ++c) dst[c] = (o[c] - mean[c]) / stdv[c];

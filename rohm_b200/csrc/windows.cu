@@ -1,0 +1,251 @@
+// Sliding-window batching of whole recordings (SURVEY.md 8f, row N4): what the reference's data loaders do on the host,
+// one clip at a time, before the rounds, and the inverse of its canonical frame after them.
+//
+//   rohm_window_encode    dataloader_video.py:160-183 / dataloader_amass.py:105-131 (windows of clip_len frames, stride
+//                         clip_len - overlap), motion_representation.py:47-110 cano_seq_smplx + other_utils.py:189-240
+//                         update_globalRT_for_smplx (canonical frame and SMPL-X global R/T), motion_representation.py:187-282
+//                         get_repr_smplx + :23-44 foot_detect (the 294 channels), dataloader_amass.py:328-329 (z-score)
+//   rohm_window_to_world  eval_prox_egobody.py:177-182 (points_coord_trans with the inverse of transf_matrix), scattered
+//                         into the recordings' frames
+#include <cmath>
+#include <cstdint>
+#include <vector>
+
+#include "common.h"
+#include "kin.cuh"
+#include "repr.cuh"
+
+namespace rohm {
+namespace {
+
+using namespace kin;
+
+constexpr int kC = 294;
+constexpr int kJ = 22;
+constexpr int kBetas = 10;
+constexpr int kPoseJ = 21;
+constexpr int kMaxClip = 160;  // frames per window: one thread per frame in one CTA
+constexpr int kChLocalPos = 22, kChLocalVel = 88, kChBodyPose = 154, kChBetas = 280, kChContact = 290;
+constexpr float kFootVel = 5e-5f;  // get_repr_smplx feet_vel_thre: squared displacement per frame
+
+// One CTA per window, one thread per window frame.  (1) the floor height (min z over the window's clip_len x 22 joints),
+// the frame-0 root XY and the frame-0 heading from hips + shoulders give transf = [Rt | -Rt o]; (2) each thread
+// canonicalises its frame's joints into shared memory and takes their root heading quaternion; (3) the first NaN
+// heading is repaired and frame 0 pinned to the identity, as traj_full_repr_kernel does over a clip; (4) frame t < clip_len
+// - 1 writes row t: the 22 trajectory channels through repr::traj_channels with the canonical SMPL-X global R/T, then local
+// positions, local velocities, body-pose 6-D, betas and foot contacts, z-scored twice (TrajNet and PoseNet statistics).
+// Input rows are the packed recording frames rec_off[win_rec[w]] + win_start[w] + t; nothing outside a window is read.
+__global__ void __launch_bounds__(kMaxClip) window_encode_kernel(
+    const float* __restrict__ joints, const float* __restrict__ go, const float* __restrict__ transl,
+    const float* __restrict__ betas, const float* __restrict__ body_pose, const int* __restrict__ win_rec,
+    const int* __restrict__ win_start, const int* __restrict__ rec_off, int clip_len, const float* __restrict__ tmean,
+    const float* __restrict__ tstd, const float* __restrict__ pmean, const float* __restrict__ pstd,
+    float* __restrict__ transf, float* __restrict__ out_traj, float* __restrict__ out_pose) {
+  __shared__ float cj[kMaxClip * kJ * 3];  // canonical joints of the window's frames
+  __shared__ float qw[kMaxClip], qz[kMaxClip];
+  __shared__ float wmin[kMaxClip / 32];
+  __shared__ float frame[7];  // x axis (xy), y axis (xy), origin (x, y, floor)
+  __shared__ int first_nan;
+  const int w = blockIdx.x, t = threadIdx.x;
+  const bool mine = t < clip_len;
+  const int64_t f = static_cast<int64_t>(rec_off[win_rec[w]]) + win_start[w] + (mine ? t : 0);
+  const float* P = joints + f * kJ * 3;
+  auto J = [&](const float* base, int j) { return V3{base[j * 3], base[j * 3 + 1], base[j * 3 + 2]}; };
+
+  // (1) canonical frame
+  float m = INFINITY;
+  if (mine)
+    for (int j = 0; j < kJ; ++j) m = fminf(m, P[j * 3 + 2]);
+  for (int s = 16; s > 0; s >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, s));
+  if ((t & 31) == 0) wmin[t >> 5] = m;
+  if (t == 0) first_nan = clip_len;
+  __syncthreads();
+  if (t == 0) {
+    float fl = wmin[0];
+    for (int i = 1; i < static_cast<int>(blockDim.x) / 32; ++i) fl = fminf(fl, wmin[i]);
+    // cano_seq_smplx: x = (r_hip - l_hip) + (sdr_r - sdr_l) = (2 - 1) + (17 - 16) without its up component, y = z x x
+    V3 x = (J(P, 2) - J(P, 1)) + (J(P, 17) - J(P, 16));
+    x.z = 0.0f;
+    x = (1.0f / sqrtf(dot(x, x))) * x;
+    V3 y = {-x.y, x.x, 0.0f};
+    y = (1.0f / sqrtf(dot(y, y))) * y;
+    const float ox = P[0], oy = P[1];
+    frame[0] = x.x, frame[1] = x.y, frame[2] = y.x, frame[3] = y.y, frame[4] = ox, frame[5] = oy, frame[6] = fl;
+    float* M = transf + static_cast<int64_t>(w) * 16;
+    M[0] = x.x, M[1] = x.y, M[2] = 0.0f, M[3] = -(x.x * ox + x.y * oy);
+    M[4] = y.x, M[5] = y.y, M[6] = 0.0f, M[7] = -(y.x * ox + y.y * oy);
+    M[8] = 0.0f, M[9] = 0.0f, M[10] = 1.0f, M[11] = -fl;
+    M[12] = 0.0f, M[13] = 0.0f, M[14] = 0.0f, M[15] = 1.0f;
+  }
+  __syncthreads();
+  const float ax = frame[0], ay = frame[1], bx = frame[2], by = frame[3], ox = frame[4], oy = frame[5], fl = frame[6];
+  // Rt (p - o) for a world point, Rt v for a world direction
+  auto to_cano = [&](V3 p) {
+    const float dx = p.x - ox, dy = p.y - oy;
+    return V3{ax * dx + ay * dy, bx * dx + by * dy, p.z - fl};
+  };
+  auto rot_cano = [&](V3 v) { return V3{ax * v.x + ay * v.y, bx * v.x + by * v.y, v.z}; };
+
+  // (2) canonical joints and headings
+  float* C0 = cj + t * kJ * 3;
+  if (mine) {
+    for (int j = 0; j < kJ; ++j) {
+      const V3 c = to_cano(J(P, j));
+      C0[j * 3] = c.x, C0[j * 3 + 1] = c.y, C0[j * 3 + 2] = c.z;
+    }
+    float q0, q1, q3;
+    repr::heading_quat(J(C0, 1), J(C0, 2), J(C0, 17), J(C0, 16), q0, q1, q3);
+    qw[t] = q0, qz[t] = q3;
+    if (isnan(q0) || isnan(q1) || isnan(q3)) atomicMin(&first_nan, t);
+  }
+  __syncthreads();
+  // (3) the reference repairs the first NaN heading only, with its predecessor (the last frame for frame 0)
+  if (t == 0) {
+    if (first_nan < clip_len) {
+      const int dst = first_nan, src = first_nan > 0 ? first_nan - 1 : clip_len - 1;
+      qw[dst] = qw[src], qz[dst] = qz[src];
+    }
+    qw[0] = 1.0f, qz[0] = 0.0f;
+  }
+  __syncthreads();
+  if (t >= clip_len - 1) return;
+
+  // (4) row t
+  const float* C1 = C0 + kJ * 3;
+  const float w0 = qw[t], z0 = qz[t], w1 = qw[t + 1], z1 = qz[t + 1];
+  const int64_t row = static_cast<int64_t>(w) * (clip_len - 1) + t;
+  float* dt = out_traj + row * kC;
+  float* dp = out_pose + row * kC;
+  auto put = [&](int c, float v) {
+    dt[c] = (v - tmean[c]) / tstd[c];
+    dp[c] = (v - pmean[c]) / pstd[c];
+  };
+  float o[repr::kTrajFull];
+  {
+    auto root = [&](int k) { return J(k == 0 ? C0 : C1, 0); };
+    // update_globalRT_for_smplx: R' = Rt R; T' = Rt (T + delta_T - o) - delta_T with delta_T = pelvis - T, i.e. the
+    // canonical pelvis - pelvis + T
+    auto rot = [&](int k) {
+      const M3 R = repr::rotvec_to_mat({go[(f + k) * 3], go[(f + k) * 3 + 1], go[(f + k) * 3 + 2]});
+      return M3{rot_cano(R.c0), rot_cano(R.c1), rot_cano(R.c2)};
+    };
+    auto tr = [&](int k, int c) {
+      const float* Ck = k == 0 ? C0 : C1;
+      return Ck[c] - (P[k * kJ * 3 + c] - transl[(f + k) * 3 + c]);
+    };
+    repr::traj_channels(o, w0, z0, w1, z1, root, rot, tr);
+  }
+#pragma unroll
+  for (int c = 0; c < repr::kTrajFull; ++c) put(c, o[c]);
+  const V3 r0 = J(C0, 0);
+  for (int j = 0; j < kJ; ++j) {
+    const V3 c0 = J(C0, j), c1 = J(C1, j);
+    const V3 lp = repr::qrot_z(w0, z0, {c0.x - r0.x, c0.y - r0.y, c0.z});
+    const V3 lv = repr::qrot_z(w0, z0, c1 - c0);
+    put(kChLocalPos + j * 3, lp.x), put(kChLocalPos + j * 3 + 1, lp.y), put(kChLocalPos + j * 3 + 2, lp.z);
+    put(kChLocalVel + j * 3, lv.x), put(kChLocalVel + j * 3 + 1, lv.y), put(kChLocalVel + j * 3 + 2, lv.z);
+  }
+  for (int k = 0; k < kPoseJ; ++k) {
+    const float* a = body_pose + f * kPoseJ * 3 + k * 3;
+    const M3 R = repr::rotvec_to_mat({a[0], a[1], a[2]});
+    const int c = kChBodyPose + k * 6;
+    put(c, R.c0.x), put(c + 1, R.c1.x), put(c + 2, R.c0.y), put(c + 3, R.c1.y), put(c + 4, R.c0.z), put(c + 5, R.c1.z);
+  }
+  for (int l = 0; l < kBetas; ++l) put(kChBetas + l, betas[f * kBetas + l]);
+  // foot_detect (up axis z): left feet 7, 10 then right feet 8, 11; height factors 0.18 (ankles), 0.15 (toes)
+  for (int s = 0; s < 4; ++s) {
+    const int j = (s & 1 ? 10 : 7) + (s >> 1);
+    const float thr = s & 1 ? 0.15f : 0.18f;
+    const V3 d = J(C1, j) - J(C0, j);
+    const bool contact = d.x * d.x + d.y * d.y + d.z * d.z < kFootVel && C0[j * 3 + 2] < thr;
+    put(kChContact + s, contact ? 1.0f : 0.0f);
+  }
+}
+
+// One thread per (window, pose frame, joint): p = R^T (c - t) for transf = [R | t], written to recording frame
+// rec_off[win_rec[w]] + win_start[w] + pose frame, which is marked covered.
+__global__ void window_to_world_kernel(const float* __restrict__ joints, const int* __restrict__ win_rec,
+                                       const int* __restrict__ win_start, const int* __restrict__ rec_off,
+                                       const float* __restrict__ transf, int W, int pose_frames, float* __restrict__ world,
+                                       unsigned char* __restrict__ covered) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<int64_t>(W) * pose_frames * kJ) return;
+  const int j = static_cast<int>(i % kJ);
+  const int64_t r = i / kJ;
+  const int w = static_cast<int>(r / pose_frames), t = static_cast<int>(r % pose_frames);
+  const float* M = transf + static_cast<int64_t>(w) * 16;
+  const float* c = joints + i * 3;
+  const V3 d = {c[0] - M[3], c[1] - M[7], c[2] - M[11]};
+  const int64_t fr = static_cast<int64_t>(rec_off[win_rec[w]]) + win_start[w] + t;
+  float* o = world + (fr * kJ + j) * 3;
+  o[0] = M[0] * d.x + M[4] * d.y + M[8] * d.z;
+  o[1] = M[1] * d.x + M[5] * d.y + M[9] * d.z;
+  o[2] = M[2] * d.x + M[6] * d.y + M[10] * d.z;
+  if (j == 0) covered[fr] = 1;
+}
+
+}  // namespace
+}  // namespace rohm
+
+using namespace rohm;
+
+extern "C" int rohm_window_encode(rohm_ctx* ctx, const float* global_orient, const float* transl, const float* betas,
+                                  const float* body_pose, const float* joints, const int* rec_off_host,
+                                  const int* rec_off, int R, int clip_len,
+                                  int overlap, const float* traj_mean, const float* traj_std, const float* pose_mean,
+                                  const float* pose_std, int max_windows, int* n_windows, int* win_rec, int* win_start,
+                                  float* transf, float* repr_traj, float* repr_pose, void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (!global_orient || !transl || !betas || !body_pose || !joints || !rec_off || !traj_mean || !traj_std || !pose_mean ||
+      !pose_std || !rec_off_host || !n_windows || !win_rec || !win_start || !transf || !repr_traj || !repr_pose || R <= 0 || max_windows < 0)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_window_encode: bad arguments");
+  if (clip_len < 3 || clip_len > kMaxClip || overlap < 0 || overlap > 2)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_window_encode: clip_len=%d overlap=%d; windows of 3 to %d frames with an "
+                "overlap of 0 to 2 frames (so that no recording frame lies in two windows' pose frames)", clip_len, overlap,
+                kMaxClip);
+  // the reference loop: window k of a recording starts at k * (clip_len - overlap) and is cut while it ends inside the
+  // recording; a recording shorter than clip_len gives none
+  const int stride = clip_len - overlap;
+  std::vector<int> tab_rec, tab_start;
+  for (int r = 0; r < R; ++r) {
+    const int n = rec_off_host[r + 1] - rec_off_host[r];
+    if (rec_off_host[r] < 0 || n < 0)
+      return fail(ctx, ROHM_ERR_INVALID, "rohm_window_encode: recording offsets must be non-negative and non-decreasing "
+                  "(rec_off[%d] = %d, rec_off[%d] = %d)", r, rec_off_host[r], r + 1, rec_off_host[r + 1]);
+    for (int s = 0; s + clip_len <= n; s += stride) tab_rec.push_back(r), tab_start.push_back(s);
+  }
+  const int W = static_cast<int>(tab_rec.size());
+  *n_windows = W;
+  if (W > max_windows)
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_window_encode: %d windows exceed the %d the outputs hold", W, max_windows);
+  if (W == 0) return ROHM_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ROHM_CUDA(ctx, cudaMemcpyAsync(win_rec, tab_rec.data(), sizeof(int) * W, cudaMemcpyHostToDevice, st));
+  ROHM_CUDA(ctx, cudaMemcpyAsync(win_start, tab_start.data(), sizeof(int) * W, cudaMemcpyHostToDevice, st));
+  window_encode_kernel<<<W, (clip_len + 31) / 32 * 32, 0, st>>>(joints, global_orient, transl, betas, body_pose, win_rec,
+                                                                win_start, rec_off, clip_len, traj_mean, traj_std, pose_mean,
+                                                                pose_std, transf, repr_traj, repr_pose);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return ROHM_OK;
+}
+
+extern "C" int rohm_window_to_world(rohm_ctx* ctx, const float* joints, const int* win_rec, const int* win_start,
+                                    const float* transf, int W, int clip_len, const int* rec_off, int64_t total_frames,
+                                    float* world, unsigned char* covered, void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (!world || !covered || !rec_off || W < 0 || clip_len < 3 || clip_len > kMaxClip || total_frames < 0 ||
+      (W > 0 && (!joints || !win_rec || !win_start || !transf)))
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_window_to_world: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (total_frames == 0) return ROHM_OK;
+  ROHM_CUDA(ctx, cudaMemsetAsync(world, 0, sizeof(float) * total_frames * kJ * 3, st));
+  ROHM_CUDA(ctx, cudaMemsetAsync(covered, 0, static_cast<size_t>(total_frames), st));
+  const int64_t n = static_cast<int64_t>(W) * (clip_len - 2) * kJ;
+  if (n == 0) return ROHM_OK;
+  window_to_world_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(joints, win_rec, win_start, rec_off, transf,
+                                                                                W, clip_len - 2, world, covered);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return ROHM_OK;
+}

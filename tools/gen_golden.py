@@ -21,6 +21,7 @@ sys.path.append('/root/reference')  # AFTER the repo: only used for the referenc
 import numpy as np
 import torch
 import torch.nn as nn
+from scipy.spatial.transform import Rotation as ref_rotation
 
 from oracle import kinematics_oracle as ko
 from rohm_b200 import synthetic
@@ -534,12 +535,124 @@ class _VertsBody(nn.Module):
         return o
 
 
+# Short windows keep the fixture small; the per-window computation is the same at every clip_len.
+WINDOW_CLIP = 24
+WINDOW_LENGTHS = (47, 24, 16)
+# (overlap, recordings) of each case: the video loaders' overlap 2 over all three (two windows of the first), the AMASS
+# loader's 0 over the first (one window)
+WINDOW_CASES = ((2, (0, 1, 2)), (0, (0,)))
+# frames whose hips and shoulders coincide: no heading, so the reference repairs their root quaternion (one per window)
+WINDOW_NAN_FRAMES = {0: (10, 35), 1: (23,)}
+
+
+def window_recordings(seed=81):
+    """Synthetic recordings for the window encoder: SMPL-X parameters, and FK joints of the synthetic body whose hips,
+    shoulders and feet are then placed by hand so that every sign and threshold the encoder decides has a margin:
+
+    * the body's heading phi(t) sets hips (1, 2) and shoulders (16, 17) around the pelvis; recording 0 starts facing
+      -y (phi(0) near 180 deg) and turns by up to pi - 0.04 within a window without crossing pi, recording 1 faces near
+      -180 deg;
+    * the feet (7, 8, 10, 11) cycle through heights 0, 0.10, 0.165, 0.30 above a floor below every other joint, in
+      segments of 4 frames, at per-frame steps of 0.003, 0.005, 0.009, 0.02: squared speeds and heights at least 38 %
+      and 0.015 away from foot_detect's thresholds (5e-5; 0.18, 0.15), and the floor is a foot at height 0 in every window.
+    """
+    g = np.random.default_rng(seed)
+    model = synthetic.smplx_like_model(0)
+    params, joints = {k: [] for k in ("global_orient", "transl", "betas", "body_pose")}, []
+    for r, n in enumerate(WINDOW_LENGTHS):
+        t = np.arange(n, dtype=np.float64)
+        if r == 0:
+            phi = np.pi - 0.02 + 3.10 * (1 - np.cos(2 * np.pi * t / 44)) / 2
+        elif r == 1:
+            phi = -np.pi + 0.02 + 0.3 * np.sin(2 * np.pi * t / 19)
+        else:
+            phi = 0.5 * t / n
+        tilt = 0.05 * np.sin(t / 13.0)
+        rz = np.stack([np.zeros(n), np.zeros(n), phi], -1)
+        rx = np.stack([tilt, np.zeros(n), np.zeros(n)], -1)
+        go = (ref_rotation.from_rotvec(rz) * ref_rotation.from_rotvec(rx)).as_rotvec()
+        transl = np.stack([0.8 * np.sin(t / 40.0) + r, 0.02 * t - r, 0.9 + 0.02 * np.sin(t / 7.0)], -1)
+        betas = np.repeat(0.5 * g.standard_normal((1, 10)), n, axis=0)
+        body_pose = 0.2 * g.standard_normal((n, 63))
+        f = lambda a: torch.from_numpy(np.asarray(a, np.float32))
+        j, _ = ko.smplx_forward(model, f(go), f(body_pose), f(betas), f(transl), return_verts=False)
+        j = j[:, 0:22].numpy().astype(np.float64)
+        right = np.stack([np.cos(phi), np.sin(phi), np.zeros(n)], -1)
+        up = np.array([0.0, 0.0, 1.0])
+        p0 = j[:, 0]
+        j[:, 2], j[:, 1] = p0 + 0.10 * right - 0.05 * up, p0 - 0.10 * right - 0.05 * up
+        j[:, 17], j[:, 16] = p0 + 0.18 * right + 0.45 * up, p0 - 0.18 * right + 0.45 * up
+        for fr in WINDOW_NAN_FRAMES.get(r, ()):
+            j[fr, 1], j[fr, 16] = j[fr, 2], j[fr, 17]
+        floor = np.delete(j, [7, 8, 10, 11], axis=1)[..., 2].min() - 0.05
+        levels, steps = (0.0, 0.10, 0.165, 0.30), (0.003, 0.005, 0.009, 0.02)
+        for k, jj in enumerate((7, 10, 8, 11)):
+            seg = (t.astype(int) // 4) + 2 * k
+            z = floor + np.array(levels)[seg % 4]
+            step = np.array(steps)[(seg // 4 + k) % 4]
+            ang = 0.37 * t + k
+            d = np.stack([step * np.cos(ang), step * np.sin(ang)], -1)  # frame t -> t + 1 moves by step[t]
+            xy = p0[0:1, 0:2] + 0.1 * k + np.concatenate([np.zeros((1, 2)), np.cumsum(d, axis=0)[:-1]], axis=0)
+            j[:, jj] = np.concatenate([xy, z[:, None]], -1)
+        for k, v in (("global_orient", go), ("transl", transl), ("betas", betas), ("body_pose", body_pose)):
+            params[k].append(np.asarray(v, np.float32))
+        joints.append(j.astype(np.float32))
+    return {k: np.concatenate(v) for k, v in params.items()}, np.concatenate(joints)
+
+
+def gen_windows(ref):
+    """The reference's loaders cut, canonicalise and encode each window of the synthetic recordings above
+    (cano_seq_smplx -> get_repr_smplx, dataloader_amass.py:152-211); points_coord_trans with the inverse transf_matrix
+    takes each window's canonical pose frames back to the world (eval_prox_egobody.py:177-182)."""
+    params, joints = window_recordings()
+    off = np.concatenate([[0], np.cumsum(WINDOW_LENGTHS)])
+    out = {"lengths": np.array(WINDOW_LENGTHS, np.int64), "clip_len": np.array(WINDOW_CLIP), "joints": joints}
+    out.update({f"param_{k}": v for k, v in params.items()})
+    for c, (overlap, recs) in enumerate(WINDOW_CASES):
+        table, tfs, reps, worlds = [], [], [], []
+        for r in recs:
+            n, k = WINDOW_LENGTHS[r], 0
+            while k * (WINDOW_CLIP - overlap) + WINDOW_CLIP <= n:  # dataloader_video.py:167-172
+                s = k * (WINDOW_CLIP - overlap)
+                rows = slice(off[r] + s, off[r] + s + WINDOW_CLIP)
+                p = {key: v[rows].copy() for key, v in params.items()}
+                cano, cano_p, tf = ref.mr.cano_seq_smplx(positions=joints[rows].copy(), smplx_params_dict=p,
+                                                         return_transf_mat=True)
+                d = ref.mr.get_repr_smplx(positions=cano, smplx_params_dict=cano_p, feet_vel_thre=5e-5)
+                rep = np.concatenate([d[key] for key in ko.REPR_LIST], axis=-1)
+                assert np.isfinite(rep).all(), (r, s)
+                # margins of the decisions an fp32 encoder has to reproduce
+                for pair, hf in ((ref.mr.fid_l, (0.18, 0.15)), (ref.mr.fid_r, (0.18, 0.15))):
+                    v2 = ((cano[1:, pair] - cano[:-1, pair]) ** 2).sum(-1)
+                    assert np.abs(v2 / 5e-5 - 1).min() > 0.3, (r, s)
+                    assert np.abs(cano[:-1, pair, 2] - np.array(hf)).min() > 0.01, (r, s)
+                ang = rep[:, 0]
+                assert np.abs(np.abs(ang) - np.pi / 2).min() > 5e-3, (r, s, np.abs(np.abs(ang) - np.pi / 2).min())
+                assert np.abs(np.abs(rep[:, 1]) - np.pi).min() > 1.0, (r, s)
+                table.append((r, s))
+                tfs.append(tf)
+                reps.append(rep.astype(np.float32))
+                worlds.append(np.stack([ref.ou.points_coord_trans(cano[t], np.linalg.inv(tf)) for t in range(WINDOW_CLIP - 2)]))
+                k += 1
+        out[f"c{c}_meta"] = np.array([overlap] + list(recs), np.int64)
+        out[f"c{c}_table"] = np.array(table, np.int64).reshape(-1, 2)
+        out[f"c{c}_transf"] = np.asarray(tfs, np.float64)
+        out[f"c{c}_repr"] = np.asarray(reps)
+        out[f"c{c}_world"] = np.asarray(worlds).astype(np.float32)
+        print(f"windows case {c}: overlap {overlap}, {len(table)} windows, |heading| up to "
+              f"{float(np.abs(np.asarray(reps)[..., 0]).max()):.4f}, contacts {float(np.asarray(reps)[..., -4:].mean()):.2f}")
+    out["n_cases"] = np.array(len(WINDOW_CASES))
+    np.savez_compressed(os.path.join(OUT, "windows.npz"), **out)
+    print("windows.npz")
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     ref = import_reference()
     which = sys.argv[1:] or ["schedules", "posenet", "trajnet", "sampling", "kinematics", "glue", "pipeline",
-                             "clip_guidance"]
+                             "clip_guidance", "windows"]
     for w in which:
         {"schedules": gen_schedules, "posenet": gen_posenet, "trajnet": gen_trajnet, "sampling": gen_sampling,
-         "kinematics": gen_kinematics, "glue": gen_glue, "pipeline": gen_pipeline, "clip_guidance": gen_clip_guidance}[w](ref)
+         "kinematics": gen_kinematics, "glue": gen_glue, "pipeline": gen_pipeline, "clip_guidance": gen_clip_guidance,
+         "windows": gen_windows}[w](ref)
