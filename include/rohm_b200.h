@@ -434,6 +434,28 @@ ROHM_API int rohm_window_encode(rohm_ctx* ctx, const float* global_orient, const
                                 int* win_rec, int* win_start, float* transf, float* repr_traj, float* repr_pose,
                                 void* stream);
 
+/* Input noise on the windows' canonical SMPL-X parameters (dataloader_amass.py:156-192, input_noise with sep_noise False).
+ * global_orient .. joints, rec_off (device int[R+1]), win_rec / win_start and transf [W,4,4] are the inputs and outputs of
+ * the rohm_window_encode call that cut these W windows of clip_len frames.  Noise, window-major like the reference's
+ * preset-noise pickle: noise_transl [W,clip_len,3] (metres), noise_betas [W,clip_len,10], noise_global_orient
+ * [W,clip_len,3] and noise_body_pose [W,clip_len,21,3] (degrees, added to scipy's extrinsic 'zxy' Euler angles of each
+ * canonical rotation; the round trip rotvec -> angles -> + n -> rotvec runs in float64 and follows scipy's gimbal-lock
+ * rule).  Output noisy_params [W*clip_len, 79]: rows of global_orient 3 | transl 3 | betas 10 | body_pose 63, float32
+ * axis-angle, window-major (row w * clip_len + t). */
+ROHM_API int rohm_window_param_noise(rohm_ctx* ctx, const float* global_orient, const float* transl, const float* betas,
+                                     const float* body_pose, const float* joints, const int* rec_off, const int* win_rec,
+                                     const int* win_start, const float* transf, int W, int clip_len,
+                                     const float* noise_transl, const float* noise_betas, const float* noise_global_orient,
+                                     const float* noise_body_pose, float* noisy_params, void* stream);
+
+/* rohm_window_encode on windows that are already canonical (the noisy windows, which the reference does not
+ * re-canonicalise): params [W*clip_len, 79] as rohm_window_param_noise writes them and joints [W*clip_len,22,3], both
+ * window-major -> repr_traj / repr_pose [W, clip_len-1, 294], get_repr_smplx of each window z-scored with traj_mean /
+ * traj_std and pose_mean / pose_std, computed by the same row code as rohm_window_encode. */
+ROHM_API int rohm_window_encode_canonical(rohm_ctx* ctx, const float* params, const float* joints, int W, int clip_len,
+                                          const float* traj_mean, const float* traj_std, const float* pose_mean,
+                                          const float* pose_std, float* repr_traj, float* repr_pose, void* stream);
+
 /* The inverse: joints [W*(clip_len-2),22,3] (each window's clip_len-2 pose frames in its canonical frame, as
  * reconstruct_outputs returns them) -> world [total_frames,22,3] packed by recording (rec_off, device int[R+1]), pose frame t
  * of window w at row rec_off[win_rec[w]] + win_start[w] + t, mapped by the inverse of transf[w] (eval_prox_egobody.py:177-182).

@@ -90,6 +90,8 @@ SIGNATURES = {
     "rohm_joints_from_traj": (_i, [_p, _p, _i, _p, _p, _i, _i, _p, _p, _i64, _i, _p, _p]),
     "rohm_window_encode": (_i, [_p, _p, _p, _p, _p, _p, C.POINTER(_i), _p, _i, _i, _i, _p, _p, _p, _p, _i,
                                 C.POINTER(_i), _p, _p, _p, _p, _p, _p]),
+    "rohm_window_param_noise": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p]),
+    "rohm_window_encode_canonical": (_i, [_p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p, _p]),
     "rohm_window_to_world": (_i, [_p, _p, _p, _p, _p, _i, _i, _p, _i64, _p, _p, _p]),
 }
 

@@ -7,6 +7,11 @@
 //                         get_repr_smplx + :23-44 foot_detect (the 294 channels), dataloader_amass.py:328-329 (z-score)
 //   rohm_window_to_world  eval_prox_egobody.py:177-182 (points_coord_trans with the inverse of transf_matrix), scattered
 //                         into the recordings' frames
+//   rohm_window_param_noise       dataloader_amass.py:156-192 (input noise on the canonical SMPL-X parameters, sep_noise
+//                                 False): transl and betas + n, rotations through scipy's 'zxy' Euler angles + n (degrees)
+//   rohm_window_encode_canonical  dataloader_amass.py:212-215 (get_repr_smplx of the noisy canonical window, not
+//                                 re-canonicalised) and :328-329 (z-score)
+#include <cfloat>
 #include <cmath>
 #include <cstdint>
 #include <vector>
@@ -27,6 +32,30 @@ constexpr int kPoseJ = 21;
 constexpr int kMaxClip = 160;  // frames per window: one thread per frame in one CTA
 constexpr int kChLocalPos = 22, kChLocalVel = 88, kChBodyPose = 154, kChBetas = 280, kChContact = 290;
 constexpr float kFootVel = 5e-5f;  // get_repr_smplx feet_vel_thre: squared displacement per frame
+// a noisy canonical parameter row: global_orient 3 | transl 3 | betas 10 | body_pose 63 (axis-angle)
+constexpr int kRowGo = 0, kRowTransl = 3, kRowBetas = 6, kRowPose = 16, kRow = 79;
+
+// A window's canonical frame, cano_seq_smplx: the canonical x and y axes in world coordinates (a, b), the frame-0 root XY
+// (ox, oy) and the floor height fl.
+struct CanoFrame {
+  float ax, ay, bx, by, ox, oy, fl;
+  // Rt (p - o) for a world point, Rt v for a world direction
+  __device__ __forceinline__ V3 to_cano(V3 p) const {
+    const float dx = p.x - ox, dy = p.y - oy;
+    return V3{ax * dx + ay * dy, bx * dx + by * dy, p.z - fl};
+  }
+  __device__ __forceinline__ V3 rot_cano(V3 v) const { return V3{ax * v.x + ay * v.y, bx * v.x + by * v.y, v.z}; }
+};
+
+// update_globalRT_for_smplx: R' = Rt R; T' = Rt (T + delta_T - o) - delta_T with delta_T = pelvis - T, i.e. component c of
+// the canonical pelvis - pelvis + T.  The encoder and the input noise both take the canonical R/T from here.
+__device__ __forceinline__ M3 cano_global_rot(const CanoFrame& F, const float* go) {
+  const M3 R = repr::rotvec_to_mat({go[0], go[1], go[2]});
+  return M3{F.rot_cano(R.c0), F.rot_cano(R.c1), F.rot_cano(R.c2)};
+}
+__device__ __forceinline__ float cano_transl(float cano_pelvis, float pelvis, float transl) {
+  return cano_pelvis - (pelvis - transl);
+}
 
 // One CTA per window, one thread per window frame.  (1) the floor height (min z over the window's clip_len x 22 joints),
 // the frame-0 root XY and the frame-0 heading from hips + shoulders give transf = [Rt | -Rt o]; (2) each thread
@@ -35,12 +64,19 @@ constexpr float kFootVel = 5e-5f;  // get_repr_smplx feet_vel_thre: squared disp
 // - 1 writes row t: the 22 trajectory channels through repr::traj_channels with the canonical SMPL-X global R/T, then local
 // positions, local velocities, body-pose 6-D, betas and foot contacts, z-scored twice (TrajNet and PoseNet statistics).
 // Input rows are the packed recording frames rec_off[win_rec[w]] + win_start[w] + t; nothing outside a window is read.
+//
+// kCanonical: the window's frames are already canonical (the noisy windows, which the reference does not re-canonicalise):
+// joints are window-major rows w * clip_len + t, the parameters are kRow-wide rows of that layout (go, transl, betas and
+// body_pose point into one row array), (1) is skipped, nothing is written to transf, and the SMPL-X R/T are used as given.
+template <bool kCanonical>
 __global__ void __launch_bounds__(kMaxClip) window_encode_kernel(
     const float* __restrict__ joints, const float* __restrict__ go, const float* __restrict__ transl,
     const float* __restrict__ betas, const float* __restrict__ body_pose, const int* __restrict__ win_rec,
     const int* __restrict__ win_start, const int* __restrict__ rec_off, int clip_len, const float* __restrict__ tmean,
     const float* __restrict__ tstd, const float* __restrict__ pmean, const float* __restrict__ pstd,
     float* __restrict__ transf, float* __restrict__ out_traj, float* __restrict__ out_pose) {
+  constexpr int kGoS = kCanonical ? kRow : 3, kTrS = kCanonical ? kRow : 3, kBeS = kCanonical ? kRow : kBetas,
+                kBpS = kCanonical ? kRow : kPoseJ * 3;
   __shared__ float cj[kMaxClip * kJ * 3];  // canonical joints of the window's frames
   __shared__ float qw[kMaxClip], qz[kMaxClip];
   __shared__ float wmin[kMaxClip / 32];
@@ -48,51 +84,55 @@ __global__ void __launch_bounds__(kMaxClip) window_encode_kernel(
   __shared__ int first_nan;
   const int w = blockIdx.x, t = threadIdx.x;
   const bool mine = t < clip_len;
-  const int64_t f = static_cast<int64_t>(rec_off[win_rec[w]]) + win_start[w] + (mine ? t : 0);
+  const int64_t f = kCanonical ? static_cast<int64_t>(w) * clip_len + (mine ? t : 0)
+                               : static_cast<int64_t>(rec_off[win_rec[w]]) + win_start[w] + (mine ? t : 0);
   const float* P = joints + f * kJ * 3;
   auto J = [&](const float* base, int j) { return V3{base[j * 3], base[j * 3 + 1], base[j * 3 + 2]}; };
+  CanoFrame F;
 
-  // (1) canonical frame
-  float m = INFINITY;
-  if (mine)
-    for (int j = 0; j < kJ; ++j) m = fminf(m, P[j * 3 + 2]);
-  for (int s = 16; s > 0; s >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, s));
-  if ((t & 31) == 0) wmin[t >> 5] = m;
-  if (t == 0) first_nan = clip_len;
-  __syncthreads();
-  if (t == 0) {
-    float fl = wmin[0];
-    for (int i = 1; i < static_cast<int>(blockDim.x) / 32; ++i) fl = fminf(fl, wmin[i]);
-    // cano_seq_smplx: x = (r_hip - l_hip) + (sdr_r - sdr_l) = (2 - 1) + (17 - 16) without its up component, y = z x x
-    V3 x = (J(P, 2) - J(P, 1)) + (J(P, 17) - J(P, 16));
-    x.z = 0.0f;
-    x = (1.0f / sqrtf(dot(x, x))) * x;
-    V3 y = {-x.y, x.x, 0.0f};
-    y = (1.0f / sqrtf(dot(y, y))) * y;
-    const float ox = P[0], oy = P[1];
-    frame[0] = x.x, frame[1] = x.y, frame[2] = y.x, frame[3] = y.y, frame[4] = ox, frame[5] = oy, frame[6] = fl;
-    float* M = transf + static_cast<int64_t>(w) * 16;
-    M[0] = x.x, M[1] = x.y, M[2] = 0.0f, M[3] = -(x.x * ox + x.y * oy);
-    M[4] = y.x, M[5] = y.y, M[6] = 0.0f, M[7] = -(y.x * ox + y.y * oy);
-    M[8] = 0.0f, M[9] = 0.0f, M[10] = 1.0f, M[11] = -fl;
-    M[12] = 0.0f, M[13] = 0.0f, M[14] = 0.0f, M[15] = 1.0f;
+  if constexpr (kCanonical) {
+    if (t == 0) first_nan = clip_len;
+    __syncthreads();
+    if (mine)
+      for (int j = 0; j < kJ * 3; ++j) cj[t * kJ * 3 + j] = P[j];
+  } else {
+    // (1) canonical frame
+    float m = INFINITY;
+    if (mine)
+      for (int j = 0; j < kJ; ++j) m = fminf(m, P[j * 3 + 2]);
+    for (int s = 16; s > 0; s >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, s));
+    if ((t & 31) == 0) wmin[t >> 5] = m;
+    if (t == 0) first_nan = clip_len;
+    __syncthreads();
+    if (t == 0) {
+      float fl = wmin[0];
+      for (int i = 1; i < static_cast<int>(blockDim.x) / 32; ++i) fl = fminf(fl, wmin[i]);
+      // cano_seq_smplx: x = (r_hip - l_hip) + (sdr_r - sdr_l) = (2 - 1) + (17 - 16) without its up component, y = z x x
+      V3 x = (J(P, 2) - J(P, 1)) + (J(P, 17) - J(P, 16));
+      x.z = 0.0f;
+      x = (1.0f / sqrtf(dot(x, x))) * x;
+      V3 y = {-x.y, x.x, 0.0f};
+      y = (1.0f / sqrtf(dot(y, y))) * y;
+      const float ox = P[0], oy = P[1];
+      frame[0] = x.x, frame[1] = x.y, frame[2] = y.x, frame[3] = y.y, frame[4] = ox, frame[5] = oy, frame[6] = fl;
+      float* M = transf + static_cast<int64_t>(w) * 16;
+      M[0] = x.x, M[1] = x.y, M[2] = 0.0f, M[3] = -(x.x * ox + x.y * oy);
+      M[4] = y.x, M[5] = y.y, M[6] = 0.0f, M[7] = -(y.x * ox + y.y * oy);
+      M[8] = 0.0f, M[9] = 0.0f, M[10] = 1.0f, M[11] = -fl;
+      M[12] = 0.0f, M[13] = 0.0f, M[14] = 0.0f, M[15] = 1.0f;
+    }
+    __syncthreads();
+    F = CanoFrame{frame[0], frame[1], frame[2], frame[3], frame[4], frame[5], frame[6]};
   }
-  __syncthreads();
-  const float ax = frame[0], ay = frame[1], bx = frame[2], by = frame[3], ox = frame[4], oy = frame[5], fl = frame[6];
-  // Rt (p - o) for a world point, Rt v for a world direction
-  auto to_cano = [&](V3 p) {
-    const float dx = p.x - ox, dy = p.y - oy;
-    return V3{ax * dx + ay * dy, bx * dx + by * dy, p.z - fl};
-  };
-  auto rot_cano = [&](V3 v) { return V3{ax * v.x + ay * v.y, bx * v.x + by * v.y, v.z}; };
 
   // (2) canonical joints and headings
   float* C0 = cj + t * kJ * 3;
   if (mine) {
-    for (int j = 0; j < kJ; ++j) {
-      const V3 c = to_cano(J(P, j));
-      C0[j * 3] = c.x, C0[j * 3 + 1] = c.y, C0[j * 3 + 2] = c.z;
-    }
+    if constexpr (!kCanonical)
+      for (int j = 0; j < kJ; ++j) {
+        const V3 c = F.to_cano(J(P, j));
+        C0[j * 3] = c.x, C0[j * 3 + 1] = c.y, C0[j * 3 + 2] = c.z;
+      }
     float q0, q1, q3;
     repr::heading_quat(J(C0, 1), J(C0, 2), J(C0, 17), J(C0, 16), q0, q1, q3);
     qw[t] = q0, qz[t] = q3;
@@ -123,15 +163,20 @@ __global__ void __launch_bounds__(kMaxClip) window_encode_kernel(
   float o[repr::kTrajFull];
   {
     auto root = [&](int k) { return J(k == 0 ? C0 : C1, 0); };
-    // update_globalRT_for_smplx: R' = Rt R; T' = Rt (T + delta_T - o) - delta_T with delta_T = pelvis - T, i.e. the
-    // canonical pelvis - pelvis + T
     auto rot = [&](int k) {
-      const M3 R = repr::rotvec_to_mat({go[(f + k) * 3], go[(f + k) * 3 + 1], go[(f + k) * 3 + 2]});
-      return M3{rot_cano(R.c0), rot_cano(R.c1), rot_cano(R.c2)};
+      if constexpr (kCanonical) {
+        const float* a = go + (f + k) * kGoS;
+        return repr::rotvec_to_mat({a[0], a[1], a[2]});
+      } else {
+        return cano_global_rot(F, go + (f + k) * 3);
+      }
     };
     auto tr = [&](int k, int c) {
-      const float* Ck = k == 0 ? C0 : C1;
-      return Ck[c] - (P[k * kJ * 3 + c] - transl[(f + k) * 3 + c]);
+      if constexpr (kCanonical) {
+        return transl[(f + k) * kTrS + c];
+      } else {
+        return cano_transl((k == 0 ? C0 : C1)[c], P[k * kJ * 3 + c], transl[(f + k) * 3 + c]);
+      }
     };
     repr::traj_channels(o, w0, z0, w1, z1, root, rot, tr);
   }
@@ -146,12 +191,12 @@ __global__ void __launch_bounds__(kMaxClip) window_encode_kernel(
     put(kChLocalVel + j * 3, lv.x), put(kChLocalVel + j * 3 + 1, lv.y), put(kChLocalVel + j * 3 + 2, lv.z);
   }
   for (int k = 0; k < kPoseJ; ++k) {
-    const float* a = body_pose + f * kPoseJ * 3 + k * 3;
+    const float* a = body_pose + f * kBpS + k * 3;
     const M3 R = repr::rotvec_to_mat({a[0], a[1], a[2]});
     const int c = kChBodyPose + k * 6;
     put(c, R.c0.x), put(c + 1, R.c1.x), put(c + 2, R.c0.y), put(c + 3, R.c1.y), put(c + 4, R.c0.z), put(c + 5, R.c1.z);
   }
-  for (int l = 0; l < kBetas; ++l) put(kChBetas + l, betas[f * kBetas + l]);
+  for (int l = 0; l < kBetas; ++l) put(kChBetas + l, betas[f * kBeS + l]);
   // foot_detect (up axis z): left feet 7, 10 then right feet 8, 11; height factors 0.18 (ankles), 0.15 (toes)
   for (int s = 0; s < 4; ++s) {
     const int j = (s & 1 ? 10 : 7) + (s >> 1);
@@ -160,6 +205,145 @@ __global__ void __launch_bounds__(kMaxClip) window_encode_kernel(
     const bool contact = d.x * d.x + d.y * d.y + d.z * d.z < kFootVel && C0[j * 3 + 2] < thr;
     put(kChContact + s, contact ? 1.0f : 0.0f);
   }
+}
+
+// ---- scipy.spatial.transform.Rotation in float64, as the noise needs it (scipy 1.18.1, _rotation_xp.py) ----
+// Quaternions are scalar-last (x, y, z, w) like scipy's.
+struct Q4 {
+  double x, y, z, w;
+};
+
+// from_rotvec: angle = |r|; scale = 0.5 - angle^2/48 + angle^4/3840 for angle <= 1e-3, sin(angle/2)/angle otherwise
+__device__ __forceinline__ Q4 quat_from_rotvec(double rx, double ry, double rz) {
+  const double a2 = rx * rx + ry * ry + rz * rz, a = sqrt(a2);
+  const double sc = a <= 1e-3 ? 0.5 - a2 / 48.0 + a2 * a2 / 3840.0 : sin(0.5 * a) / a;
+  return {sc * rx, sc * ry, sc * rz, cos(0.5 * a)};
+}
+
+// from_matrix (Shepperd: the largest of the diagonal and the trace picks the stable formula; scipy's order of the
+// comparisons, the first maximum wins), then normalised.  m(i, j) is row i, column j.  One branch per choice, so the
+// quaternion stays in registers.
+template <class M>
+__device__ __forceinline__ Q4 quat_from_matrix(M m) {
+  const double d0 = m(0, 0), d1 = m(1, 1), d2 = m(2, 2), tr = d0 + d1 + d2;
+  int c = 0;  // argmax over (d0, d1, d2, tr)
+  double best = d0;
+  if (d1 > best) c = 1, best = d1;
+  if (d2 > best) c = 2, best = d2;
+  if (tr > best) c = 3;
+  Q4 q;
+  if (c == 0) {
+    q = {1.0 - tr + 2.0 * d0, m(1, 0) + m(0, 1), m(2, 0) + m(0, 2), m(2, 1) - m(1, 2)};
+  } else if (c == 1) {
+    q = {m(0, 1) + m(1, 0), 1.0 - tr + 2.0 * d1, m(2, 1) + m(1, 2), m(0, 2) - m(2, 0)};
+  } else if (c == 2) {
+    q = {m(0, 2) + m(2, 0), m(1, 2) + m(2, 1), 1.0 - tr + 2.0 * d2, m(1, 0) - m(0, 1)};
+  } else {
+    q = {m(2, 1) - m(1, 2), m(0, 2) - m(2, 0), m(1, 0) - m(0, 1), 1.0 + tr};
+  }
+  const double n = sqrt(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
+  return {q.x / n, q.y / n, q.z / n, q.w / n};
+}
+
+// scipy's wrap of an Euler angle: one turn added or taken away where it lies outside [-pi, pi] (an exact +-pi stays)
+__device__ __forceinline__ double wrap_pi(double a) {
+  return a < -M_PI ? a + 2.0 * M_PI : (a > M_PI ? a - 2.0 * M_PI : a);
+}
+
+// as_euler('zxy') (extrinsic z, then x, then y) by Bernardes & Viollet's quaternion method, the algorithm scipy uses
+// since 1.10 (scipy 1.8.0, which the reference pins, goes through the matrix; both agree away from the lock): axes
+// (i, j, k) = (z, x, y), sign +1, a = w - x, b = z + y, c = x + w, d = y - z.  The middle angle is 2 atan2(|(c, d)|,
+// |(a, b)|) - pi/2 in [-pi/2, pi/2].  Within 1e-7 rad of the lock (middle angle +-pi/2) the third angle is 0 and the first
+// carries the whole rotation about the vertical: 2 atan2(b, a) at -pi/2, -2 atan2(d, c) at +pi/2 - scipy's rule and
+// threshold.  Every angle is then brought into [-pi, pi] as wrap_pi does.
+__device__ __forceinline__ void euler_zxy(const Q4& q, double e[3]) {
+  const double a = q.w - q.x, b = q.z + q.y, c = q.x + q.w, d = q.y - q.z;
+  const double hs = atan2(b, a), hd = atan2(d, c);
+  const double th = 2.0 * atan2(hypot(c, d), hypot(a, b));
+  const bool lock0 = fabs(th) <= 1e-7, lock1 = fabs(th - M_PI) <= 1e-7;
+  if (lock0 || lock1) {
+    e[0] = lock0 ? 2.0 * hs : -2.0 * hd;
+    e[2] = 0.0;
+  } else {
+    e[0] = hs - hd;
+    e[2] = hs + hd;
+  }
+  e[1] = th - 0.5 * M_PI;
+  for (int i = 0; i < 3; ++i) e[i] = wrap_pi(e[i]);
+}
+
+// from_euler('zxy', e): q = q_y(e2) q_x(e1) q_z(e0), elementary q_axis(t) = (sin(t/2) axis, cos(t/2))
+__device__ __forceinline__ Q4 quat_from_euler_zxy(const double e[3]) {
+  double sz, cz, sx, cx, sy, cy;
+  sincos(0.5 * e[0], &sz, &cz);
+  sincos(0.5 * e[1], &sx, &cx);
+  sincos(0.5 * e[2], &sy, &cy);
+  // q_x q_z = (sx cz, -sx sz... ): (cx, sx, 0, 0) * (cz, 0, 0, sz) in (w, x, y, z)
+  const double w1 = cx * cz, x1 = sx * cz, y1 = -sx * sz, z1 = cx * sz;
+  // q_y * q1 with q_y = (cy, 0, sy, 0)
+  return {cy * x1 + sy * z1, cy * y1 + sy * w1, cy * z1 - sy * x1, cy * w1 - sy * y1};
+}
+
+// as_rotvec: the quaternion in scipy's canonical sign (w > 0; at w == 0 the first non-zero of x, y, z positive), angle = 2 atan2(|v|, w), scale = 2 + angle^2/12 +
+// 7 angle^4/2880 for angle <= 1e-3, angle / sin(angle/2) otherwise
+__device__ __forceinline__ void rotvec_from_quat(Q4 q, float* out) {
+  const bool flip = q.w < 0.0 || (q.w == 0.0 && (q.x < 0.0 || (q.x == 0.0 && (q.y < 0.0 || (q.y == 0.0 && q.z < 0.0)))));
+  if (flip) q = {-q.x, -q.y, -q.z, -q.w};
+  const double n = sqrt(q.x * q.x + q.y * q.y + q.z * q.z);
+  const double a = 2.0 * atan2(n, q.w), a2 = a * a;
+  const double sc = a <= 1e-3 ? 2.0 + a2 / 12.0 + 7.0 * a2 * a2 / 2880.0 : a / sin(0.5 * a);
+  out[0] = static_cast<float>(sc * q.x), out[1] = static_cast<float>(sc * q.y), out[2] = static_cast<float>(sc * q.z);
+}
+
+// One rotation + n degrees of zxy Euler noise, in float64: the reference's as_euler('zxy', degrees=True) + n ->
+// from_euler('zxy', degrees=True) -> as_rotvec.
+__device__ __forceinline__ void add_euler_noise(const Q4& q, const float* n_deg, float* out) {
+  double e[3];
+  euler_zxy(q, e);
+  constexpr double kDeg = M_PI / 180.0;
+  for (int i = 0; i < 3; ++i) e[i] += static_cast<double>(n_deg[i]) * kDeg;
+  rotvec_from_quat(quat_from_euler_zxy(e), out);
+}
+
+// One thread per (window, frame, rotation): rotation 0 is the canonical global orientation (that thread also writes the
+// canonical translation and the betas, each + n), rotations 1..21 the body-pose joints.  The canonical R/T come from the
+// encoder's own functions (cano_global_rot, cano_transl) on the window's frame, rebuilt from transf and the window's
+// frame-0 root, so the clean parameters under the noise are those the clean rows were encoded from.  Noise arrays are
+// window-major [W, clip_len, .]; out is [W * clip_len, kRow].
+__global__ void window_param_noise_kernel(const float* __restrict__ joints, const float* __restrict__ go,
+                                          const float* __restrict__ transl, const float* __restrict__ betas,
+                                          const float* __restrict__ body_pose, const int* __restrict__ win_rec,
+                                          const int* __restrict__ win_start, const int* __restrict__ rec_off,
+                                          const float* __restrict__ transf, int W, int clip_len,
+                                          const float* __restrict__ n_transl, const float* __restrict__ n_betas,
+                                          const float* __restrict__ n_go, const float* __restrict__ n_pose,
+                                          float* __restrict__ out) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<int64_t>(W) * clip_len * (kPoseJ + 1)) return;
+  const int r = static_cast<int>(i % (kPoseJ + 1));
+  const int64_t row = i / (kPoseJ + 1);  // w * clip_len + t
+  const int w = static_cast<int>(row / clip_len), t = static_cast<int>(row % clip_len);
+  const int64_t f0 = static_cast<int64_t>(rec_off[win_rec[w]]) + win_start[w], f = f0 + t;
+  float* o = out + row * kRow;
+  if (r > 0) {
+    const float* a = body_pose + f * kPoseJ * 3 + (r - 1) * 3;
+    add_euler_noise(quat_from_rotvec(a[0], a[1], a[2]), n_pose + (row * kPoseJ + (r - 1)) * 3, o + kRowPose + (r - 1) * 3);
+    return;
+  }
+  const float* M = transf + static_cast<int64_t>(w) * 16;
+  const float* P0 = joints + f0 * kJ * 3;
+  const CanoFrame F{M[0], M[1], M[4], M[5], P0[0], P0[1], -M[11]};
+  const float* P = joints + f * kJ * 3;
+  const V3 pelvis = F.to_cano({P[0], P[1], P[2]});
+  const float cp[3] = {pelvis.x, pelvis.y, pelvis.z};
+  for (int c = 0; c < 3; ++c) o[kRowTransl + c] = cano_transl(cp[c], P[c], transl[f * 3 + c]) + n_transl[row * 3 + c];
+  for (int l = 0; l < kBetas; ++l) o[kRowBetas + l] = betas[f * kBetas + l] + n_betas[row * kBetas + l];
+  const M3 R = cano_global_rot(F, go + f * 3);
+  auto m = [&](int a, int b) {
+    const V3 col = b == 0 ? R.c0 : (b == 1 ? R.c1 : R.c2);
+    return static_cast<double>(a == 0 ? col.x : (a == 1 ? col.y : col.z));
+  };
+  add_euler_noise(quat_from_matrix(m), n_go + row * 3, o + kRowGo);
 }
 
 // One thread per (window, pose frame, joint): p = R^T (c - t) for transf = [R | t], written to recording frame
@@ -223,9 +407,45 @@ extern "C" int rohm_window_encode(rohm_ctx* ctx, const float* global_orient, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ROHM_CUDA(ctx, cudaMemcpyAsync(win_rec, tab_rec.data(), sizeof(int) * W, cudaMemcpyHostToDevice, st));
   ROHM_CUDA(ctx, cudaMemcpyAsync(win_start, tab_start.data(), sizeof(int) * W, cudaMemcpyHostToDevice, st));
-  window_encode_kernel<<<W, (clip_len + 31) / 32 * 32, 0, st>>>(joints, global_orient, transl, betas, body_pose, win_rec,
+  window_encode_kernel<false><<<W, (clip_len + 31) / 32 * 32, 0, st>>>(joints, global_orient, transl, betas, body_pose, win_rec,
                                                                 win_start, rec_off, clip_len, traj_mean, traj_std, pose_mean,
                                                                 pose_std, transf, repr_traj, repr_pose);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return ROHM_OK;
+}
+
+extern "C" int rohm_window_param_noise(rohm_ctx* ctx, const float* global_orient, const float* transl,
+                                       const float* betas, const float* body_pose, const float* joints, const int* rec_off,
+                                       const int* win_rec, const int* win_start, const float* transf, int W, int clip_len,
+                                       const float* noise_transl, const float* noise_betas, const float* noise_global_orient,
+                                       const float* noise_body_pose, float* noisy_params, void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (W < 0 || clip_len < 3 || clip_len > kMaxClip ||
+      (W > 0 && (!global_orient || !transl || !betas || !body_pose || !joints || !rec_off || !win_rec || !win_start ||
+                 !transf || !noise_transl || !noise_betas || !noise_global_orient || !noise_body_pose || !noisy_params)))
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_window_param_noise: bad arguments");
+  const int64_t n = static_cast<int64_t>(W) * clip_len * (kPoseJ + 1);
+  if (n == 0) return ROHM_OK;
+  window_param_noise_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(
+      joints, global_orient, transl, betas, body_pose, win_rec, win_start, rec_off, transf, W, clip_len, noise_transl,
+      noise_betas, noise_global_orient, noise_body_pose, noisy_params);
+  ROHM_CUDA(ctx, cudaGetLastError());
+  return ROHM_OK;
+}
+
+extern "C" int rohm_window_encode_canonical(rohm_ctx* ctx, const float* params, const float* joints, int W, int clip_len,
+                                            const float* traj_mean, const float* traj_std, const float* pose_mean,
+                                            const float* pose_std, float* repr_traj, float* repr_pose, void* stream) {
+  if (ctx == nullptr) return ROHM_ERR_INVALID;
+  rohm::DeviceGuard device_guard__(ctx);
+  if (W < 0 || clip_len < 3 || clip_len > kMaxClip ||
+      (W > 0 && (!params || !joints || !traj_mean || !traj_std || !pose_mean || !pose_std || !repr_traj || !repr_pose)))
+    return fail(ctx, ROHM_ERR_INVALID, "rohm_window_encode_canonical: bad arguments");
+  if (W == 0) return ROHM_OK;
+  window_encode_kernel<true><<<W, (clip_len + 31) / 32 * 32, 0, static_cast<cudaStream_t>(stream)>>>(
+      joints, params + kRowGo, params + kRowTransl, params + kRowBetas, params + kRowPose, nullptr, nullptr, nullptr,
+      clip_len, traj_mean, traj_std, pose_mean, pose_std, nullptr, repr_traj, repr_pose);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }

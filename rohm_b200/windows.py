@@ -7,6 +7,10 @@ builds them without input noise (dataloader_amass.py:319-341).  ``to_recordings`
 world frame of its recording (the inverse of transf_matrix, eval_prox_egobody.py:177-182).  Both are one kernel launch
 (rohm_window_encode / rohm_window_to_world); tensors stay on the GPU.
 
+``encode(..., noise=InputNoise...)`` adds the reference's input noise (dataloader_amass.py:156-227 with sep_noise False,
+the paper's setup): noise on each window's canonical SMPL-X parameters (rohm_window_param_noise), FK of the noisy
+parameters with the body model, and their representation without re-canonicalisation (rohm_window_encode_canonical).
+
 Only full windows are cut, so a recording shorter than ``clip_len`` gives none, and the frames after a recording's last
 window are not covered.  A window's results cover its first clip_len - 2 frames (the PoseNet frames): with overlap 2
 consecutive windows tile the recording, with overlap 0 each leaves a 2-frame gap.  ``to_recordings`` reports which frames
@@ -17,13 +21,19 @@ import ctypes as C
 import numpy as np
 import torch
 
-from . import _lib, glue
+from . import _lib, glue, noise_streams, ops
 from ._lib import RohmB200Error
 
 MAX_CLIP_LEN = 160  # one CTA of one thread per window frame
 # channels of the 294-wide row the TrajNet condition keeps with repr_abs_only (dataloader_amass.py:337)
 ABS_TRAJ_CHANNELS = (0, 2, 3, 6, 7, 8, 9, 10, 11, 12, 16, 17, 18)
 PARAMS = (('global_orient', 3), ('transl', 3), ('betas', 10), ('body_pose', 63))
+# a row of Windows.noisy_params: the PARAMS in order, 79 floats
+NOISY_ROW = {'global_orient': slice(0, 3), 'transl': slice(3, 6), 'betas': slice(6, 16), 'body_pose': slice(16, 79)}
+NOISY_WIDTH = 79
+# the reference's order of draws (dataloader_amass.py:159) and each draw's channels per frame
+NOISE_DRAWS = (('transl', 3), ('body_pose', 63), ('betas', 10), ('global_orient', 3))
+NOISE_SHAPES = {'transl': (3,), 'betas': (10,), 'global_orient': (3,), 'body_pose': (21, 3)}
 
 
 def window_table(lengths, clip_len=145, overlap=2):
@@ -35,14 +45,112 @@ def window_table(lengths, clip_len=145, overlap=2):
 
 class Windows:
     """The windows of one ``encode`` call: ``recording`` / ``start`` (int32 device [W]), ``transf`` (world -> canonical
-    [W,4,4]), and the recordings' ``lengths`` (ints), ``offsets`` (int32 device [R+1]), ``clip_len`` and ``overlap``."""
+    [W,4,4]), and the recordings' ``lengths`` (ints), ``offsets`` (int32 device [R+1]), ``clip_len`` and ``overlap``.
+    With input noise, ``noisy_params`` holds the noisy canonical SMPL-X parameters [W, clip_len, 79] (rows of
+    global_orient 3 | transl 3 | betas 10 | body_pose 63 axis-angle, see NOISY_ROW); None without."""
 
-    def __init__(self, recording, start, transf, lengths, offsets, clip_len, overlap):
+    def __init__(self, recording, start, transf, lengths, offsets, clip_len, overlap, noisy_params=None):
         self.recording, self.start, self.transf = recording, start, transf
         self.lengths, self.offsets, self.clip_len, self.overlap = lengths, offsets, clip_len, overlap
+        self.noisy_params = noisy_params
 
     def __len__(self):
         return int(self.recording.shape[0])
+
+
+class InputNoise:
+    """The input noise of W windows, one entry per window in window order (``window_table``), in the layout and units of
+    the reference's preset-noise pickle (smplx_noise_level_*.pkl, one entry per clip): transl [W, clip_len, 3] metres,
+    betas [W, clip_len, 10] (per frame), global_orient [W, clip_len, 3] and body_pose [W, clip_len, 21, 3] degrees, added
+    to scipy's extrinsic 'zxy' Euler angles of the canonical rotations.  Build it with ``given`` or ``drawn``."""
+
+    def __init__(self, tensors=None, generators=None, stds=None):
+        self._tensors, self._generators, self._stds = tensors, generators, stds
+
+    @classmethod
+    def given(cls, transl, betas, global_orient, body_pose):
+        """Preset noise (load_noise=True): float32 CUDA tensors on one device, shapes as in the class docstring."""
+        t = {'transl': transl, 'betas': betas, 'global_orient': global_orient, 'body_pose': body_pose}
+        dev = None
+        for name, v in t.items():
+            if not torch.is_tensor(v):
+                raise RohmB200Error(f"InputNoise.given: {name} must be a torch tensor, got {type(v).__name__}")
+            if v.device.type != 'cuda':
+                raise RohmB200Error(f"InputNoise.given: {name} must be a CUDA tensor, got one on {v.device}")
+            if v.dtype != torch.float32:
+                raise RohmB200Error(f"InputNoise.given: {name} must be float32, got {v.dtype}")
+            if dev is not None and v.device != dev:
+                raise RohmB200Error(f"InputNoise.given: {name} lives on {v.device}, transl on {dev}")
+            dev = v.device
+            want = 2 + len(NOISE_SHAPES[name])
+            if v.dim() != want or tuple(v.shape[2:]) != NOISE_SHAPES[name]:
+                raise RohmB200Error(f"InputNoise.given: {name} must be [W, clip_len, {', '.join(map(str, NOISE_SHAPES[name]))}]"
+                                    f", got {tuple(v.shape)}")
+            if tuple(v.shape[:2]) != tuple(transl.shape[:2]):
+                raise RohmB200Error(f"InputNoise.given: {name} covers [W, clip_len] = {tuple(v.shape[:2])}, transl "
+                                    f"{tuple(transl.shape[:2])}")
+        return cls(tensors={k: v.contiguous() for k, v in t.items()})
+
+    @classmethod
+    def drawn(cls, generators, std_global_rot=3.0, std_body_rot=3.0, std_transl=0.03, std_betas=0.1):
+        """Noise drawn on the device from one CUDA torch.Generator per window (defaults: test_amass_full.py's noise level
+        3).  Window w gets exactly ``std * torch.randn(shape, generator=generators[w])`` for each parameter, in the
+        reference's order (transl [clip_len, 3], body_pose [clip_len*21, 3], betas [clip_len, 10], global_orient
+        [clip_len, 3]), and each generator's offset advances as those four torch draws would advance it.  The draws
+        happen in ``encode``, after its checks."""
+        if not isinstance(generators, (list, tuple)):
+            raise RohmB200Error(f"InputNoise.drawn: generators must be a list or tuple of torch.Generator, got "
+                                f"{type(generators).__name__}")
+        stds = {'global_orient': std_global_rot, 'body_pose': std_body_rot, 'transl': std_transl, 'betas': std_betas}
+        for name, v in stds.items():
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not np.isfinite(v) or v < 0:
+                raise RohmB200Error(f"InputNoise.drawn: the standard deviation of {name} must be a finite number >= 0, "
+                                    f"got {v!r}")
+        return cls(generators=list(generators), stds={k: float(v) for k, v in stds.items()})
+
+    def _check(self, W, clip_len, dev):
+        """Refuses a noise that does not fit W windows of clip_len frames on `dev`, before anything runs."""
+        if W == 0:
+            raise RohmB200Error("windows.encode: input noise for a batch that cuts no window (every recording is shorter "
+                                "than clip_len)")
+        if self._tensors is not None:
+            got = tuple(self._tensors['transl'].shape[:2])
+            if got != (W, clip_len):
+                raise RohmB200Error(f"windows.encode: the input noise covers [W, clip_len] = {got}, the recordings cut "
+                                    f"{W} windows of {clip_len} frames")
+            if self._tensors['transl'].device != dev:
+                raise RohmB200Error(f"windows.encode: the input noise lives on {self._tensors['transl'].device}, the "
+                                    f"parameters on {dev}")
+            return
+        gens = self._generators
+        if len(gens) != W:
+            raise RohmB200Error(f"windows.encode: InputNoise.drawn holds {len(gens)} generators, the recordings cut {W} "
+                                "windows; give every window its own")
+        if len({id(g) for g in gens}) != len(gens):
+            raise RohmB200Error("InputNoise.drawn: the same generator object appears twice; give every window its own")
+        step = noise_streams.MAX_CLIPS
+        for i in range(0, W, step):
+            try:
+                noise_streams.check_generators({'generators': gens[i:i + step]}, len(gens[i:i + step]), dev)
+            except RohmB200Error as e:
+                raise RohmB200Error(f"InputNoise.drawn (windows {i}..): {e}") from None
+
+    def _tensors_for(self, clip_len, dev):
+        """The noise tensors: the given ones, or the draws (at most MAX_CLIPS generators per launch; every generator's
+        draws are its own, so the chunking changes no bit)."""
+        if self._tensors is not None:
+            return self._tensors
+        W = len(self._generators)
+        out = {}
+        for name, width in NOISE_DRAWS:
+            t = torch.empty(W, clip_len, width, device=dev)
+            for i in range(0, W, noise_streams.MAX_CLIPS):
+                chunk = self._generators[i:i + noise_streams.MAX_CLIPS]
+                streams = noise_streams.NoiseStreams(chunk, dev)
+                t[i:i + len(chunk)] = ops.randn_clips(streams, [len(chunk), clip_len, width], True)
+                streams.close()
+            out[name] = t.mul_(self._stds[name]).reshape(W, clip_len, *NOISE_SHAPES[name])
+        return out
 
 
 def _check_shape(clip_len, overlap):
@@ -51,7 +159,7 @@ def _check_shape(clip_len, overlap):
                             "overlap of 0 to 2 frames (so that no recording frame lies in two windows' pose frames)")
 
 
-def encode(body_model, params, lengths, pose_dataset, traj_dataset, clip_len=145, overlap=2):
+def encode(body_model, params, lengths, pose_dataset, traj_dataset, clip_len=145, overlap=2, noise=None):
     """params: SMPL-X parameters of R recordings packed frame after frame (CUDA tensors global_orient [N,3], transl [N,3],
     betas [N,10], body_pose [N,63] axis-angle, N = sum of lengths, z up); lengths: frames per recording (ints).  World joints
     come from ``body_model`` (FK only).  Returns (test_batch_traj, test_batch_pose, windows):
@@ -62,23 +170,53 @@ def encode(body_model, params, lengths, pose_dataset, traj_dataset, clip_len=145
     * test_batch_pose: motion_repr_clean / motion_repr_noisy z-scored with pose_dataset's statistics;
     * windows: the window table and transf (``Windows``), for ``to_recordings``.
 
-    Each window's rows depend on its own frames only: the same in any batch, order or packing of recordings."""
+    Each window's rows depend on its own frames only: the same in any batch, order or packing of recordings.
+
+    noise: an ``InputNoise`` for the W windows, or None (motion_repr_noisy is then a copy of motion_repr_clean).  With
+    noise, the dicts are the ones DataloaderAMASS.__getitem__ builds with input_noise (dataloader_amass.py:317-341):
+    motion_repr_noisy is the representation of the noisy window, in test_batch_pose with its first
+    pose_dataset.traj_feat_dim channels replaced by the clean ones; test_batch_traj's cond is the noisy trajectory and
+    control_cond the clean local pose; both dicts get noisy_joints [W, clip_len, 22, 3] (canonical, from FK of the noisy
+    parameters with ``body_model``), and windows.noisy_params the noisy parameters.  One deliberate difference: with
+    load_noise=False the reference's pose and traj datasets each draw their own noise from numpy's global stream; here
+    one noise per window feeds both dicts, as the reference's default load_noise=True does.  Each window's noisy rows
+    depend on its own frames and its own noise only."""
+    _check_noise_type(noise)
     p, lengths = _packed_params(params, lengths, clip_len, overlap)
+    W = len(window_table(lengths, clip_len, overlap))
+    _check_noise(noise, W, clip_len, p['transl'].device)
     joints = None
-    if window_table(lengths, clip_len, overlap):
+    if W:
         joints = body_model(transl=p['transl'], global_orient=p['global_orient'], body_pose=p['body_pose'],
                             betas=p['betas'], return_verts=False).joints[:, 0:22].contiguous()
-    return _encode(p, joints, lengths, pose_dataset, traj_dataset, clip_len, overlap)
+    return _encode(p, joints, lengths, pose_dataset, traj_dataset, clip_len, overlap, noise, body_model)
 
 
-def encode_joints(params, joints, lengths, pose_dataset, traj_dataset, clip_len=145, overlap=2):
+def encode_joints(params, joints, lengths, pose_dataset, traj_dataset, clip_len=145, overlap=2, noise=None,
+                  body_model=None):
     """``encode`` with the recordings' 22-joint world positions given (joints [N,22,3], packed like params), as the
-    reference loaders read them from preprocessed files."""
+    reference loaders read them from preprocessed files.  With ``noise``, ``body_model`` gives the noisy joints by FK, as
+    the AMASS loader does (dataloader_amass.py:194-206)."""
+    _check_noise_type(noise)
+    if noise is not None and body_model is None:
+        raise RohmB200Error("windows.encode_joints: input noise needs body_model, which gives the noisy joints by FK")
     p, lengths = _packed_params(params, lengths, clip_len, overlap)
     joints = glue._f32c(joints, "windows.encode_joints: joints")
     if joints.numel() != sum(lengths) * 66:
         raise RohmB200Error(f"windows.encode_joints: joints must hold [{sum(lengths)}, 22, 3], got {tuple(joints.shape)}")
-    return _encode(p, joints, lengths, pose_dataset, traj_dataset, clip_len, overlap)
+    _check_noise(noise, len(window_table(lengths, clip_len, overlap)), clip_len, p['transl'].device)
+    return _encode(p, joints, lengths, pose_dataset, traj_dataset, clip_len, overlap, noise, body_model)
+
+
+def _check_noise_type(noise):
+    if noise is not None and not isinstance(noise, InputNoise):
+        raise RohmB200Error(f"windows.encode: noise must be an InputNoise (InputNoise.given / .drawn) or None, got "
+                            f"{type(noise).__name__}")
+
+
+def _check_noise(noise, W, clip_len, dev):
+    if noise is not None:
+        noise._check(W, clip_len, dev)
 
 
 def _packed_params(params, lengths, clip_len, overlap):
@@ -97,7 +235,7 @@ def _packed_params(params, lengths, clip_len, overlap):
     return p, lengths
 
 
-def _encode(p, joints, lengths, pose_dataset, traj_dataset, clip_len, overlap):
+def _encode(p, joints, lengths, pose_dataset, traj_dataset, clip_len, overlap, noise=None, body_model=None):
     dev = p['transl'].device
     tm, ts = glue.stats_on(traj_dataset, dev)
     pm, ps = glue.stats_on(pose_dataset, dev)
@@ -123,11 +261,40 @@ def _encode(p, joints, lengths, pose_dataset, traj_dataset, clip_len, overlap):
         if n.value != W:
             raise RohmB200Error(f"windows.encode: the library cut {n.value} windows, the window rule {W}")
     tfd, pfd = traj_dataset.traj_feat_dim, traj_dataset.pose_feat_dim
-    cond = rt[..., list(ABS_TRAJ_CHANNELS)] if tfd == len(ABS_TRAJ_CHANNELS) else rt[..., 0:tfd].clone()
-    test_batch_traj = {'motion_repr_clean': rt, 'motion_repr_noisy': rt.clone(), 'cond': cond,
-                       'control_cond': rt[..., -pfd:].contiguous()}
-    test_batch_pose = {'motion_repr_clean': rp, 'motion_repr_noisy': rp.clone()}
-    return test_batch_traj, test_batch_pose, Windows(rec, start, transf, lengths, offsets, clip_len, overlap)
+    win = Windows(rec, start, transf, lengths, offsets, clip_len, overlap)
+    if noise is None:
+        cond = rt[..., list(ABS_TRAJ_CHANNELS)] if tfd == len(ABS_TRAJ_CHANNELS) else rt[..., 0:tfd].clone()
+        test_batch_traj = {'motion_repr_clean': rt, 'motion_repr_noisy': rt.clone(), 'cond': cond,
+                           'control_cond': rt[..., -pfd:].contiguous()}
+        test_batch_pose = {'motion_repr_clean': rp, 'motion_repr_noisy': rp.clone()}
+        return test_batch_traj, test_batch_pose, win
+
+    # dataloader_amass.py:156-215: noisy canonical parameters, their FK, their representation (not re-canonicalised)
+    n = noise._tensors_for(clip_len, dev)
+    lib, ctx = _lib.load(), _lib.ctx(dev.index)
+    noisy = torch.empty(W * clip_len, NOISY_WIDTH, device=dev)
+    rc = lib.rohm_window_param_noise(ctx, glue._p(p['global_orient']), glue._p(p['transl']), glue._p(p['betas']),
+                                     glue._p(p['body_pose']), glue._p(joints), glue._p(offsets), glue._p(rec),
+                                     glue._p(start), glue._p(transf), W, clip_len, glue._p(n['transl']),
+                                     glue._p(n['betas']), glue._p(n['global_orient']), glue._p(n['body_pose']),
+                                     glue._p(noisy), glue._stream(dev))
+    _lib.check(rc, ctx)
+    nj = body_model(**{k: noisy[:, s] for k, s in NOISY_ROW.items()}, return_verts=False).joints[:, 0:22].contiguous()
+    nt = torch.empty(W, T1, glue.BODY_FEAT_DIM, device=dev)
+    npose = torch.empty(W, T1, glue.BODY_FEAT_DIM, device=dev)
+    rc = lib.rohm_window_encode_canonical(ctx, glue._p(noisy), glue._p(nj), W, clip_len, glue._p(tm), glue._p(ts),
+                                          glue._p(pm), glue._p(ps), glue._p(nt), glue._p(npose), glue._stream(dev))
+    _lib.check(rc, ctx)
+    # __getitem__ (:317-341): PoseNet is conditioned on the clean trajectory (task 'pose'); TrajNet on the noisy trajectory
+    # with the clean local pose as its control signal (task 'traj')
+    npose[..., 0:pose_dataset.traj_feat_dim] = rp[..., 0:pose_dataset.traj_feat_dim]
+    noisy_joints = nj.reshape(W, clip_len, 22, 3)
+    cond = nt[..., list(ABS_TRAJ_CHANNELS)] if tfd == len(ABS_TRAJ_CHANNELS) else nt[..., 0:tfd].clone()
+    test_batch_traj = {'motion_repr_clean': rt, 'motion_repr_noisy': nt, 'cond': cond,
+                       'control_cond': rt[..., -pfd:].contiguous(), 'noisy_joints': noisy_joints}
+    test_batch_pose = {'motion_repr_clean': rp, 'motion_repr_noisy': npose, 'noisy_joints': noisy_joints.clone()}
+    win.noisy_params = noisy.reshape(W, clip_len, NOISY_WIDTH)
+    return test_batch_traj, test_batch_pose, win
 
 
 def to_recordings(windows, joints):

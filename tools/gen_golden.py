@@ -646,13 +646,169 @@ def gen_windows(ref):
     print("windows.npz")
 
 
+# Input noise (dataloader_amass.py:156-227): 24-frame windows with overlap 2 over the first two recordings (three windows),
+# each with its own noise scale relative to test_amass_full.py's level 3 (3 deg, 3 deg, 0.03 m, 0.1)
+NOISE_LENGTHS = (47, 24)
+NOISE_SCALES = (1.0, 1.0 / 30.0, 0.3)
+NOISE_LOCK_JOINT, NOISE_NEAR_JOINT = 17, 18  # body_pose rotations (elbows: they move no foot, hip or shoulder)
+NOISE_KEEP_LOCK_WINDOW = 1  # the window whose middle-angle noise on those two joints is zero
+
+
+def _lock_rotvec(g, middle_deg, want):
+    """A float32 rotvec whose 'zxy' middle angle is middle_deg, with random first and third angles, whose lock distance
+    (float64, from the float32 values) is below 3e-8 rad (want='lock') or within 1e-5 of 1e-3 rad (want='near'): well
+    clear of scipy's 1e-7 threshold either way."""
+    from oracle import windows_noise_oracle as wno
+    while True:
+        e = [g.uniform(-170, 170), middle_deg, g.uniform(-170, 170)]
+        rv = ref_rotation.from_euler('zxy', e, degrees=True).as_rotvec().astype(np.float32)
+        d = float(wno.lock_distance(wno.quat_from_rotvec(rv.astype(np.float64))))
+        if (want == 'lock' and d < 3e-8) or (want == 'near' and abs(d - 1e-3) < 1e-5):
+            return rv
+
+
+def noise_recordings(seed=91):
+    """Recordings whose joints are FK of their parameters on the synthetic body, as AMASS's preprocessed joints are: the
+    global orientation turns about z near +-180 deg (recording 0 from 178 deg through 180, recording 1 near -179 deg) with
+    a small tilt; the translation moves slowly (0 to 4 mm per frame) so that feet come into contact; the body pose is
+    smooth, except the two elbow rotations: NOISE_LOCK_JOINT is exactly at the 'zxy' gimbal lock (middle angle +90 deg on
+    even frames, -90 on odd), NOISE_NEAR_JOINT 1e-3 rad from it."""
+    g = np.random.default_rng(seed)
+    model = synthetic.smplx_like_model(0)
+    params, joints = {k: [] for k in ("global_orient", "transl", "betas", "body_pose")}, []
+    near = 90.0 - np.degrees(1e-3)
+    for r, n in enumerate(NOISE_LENGTHS):
+        t = np.arange(n, dtype=np.float64)
+        phi = (np.pi - 0.035 + 0.07 * t / n) if r == 0 else (-np.pi + 0.02 + 0.01 * np.sin(t / 5.0))
+        tilt = 0.05 * np.sin(t / 13.0)
+        go = (ref_rotation.from_rotvec(np.stack([0 * t, 0 * t, phi], -1)) *
+              ref_rotation.from_rotvec(np.stack([tilt, 0 * t, 0 * t], -1))).as_rotvec()
+        speed = 0.002 * (1 + np.sin(t / 4.0 + r))  # metres per frame, 0 .. 4 mm
+        transl = np.stack([0.3 * r + np.cumsum(speed) * 0.6, np.cumsum(speed) * 0.8 - r, 0.9 + 0.002 * np.sin(t / 7.0)], -1)
+        betas = np.repeat(0.5 * g.standard_normal((1, 10)), n, axis=0)
+        body_pose = 0.15 * g.standard_normal((1, 63)) + 0.02 * np.sin(t[:, None] / 9.0 + np.arange(63))
+        for fr in range(n):
+            body_pose[fr, NOISE_LOCK_JOINT * 3:NOISE_LOCK_JOINT * 3 + 3] = _lock_rotvec(g, 90.0 if fr % 2 == 0 else -90.0, 'lock')
+            body_pose[fr, NOISE_NEAR_JOINT * 3:NOISE_NEAR_JOINT * 3 + 3] = _lock_rotvec(g, near if fr % 2 else -near, 'near')
+        f = lambda a: torch.from_numpy(np.asarray(a, np.float32))
+        j, _ = ko.smplx_forward(model, f(go), f(body_pose), f(betas), f(transl), return_verts=False)
+        for k, v in (("global_orient", go), ("transl", transl), ("betas", betas), ("body_pose", body_pose)):
+            params[k].append(np.asarray(v, np.float32))
+        joints.append(j[:, 0:22].numpy().astype(np.float32))
+    return {k: np.concatenate(v) for k, v in params.items()}, np.concatenate(joints)
+
+
+def gen_windows_noise(ref):
+    """The reference's own AMASS loader with input noise (input_noise=True, sep_noise=False, load_noise=True): a
+    DataloaderAMASS made with object.__new__, its clip lists set to the windows of the recordings above and its preset
+    noise to the arrays below, then create_body_repr and __getitem__ for task 'pose' (repr_abs_only=False) and task
+    'traj' (repr_abs_only=True).  The stub smplx body stands in for the SMPL-X model, as everywhere in this file."""
+    import pickle
+    import tempfile
+    sys.path.insert(0, '/root/reference')
+    import data_loaders.dataloader_amass as dla
+    sys.path.pop(0)
+    from oracle import windows_oracle as wo
+    from oracle import windows_noise_oracle as wno
+    params, joints = noise_recordings()
+    L, overlap = WINDOW_CLIP, 2
+    off = np.concatenate([[0], np.cumsum(NOISE_LENGTHS)])
+    table = wo.window_table(NOISE_LENGTHS, L, overlap)
+    assert len(table) == len(NOISE_SCALES), table
+    g = np.random.default_rng(92)
+    noise = {'transl': [], 'betas': [], 'global_orient': [], 'body_pose': []}
+    for w, sc in enumerate(NOISE_SCALES):
+        bp = (sc * 3.0 * g.standard_normal((L, 21, 3))).astype(np.float32)
+        if w == NOISE_KEEP_LOCK_WINDOW:  # the noisy middle angle stays at the lock / 1e-3 rad from it
+            bp[:, NOISE_LOCK_JOINT, 1] = 0.0
+            bp[:, NOISE_NEAR_JOINT, 1] = 0.0
+        else:
+            # middle-angle noise of at least 2 deg: at the lock, (first, third) = (a, 0) and any other split of the same
+            # rotation, e.g. (a - s, s), give noisy rotations s * |n_x| apart, so these windows pin scipy's split
+            bp[:, NOISE_LOCK_JOINT, 1] = np.where(np.arange(L) % 2 == 0, 1.0, -1.0) * (2.0 + np.abs(bp[:, NOISE_LOCK_JOINT, 1]))
+        noise['transl'].append((sc * 0.03 * g.standard_normal((L, 3))).astype(np.float32))
+        noise['betas'].append((sc * 0.1 * g.standard_normal((L, 10))).astype(np.float32))
+        noise['global_orient'].append((sc * 3.0 * g.standard_normal((L, 3))).astype(np.float32))
+        noise['body_pose'].append(bp)
+    noise = {k: np.asarray(v) for k, v in noise.items()}
+    ds_pose = synthetic.make_dataset('pose', seed=3, realistic_std=True)
+    ds_traj = synthetic.make_dataset('traj', seed=3, realistic_std=True)
+    d = object.__new__(dla.DataloaderAMASS)
+    rows = [slice(off[r] + s, off[r] + s + L) for r, s in table]
+    d.joints_clip_list = [joints[rw].copy() for rw in rows]
+    d.smplx_clip_list = [np.concatenate([params['global_orient'][rw], params['transl'][rw], params['betas'][rw],
+                                         params['body_pose'][rw]], axis=-1) for rw in rows]
+    d.n_samples, d.spacing, d.joints_num, d.clip_len, d.device, d.split = len(rows), 1, 22, L, 'cpu', 'test'
+    d.smplx_neutral = _StubBody()
+    d.input_noise, d.sep_noise, d.load_noise = True, False, True
+    d.loaded_smplx_noise_dict = {k: v.astype(np.float64) for k, v in noise.items()}
+    d.noise_std_params_dict = {'global_orient': 3.0, 'transl': 0.03, 'body_pose': 3.0, 'betas': 0.1}
+    d.repr_list_dict = {k: [] for k in ko.REPR_LIST}
+    d.repr_list_dict_noisy = {k: [] for k in ko.REPR_LIST}
+    d.smplx_params_list_dict = {k: [] for k in ('global_orient', 'transl', 'body_pose', 'betas')}
+    d.joints_clean_list, d.joints_noisy_list = [], []
+    noisy_params = []
+    real_fk = d.smplx_neutral.forward
+
+    def recording_fk(**kw):  # the noisy parameters as the FK receives them (float32)
+        noisy_params.append({k: kw[k].numpy().copy() for k in ('global_orient', 'transl', 'betas', 'body_pose')})
+        return real_fk(**kw)
+
+    d.smplx_neutral.forward = recording_fk
+    with tempfile.TemporaryDirectory() as tmp:
+        cur = 0
+        mean, std = {}, {}
+        for k in ko.REPR_LIST:
+            mean[k] = ds_pose.Mean[cur:cur + ko.REPR_DIM_DICT[k]]
+            std[k] = ds_pose.Std[cur:cur + ko.REPR_DIM_DICT[k]]
+            cur += ko.REPR_DIM_DICT[k]
+        for name, v in (('AMASS_mean.pkl', mean), ('AMASS_std.pkl', std)):
+            with open(os.path.join(tmp, name), 'wb') as fh:
+                pickle.dump(v, fh)
+        d.logdir = tmp
+        d.create_body_repr()
+    out = {"lengths": np.array(NOISE_LENGTHS, np.int64), "clip_len": np.array(L), "overlap": np.array(overlap),
+           "joints": joints, "table": np.array(table, np.int64), "scales": np.array(NOISE_SCALES)}
+    out.update({f"param_{k}": v for k, v in params.items()})
+    out.update({f"noise_{k}": v for k, v in noise.items()})
+    out["noisy_param_global_orient"] = np.asarray([p['global_orient'] for p in noisy_params])
+    out["noisy_param_transl"] = np.asarray([p['transl'] for p in noisy_params])
+    out["noisy_param_betas"] = np.asarray([p['betas'] for p in noisy_params])
+    out["noisy_param_body_pose"] = np.asarray([p['body_pose'] for p in noisy_params]).reshape(len(rows), L, 63)
+    out["noisy_joints"] = np.asarray(d.joints_noisy_list, np.float32)
+    noisy_repr = np.asarray([np.concatenate([d.repr_list_dict_noisy[k][w] for k in ko.REPR_LIST], axis=-1)
+                             for w in range(len(rows))])
+    out["noisy_contacts"] = noisy_repr[..., 290:].astype(np.float32)
+    for task, ds, abs_only in (('pose', ds_pose, False), ('traj', ds_traj, True)):
+        d.task, d.repr_abs_only = task, abs_only
+        d.traj_feat_dim, d.pose_feat_dim = ds.traj_feat_dim, ds.pose_feat_dim
+        d.Mean, d.Std = ds.Mean, ds.Std
+        items = [d.__getitem__(w) for w in range(len(rows))]
+        # motion_repr_clean is windows.npz's business; noisy_joints is stored once above
+        for key in set(items[0]) - {'motion_repr_clean', 'noisy_joints'}:
+            out[f"{task}_{key}"] = np.asarray([it[key] for it in items])
+        assert all(np.array_equal(it['noisy_joints'], out["noisy_joints"][w]) for w, it in enumerate(items))
+    # margins of the noisy contact decisions (the noisy joints are canonical already)
+    nj = out["noisy_joints"].astype(np.float64)
+    feet = [7, 10, 8, 11]
+    v2 = ((nj[:, 1:, feet] - nj[:, :-1, feet]) ** 2).sum(-1)
+    hz = nj[:, :-1, feet, 2] - np.array([0.18, 0.15, 0.18, 0.15])
+    out["noisy_speed_margin"] = np.abs(v2 / 5e-5 - 1)
+    out["noisy_height_margin"] = np.abs(hz)
+    lab = out["noisy_contacts"]
+    np.savez_compressed(os.path.join(OUT, "windows_noise.npz"), **out)
+    print(f"windows_noise.npz: {len(rows)} windows, noisy contacts {float(lab.mean()):.2f}, per window "
+          f"{lab.mean(axis=(1, 2)).round(2).tolist()}, speed margin {float(out['noisy_speed_margin'].min()):.2e}, "
+          f"height margin {float(out['noisy_height_margin'].min()):.2e}")
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     ref = import_reference()
     which = sys.argv[1:] or ["schedules", "posenet", "trajnet", "sampling", "kinematics", "glue", "pipeline",
-                             "clip_guidance", "windows"]
+                             "clip_guidance", "windows", "windows_noise"]
     for w in which:
         {"schedules": gen_schedules, "posenet": gen_posenet, "trajnet": gen_trajnet, "sampling": gen_sampling,
          "kinematics": gen_kinematics, "glue": gen_glue, "pipeline": gen_pipeline, "clip_guidance": gen_clip_guidance,
-         "windows": gen_windows}[w](ref)
+         "windows": gen_windows, "windows_noise": gen_windows_noise}[w](ref)

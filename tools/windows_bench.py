@@ -1,5 +1,7 @@
 """Cost of sliding-window batching: rohm_b200.windows.encode (SMPL-X FK of every frame, then the window encoder) and
-encode_joints (the encoder alone), and to_recordings, on R recordings of N frames cut into 145-frame windows with overlap 2.
+encode_joints (the encoder alone), encode with input noise (noise_given: preset noise tensors; noise_drawn: one CUDA
+generator per window, the draws included; both add the noise kernel, FK of the W x 145 noisy rows and the canonical
+encoder), and to_recordings, on R recordings of N frames cut into 145-frame windows with overlap 2.
 
     python tools/windows_bench.py [--recordings R] [--frames N] [--iters K] [--rounds M] [--oracle-windows V] [--json PATH]
 
@@ -22,7 +24,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from oracle import windows_oracle  # noqa: E402
+from oracle import windows_noise_oracle, windows_oracle  # noqa: E402
 from rohm_b200 import synthetic, windows  # noqa: E402
 from rohm_b200.body_model import BodyModel  # noqa: E402
 
@@ -80,8 +82,15 @@ def main():
     _, pose, win = windows.encode(bm, params, lengths, ds_p, ds_t)
     W = len(win)
     cano = torch.randn(W, 143, 22, 3, device=dev)
+    g = torch.Generator(device=dev).manual_seed(1)
+    level3 = {'transl': (0.03, (3,)), 'betas': (0.1, (10,)), 'global_orient': (3.0, (3,)), 'body_pose': (3.0, (21, 3))}
+    n = {k: s * torch.randn((W, 145) + shape, generator=g, device=dev) for k, (s, shape) in level3.items()}
+    given = windows.InputNoise.given(n['transl'], n['betas'], n['global_orient'], n['body_pose'])
+    gens = [torch.Generator(device=dev).manual_seed(100 + w) for w in range(W)]
     calls = {"encode": lambda: windows.encode(bm, params, lengths, ds_p, ds_t),
              "encode_joints": lambda: windows.encode_joints(params, joints, lengths, ds_p, ds_t),
+             "noise_given": lambda: windows.encode(bm, params, lengths, ds_p, ds_t, noise=given),
+             "noise_drawn": lambda: windows.encode(bm, params, lengths, ds_p, ds_t, noise=windows.InputNoise.drawn(gens)),
              "to_recordings": lambda: windows.to_recordings(win, cano)}
     ms = {k: [] for k in calls}
     for _ in range(a.rounds):
@@ -102,8 +111,16 @@ def main():
                                      host['body_pose'][rows], m)
     oracle_ms = (time.perf_counter() - t0) * 1e3 / len(table)
     print(f"oracle (float64 numpy, CPU, 1 thread): {oracle_ms:.3f} ms per window")
+    # the noisy path on the first recording's windows
+    W0 = len(windows.window_table([a.frames]))
+    nh = {k: v[:W0].cpu().numpy() for k, v in n.items()}
+    model = synthetic.smplx_like_model(0)
+    t0 = time.perf_counter()
+    windows_noise_oracle.encode_noisy({k: v[:a.frames] for k, v in host.items()}, jh[:a.frames], [a.frames], nh, model)
+    noisy_ms = (time.perf_counter() - t0) * 1e3 / W0
+    print(f"oracle noisy path (float64, CPU, 1 thread): {noisy_ms:.3f} ms per window")
     line = {"card": info, "recordings": a.recordings, "frames": a.frames, "windows": W, **{k: v for k, v in res.items()},
-            "oracle_cpu_ms_per_window": oracle_ms}
+            "oracle_cpu_ms_per_window": oracle_ms, "oracle_noisy_cpu_ms_per_window": noisy_ms}
     print(json.dumps(line))
     if a.json:
         os.makedirs(os.path.dirname(os.path.abspath(a.json)), exist_ok=True)
