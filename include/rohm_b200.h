@@ -193,17 +193,20 @@ ROHM_API int rohm_posenet_sample_step_clips(rohm_posenet* pn, const float* x_t, 
                                             float* x_next, const float* coef_row, const uint64_t* streams, uint64_t draw,
                                             uint64_t* offset_increments, int B, int T, void* stream);
 
-/* Same as rohm_posenet_forward but with CUDA events recorded on `stream` around every kernel launch; synchronises the
- * stream and returns, per category {0: tensor-core GEMM, 1: attention, 2: LayerNorm, 3: pack/unpack/time-token}, the
+/* Same as rohm_posenet_forward but with CUDA events recorded on `stream` around every kernel launch, always as the serial
+ * layer chain on that one stream; synchronises the stream and returns, per category {0: tensor-core GEMM, 1: attention, 2: LayerNorm, 3: pack/unpack/time-token}, the
  * summed device milliseconds (host float[4]) and the number of launches (host int[4]).  For bench.py's roofline. */
 ROHM_API int rohm_posenet_profile(rohm_posenet* pn, const float* x_t, const int64_t* timesteps, float* out, int B, int T,
                          void* stream, float* ms_by_category, int* launches_by_category);
 
 /* Options: 0 = replay the forward as a CUDA graph (default 1; the graph is captured on first use per (B, T) and its
- * three caller-memory pointers are patched per call); 1 = programmatic dependent launch on the GEMMs (default 1). */
+ * three caller-memory pointers are patched per call); 1 = programmatic dependent launch on the GEMMs (default 1);
+ * 2 = clip groups of uniform clips: 0 = chosen from B and T (default: two concurrent groups when the batch's QKV GEMM
+ * has more tiles than the GPU has SMs), 1 = the serial layer chain, 2 = two groups whenever B >= 2 (for timing the two
+ * against each other; the results are the same bits). */
 ROHM_API int rohm_posenet_set_option(rohm_posenet* pn, int option, int value);
 
-/* Kernel launches issued by the last forward (for bench.py's gpu_launches accounting). */
+/* Kernel launches issued by the last forward outside rohm_posenet_profile (for bench.py's gpu_launches accounting). */
 ROHM_API int rohm_posenet_launches_per_forward(const rohm_posenet* pn);
 
 /* ------------------------------------------------------------------------------------------------------------

@@ -14,6 +14,23 @@ cudaError_t KernelPatch::apply(cudaGraphExec_t exec, cudaGraphNode_t node, const
   return cudaGraphExecKernelNodeSetParams(exec, node, &kp);
 }
 
+BranchEvents::~BranchEvents() {
+  for (cudaEvent_t e : events_) cudaEventDestroy(e);
+}
+
+int BranchEvents::order_after(rohm_ctx* ctx, cudaStream_t from, cudaStream_t to) {
+  if (from == to) return ROHM_OK;
+  if (next_ == events_.size()) {
+    cudaEvent_t e = nullptr;
+    ROHM_CUDA(ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    events_.push_back(e);
+  }
+  cudaEvent_t e = events_[next_++];
+  ROHM_CUDA(ctx, cudaEventRecord(e, from));
+  ROHM_CUDA(ctx, cudaStreamWaitEvent(to, e, 0));
+  return ROHM_OK;
+}
+
 ForwardGraphs::~ForwardGraphs() {
   if (capture_stream_) cudaStreamDestroy(capture_stream_);
 }

@@ -60,6 +60,23 @@ class KernelPatch {
   int n_ = 0;
 };
 
+// Fork / join between the streams of a forward's parallel branches.  order_after(from, to): everything issued on `from` so
+// far happens-before what is issued on `to` afterwards (event record + wait; during stream capture this adds a graph
+// edge).  The events are reused from forward to forward: rewind() before each one.
+class BranchEvents {
+ public:
+  BranchEvents() = default;
+  BranchEvents(const BranchEvents&) = delete;
+  BranchEvents& operator=(const BranchEvents&) = delete;
+  ~BranchEvents();
+  void rewind() { next_ = 0; }
+  int order_after(rohm_ctx* ctx, cudaStream_t from, cudaStream_t to);
+
+ private:
+  std::vector<cudaEvent_t> events_;
+  size_t next_ = 0;
+};
+
 // What a forward graph appends to the forward: nothing, the single-stream update (DdpmStep) or the per-clip one
 // (DdpmClipStep).  Part of the graph key, since the two updates are different kernels.
 enum StepKind : int { kNoStep = 0, kStepSingleStream = 1, kStepPerClip = 2 };

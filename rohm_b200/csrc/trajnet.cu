@@ -312,8 +312,7 @@ struct rohm_trajnet {
   // (11 to 96 tiles), so running them side by side shortens the critical path at no cost.  ROHM_B200_TRAJ_PARALLEL=0: serial.
   bool parallel = true;
   cudaStream_t side[3] = {nullptr, nullptr, nullptr};  // 0: TrajControl branch, 1 / 2: residual convolutions of branch 0 / 1
-  std::vector<cudaEvent_t> events;
-  size_t ev_next = 0;
+  BranchEvents events;
   int cond_B = -1;
   int launches = 0;
   ForwardGraphs graphs;  // CUDA graph of one forward per batch size and lengths
@@ -334,7 +333,6 @@ struct rohm_trajnet {
   ~rohm_trajnet() {
     for (cudaStream_t q : side)
       if (q) cudaStreamDestroy(q);
-    for (cudaEvent_t e : events) cudaEventDestroy(e);
   }
 };
 
@@ -641,32 +639,17 @@ int run_gn(rohm_trajnet* tn, const Conv& cv, const GroupNorm& gn, int B, const f
   return ROHM_OK;
 }
 
-// fork: everything recorded on `from` so far happens-before what is launched on `to` afterwards (event record + wait; during
-// stream capture this adds a graph edge)
-int order_after(rohm_trajnet* tn, cudaStream_t from, cudaStream_t to) {
-  if (from == to) return ROHM_OK;
-  if (tn->ev_next == tn->events.size()) {
-    cudaEvent_t e = nullptr;
-    ROHM_CUDA(tn->ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    tn->events.push_back(e);
-  }
-  cudaEvent_t e = tn->events[tn->ev_next++];
-  ROHM_CUDA(tn->ctx, cudaEventRecord(e, from));
-  ROHM_CUDA(tn->ctx, cudaStreamWaitEvent(to, e, 0));
-  return ROHM_OK;
-}
-
 // Executes a ResidualTemporalBlock on `st`, its 1x1 residual convolution on `side`
 int run_rtb(rohm_trajnet* tn, Rtb& r, int B, cudaStream_t st, cudaStream_t side) {
   if (r.has_res) {  // the 1x1 residual convolution only reads the block's input: run it next to the main chain
-    TRY(order_after(tn, st, side));
+    TRY(tn->events.order_after(tn->ctx, st, side));
     TRY(run_conv(tn, r.res, B, side));
   }
   TRY(run_conv(tn, r.c1, B, st));
   const float* tp = r.tp_off >= 0 ? tn->tp + r.tp_off : nullptr;
   TRY(run_gn(tn, r.c1, r.gn[0], B, tp, nullptr, nullptr, r.a1, st));
   TRY(run_conv(tn, r.c2, B, st));
-  if (r.has_res) TRY(order_after(tn, side, st));
+  if (r.has_res) TRY(tn->events.order_after(tn->ctx, side, st));
   return run_gn(tn, r.c2, r.gn[1], B, nullptr, r.residual, r.extra, r.out, st);
 }
 
@@ -989,7 +972,7 @@ static int trajnet_forward_launches(rohm_trajnet* tn, const float* x_t, const in
 
   // Parallel branches (see rohm_trajnet::parallel): sC carries the TrajControl branch, r0 / r1 the residual 1x1 convolutions
   // (and the odd phases of the transposed convolutions) of the U-Net / TrajControl blocks.
-  tn->ev_next = 0;
+  tn->events.rewind();
   if (tn->parallel)
     for (cudaStream_t& q : tn->side)
       if (q == nullptr) ROHM_CUDA(ctx, cudaStreamCreateWithFlags(&q, cudaStreamNonBlocking));
@@ -998,7 +981,7 @@ static int trajnet_forward_launches(rohm_trajnet* tn, const float* x_t, const in
   cudaStream_t r1 = tn->parallel ? tn->side[2] : sC;
   if (tn->control) {
     auto& ctl = tn->ctl;
-    TRY(order_after(tn, st, sC));  // fork after pack + time
+    TRY(tn->events.order_after(tn->ctx, st, sC));  // fork after pack + time
     for (int l = 0; l < 4; ++l) {
       TRY(run_rtb(tn, ctl.enc[l], B, sC, r1));
       TRY(run_conv(tn, ctl.zero[l], B, sC));
@@ -1013,14 +996,14 @@ static int trajnet_forward_launches(rohm_trajnet* tn, const float* x_t, const in
     TRY(run_conv(tn, tn->down[l], B, st));
   }
   TRY(run_rtb(tn, tn->mid_block[0], B, st, r0));
-  if (tn->control) TRY(order_after(tn, sC, st));  // join: the decoder adds the TrajControl residuals
+  if (tn->control) TRY(tn->events.order_after(tn->ctx, sC, st));  // join: the decoder adds the TrajControl residuals
   TRY(run_rtb(tn, tn->mid_block[1], B, st, r0));
   for (int l = 3; l >= 0; --l) {
     // ConvTranspose1d = two independent GEMMs (even / odd output frames) with row-interleaved stores
-    TRY(order_after(tn, st, r0));
+    TRY(tn->events.order_after(tn->ctx, st, r0));
     TRY(run_conv(tn, tn->up_odd[l], B, r0));
     TRY(run_conv(tn, tn->up_even[l], B, st));
-    TRY(order_after(tn, r0, st));
+    TRY(tn->events.order_after(tn->ctx, r0, st));
     TRY(run_rtb(tn, tn->dec[l], B, st, r0));
   }
   TRY(run_conv(tn, tn->final_c, B, st));
