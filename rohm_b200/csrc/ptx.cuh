@@ -207,28 +207,35 @@ __device__ __forceinline__ void wgmma_f16_rs_tb(float (&d)[64], const uint32_t (
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
 }
 
-// Round-to-nearest TF32 (10-bit mantissa), result kept in an fp32 container.
+// Round-to-nearest TF32 (10-bit mantissa, ties away from zero), result kept in an fp32 container.  fp32 subnormals round
+// like normal values.  The TF32 pair (hi = to_tf32(x), lo = x - hi) is exact for every finite x below the top binade; in it,
+// |x| >= 2^128 (1 - 2^-12) rounds to hi = +-inf, lo = -+inf: a NaN pair.  +-inf gives (+-inf, NaN).  A NaN is truncated,
+// not rounded: hi keeps the top 10 bits of its payload (+-inf when the payload lies in the low 13 bits) and lo is NaN.
 __device__ __forceinline__ float to_tf32(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
 }
 
-// Two-term fp16 split x ~= hi + lo (2 x 11 significant bits, the same 22 bits a TF32 hi/lo pair carries).  hi is
-// clamped to the fp16 range so values up to 2 x 65504 still split into finite halves; below 2^-14 the halves go
-// subnormal and the split degrades gracefully to an absolute error of 2^-25 per element.
+// Two-term fp16 split x ~= hi + lo (2 x 11 significant bits, the same 22 bits a TF32 hi/lo pair carries):
+//   hi = rn_f16(x) saturated to +-65504 (NaN stays NaN),  lo = rn_f16(x - hi), not saturated.
+// So the pair is finite exactly when |x| < 65504 + 65520 = 131024, and +-inf beyond: an out-of-range value is never
+// stored as a plausible finite one.  NaN gives NaN in both halves.  Below 2^-14 the halves go subnormal and the split
+// degrades gracefully to an absolute error of 2^-25 per element.  cvt.rn.satfinite rounds hi to nearest and saturates it
+// (NaN stays NaN); lo is converted without .satfinite, which would turn an overflowing lo into 65504 as well.
 __device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
-  const float c = fminf(fmaxf(x, -65504.0f), 65504.0f);
-  hi = __float2half_rn(c);
+  uint16_t h;
+  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(x));
+  hi = __ushort_as_half(h);
   lo = __float2half_rn(x - __half2float(hi));
 }
-// Packed form: (x, y) -> half2 words {x in the low half}.  cvt.rn.satfinite.f16x2.f32 rounds to nearest and saturates at
-// +-65504, which is the clamp split_f16 applies; bit-identical to two split_f16 calls in 6 instructions.
+// Packed form: (x, y) -> half2 words {x in the low half}, in 6 instructions, with the same two conversions.
+// Bit-identical to two split_f16 calls for every non-NaN input (for NaN both give NaN halves, possibly with other payloads).
 __device__ __forceinline__ void split_f16x2(float x, float y, uint32_t& hi, uint32_t& lo) {
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(y), "f"(x));
   const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
   const float lx = x - hf.x, ly = y - hf.y;
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(ly), "f"(lx));
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(ly), "f"(lx));
 }
 // (x, y, z, w) -> four hi halves and four lo halves packed for 8-byte stores
 __device__ __forceinline__ void split_f16x4(const float4& v, uint2& hi, uint2& lo) {

@@ -67,6 +67,7 @@ def lib():
         _lib = C.CDLL(LIB_PATH)
         _lib.probe_gemm.argtypes = [C.POINTER(Gemm), C.c_int]
         _lib.probe_split.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float]
+        _lib.probe_pair_forms.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.probe_f16_weight_scale.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_float)]
         _lib.probe_attention.argtypes = [C.POINTER(Attn), C.c_int]
         _lib.probe_group_norm.argtypes = [C.POINTER(GnArgs), C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -85,6 +86,18 @@ def split(kind, x, scale=1.0):
     hi, lo = torch.empty_like(x, dtype=dt), torch.empty_like(x, dtype=dt)
     assert lib().probe_split(kind, x.data_ptr(), hi.data_ptr(), lo.data_ptr(), x.numel(), scale) == 0
     return hi, lo
+
+
+def pair_forms(x):
+    """The operand-pair helpers of rohm_b200/csrc/ptx.cuh on a 1-D fp32 device tensor (length a multiple of 4): fp16 halves
+    (hi, lo), each [3, n] with the rows from split_f16, split_f16x2 and split_f16x4, and the TF32 pair (hi, lo), each [n]."""
+    x = x.contiguous()
+    n = x.numel()
+    hi = torch.empty(3, n, dtype=torch.float16, device=x.device)
+    lo = torch.empty_like(hi)
+    t_hi, t_lo = torch.empty_like(x), torch.empty_like(x)
+    assert lib().probe_pair_forms(x.data_ptr(), n, hi.data_ptr(), lo.data_ptr(), t_hi.data_ptr(), t_lo.data_ptr()) == 0
+    return hi, lo, t_hi, t_lo
 
 
 def pair_value(hi, lo):

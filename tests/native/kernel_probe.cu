@@ -1,6 +1,6 @@
 // Test-only entry points into the GEMM, attention and GroupNorm kernels (rohm_b200/csrc/gemm.cu, attention.cu,
-// groupnorm.cu), driven from Python through ctypes by tests/kernel_probe.py and linked against the product's own objects of
-// those sources.  Every function takes plain structs / device pointers, builds the tensor maps itself with the library's own
+// groupnorm.cu) and the operand-pair helpers of ptx.cuh, driven from Python through ctypes by tests/kernel_probe.py and
+// linked against the product's own objects of those sources.  Every function takes plain structs / device pointers, builds the tensor maps itself with the library's own
 // helpers and returns 0, a cudaError_t (> 0) or -CUresult of a failed tensor-map encoding.  The launching probes run their
 // launch `reps` >= 1 times back to back on the default stream, set-up done once, so that tools can time them.  The product
 // library (librohm_b200.so, include/rohm_b200.h) exports none of this.
@@ -20,6 +20,29 @@ int repeat(int reps, F launch) {
   cudaError_t rc = cudaSuccess;
   for (int i = 0; i < reps && rc == cudaSuccess; ++i) rc = launch();
   return static_cast<int>(rc);
+}
+
+// Every operand-pair form of ptx.cuh applied to the same elements, four per thread: the scalar fp16 split, the packed fp16x2
+// and fp16x4 splits (element 2k in the low half of word k) and the TF32 pair the kernels write (hi = to_tf32(x), lo = x - hi).
+__global__ void pair_forms_kernel(const float4* __restrict__ x, int64_t n4, __half* __restrict__ s_hi,
+                                  __half* __restrict__ s_lo, uint32_t* __restrict__ x2_hi, uint32_t* __restrict__ x2_lo,
+                                  uint2* __restrict__ x4_hi, uint2* __restrict__ x4_lo, float4* __restrict__ t_hi,
+                                  float4* __restrict__ t_lo) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const float4 v = x[i];
+    ptx::split_f16(v.x, s_hi[4 * i], s_lo[4 * i]);
+    ptx::split_f16(v.y, s_hi[4 * i + 1], s_lo[4 * i + 1]);
+    ptx::split_f16(v.z, s_hi[4 * i + 2], s_lo[4 * i + 2]);
+    ptx::split_f16(v.w, s_hi[4 * i + 3], s_lo[4 * i + 3]);
+    ptx::split_f16x2(v.x, v.y, x2_hi[2 * i], x2_lo[2 * i]);
+    ptx::split_f16x2(v.z, v.w, x2_hi[2 * i + 1], x2_lo[2 * i + 1]);
+    ptx::split_f16x4(v, x4_hi[i], x4_lo[i]);
+    float4 h, l;
+    h.x = ptx::to_tf32(v.x), h.y = ptx::to_tf32(v.y), h.z = ptx::to_tf32(v.z), h.w = ptx::to_tf32(v.w);
+    l.x = v.x - h.x, l.y = v.y - h.y, l.z = v.z - h.z, l.w = v.w - h.w;
+    t_hi[i] = h, t_lo[i] = l;
+  }
 }
 
 }  // namespace
@@ -114,6 +137,22 @@ int probe_gemm(ProbeGemm* g, int reps) {
 int probe_split(int kind, const float* x, void* hi, void* lo, int64_t n, float scale) {
   if (kind == kKindF16) return static_cast<int>(launch_split_f16(x, hi, lo, n, scale, nullptr));
   return static_cast<int>(launch_split_tf32(x, static_cast<float*>(hi), static_cast<float*>(lo), n, nullptr));
+}
+
+// The operand-pair helpers of ptx.cuh on n fp32 values (n a multiple of 4, 16-byte aligned buffers): f16_hi / f16_lo
+// [3][n] halves from split_f16, split_f16x2 and split_f16x4 in that order, tf32_hi / tf32_lo [n] the TF32 pair.
+int probe_pair_forms(const float* x, int64_t n, void* f16_hi, void* f16_lo, float* tf32_hi, float* tf32_lo) {
+  if (n <= 0 || n % 4 != 0) return static_cast<int>(cudaErrorInvalidValue);
+  __half* h = static_cast<__half*>(f16_hi);
+  __half* l = static_cast<__half*>(f16_lo);
+  const int64_t n4 = n / 4;
+  const int threads = 256;
+  const int64_t blocks = (n4 + threads - 1) / threads < 4096 ? (n4 + threads - 1) / threads : 4096;
+  pair_forms_kernel<<<static_cast<unsigned>(blocks), threads>>>(
+      reinterpret_cast<const float4*>(x), n4, h, l, reinterpret_cast<uint32_t*>(h + n), reinterpret_cast<uint32_t*>(l + n),
+      reinterpret_cast<uint2*>(h + 2 * n), reinterpret_cast<uint2*>(l + 2 * n), reinterpret_cast<float4*>(tf32_hi),
+      reinterpret_cast<float4*>(tf32_lo));
+  return static_cast<int>(cudaGetLastError());
 }
 
 // The engines' weight scale for fp16 pairs (synchronous).

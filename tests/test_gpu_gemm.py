@@ -427,8 +427,8 @@ def _model_case(dev, a, w, block_n=128):
 
 @pytest.mark.parametrize("a_scale", [1.0, 1e-3, 300.0, 1.3e5])
 def test_f16_kernel_equals_the_cpu_model(dev, a_scale):
-    """Activations at 1e-3 (lo halves subnormal), 300 and 1.3e5 (the documented limit: above 65504 the hi half saturates and
-    the lo half carries the rest, so the reference is the model, not fp32 grade)."""
+    """Activations at 1e-3 (lo halves subnormal), 300 and up to 1.3e5 (inside the pair's range |x| < 131024: above 65504 the
+    hi half saturates and the lo half carries the rest, so the reference is the model, not fp32 grade)."""
     M, N, K = 256, 192, 512
     if a_scale > 65504.0:  # uniform up to the limit
         a = ((torch.rand(M, K, generator=_gen(300)) * 2.0 - 1.0) * a_scale).to(dev)

@@ -8,7 +8,7 @@ import re
 import numpy as np
 from scipy.special import erf
 
-from arith_model import gemm_f16x2, split_f16, weight_scale
+from arith_model import F16_MAX, F16_PAIR_LIMIT, gemm_f16x2, split_f16, split_tf32, weight_scale
 from helpers import ROOT
 
 f16, f32, f64 = np.float16, np.float32, np.float64
@@ -37,7 +37,96 @@ def test_pair_split_keeps_22_bits_and_degrades_gracefully():
     big = np.array([70000.0, -120000.0, 131000.0], dtype=f32)  # beyond fp16's largest finite value
     hi, lo = split_f16(big)
     assert np.all(np.isfinite(hi)) and np.all(np.isfinite(lo))
-    assert np.abs((hi + lo) - big).max() <= 64.0               # still 11+ bits; the documented range limit is 1.3e5
+    assert np.abs((hi + lo) - big).max() <= 64.0               # still 11+ bits; the pair's range ends at 131024
+
+
+def _f32_range(lo, hi):
+    """Every float32 in [lo, hi] (0 <= lo <= hi), in order."""
+    a, b = np.array([lo, hi], dtype=f32).view(np.uint32)
+    return np.arange(a, b + 1, dtype=np.uint32).view(f32)
+
+
+def test_f16_pair_is_finite_exactly_below_131024():
+    """hi saturates at 65504 and lo does not: every float32 with |x| < 65504 + 65520 has a finite pair, every larger one
+    (and +-inf) a pair of +-inf with the sign of x, never a plausible finite value.  NaN gives NaN in both halves."""
+    x = _f32_range(60000.0, 140000.0)
+    x = np.concatenate([x, -x, np.array([np.inf, -np.inf, 2e5, -2e5, 1e30, -1e30, 3.4028235e38], dtype=f32)])
+    hi, lo = split_f16(x)
+    pair = hi.astype(f64) + lo.astype(f64)
+    below = np.abs(x) < F16_PAIR_LIMIT
+    assert np.isfinite(pair[below]).all() and np.isfinite(hi).all()
+    assert (np.abs(hi[np.abs(x) >= F16_MAX]) == F16_MAX).all()
+    assert np.isinf(pair[~below]).all() and (np.sign(pair[~below]) == np.sign(x[~below])).all()
+    assert np.nextafter(f32(F16_PAIR_LIMIT), f32(0.0)) in x[below] and f32(F16_PAIR_LIMIT) in x[~below]
+    # the largest finite pair value: 65504 + 65504
+    assert pair[below].max() == 2 * F16_MAX and pair[below].min() == -2 * F16_MAX
+    # above the fp16 range the pair still carries 11 significant bits (lo = rn_f16(x - 65504))
+    mid = below & (np.abs(x) > F16_MAX)
+    assert (np.abs(pair[mid] - x[mid]) <= 2.0 ** -12 * np.abs(x[mid])).all()
+    hi, lo = split_f16(np.array([np.nan, -np.nan], dtype=f32))
+    assert np.isnan(hi).all() and np.isnan(lo).all()
+
+
+def test_f16_pair_error_is_2_22_relative_or_2_25_absolute():
+    """|hi + lo - x| <= max(2^-22 |x|, 2^-25) for every finite |x| <= 65504: 2 x 11 significant bits while lo is normal,
+    an absolute 2^-25 (half the smallest fp16 subnormal) once lo or hi goes subnormal.  Random bit patterns over the whole
+    fp32 range, the fp16 subnormal range 2^-24 .. 2^-14 densely, fp32 subnormals, and hi / lo rounding ties."""
+    rng = np.random.default_rng(7)
+    x = rng.integers(0, 2 ** 32, size=2 ** 20, dtype=np.uint64).astype(np.uint32).view(f32)
+    ties = np.array([1.0 + 2.0 ** -11, 1.0 + 3 * 2.0 ** -11, 1.0 + 2.0 ** -11 + 2.0 ** -22, 1.0 + 2.0 ** -11 + 3 * 2.0 ** -22,
+                     2048.0 + 1.0, 2048.0 + 3.0, 65504.0 - 16.0, 2.0 ** -14 + 2.0 ** -25, 2.0 ** -24 + 2.0 ** -25,
+                     2.0 ** -25, 3 * 2.0 ** -25], dtype=f32)
+    x = np.concatenate([x, _f32_range(2.0 ** -24, 2.0 ** -14)[::7], _f32_range(1e-45, 1.1754942e-38)[::4099], ties,
+                        np.array([0.0, 65504.0, 65519.996], dtype=f32)])
+    x = np.concatenate([x, -x])
+    x = x[np.isfinite(x) & (np.abs(x) <= F16_MAX)]
+    hi, lo = split_f16(x)
+    err = np.abs(hi.astype(f64) + lo.astype(f64) - x.astype(f64))
+    assert (err <= np.maximum(2.0 ** -22 * np.abs(x.astype(f64)), 2.0 ** -25)).all()
+    # hi is x rounded to fp16: |x - hi| <= half an ulp of hi, and lo never exceeds it
+    assert (np.abs(lo) <= np.maximum(2.0 ** -11 * np.abs(hi.astype(f64)), 2.0 ** -25)).all()
+
+
+def test_tf32_model_rounds_half_away_to_11_bits():
+    """split_tf32's bit operations against the same rounding done in float64: hi = x rounded half away from zero to a
+    multiple of 2^(max(e, -126) - 10), e = floor(log2 |x|) -- the 11 significant bits of TF32 in the normal range, the
+    fixed 2^-136 grid of the smallest binade for fp32 subnormals."""
+    rng = np.random.default_rng(8)
+    x = rng.integers(0, 2 ** 32, size=2 ** 20, dtype=np.uint64).astype(np.uint32).view(f32)
+    ties = np.array([1.0 + 2.0 ** -11, 1.0 + 3 * 2.0 ** -11, 2.0 - 2.0 ** -11, 2.0 ** -130 + 2.0 ** -137,
+                     2.0 ** -126 - 2.0 ** -137], dtype=f32)
+    x = np.concatenate([x, ties, -ties, _f32_range(1e-45, 1.1754942e-38)[::997]])
+    x = x[np.isfinite(x) & (np.abs(x) < 2.0 ** 127)]
+    hi, lo = split_tf32(x)
+    a = np.abs(x.astype(f64))
+    e = np.floor(np.log2(np.where(a > 0, a, 1.0)))
+    q = np.exp2(np.maximum(e, -126.0) - 10.0)
+    want = np.copysign(np.floor(a / q + 0.5) * q, x.astype(f64))
+    assert (hi.astype(f64) == want).all()
+    assert ((hi.view(np.uint32) & 0x1FFF) == 0).all()
+
+
+def test_tf32_pair_is_exact_below_the_top_binade():
+    """lo = x - hi is exact in fp32, so hi + lo == x for every finite x below 2^127 (fp32 subnormals included).  In the
+    top binade |x| >= 2^128 (1 - 2^-12) rounds to hi = +-inf and the pair is NaN (the kernels' behaviour, recorded in
+    DESIGN.md section 2); +-inf gives (+-inf, NaN), NaN a NaN lo."""
+    rng = np.random.default_rng(9)
+    x = rng.integers(0, 2 ** 32, size=2 ** 20, dtype=np.uint64).astype(np.uint32).view(f32)
+    x = np.concatenate([x, _f32_range(1e-45, 1.1754942e-38)[::997], np.array([0.0, -0.0], dtype=f32)])
+    x = x[np.isfinite(x) & (np.abs(x) < 2.0 ** 127)]
+    hi, lo = split_tf32(x)
+    assert (hi.astype(f64) + lo.astype(f64) == x.astype(f64)).all()
+    top = _f32_range(2.0 ** 127, 3.4028235e38)
+    hi, lo = split_tf32(top)
+    edge = f32(2.0 ** 128 * (1.0 - 2.0 ** -12))
+    fin = top < edge
+    assert (hi[fin].astype(f64) + lo[fin].astype(f64) == top[fin].astype(f64)).all()
+    assert np.isposinf(hi[~fin]).all() and np.isneginf(lo[~fin]).all() and edge in top[~fin]
+    hi, lo = split_tf32(np.array([np.inf, -np.inf, np.nan], dtype=f32))
+    assert hi[0] == np.inf and hi[1] == -np.inf and np.isnan(lo).all() and np.isnan(hi[2])
+    # NaNs are truncated, not rounded: a payload in the low 13 bits leaves hi = +-inf, but the pair is NaN either way
+    hi, lo = split_tf32(np.array([0x7F800001, 0xFF801FFF, 0x7F802000, 0x7FFFFFFF], dtype=np.uint32).view(f32))
+    assert hi[0] == np.inf and hi[1] == -np.inf and np.isnan(hi[2:]).all() and np.isnan(lo).all()
 
 
 def test_three_product_gemm_is_fp32_grade():
@@ -92,6 +181,8 @@ def test_branch_free_erf_gelu_constants_match_float64():
     ref = 0.5 * x64 * (1.0 + erf(x64 / math.sqrt(2.0)))
     assert np.abs(gelu - ref).max() < 3e-7  # tools/fit_gelu_erf.py reports 2.5e-7 (fp32 erff formulation: 4.5e-7)
     assert gelu[x > 8.0].tolist() == x64[x > 8.0].tolist() and np.all(np.abs(gelu[x < -8.0]) < 3e-8)  # saturation
+    # below -6.5 the tail |x| Phi(-|x|) is taken as |x| 2^Q(6.5): the slope of the extra error gemm.cu documents
+    assert 3.4e-11 < float(p[np.abs(x) >= clamp][0]) < 3.6e-11
 
 
 def test_split_k_partials_added_in_order_stay_fp32_grade():
