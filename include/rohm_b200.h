@@ -286,16 +286,19 @@ ROHM_API int rohm_body_create(rohm_ctx* ctx, const float* v_template, const floa
                               const int* parents_host, int num_verts, int64_t max_frames, int with_vertices,
                               int precision, rohm_body** out);
 ROHM_API void rohm_body_destroy(rohm_body* bd);
-/* 1 if rohm_body_forward computes the vertices with the fused blend-GEMM + skinning launch, 0 if the handle uses the
- * two-kernel path (no vertex support, TF32 precision, ROHM_B200_FUSED_LBS=0, or a body model whose 32-vertex tiles touch
- * more than 16 bones).  Introspection only. */
-ROHM_API int rohm_body_uses_fused_lbs(const rohm_body* bd);
+/* The skinning path rohm_body_forward takes for the vertices, chosen at rohm_body_create from the model's weights:
+ *   0  fused: blend GEMM with the skinning in its epilogue, one launch (fp16 pairs, every 32-vertex tile touches <= 16 bones);
+ *   1  sparse two-kernel: blend GEMM -> v_posed chunks -> skinning kernel (otherwise, every vertex has <= 8 bones);
+ *   2  dense two-kernel: blend GEMM -> v_posed chunks -> dense skinning kernel (some vertex has > 8 bones);
+ *  -1  the handle has no vertex support (or is NULL).
+ * ROHM_B200_FUSED_LBS=0 and ROHM_B200_DENSE_SKIN=1 move a handle to a later path.  Introspection only. */
+ROHM_API int rohm_body_skin_path(const rohm_body* bd);
 
 /* Row pitch, in floats, of the `vertices` buffers handed to rohm_body_forward / rohm_body_from_repr from now on:
  * frame n's vertices start at vertices + n * pitch.  0 (the default) = dense [N, V, 3] as smplx returns them
  * (reference: body_model output `.vertices`, test_amass_full.py:392-428).  A pitch that is a multiple of 4 floats (>= 3 V;
  * 16-byte-aligned buffer) lets the fused launch write the vertices with TMA bulk stores instead of 4-byte stores (3 V =
- * 31425 floats is not 16-byte divisible); only valid when rohm_body_uses_fused_lbs() is 1. */
+ * 31425 floats is not 16-byte divisible); only valid when rohm_body_skin_path() is 0. */
 ROHM_API int rohm_body_set_vertex_pitch(rohm_body* bd, int64_t pitch_floats);
 
 /* SMPLX.forward with jaw / eyes / hands / expression = 0 (exactly how RoHM calls it): global_orient [N,3], body_pose

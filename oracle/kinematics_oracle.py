@@ -129,9 +129,9 @@ def batch_rodrigues(aa):
     d = aa / angle
     cos, sin = torch.cos(angle)[:, None], torch.sin(angle)[:, None]
     rx, ry, rz = torch.split(d, 1, dim=1)
-    zeros = torch.zeros((n, 1), dtype=aa.dtype)
+    zeros = torch.zeros((n, 1), dtype=aa.dtype, device=aa.device)
     K = torch.cat([zeros, -rz, ry, rz, zeros, -rx, -ry, rx, zeros], dim=1).view(n, 3, 3)
-    ident = torch.eye(3, dtype=aa.dtype).unsqueeze(0)
+    ident = torch.eye(3, dtype=aa.dtype, device=aa.device).unsqueeze(0)
     return ident + sin * K + (1 - cos) * torch.bmm(K, K)
 
 
@@ -156,13 +156,15 @@ def batch_rigid_transform(rot_mats, joints, parents):
 def smplx_forward(model, global_orient, body_pose, betas, transl, return_verts=True, dtype=None):
     """SMPLX.forward as RoHM calls it (motion_representation.py:379-389): jaw/eyes/hands/expression are zeros.
     model: dict with v_template [V,3], shapedirs [V,3,20], posedirs [486, V*3], J_regressor [55,V],
-    lbs_weights [V,55], parents (list of 55).  Returns (joints [N,55,3], vertices [N,V,3] or None)."""
+    lbs_weights [V,55], parents (list of 55).  Returns (joints [N,55,3], vertices [N,V,3] or None).
+    Runs on the device of ``global_orient``; the model's tensors are moved there."""
     dtype = dtype or global_orient.dtype
-    m = {k: (v.to(dtype) if torch.is_tensor(v) else v) for k, v in model.items()}
+    dev = global_orient.device
+    m = {k: (v.to(device=dev, dtype=dtype) if torch.is_tensor(v) else v) for k, v in model.items()}
     N = global_orient.shape[0]
-    full_pose = torch.cat([global_orient.reshape(N, 1, 3), body_pose.reshape(N, 21, 3),
-                           torch.zeros(N, 33, 3, dtype=dtype)], dim=1).to(dtype)
-    shape_comps = torch.cat([betas.to(dtype), torch.zeros(N, 10, dtype=dtype)], dim=-1)
+    full_pose = torch.cat([global_orient.reshape(N, 1, 3).to(dtype), body_pose.reshape(N, 21, 3).to(dtype),
+                           torch.zeros(N, 33, 3, dtype=dtype, device=dev)], dim=1)
+    shape_comps = torch.cat([betas.to(dtype), torch.zeros(N, 10, dtype=dtype, device=dev)], dim=-1)
     v_shaped = m["v_template"] + torch.einsum('bl,mkl->bmk', shape_comps, m["shapedirs"])
     J = torch.einsum('bik,ji->bjk', v_shaped, m["J_regressor"])
     R = batch_rodrigues(full_pose.reshape(-1, 3)).view(N, 55, 3, 3)
@@ -170,11 +172,11 @@ def smplx_forward(model, global_orient, body_pose, betas, transl, return_verts=T
     joints = posed + transl.to(dtype).unsqueeze(1)
     if not return_verts:
         return joints, None
-    ident = torch.eye(3, dtype=dtype)
+    ident = torch.eye(3, dtype=dtype, device=dev)
     pose_feature = (R[:, 1:] - ident).reshape(N, -1)
     v_posed = v_shaped + torch.matmul(pose_feature, m["posedirs"]).view(N, -1, 3)
     Tm = torch.matmul(m["lbs_weights"], A.reshape(N, 55, 16)).view(N, -1, 4, 4)
-    vh = torch.cat([v_posed, torch.ones(N, v_posed.shape[1], 1, dtype=dtype)], dim=2)
+    vh = torch.cat([v_posed, torch.ones(N, v_posed.shape[1], 1, dtype=dtype, device=dev)], dim=2)
     verts = torch.matmul(Tm, vh.unsqueeze(-1))[:, :, :3, 0]
     return joints, verts + transl.to(dtype).unsqueeze(1)
 

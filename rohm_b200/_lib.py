@@ -15,6 +15,7 @@ ROHM_OK = 0
 PRECISION_TF32X3 = 3
 PRECISION_F16X2 = 2
 PRECISION_TF32 = 1
+SKIN_FUSED, SKIN_SPARSE, SKIN_DENSE = 0, 1, 2  # rohm_body_skin_path
 DDPM_COEFS = 8
 
 
@@ -74,7 +75,7 @@ SIGNATURES = {
     "rohm_trajnet_launches_per_forward": (_i, [_p]),
     "rohm_body_create": (_i, [_p, _p, _p, _i, _p, _p, _p, C.POINTER(C.c_int), _i, _i64, _i, _i, C.POINTER(_p)]),
     "rohm_body_destroy": (None, [_p]),
-    "rohm_body_uses_fused_lbs": (_i, [_p]),
+    "rohm_body_skin_path": (_i, [_p]),
     "rohm_body_set_vertex_pitch": (_i, [_p, _i64]),
     "rohm_body_forward": (_i, [_p, _p, _p, _p, _p, _i64, _p, _i, _p, _p]),
     "rohm_body_from_repr": (_i, [_p, _p, _i, _p, _p, _i, _i, _p, _p, _i64, _p, _i, _p, _p]),

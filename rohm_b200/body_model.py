@@ -58,8 +58,9 @@ class BodyKernels:
         # The fused blend + skinning launch writes the vertices with TMA bulk stores when every frame's row starts on a 16-byte
         # boundary: 3 V = 31425 floats does not, so the buffer gets 3 pad floats per frame and the caller a strided [N, V, 3]
         # view of it (same values, `.contiguous()` gives smplx's dense layout).  ROHM_B200_LBS_TMA_STORE=0: dense rows, 4-byte stores.
+        self.skin_path = self.lib.rohm_body_skin_path(handle)  # _lib.SKIN_FUSED / SKIN_SPARSE / SKIN_DENSE, -1 without vertices
         self.vertex_pitch = 0
-        if with_vertices and self.lib.rohm_body_uses_fused_lbs(handle) and os.environ.get("ROHM_B200_LBS_TMA_STORE", "1") != "0":
+        if self.skin_path == _lib.SKIN_FUSED and os.environ.get("ROHM_B200_LBS_TMA_STORE", "1") != "0":
             pitch = -(-self.V * 3 // 4) * 4
             _lib.check(self.lib.rohm_body_set_vertex_pitch(handle, pitch), self.ctx)
             self.vertex_pitch = pitch

@@ -40,7 +40,6 @@ constexpr int kBetas = 10;
 constexpr int kPoseFeat = 189;  // (22 - 1) * 9 non-zero pose-corrective features (hands / jaw / eyes are identity)
 constexpr int kBlendK = 256;    // 189 pose features + 10 betas + 1 (template), zero-padded to whole K blocks (64 fp16 / 32 TF32)
 constexpr int kMaxBones = 8;    // compressed skinning weights per vertex
-constexpr int64_t kLbsChunk = 384;  // frames per (blend GEMM -> skinning) chunk: 384 x 31488 x 4 B = 48 MB of v_posed
 
 __constant__ int c_parents[kJ];
 
@@ -734,8 +733,10 @@ extern "C" int rohm_body_create(rohm_ctx* ctx, const float* v_template, const fl
     bd->a_frame_stride = round_up(F, 128);  // whole 128-frame row tiles: the epilogue's bulk copies never leave a row
     bd->A = bd->pool.floats(bd->a_frame_stride * kJ * 12);
     bd->feat_h = bd->pool.floats(F * kBlendK), bd->feat_l = bd->pool.floats(F * kBlendK);
-    // two-kernel path: v_posed lives for one chunk of frames at a time (the blend GEMM writes it, the skinning kernel reads
-    // it back); a chunk small enough for the 50 MB L2 (ROHM_B200_LBS_CHUNK=384: 48 MB) keeps that round trip out of HBM
+    // two-kernel path: v_posed lives for one chunk of bd->chunk frames at a time (the blend GEMM writes it, the skinning
+    // kernel reads it back), in two buffers so that the next chunk's GEMM can run beside this chunk's skinning.  The default
+    // chunk of 4608 frames is 4608 x 31 488 x 4 B = 580 MB per buffer; a chunk small enough for the 50 MB L2 (384 frames:
+    // 48 MB) would keep the round trip out of HBM at the price of more, smaller launches
     if (const char* env = getenv("ROHM_B200_LBS_CHUNK")) {  // developer switch: frames per chunk (multiple of 128)
       const long v = atol(env);
       if (v >= 128 && v % 128 == 0) bd->chunk = v;
@@ -889,7 +890,10 @@ extern "C" int rohm_body_create(rohm_ctx* ctx, const float* v_template, const fl
 
 extern "C" void rohm_body_destroy(rohm_body* bd) { delete bd; }
 
-extern "C" int rohm_body_uses_fused_lbs(const rohm_body* bd) { return bd != nullptr && bd->fused_lbs ? 1 : 0; }
+extern "C" int rohm_body_skin_path(const rohm_body* bd) {
+  if (bd == nullptr || bd->vposed == nullptr) return -1;
+  return bd->fused_lbs ? 0 : (bd->sparse_ok ? 1 : 2);
+}
 
 extern "C" int rohm_body_set_vertex_pitch(rohm_body* bd, int64_t pitch_floats) {
   if (bd == nullptr) return ROHM_ERR_INVALID;
@@ -944,8 +948,9 @@ extern "C" int rohm_body_forward(rohm_body* bd, const float* global_orient, cons
     }
     ROHM_CUDA(ctx, launch_gemm(g, static_cast<int>(N), bd->blend.Np, 96, bd->passes, st, false, bd->kind));
   } else if (verts) {
-    // Pipeline over chunks of kLbsChunk frames: blend GEMM of chunk i on the caller's stream into v_posed buffer i % 2,
-    // skinning of chunk i on a second stream (HBM-bound next to the tensor-bound GEMM of chunk i + 1).
+    // Pipeline over chunks of bd->chunk frames (4608 by default, ROHM_B200_LBS_CHUNK): blend GEMM of chunk i on the caller's
+    // stream into v_posed buffer i % 2, skinning of chunk i on a second stream (HBM-bound next to the tensor-bound GEMM of
+    // chunk i + 1).  One chunk, or ROHM_B200_LBS_OVERLAP=0, runs everything on the caller's stream with one buffer.
     const int vblocks = (bd->V + 255) / 256;
     int occ = 0;  // resident CTAs per SM (registers / the 42 KB of shared memory decide)
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, skin_kernel, 256, 0) != cudaSuccess || occ < 1) occ = 3;

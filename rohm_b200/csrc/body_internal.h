@@ -38,7 +38,7 @@ struct rohm_body {
   float* skin_w = nullptr;
   // full LBS pipeline: v_posed double buffer (one chunk each), second stream for the skinning kernels
   int64_t vposed_stride = 0;
-  // frames per chunk (ROHM_B200_LBS_CHUNK; the default is one pass over the batch)
+  // frames per two-kernel chunk (ROHM_B200_LBS_CHUNK, a multiple of 128)
   int64_t chunk = 4608;
   CUtensorMap st_out_b{};
   cudaStream_t skin_stream = nullptr;

@@ -13,7 +13,7 @@ import torch
 from helpers import ROOT, TOL, golden
 from oracle import glue_oracle as go
 from oracle import kinematics_oracle as ko
-from rohm_b200 import glue, synthetic
+from rohm_b200 import _lib, glue, synthetic
 from rohm_b200.body_model import BodyModel, kernels_for
 from rohm_b200.motion_representation import recover_from_repr_smpl, split_repr
 from rohm_b200.posenet import PoseNet
@@ -299,10 +299,10 @@ def test_eval_loss_dictionaries_match_reference(body, cuda_device):
     _check_losses(got, g["traj_loss_names"], g["traj_loss_values"])
 
 
-def test_fused_lbs_falls_back_when_a_tile_touches_too_many_bones(cuda_device):
+def test_skin_path_falls_back_to_sparse_when_a_tile_touches_too_many_bones(cuda_device):
     """The fused blend + skinning launch needs at most 16 distinct bones per 32 consecutive vertices.  A body model whose
-    vertices are in random order breaks that: the handle must choose the two-kernel path by itself and stay correct; the
-    body-part-ordered model takes the fused path."""
+    vertices are in random order breaks that: rohm_body_skin_path must report the sparse two-kernel path, chosen by the handle
+    itself, and the vertices stay correct; the body-part-ordered model takes the fused path."""
     t = synthetic.smplx_like_model(0)
     V = t['v_template'].shape[0]
     perm = torch.randperm(V, generator=torch.Generator().manual_seed(5))
@@ -314,10 +314,10 @@ def test_fused_lbs_falls_back_when_a_tile_touches_too_many_bones(cuda_device):
     N = 40
     gor, bp = 0.3 * torch.randn(N, 3, generator=g), 0.3 * torch.randn(N, 63, generator=g)
     be, tr = torch.randn(N, 10, generator=g), torch.randn(N, 3, generator=g)
-    for tensors, fused in ((shuffled, 0), (t, 1)):
+    for tensors, path in ((shuffled, _lib.SKIN_SPARSE), (t, _lib.SKIN_FUSED)):
         bm = BodyModel(tensors).to(cuda_device)
         out = bm(transl=tr.to(cuda_device), global_orient=gor.to(cuda_device), body_pose=bp.to(cuda_device), betas=be.to(cuda_device))
         k = kernels_for(bm, cuda_device, N, with_vertices=True)
-        assert k.lib.rohm_body_uses_fused_lbs(k.handle) == fused
+        assert k.lib.rohm_body_skin_path(k.handle) == path == k.skin_path
         _, v = ko.smplx_forward(tensors, gor, bp, be, tr, return_verts=True, dtype=torch.float64)
         assert float((out.vertices.cpu().double() - v).abs().max()) < 5e-5
