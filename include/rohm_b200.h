@@ -470,6 +470,43 @@ ROHM_API int rohm_window_to_world(rohm_ctx* ctx, const float* joints, const int*
                                   const float* transf, int W, int clip_len, const int* rec_off, int64_t total_frames,
                                   float* world, unsigned char* covered, void* stream);
 
+/* The video loader's windows (dataloader_video.py, DataloaderVideo for PROX and EgoBody): the recordings' per-frame
+ * SMPL-X fits and their FK joints are in each recording's camera frame; cam [R,12] holds rows of [A | b], the camera ->
+ * z-up scene map (PROX: cam2world; EgoBody, whose scene is y-up: Q cam2world with Q = Rx(+90 deg), (x, y, z) -> (x, -z,
+ * y), which turns cano_seq_smplx_egobody into cano_seq_smplx, DESIGN §4.14), and y_up = 1 for EgoBody.  floor [R]: a preset
+ * floor height per recording, 0 for the window minimum (the reference's `if preset_floor_height:`).  Windows are cut as
+ * rohm_window_encode cuts them, and repr_traj / repr_pose are computed by its row code.  transf [W,4,4] is the
+ * reference's scene -> canonical transf_matrix (T_z Q for y_up).  Further outputs per window frame, including the last,
+ * window-major: cano_joints and scene_joints [W*clip_len,22,3] (canonical; scene frame, y up for y_up) and cano_params
+ * [W*clip_len,79] (the canonical SMPL-X parameters, rows as rohm_window_param_noise writes them). */
+ROHM_API int rohm_window_encode_video(rohm_ctx* ctx, const float* global_orient, const float* transl, const float* betas,
+                                      const float* body_pose, const float* joints, const int* rec_off_host,
+                                      const int* rec_off, int R, int clip_len, int overlap, const float* cam,
+                                      const float* floor, int y_up, const float* traj_mean, const float* traj_std,
+                                      const float* pose_mean, const float* pose_std, int max_windows, int* n_windows,
+                                      int* win_rec, int* win_start, float* transf, float* repr_traj, float* repr_pose,
+                                      float* cano_joints, float* scene_joints, float* cano_params, void* stream);
+
+/* The video loader's 2-D inputs of W windows (dataloader_video.py:441-484): keypoints25 [N,25,3] (OpenPose BODY_25 x, y,
+ * confidence per packed recording frame, zeros where no person was found) and depth_mask [N,25] (mask_joint.npy, SMPL-X
+ * joint order).  conf64 [R] (bytes, device): 1 where the recording's keypoint array is float64 in the loader (some frame
+ * had no person), so that conf > 0.2 and PROX's flip are evaluated in float64; 0 for float32.  undistort = 1 (PROX):
+ * x -> 1919 - x, cv2.undistortPoints with P = camera_mtx (camera_mtx [R,3,3] and dist [R,14], zero-padded distortion,
+ * float64; 5 fixed iterations), flipped back.  Outputs, window-major: keypoints [W*clip_len,22,3] (SMPL topology),
+ * mask_joint_vis [W*clip_len,22] and mask_vec_vis [W*clip_len,294]. */
+ROHM_API int rohm_window_keypoints(rohm_ctx* ctx, const float* keypoints25, const float* depth_mask,
+                                   const unsigned char* conf64, const double* camera_mtx, const double* dist,
+                                   int undistort, const int* rec_off, const int* win_rec, const int* win_start, int W,
+                                   int clip_len, float* keypoints, float* mask_joint_vis, float* mask_vec_vis,
+                                   void* stream);
+
+/* joints [N,22,3] (packed recording frames) mapped by their recording's cam [R,12] (rows of [A | b]) and gathered into
+ * the W windows' frames: out [W*clip_len,22,3] (EgoBody's ground-truth joints in the scene frame, dataloader_video.py
+ * :312-314). */
+ROHM_API int rohm_window_scene_joints(rohm_ctx* ctx, const float* joints, const float* cam, const int* rec_off,
+                                      const int* win_rec, const int* win_start, int W, int clip_len, float* out,
+                                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -94,6 +94,10 @@ SIGNATURES = {
     "rohm_window_param_noise": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p]),
     "rohm_window_encode_canonical": (_i, [_p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p, _p]),
     "rohm_window_to_world": (_i, [_p, _p, _p, _p, _p, _i, _i, _p, _i64, _p, _p, _p]),
+    "rohm_window_encode_video": (_i, [_p, _p, _p, _p, _p, _p, C.POINTER(_i), _p, _i, _i, _i, _p, _p, _i, _p, _p, _p, _p,
+                                      _i, C.POINTER(_i), _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "rohm_window_keypoints": (_i, [_p, _p, _p, _p, _p, _p, _i, _p, _p, _p, _i, _i, _p, _p, _p, _p]),
+    "rohm_window_scene_joints": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p]),
 }
 
 _lock = threading.Lock()

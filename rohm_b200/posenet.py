@@ -435,19 +435,49 @@ class PoseNet(nn.Module):
     def _camera_affine(self, batch, device):
         """[B, 3, 4] canonical -> camera map of guide_2d_projection_with_smpl (reference posenet.py:285-297):
         p_cam = inv(cam_R) (inv(transf_matrix) p_cano - cam_t).  Per-clip 4x4 inverses: host-sized work, cached per
-        transf_matrix tensor so the guided steps of one loop compute it once."""
+        transf_matrix tensor so the guided steps of one loop compute it once.
+
+        With batch['cam2world'] [B,4,4] (windows.encode_video puts it there), clip b's camera is cam2world[b] instead of
+        the dataset's cam_R / cam_t, so one batch can hold windows of recordings with different cameras.  A batch of one
+        camera takes the dataset-camera path's operations (the same bits as that camera in the dataset); a batch of
+        several computes each clip's affine as that clip alone would, so each clip gets the bits of its own run."""
         tm = batch['transf_matrix']
+        c2w = batch.get('cam2world')
+        c2w_version = None if c2w is None else c2w._version
         cache = getattr(self, "_cam_cache", None)
-        if cache is not None and cache[0] is tm and cache[1] == tm._version:
-            return cache[2]
+        if cache is not None and cache[0] is tm and cache[1] == tm._version and cache[2] is c2w and \
+                cache[3] == c2w_version:
+            return cache[4]
         cano2scene = torch.linalg.inv(tm.to(device=device, dtype=torch.float32))  # [B, 4, 4]
-        cam_R = torch.as_tensor(self.dataset.cam_R, dtype=torch.float32, device=device).reshape(3, 3)
-        cam_t = torch.as_tensor(self.dataset.cam_t, dtype=torch.float32, device=device).reshape(3)
-        Rinv = torch.linalg.inv(cam_R)
-        M = Rinv @ cano2scene[:, 0:3, 0:3]                                   # [B, 3, 3]
-        m = (Rinv @ (cano2scene[:, 0:3, 3] - cam_t).unsqueeze(-1))           # [B, 3, 1]
-        aff = torch.cat([M, m], dim=-1).contiguous()
-        self._cam_cache = (tm, tm._version, aff)
+
+        def affine(cam_R, cam_t, c2s):
+            Rinv = torch.linalg.inv(cam_R)
+            M = Rinv @ c2s[:, 0:3, 0:3]                                       # [B, 3, 3]
+            m = (Rinv @ (c2s[:, 0:3, 3] - cam_t).unsqueeze(-1))               # [B, 3, 1]
+            return torch.cat([M, m], dim=-1)
+
+        if c2w is None:
+            cam_R = torch.as_tensor(self.dataset.cam_R, dtype=torch.float32, device=device).reshape(3, 3)
+            cam_t = torch.as_tensor(self.dataset.cam_t, dtype=torch.float32, device=device).reshape(3)
+            aff = affine(cam_R, cam_t, cano2scene).contiguous()
+        else:
+            B = cano2scene.shape[0]
+            cams = c2w.to(device=device, dtype=torch.float32)
+            if cams.shape != (B, 4, 4):
+                raise RohmB200Error(f"guide_2d_projection_with_smpl: batch['cam2world'] must be [{B}, 4, 4], got "
+                                    f"{tuple(cams.shape)}")
+            # one camera (compared by bit pattern, so -0.0 and 0.0 differ; a host sync per new camera tensor, the affine
+            # is cached for the loop's guided steps): the dataset-camera path's batched operations, and its bits
+            rows16 = cams.reshape(B, 16).view(torch.int32).cpu()
+            if bool((rows16 == rows16[0]).all()):
+                aff = affine(cams[0, 0:3, 0:3], cams[0, 0:3, 3], cano2scene).contiguous()
+            else:
+                # several cameras: each clip by itself, with the operations and shapes of that clip run alone with its
+                # camera as dataset.cam_R / cam_t (batched inverses and matrix products may round per batch size)
+                tmd = tm.to(device=device, dtype=torch.float32)
+                aff = torch.cat([affine(cams[b, 0:3, 0:3], cams[b, 0:3, 3], torch.linalg.inv(tmd[b:b + 1]))
+                                 for b in range(B)]).contiguous()
+        self._cam_cache = (tm, tm._version, c2w, c2w_version, aff)
         return aff
 
     def guide_2d_projection_with_smpl(self, batch, out, denoise_t, compute_grad='x_t'):

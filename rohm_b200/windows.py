@@ -7,6 +7,12 @@ builds them without input noise (dataloader_amass.py:319-341).  ``to_recordings`
 world frame of its recording (the inverse of transf_matrix, eval_prox_egobody.py:177-182).  Both are one kernel launch
 (rohm_window_encode / rohm_window_to_world); tensors stay on the GPU.
 
+``encode_video`` builds the batches of the video loader (DataloaderVideo, PROX and EgoBody) from recordings whose
+per-frame fits are in each recording's camera frame: the camera instance of the encoder (rohm_window_encode_video), the
+keypoints and visibility masks (rohm_window_keypoints) and, for EgoBody, the ground-truth joints in the scene frame
+(rohm_window_scene_joints).  Each window's ``cam2world`` rides along in test_batch_pose, so PoseNet's projection guidance
+can take a batch of windows of recordings with different cameras.
+
 ``encode(..., noise=InputNoise...)`` adds the reference's input noise (dataloader_amass.py:156-227 with sep_noise False,
 the paper's setup): noise on each window's canonical SMPL-X parameters (rohm_window_param_noise), FK of the noisy
 parameters with the body model, and their representation without re-canonicalisation (rohm_window_encode_canonical).
@@ -295,6 +301,166 @@ def _encode(p, joints, lengths, pose_dataset, traj_dataset, clip_len, overlap, n
     test_batch_pose = {'motion_repr_clean': rp, 'motion_repr_noisy': npose, 'noisy_joints': noisy_joints.clone()}
     win.noisy_params = noisy.reshape(W, clip_len, NOISY_WIDTH)
     return test_batch_traj, test_batch_pose, win
+
+
+VIDEO_DATASETS = ('prox', 'egobody')
+DIST_LENGTHS = (4, 5, 8)  # OpenCV distortion vectors the video loaders' Color.json carry: k1 k2 p1 p2 [k3 [k4 k5 k6]]
+# Q = Rx(+90 deg): (x, y, z) -> (x, -z, y), EgoBody's y-up scene frame to the z-up frame cano_seq_smplx takes (DESIGN §4.14)
+Y_UP_TO_Z_UP = np.array([[1.0, 0.0, 0.0], [0.0, 0.0, -1.0], [0.0, 1.0, 0.0]])
+
+
+def _host64(v, name, shape):
+    """A small per-recording array as finite float64 numpy of `shape` (None entries: any size), refused otherwise."""
+    a = v.detach().cpu().double().numpy() if torch.is_tensor(v) else np.asarray(v, dtype=np.float64)
+    if a.ndim != len(shape) or any(w is not None and a.shape[i] != w for i, w in enumerate(shape)):
+        want = ", ".join("n" if w is None else str(w) for w in shape)
+        raise RohmB200Error(f"windows.encode_video: {name} must be [{want}], got {tuple(a.shape)}")
+    if not np.isfinite(a).all():
+        raise RohmB200Error(f"windows.encode_video: {name} holds a non-finite value")
+    return a
+
+
+def encode_video(body_model, params, lengths, dataset, cam2world, focal_length, camera_center, camera_mtx, dist,
+                 keypoints, depth_mask, pose_dataset, traj_dataset, floor=None, clip_len=145, overlap=2,
+                 keypoints_float64=None, gt_params=None, gt_body_model=None, master2world=None, noise=None):
+    """The batches of the reference's DataloaderVideo (dataloader_video.py) for R recordings packed frame after frame.
+
+    params: the initial SMPL-X fits in each recording's camera frame, as the per-frame 000.pkl holds them (CUDA tensors
+    global_orient [N,3], transl [N,3], betas [N,10], body_pose [N,63]); lengths: frames per recording; dataset: 'prox'
+    (z-up scene) or 'egobody' (y-up scene).  Per recording (tensors or arrays, any device): cam2world [R,4,4] (for an
+    EgoBody sub view, master2world @ trans_subtomain as the loader composes it), the colour camera focal_length [R,2],
+    camera_center [R,2], camera_mtx [R,3,3] and dist [R,n], n in (4, 5, 8), and floor [R] (None: every window takes its
+    own minimum; a preset height, where 0.0 also takes the window minimum, as the reference's ``if
+    preset_floor_height:`` does).  Per frame (CUDA): keypoints [N,25,3] (OpenPose BODY_25 from the json, zeros where no
+    person was found) and depth_mask [N,25] (mask_joint.npy).  keypoints_float64 [R] bools: the recording's keypoint
+    array is float64 in the loader (a frame had no person, np.zeros is float64), which sets the precision of conf > 0.2;
+    None derives it from the frames whose keypoints are all zero.  For EgoBody with ground truth: gt_params (fits in the
+    master camera frame, packed like params), gt_body_model and master2world [R,4,4].
+
+    Returns (test_batch_traj, test_batch_pose, windows): every key DataloaderVideo.__getitem__ emits for task 'traj' and
+    'pose' as CUDA float32 tensors with a leading W, except frame_name (host strings: windows.recording / start index the
+    caller's own name lists); test_batch_pose also carries cam2world [W,4,4], the camera of each window's recording, which
+    PoseNet's projection guidance uses in place of dataset.cam_R / cam_t.  windows.transf is the reference's scene ->
+    canonical transf_matrix, so ``to_recordings`` returns scene coordinates (y up for EgoBody).  The video loader adds no
+    input noise: passing ``noise`` is refused."""
+    if noise is not None:
+        raise RohmB200Error("windows.encode_video: the video loader adds no input noise; noise must be None")
+    if dataset not in VIDEO_DATASETS:
+        raise RohmB200Error(f"windows.encode_video: dataset must be one of {VIDEO_DATASETS}, got {dataset!r}")
+    _check_shape(clip_len, overlap)
+    lengths = tuple(int(n) for n in lengths)
+    if not lengths or min(lengths) < 0:
+        raise RohmB200Error(f"windows.encode_video: lengths must be one frame count >= 0 per recording, got {lengths}")
+    R, N = len(lengths), sum(lengths)
+    c2w = _host64(cam2world, "cam2world", (R, 4, 4))
+    f = _host64(focal_length, "focal_length", (R, 2))
+    c = _host64(camera_center, "camera_center", (R, 2))
+    K = _host64(camera_mtx, "camera_mtx", (R, 3, 3))
+    k = _host64(dist, "dist", (R, None))
+    if k.shape[1] not in DIST_LENGTHS:
+        raise RohmB200Error(f"windows.encode_video: dist must hold {DIST_LENGTHS} coefficients per recording, got "
+                            f"{k.shape[1]}")
+    fl = np.zeros(R) if floor is None else _host64(floor, "floor", (R,))
+    for name, t, shape in (("keypoints", keypoints, (N, 25, 3)), ("depth_mask", depth_mask, (N, 25))):
+        if not hasattr(t, "shape") or tuple(t.shape) != shape:
+            raise RohmB200Error(f"windows.encode_video: {name} must be {list(shape)}, got "
+                                f"{tuple(getattr(t, 'shape', ()))}")
+    if keypoints_float64 is not None and len(keypoints_float64) != R:
+        raise RohmB200Error(f"windows.encode_video: keypoints_float64 must hold one flag per recording ({R}), got "
+                            f"{len(keypoints_float64)}")
+    with_gt = gt_params is not None
+    if with_gt != (gt_body_model is not None) or with_gt != (master2world is not None):
+        raise RohmB200Error("windows.encode_video: the ground truth needs gt_params, gt_body_model and master2world "
+                            "together")
+    if with_gt and dataset != 'egobody':
+        raise RohmB200Error("windows.encode_video: ground-truth fits are an EgoBody input")
+    m2w = _host64(master2world, "master2world", (R, 4, 4)) if with_gt else None
+    p, _ = _packed_params(params, lengths, clip_len, overlap)
+    dev = p['transl'].device
+    kp = glue._f32c(keypoints, "windows.encode_video: keypoints")
+    dm = glue._f32c(depth_mask, "windows.encode_video: depth_mask")
+    gp = _packed_params(gt_params, lengths, clip_len, overlap)[0] if with_gt else None
+    for name, t in (("keypoints", kp), ("depth_mask", dm)) + ((("gt_params", gp['transl']),) if with_gt else ()):
+        if t.device != dev:
+            raise RohmB200Error(f"windows.encode_video: {name} lives on {t.device}, the parameters on {dev}")
+    tm, ts = glue.stats_on(traj_dataset, dev)
+    pm, ps = glue.stats_on(pose_dataset, dev)
+    if any(t.numel() != glue.BODY_FEAT_DIM for t in (tm, ts, pm, ps)):
+        raise RohmB200Error("windows.encode_video: the datasets' Mean / Std must have 294 entries")
+
+    # the recording's camera -> z-up scene map, in float32 as the loader applies cam2world.float(); for EgoBody Q is a
+    # permutation with one sign, so Q A is exact
+    c2w32 = c2w.astype(np.float32)
+    A = c2w32[:, 0:3, :]
+    if dataset == 'egobody':
+        A = np.stack([A[:, 0], -A[:, 2], A[:, 1]], axis=1)
+    cam = torch.from_numpy(np.ascontiguousarray(A.reshape(R, 12))).to(dev)
+    floors = torch.from_numpy(fl.astype(np.float32)).to(dev)
+    W, L, T1 = len(window_table(lengths, clip_len, overlap)), clip_len, clip_len - 1
+    off = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int32)
+    offsets = torch.from_numpy(off).to(dev)
+    rec = torch.empty(W, dtype=torch.int32, device=dev)
+    start = torch.empty(W, dtype=torch.int32, device=dev)
+    transf = torch.empty(W, 4, 4, device=dev)
+    rt = torch.empty(W, T1, glue.BODY_FEAT_DIM, device=dev)
+    rp = torch.empty(W, T1, glue.BODY_FEAT_DIM, device=dev)
+    cano_joints = torch.empty(W, L, 22, 3, device=dev)
+    scene_joints = torch.empty(W, L, 22, 3, device=dev)
+    cano_params = torch.empty(W, L, NOISY_WIDTH, device=dev)
+    kp_out = torch.empty(W, L, 22, 3, device=dev)
+    vis = torch.empty(W, L, 22, device=dev)
+    vec = torch.empty(W, L, glue.BODY_FEAT_DIM, device=dev)
+    gt_scene = torch.empty(W, L, 22, 3, device=dev) if with_gt else None
+    if W > 0:
+        lib, ctx = _lib.load(), _lib.ctx(dev.index)
+        joints = body_model(transl=p['transl'], global_orient=p['global_orient'], body_pose=p['body_pose'],
+                            betas=p['betas'], return_verts=False).joints[:, 0:22].contiguous()
+        n = C.c_int(0)
+        rc = lib.rohm_window_encode_video(ctx, glue._p(p['global_orient']), glue._p(p['transl']), glue._p(p['betas']),
+                                          glue._p(p['body_pose']), glue._p(joints), (C.c_int * len(off))(*off.tolist()),
+                                          glue._p(offsets), R, clip_len, overlap, glue._p(cam), glue._p(floors),
+                                          int(dataset == 'egobody'), glue._p(tm), glue._p(ts), glue._p(pm), glue._p(ps),
+                                          W, C.byref(n), glue._p(rec), glue._p(start), glue._p(transf), glue._p(rt),
+                                          glue._p(rp), glue._p(cano_joints), glue._p(scene_joints),
+                                          glue._p(cano_params), glue._stream(dev))
+        _lib.check(rc, ctx)
+        if n.value != W:
+            raise RohmB200Error(f"windows.encode_video: the library cut {n.value} windows, the window rule {W}")
+        if keypoints_float64 is None:
+            empty = (kp.reshape(N, 75) == 0).all(dim=1).cpu().numpy()
+            conf64 = torch.tensor([int(empty[off[r]:off[r + 1]].any()) for r in range(R)], dtype=torch.uint8, device=dev)
+        else:
+            conf64 = torch.tensor([1 if b else 0 for b in keypoints_float64], dtype=torch.uint8, device=dev)
+        kpad = np.zeros((R, 14))
+        kpad[:, :k.shape[1]] = k
+        Kd = torch.from_numpy(np.ascontiguousarray(K.reshape(R, 9))).to(dev)
+        kd = torch.from_numpy(kpad).to(dev)
+        rc = lib.rohm_window_keypoints(ctx, glue._p(kp), glue._p(dm), glue._p(conf64), glue._p(Kd), glue._p(kd),
+                                       int(dataset == 'prox'), glue._p(offsets), glue._p(rec), glue._p(start), W, L,
+                                       glue._p(kp_out), glue._p(vis), glue._p(vec), glue._stream(dev))
+        _lib.check(rc, ctx)
+        if with_gt:
+            gj = gt_body_model(transl=gp['transl'], global_orient=gp['global_orient'], body_pose=gp['body_pose'],
+                               betas=gp['betas'], return_verts=False).joints[:, 0:22].contiguous()
+            mcam = torch.from_numpy(np.ascontiguousarray(m2w.astype(np.float32)[:, 0:3, :].reshape(R, 12))).to(dev)
+            rc = lib.rohm_window_scene_joints(ctx, glue._p(gj), glue._p(mcam), glue._p(offsets), glue._p(rec),
+                                              glue._p(start), W, L, glue._p(gt_scene), glue._stream(dev))
+            _lib.check(rc, ctx)
+    ri = rec.long()
+    per_rec = lambda a: torch.from_numpy(np.ascontiguousarray(a.astype(np.float32))).to(dev)[ri]
+    common = {'noisy_joints': cano_joints, 'noisy_joints_scene_coord': scene_joints, 'transf_matrix': transf,
+              'cano_smplx_params_dict': {k_: cano_params[..., s_].contiguous() for k_, s_ in NOISY_ROW.items()},
+              'focal_length': per_rec(f), 'camera_center': per_rec(c), 'keypoints_2d': kp_out,
+              'mask_joint_vis': vis, 'mask_vec_vis': vec}
+    if with_gt:
+        common['gt_joints_scene_coord'] = gt_scene
+    tfd, pfd = traj_dataset.traj_feat_dim, traj_dataset.pose_feat_dim
+    cond = rt[..., list(ABS_TRAJ_CHANNELS)] if tfd == len(ABS_TRAJ_CHANNELS) else rt[..., 0:tfd].clone()
+    test_batch_traj = dict(common, motion_repr_noisy=rt, cond=cond, control_cond=rt[..., -pfd:].contiguous())
+    test_batch_pose = {key: ({a: b.clone() for a, b in v.items()} if isinstance(v, dict) else v.clone())
+                       for key, v in common.items()}
+    test_batch_pose.update(motion_repr_noisy=rp, cam2world=per_rec(c2w))
+    return test_batch_traj, test_batch_pose, Windows(rec, start, transf, lengths, offsets, clip_len, overlap)
 
 
 def to_recordings(windows, joints):

@@ -802,13 +802,249 @@ def gen_windows_noise(ref):
           f"height margin {float(out['noisy_height_margin'].min()):.2e}")
 
 
+# The video loader (DataloaderVideo): 24-frame windows, overlap 2.  Each case is one recording, as the loader takes one:
+# (name, dataset, scene from the reference's floor tables, view, frames, use_scene_floor_height, floor override)
+VIDEO_CLIP = 24
+VIDEO_Q_TRIALS = 4  # random float64 windows through the reference's cano_seq_smplx_egobody
+ABS_CHANNELS = (0, 2, 3, 6, 7, 8, 9, 10, 11, 12, 16, 17, 18)  # repr_abs_only's trajectory channels
+VIDEO_CASES = (("N3Office_00034_01", 'prox', 'N3Office', None, 46, True, None),
+               ("Werkraum_03403_01", 'prox', 'Werkraum', None, 24, True, 0.0),    # a preset floor of 0.0: window minimum
+               ("recording_20210907_S02_S01_01", 'egobody', 'seminar_g110', 'master', 24, True, None),
+               ("recording_20210911_S07_S06_02", 'egobody', 'seminar_d78', 'sub_2', 46, False, None))
+# PROX's colour camera (Kinect v2, k1 k2 p1 p2 k3) and EgoBody's per-view ones (k1 k2 p1 p2 k3 k4 k5 k6)
+VIDEO_PROX_CAM = {'f': [1060.53, 1060.38], 'c': [951.30, 536.77],
+                  'camera_mtx': [[1060.53, 0.0, 951.30], [0.0, 1060.38, 536.77], [0.0, 0.0, 1.0]],
+                  'k': [0.0548, -0.0489, 0.0009, -0.0012, 0.0102]}
+VIDEO_EGO_CAM = {'f': [918.72, 918.64], 'c': [956.13, 548.89],
+                 'camera_mtx': [[918.72, 0.0, 956.13], [0.0, 918.64, 548.89], [0.0, 0.0, 1.0]],
+                 'k': [0.4761, -2.7413, 0.0004, -0.0002, 1.5812, 0.3563, -2.5628, 1.5138]}
+
+
+def _rigid(rotvec, t):
+    m = np.eye(4)
+    m[:3, :3] = ref_rotation.from_rotvec(rotvec).as_matrix()
+    m[:3, 3] = t
+    return m
+
+
+def video_recording(g, n, cam2world, y_up, heading):
+    """Camera-frame SMPL-X fits of a body that walks in the scene with its heading near `heading` (radians about the
+    scene's up axis) and a small tilt, so that after the camera transform the global rotation is near pi; FK on the
+    synthetic body gives the pelvis offset delta_T = pelvis - transl, which the scene -> camera inversion keeps."""
+    model = synthetic.smplx_like_model(0)
+    t = np.arange(n, dtype=np.float64)
+    phi = heading + 0.03 * np.sin(t / 5.0)
+    go_z = (ref_rotation.from_rotvec(np.stack([0 * t, 0 * t, phi], -1)) *
+            ref_rotation.from_rotvec(np.stack([0.05 * np.sin(t / 13.0), 0 * t, 0 * t], -1)))
+    T_z = np.stack([0.6 * np.sin(t / 30.0), 0.004 * t, 0.9 + 0.01 * np.sin(t / 7.0)], -1)
+    betas = np.repeat(0.5 * g.standard_normal((1, 10)), n, axis=0).astype(np.float32)
+    body_pose = (0.15 * g.standard_normal((1, 63)) + 0.05 * np.sin(t[:, None] / 6.0 + np.arange(63))).astype(np.float32)
+    f = lambda a: torch.from_numpy(np.asarray(a, np.float32))
+    j0, _ = ko.smplx_forward(model, f(np.zeros((n, 3))), f(body_pose), f(betas), f(np.zeros((n, 3))), return_verts=False)
+    delta = j0[:, 0].numpy().astype(np.float64)
+    Qm = np.array([[1.0, 0, 0], [0, 0, -1], [0, 1, 0]])
+    go_s, T_s = go_z, T_z
+    if y_up:  # the body walks in a y-up scene: Q^T of the z-up motion
+        go_s = ref_rotation.from_matrix(Qm.T) * go_z
+        T_s = (T_z + delta) @ Qm - delta
+    Rc, tc = cam2world[:3, :3], cam2world[:3, 3]
+    go_c = (ref_rotation.from_matrix(Rc.T) * go_s).as_rotvec()
+    T_c = (T_s + delta - tc) @ Rc - delta
+    return {'global_orient': go_c.astype(np.float32), 'transl': T_c.astype(np.float32), 'betas': betas,
+            'body_pose': body_pose}
+
+
+def video_keypoints(g, n, no_person=()):
+    """OpenPose BODY_25 rows [n,25,3] (float32): pixels over the image, its corners and far outside it; confidences with
+    0.2f and its float32 neighbours; frames in no_person have no person (zeros)."""
+    xy = np.stack([g.uniform(0, 1920, (n, 25)), g.uniform(0, 1080, (n, 25))], -1)
+    xy[0, 8], xy[0, 12] = (0.0, 0.0), (1919.0, 1079.0)
+    xy[1, 9], xy[1, 13] = (0.0, 1079.0), (1919.0, 0.0)
+    xy[2, 8], xy[2, 1] = (-6000.0, 9000.0), (12000.0, -7000.0)  # far outside: OpenCV's negative icdist branch
+    conf = g.uniform(0, 1, (n, 25))
+    c2 = np.float32(0.2)
+    conf[:, 5] = c2
+    conf[:, 2] = np.nextafter(c2, np.float32(1))
+    conf[:, 6] = np.nextafter(c2, np.float32(0))
+    kp = np.concatenate([xy, conf[..., None]], -1).astype(np.float32)
+    for fr in no_person:
+        kp[fr] = 0
+    return kp
+
+
+def gen_windows_video(ref):
+    """The reference's own DataloaderVideo on tiny PROX and EgoBody recordings written to a temporary directory in the
+    loader's layout (per-frame 000.pkl fits and keypoint jsons, mask_joint.npy, cam2world / calibration jsons, Color.json,
+    egobody_rohm_info.csv and data_splits.csv, AMASS_mean / std.pkl), for task 'pose' (repr_abs_only False) and 'traj'
+    (repr_abs_only True).  The stub smplx body stands in for the neutral and gendered SMPL-X models."""
+    import json
+    import pickle
+    import tempfile
+    sys.path.insert(0, '/root/reference')
+    import data_loaders.dataloader_video as dlv
+    sys.path.pop(0)
+    g = np.random.default_rng(111)
+    ds_pose = synthetic.make_dataset('pose', seed=3, realistic_std=True)
+    ds_traj = synthetic.make_dataset('traj', seed=3, realistic_std=True)
+    assert ds_traj.traj_feat_dim == len(ABS_CHANNELS)
+    out = {"clip_len": np.array(VIDEO_CLIP), "overlap": np.array(2), "n_cases": np.array(len(VIDEO_CASES))}
+    for key, cam in (("prox", VIDEO_PROX_CAM), ("egobody", VIDEO_EGO_CAM)):
+        out[f"{key}_f"], out[f"{key}_c"] = np.array(cam['f']), np.array(cam['c'])
+        out[f"{key}_camera_mtx"], out[f"{key}_k"] = np.array(cam['camera_mtx']), np.array(cam['k'])
+
+    def dump(path, obj, mode='w'):
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        with open(path, mode) as fh:
+            (pickle.dump if mode == 'wb' else json.dump)(obj, fh)
+
+    def write_fits(root, prm, n):
+        for fr in range(n):
+            dump(os.path.join(root, f"frame_{fr:05d}", "000.pkl"), {k: v[fr:fr + 1] for k, v in prm.items()}, 'wb')
+
+    with tempfile.TemporaryDirectory() as tmp:
+        base, init = os.path.join(tmp, "base"), os.path.join(tmp, "init")
+        logs = {}
+        # one set of statistics for both tasks (the pose model's): the rows are then the same and stored once
+        for task, ds in (("pose", ds_pose), ("traj", ds_pose)):
+            logs[task] = os.path.join(tmp, f"log_{task}")
+            cur, mean, std = 0, {}, {}
+            for k in ko.REPR_LIST:
+                mean[k], std[k] = ds.Mean[cur:cur + ko.REPR_DIM_DICT[k]], ds.Std[cur:cur + ko.REPR_DIM_DICT[k]]
+                cur += ko.REPR_DIM_DICT[k]
+            dump(os.path.join(logs[task], "AMASS_mean.pkl"), mean, 'wb')
+            dump(os.path.join(logs[task], "AMASS_std.pkl"), std, 'wb')
+        dump(os.path.join(base, "calibration", "Color.json"), VIDEO_PROX_CAM)
+        ego = [c for c in VIDEO_CASES if c[1] == 'egobody']
+        import pandas as pd
+        os.makedirs(base, exist_ok=True)
+        pd.DataFrame({'recording_name': [c[0] for c in ego], 'target_idx': [1, 0], 'target_gender': ['male', 'female'],
+                      'view': [c[3] for c in ego], 'scene_name': [c[2] for c in ego],
+                      'body_idx_fpv': ['1 male', '1 male']}).to_csv(os.path.join(base, "egobody_rohm_info.csv"))
+        pd.DataFrame({'train': ['a', 'b'], 'val': ['c', 'd'], 'test': [ego[0][0], ego[1][0]]}).to_csv(
+            os.path.join(base, "data_splits.csv"))
+        for view in ('master', 'sub_2'):
+            dump(os.path.join(base, "kinect_cam_params", f"kinect_{view}", "Color.json"), VIDEO_EGO_CAM)
+        saved_floor = {}
+        for c, (name, dataset, scene, view, n, use_floor, floor_override) in enumerate(VIDEO_CASES):
+            y_up = dataset == 'egobody'
+            # cameras: PROX looks down at the room from 2.5 m; EgoBody's master and a sub view 60 deg around it
+            cam = _rigid([-2.0, 0.3, 0.4], [1.0 + 0.1 * c, -2.0, 2.5]) if not y_up else \
+                _rigid([0.2, 2.9, 0.1], [0.5, 1.4, 2.0 + 0.2 * c])
+            master = cam
+            if view not in (None, 'master'):
+                sub2main = _rigid([0.05, 1.05, -0.02], [1.8, 0.02, 0.9])
+                cam = master @ sub2main
+            heading = (np.pi - 0.02) if c % 2 == 0 else (-np.pi + 0.015)
+            prm = video_recording(g, n, cam, y_up, heading)
+            no_person = (3, 17) if c in (0, 3) else ()
+            kp = video_keypoints(g, n, no_person)
+            mask = g.uniform(0, 1, (n, 25)) > 0.15
+            mask[4, 7] = mask[5, 8] = mask[6, 10] = mask[7, 11] = False  # a zero on each foot joint
+            mask[8:12, [7, 8, 10, 11]] = True
+            kp[8:12, [14, 11, 19, 20, 21, 22, 23, 24], 2] = 0.9  # feet seen on frames 8-11: both contact masks occur
+            if y_up:
+                fit_dir = os.path.join(init, name, "body_idx_1" if c == 2 else "body_idx_0", "results")
+                gt_root = os.path.join(base, "smplx_interactee_test" if c == 2 else "smplx_camera_wearer_test", name,
+                                       "body_idx_1" if c == 2 else "body_idx_0", "results")
+                gt = video_recording(g, n, master, True, heading + 0.1)
+                write_fits(gt_root, gt, n)
+                calib = os.path.join(base, "calibrations", name, "cal_trans")
+                dump(os.path.join(calib, "kinect12_to_world", scene + ".json"), {'trans': master.tolist()})
+                if view != 'master':
+                    dump(os.path.join(calib, "kinect_13to12_color.json"), {'trans': sub2main.tolist()})
+                kp_dir = os.path.join(base, "keypoints_cleaned", name, view)
+                mask_path = os.path.join(base, "mask_joint", name, view, "mask_joint.npy")
+            else:
+                fit_dir = os.path.join(init, name, "results")
+                dump(os.path.join(base, "cam2world", scene + ".json"), cam.tolist())
+                kp_dir = os.path.join(base, "keypoints_openpose", name)
+                mask_path = os.path.join(base, "mask_joint", name, "mask_joint.npy")
+            write_fits(fit_dir, prm, n)
+            body_idx = 1 if c == 2 else 0
+            for fr in range(n):
+                people = [] if fr in no_person else [{'pose_keypoints_2d': [0.0] * 75}] * body_idx + \
+                    [{'pose_keypoints_2d': kp[fr].reshape(-1).tolist()}]
+                dump(os.path.join(kp_dir, f"frame_{fr:05d}_keypoints.json"), {'people': people})
+            os.makedirs(os.path.dirname(mask_path), exist_ok=True)
+            np.save(mask_path, mask)
+            table = dlv.prox_floor_height if dataset == 'prox' else dlv.egobody_floor_height
+            if floor_override is not None:
+                saved_floor[scene] = table[scene]
+                table[scene] = floor_override
+            items = {}
+            try:
+                for task in ("pose", "traj"):
+                    d = dlv.DataloaderVideo(dataset=dataset, init_root=init, base_dir=base, body_model_path='',
+                                            recording_name=name, use_scene_floor_height=use_floor,
+                                            repr_abs_only=task == 'traj', task=task, overlap_len=2, clip_len=VIDEO_CLIP,
+                                            logdir=logs[task], device='cpu')
+                    items[task] = [d[w] for w in range(len(d))]
+                if floor_override is not None:  # the same recording without a preset floor: the same windows
+                    d0 = dlv.DataloaderVideo(dataset=dataset, init_root=init, base_dir=base, body_model_path='',
+                                             recording_name=name, use_scene_floor_height=False, task='pose',
+                                             overlap_len=2, clip_len=VIDEO_CLIP, logdir=logs['pose'], device='cpu')
+                    for a, b in zip(items['pose'], [d0[w] for w in range(len(d0))]):
+                        assert np.array_equal(a['transf_matrix'], b['transf_matrix'])
+                        assert np.array_equal(a['motion_repr_noisy'], b['motion_repr_noisy'])
+            finally:
+                for k, v in saved_floor.items():
+                    table[k] = v
+                saved_floor.clear()
+            fl = table[scene] if (use_floor and floor_override is None) else (floor_override or 0.0)
+            out[f"c{c}_meta"] = np.array([int(y_up), n, int(view not in (None, 'master'))])
+            out[f"c{c}_name"] = np.array(name)
+            out[f"c{c}_floor"] = np.array(fl if use_floor else 0.0)
+            out[f"c{c}_cam2world"], out[f"c{c}_master2world"] = cam, master
+            out[f"c{c}_keypoints25"], out[f"c{c}_depth_mask"] = kp, mask
+            out[f"c{c}_kp_float64"] = np.array(len(no_person) > 0)
+            for k, v in prm.items():
+                out[f"c{c}_param_{k}"] = v
+            if y_up:
+                for k, v in gt.items():
+                    out[f"c{c}_gt_{k}"] = v
+            pose, traj = items["pose"], items["traj"]
+            for key in pose[0]:
+                if key == 'frame_name':
+                    assert [it['frame_name'][0] for it in pose] == [f"frame_{s:05d}" for s in range(0, n - VIDEO_CLIP + 1,
+                                                                                                     VIDEO_CLIP - 2)]
+                    continue
+                if key == 'cano_smplx_params_dict':
+                    for k in ('global_orient', 'transl', 'betas', 'body_pose'):
+                        out[f"c{c}_cano_{k}"] = np.asarray([it[key][k] for it in pose])
+                    continue
+                out[f"c{c}_{key}"] = np.asarray([it[key] for it in pose])
+                assert all(np.array_equal(np.asarray(a[key]), np.asarray(b[key])) for a, b in zip(pose, traj)), key
+            for a in traj:  # the TrajNet inputs are channels of the same rows (repr_abs_only True)
+                assert np.array_equal(a['cond'], a['motion_repr_noisy'][:, list(ABS_CHANNELS)])
+                assert np.array_equal(a['control_cond'], a['motion_repr_noisy'][:, -ds_traj.pose_feat_dim:])
+            print(f"windows_video case {c} ({dataset}, {name}): {len(pose)} windows, floor {fl}, "
+                  f"keypoints dtype {pose[0]['keypoints_2d'].dtype}")
+    # the EgoBody canonical frame as the reference computes it, in float64 on random joints and parameters (both floor
+    # modes): the tests hold T_z Q and cano_seq_smplx of Q p against these (DESIGN §4.14)
+    gq = np.random.default_rng(9)
+    for trial in range(VIDEO_Q_TRIALS):
+        j = gq.standard_normal((4, 22, 3))
+        p = {"global_orient": gq.standard_normal((4, 3)), "transl": gq.standard_normal((4, 3)),
+             "betas": gq.standard_normal((4, 10)), "body_pose": gq.standard_normal((4, 63))}
+        floor = 0.0 if trial % 2 else float(gq.uniform(-2, -0.5))
+        cano, cano_p, tf = ref.mr.cano_seq_smplx_egobody(j.copy(), {k: v.copy() for k, v in p.items()},
+                                                         preset_floor_height=floor or None, return_transf_mat=True)
+        out[f"q{trial}_joints"], out[f"q{trial}_floor"] = j, np.array(floor)
+        out[f"q{trial}_global_orient"], out[f"q{trial}_transl"] = p['global_orient'], p['transl']
+        out[f"q{trial}_cano_joints"], out[f"q{trial}_transf"] = cano, tf
+        out[f"q{trial}_cano_global_orient"], out[f"q{trial}_cano_transl"] = cano_p['global_orient'], cano_p['transl']
+    out["q_trials"] = np.array(VIDEO_Q_TRIALS)
+    np.savez_compressed(os.path.join(OUT, "windows_video.npz"), **out)
+    print("windows_video.npz", os.path.getsize(os.path.join(OUT, "windows_video.npz")), "bytes")
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     ref = import_reference()
     which = sys.argv[1:] or ["schedules", "posenet", "trajnet", "sampling", "kinematics", "glue", "pipeline",
-                             "clip_guidance", "windows", "windows_noise"]
+                             "clip_guidance", "windows", "windows_noise", "windows_video"]
     for w in which:
         {"schedules": gen_schedules, "posenet": gen_posenet, "trajnet": gen_trajnet, "sampling": gen_sampling,
          "kinematics": gen_kinematics, "glue": gen_glue, "pipeline": gen_pipeline, "clip_guidance": gen_clip_guidance,
-         "windows": gen_windows, "windows_noise": gen_windows_noise}[w](ref)
+         "windows": gen_windows, "windows_noise": gen_windows_noise, "windows_video": gen_windows_video}[w](ref)

@@ -4,6 +4,7 @@ generator per window, the draws included; both add the noise kernel, FK of the W
 encoder), and to_recordings, on R recordings of N frames cut into 145-frame windows with overlap 2.
 
     python tools/windows_bench.py [--recordings R] [--frames N] [--iters K] [--rounds M] [--oracle-windows V] [--json PATH]
+    python tools/windows_bench.py --video [...]   # encode_video (PROX: camera map, undistorted keypoints, masks) vs encode
 
 Each call is timed with CUDA events around --iters calls after warm-up calls; the median over --rounds is reported as
 windows per second.  Next to it, the float64 CPU oracle's time per window (oracle/windows_oracle.py, one thread, over
@@ -24,7 +25,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from oracle import windows_noise_oracle, windows_oracle  # noqa: E402
+from oracle import windows_noise_oracle, windows_oracle, windows_video_oracle  # noqa: E402
 from rohm_b200 import synthetic, windows  # noqa: E402
 from rohm_b200.body_model import BodyModel  # noqa: E402
 
@@ -69,10 +70,13 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--oracle-windows", type=int, default=20)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--video", action="store_true", help="encode_video against encode, alternated per round")
     a = ap.parse_args()
     dev = torch.device("cuda:0")
     info = card()
     print("card, power limit, SM clock, max SM clock:", info)
+    if a.video:
+        return video(a, dev, info)
     ds_p, ds_t = synthetic.make_dataset('pose', seed=3, realistic_std=True), synthetic.make_dataset('traj', seed=3, realistic_std=True)
     bm = BodyModel.create('', device=dev, seed=0)
     host = recordings(a.recordings, a.frames)
@@ -121,6 +125,57 @@ def main():
     print(f"oracle noisy path (float64, CPU, 1 thread): {noisy_ms:.3f} ms per window")
     line = {"card": info, "recordings": a.recordings, "frames": a.frames, "windows": W, **{k: v for k, v in res.items()},
             "oracle_cpu_ms_per_window": oracle_ms, "oracle_noisy_cpu_ms_per_window": noisy_ms}
+    print(json.dumps(line))
+    if a.json:
+        os.makedirs(os.path.dirname(os.path.abspath(a.json)), exist_ok=True)
+        with open(a.json, "w") as f:
+            json.dump(line, f, indent=1)
+
+
+def video(a, dev, info):
+    """encode_video on PROX-like recordings (a rotated camera, Kinect-like distortion, keypoints over the image) against
+    encode on the same parameters; each call's host work is inside the timed region."""
+    ds_p, ds_t = synthetic.make_dataset('pose', seed=3, realistic_std=True), synthetic.make_dataset('traj', seed=3, realistic_std=True)
+    bm = BodyModel.create('', device=dev, seed=0)
+    host = recordings(a.recordings, a.frames)
+    params = {k: torch.from_numpy(v).to(dev) for k, v in host.items()}
+    R, N = a.recordings, a.recordings * a.frames
+    lengths = [a.frames] * R
+    g = np.random.default_rng(2)
+    c2w = np.repeat(np.eye(4)[None], R, 0)
+    c2w[:, :3, :3] = np.array([[1.0, 0, 0], [0, 0, 1], [0, -1, 0]])
+    c2w[:, :3, 3] = g.uniform(-1, 1, (R, 3))
+    K = np.array([[1060.5, 0.0, 951.3], [0.0, 1060.4, 536.8], [0.0, 0.0, 1.0]])
+    kp = np.concatenate([g.uniform(0, 1920, (N, 25, 1)), g.uniform(0, 1080, (N, 25, 1)), g.uniform(0, 1, (N, 25, 1))], -1)
+    cam = dict(cam2world=c2w, focal_length=np.repeat([[1060.5, 1060.4]], R, 0), camera_center=np.repeat([[951.3, 536.8]], R, 0),
+               camera_mtx=np.repeat(K[None], R, 0), dist=np.repeat([[0.0548, -0.0489, 0.0009, -0.0012, 0.0102]], R, 0),
+               keypoints=torch.from_numpy(kp.astype(np.float32)).to(dev),
+               depth_mask=torch.from_numpy((g.uniform(0, 1, (N, 25)) > 0.1).astype(np.float32)).to(dev),
+               keypoints_float64=[False] * R)
+    calls = {"encode_video": lambda: windows.encode_video(bm, params, lengths, 'prox', pose_dataset=ds_p, traj_dataset=ds_t,
+                                                          **cam),
+             "encode": lambda: windows.encode(bm, params, lengths, ds_p, ds_t)}
+    W = len(windows.window_table(lengths))
+    ms = {k: [] for k in calls}
+    for _ in range(a.rounds):
+        for k, fn in calls.items():
+            ms[k].append(time_ms(fn, a.iters))
+    res = {k: {"ms": statistics.median(v), "windows_per_s": W / (statistics.median(v) / 1e3)} for k, v in ms.items()}
+    for k, v in res.items():
+        print(f"{k:14s} {W} windows: {v['ms']:.3f} ms  ({v['windows_per_s']:.0f} windows/s)")
+    torch.set_num_threads(1)
+    jh = bm(**params, return_verts=False).joints[:, 0:22].cpu().numpy()
+    table = windows.window_table(lengths)[:a.oracle_windows]
+    t0 = time.perf_counter()
+    for r, s in table:
+        rows = slice(r * a.frames + s, r * a.frames + s + 145)
+        windows_video_oracle.encode_window_video(jh[rows], {k: v[rows] for k, v in host.items()}, c2w[r], False)
+        windows_video_oracle.keypoints_window(kp[rows].astype(np.float32), np.ones((145, 25)), True, K,
+                                              cam['dist'][r], False)
+    oracle_ms = (time.perf_counter() - t0) * 1e3 / len(table)
+    print(f"oracle video path (float64 numpy, CPU, 1 thread): {oracle_ms:.3f} ms per window")
+    line = {"card": info, "recordings": R, "frames": a.frames, "windows": W, **res,
+            "oracle_video_cpu_ms_per_window": oracle_ms}
     print(json.dumps(line))
     if a.json:
         os.makedirs(os.path.dirname(os.path.abspath(a.json)), exist_ok=True)
