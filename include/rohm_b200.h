@@ -402,10 +402,14 @@ ROHM_API int rohm_pose_to_control_cond(rohm_ctx* ctx, const float* pose_out, int
  * [B,src_T,294]) with channels [0,22) replaced by traj_full [B,Tp,22] (NULL keeps src) and channels >= 22 zeroed where
  * chan_keep[c] == 0 (294 bytes, NULL = keep all: the 'lower' / 'upper' joint masks), where frame_lo[b] <= t < frame_hi[b]
  * (int [B], NULL = none: the 'full' scheme) and, with zero_contact, in the 4 contact channels.  With lengths
- * (1 <= lengths[b] <= Tp): frames past a clip are zeros in every channel. */
+ * (1 <= lengths[b] <= Tp): frames past a clip are zeros in every channel.  With vis_mask (test_prox_egobody.py:302-309,
+ * channels-last [B,vis_T,294] with vis_T >= Tp, frames [0,Tp) read; NULL = none; not with lengths): after the occlusion
+ * zeroing every channel of frame t is multiplied by vis_mask[b,t,c] (IEEE products: -x*0 = -0, NaN*1 = NaN, Inf*0 = NaN),
+ * and the contact zeroing comes after the multiply. */
 ROHM_API int rohm_build_pose_cond(rohm_ctx* ctx, const float* src, int src_channel_major, int src_T, const float* traj_full,
                                   const unsigned char* chan_keep, const int* frame_lo, const int* frame_hi,
-                                  int zero_contact, int B, int Tp, const int* lengths, float* cond_out, void* stream);
+                                  int zero_contact, int B, int Tp, const int* lengths, const float* vis_mask, int vis_T,
+                                  float* cond_out, void* stream);
 
 /* rot6d_to_rotmat (quaternion.py:482-501) and rotation_matrix_to_angle_axis (konia_transform.py:317-340 -> :350-444 ->
  * :561-631) on n 6-D rotations: aa [n,3] and/or rotmat [n,9] (row-major), either may be NULL. */

@@ -86,7 +86,7 @@ SIGNATURES = {
     "rohm_traj_glue": (_i, [_p, _p, _i, _p, _p, _p, _p, _p, _i, _i, _p, _p, _i64, _p, _p, _p]),
     "rohm_traj_repr_from_joints": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p]),
     "rohm_pose_to_control_cond": (_i, [_p, _p, _i, _i, _i, _i, _i, _p, _p, _p]),
-    "rohm_build_pose_cond": (_i, [_p, _p, _i, _i, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p]),
+    "rohm_build_pose_cond": (_i, [_p, _p, _i, _i, _p, _p, _p, _p, _i, _i, _i, _p, _p, _i, _p, _p]),
     "rohm_rot6d_to_aa": (_i, [_p, _p, _i64, _p, _p, _p]),
     "rohm_joints_from_traj": (_i, [_p, _p, _i, _p, _p, _i, _i, _p, _p, _i64, _i, _p, _p]),
     "rohm_window_encode": (_i, [_p, _p, _p, _p, _p, _p, C.POINTER(_i), _p, _i, _i, _i, _p, _p, _p, _p, _i,

@@ -181,12 +181,17 @@ __global__ void pose_to_control_kernel(const float* __restrict__ pose_out, int T
 
 // PoseNet condition [B, 294, 1, Tp] from a source in either layout, the trajectory block and the occlusion masks.
 // kLengths: clip b has lengths[b] <= Tp frames; later frames are written as zeros, src and traj_full are not read there.
-template <bool kLengths>
+// kVis (video driver, test_prox_egobody.py:302-309): after the occlusion zeroing every channel is multiplied by
+// vis_mask[b, t, c] ([B, vis_T, 294], vis_T >= Tp), then the contact channels are zeroed.  A multiply, not a select: the
+// reference's -x * 0 = -0, NaN * 1 = NaN and Inf * 0 = NaN are kept.
+template <bool kLengths, bool kVis = false>
 __global__ void build_pose_cond_kernel(const float* __restrict__ src, int src_channel_major, int src_T,
                                        const float* __restrict__ traj_full, const unsigned char* __restrict__ chan_keep,
                                        const int* __restrict__ frame_lo, const int* __restrict__ frame_hi,
                                        int zero_contact, int Tp, float* __restrict__ out,
-                                       const int* __restrict__ lengths) {
+                                       const int* __restrict__ lengths, const float* __restrict__ vis_mask = nullptr,
+                                       int vis_T = 0) {
+  static_assert(!(kLengths && kVis), "the visibility mask applies to whole clips");
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
@@ -203,6 +208,30 @@ __global__ void build_pose_cond_kernel(const float* __restrict__ src, int src_ch
       const int t = t0 + j, c = c0 + tx;
       tile[tx][j] = (c < kC && t < len) ? src[(static_cast<int64_t>(b) * src_T + t) * kC + c] : 0.0f;
     }
+  }
+  if constexpr (kVis) {
+    // the mask is channels-last: staged through shared memory like a channels-last source, so both reads coalesce
+    __shared__ float vtile[32][33];
+    for (int j = ty; j < 32; j += 8) {
+      const int t = t0 + j, c = c0 + tx;
+      vtile[tx][j] = (c < kC && t < Tp) ? vis_mask[(static_cast<int64_t>(b) * vis_T + t) * kC + c] : 0.0f;
+    }
+    __syncthreads();
+    const int lo = frame_lo != nullptr ? frame_lo[b] : 0, hi = frame_hi != nullptr ? frame_hi[b] : 0;
+    for (int j = ty; j < 32; j += 8) {
+      const int c = c0 + j, t = t0 + tx;
+      if (c >= kC || t >= Tp) continue;
+      float v = tile[j][tx];
+      if (c < kTrajFull) {
+        if (traj_full != nullptr) v = traj_full[(static_cast<int64_t>(b) * Tp + t) * kTrajFull + c];
+      } else if ((chan_keep != nullptr && chan_keep[c] == 0) || (t >= lo && t < hi)) {
+        v = 0.0f;
+      }
+      v = v * vtile[j][tx];
+      if (zero_contact && c >= kChContact) v = 0.0f;
+      out[(static_cast<int64_t>(b) * kC + c) * Tp + t] = v;
+    }
+    return;
   }
   __syncthreads();
   const int lo = frame_lo != nullptr ? frame_lo[b] : 0, hi = frame_hi != nullptr ? frame_hi[b] : 0;
@@ -519,15 +548,18 @@ extern "C" int rohm_pose_to_control_cond(rohm_ctx* ctx, const float* pose_out, i
 extern "C" int rohm_build_pose_cond(rohm_ctx* ctx, const float* src, int src_channel_major, int src_T,
                                     const float* traj_full, const unsigned char* chan_keep, const int* frame_lo,
                                     const int* frame_hi, int zero_contact, int B, int Tp, const int* lengths,
-                                    float* cond_out, void* stream) {
+                                    const float* vis_mask, int vis_T, float* cond_out, void* stream) {
   if (ctx == nullptr) return ROHM_ERR_INVALID;
   rohm::DeviceGuard device_guard__(ctx);
-  if (!src || !cond_out || B <= 0 || Tp <= 0 || src_T < Tp || B > 65535 || ((frame_lo == nullptr) != (frame_hi == nullptr)))
+  if (!src || !cond_out || B <= 0 || Tp <= 0 || src_T < Tp || B > 65535 || ((frame_lo == nullptr) != (frame_hi == nullptr)) ||
+      (vis_mask != nullptr && (vis_T < Tp || lengths != nullptr)))
     return fail(ctx, ROHM_ERR_INVALID, "rohm_build_pose_cond: bad arguments");
   dim3 grid((Tp + 31) / 32, (kC + 31) / 32, B);
-  const auto kernel = lengths != nullptr ? build_pose_cond_kernel<true> : build_pose_cond_kernel<false>;
+  const auto kernel = vis_mask != nullptr ? build_pose_cond_kernel<false, true>
+                      : lengths != nullptr ? build_pose_cond_kernel<true> : build_pose_cond_kernel<false>;
   kernel<<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
-      src, src_channel_major, src_T, traj_full, chan_keep, frame_lo, frame_hi, zero_contact, Tp, cond_out, lengths);
+      src, src_channel_major, src_T, traj_full, chan_keep, frame_lo, frame_hi, zero_contact, Tp, cond_out, lengths,
+      vis_mask, vis_T);
   ROHM_CUDA(ctx, cudaGetLastError());
   return ROHM_OK;
 }

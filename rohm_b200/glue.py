@@ -159,11 +159,14 @@ def channel_keep_mask(mask_scheme, traj_feat_dim=22):
 
 
 def build_pose_cond(src, traj_full=None, chan_keep=None, frame_lo=None, frame_hi=None, zero_contact=False, frames=None,
-                    lengths=None):
+                    lengths=None, vis_mask=None):
     """PoseNet condition [B,294,1,Tp] (test_amass_full.py:320-370): ``src`` is [B,Ts,294] (driver tensors) or [B,294,1,Ts]
     (a previous PoseNet output), Tp = ``frames`` (default Ts); channels [0,22) <- traj_full [B,Tp,22]; channels >= 22 are
     zeroed where chan_keep == 0, inside [frame_lo[b], frame_hi[b]) and (zero_contact) in the contact channels.
-    lengths (int32 device [B], pose frames per clip): frames past a clip are zeros, src / traj_full are not read there."""
+    lengths (int32 device [B], pose frames per clip): frames past a clip are zeros, src / traj_full are not read there.
+    vis_mask (float32 CUDA [B,vis_T,294], vis_T >= Tp; the video loader's mask_vec_vis, test_prox_egobody.py:302-309): after
+    the occlusion zeroing every channel of frame t < Tp is multiplied by vis_mask[b,t] -- a multiply, so -x * 0 = -0.0,
+    NaN * 1 = NaN and Inf * 0 = NaN as in the reference -- and the contact zeroing comes after it.  Not with lengths."""
     src = _f32c(src, "src")
     if src.dim() == 4:
         B, Cc, _, Ts = src.shape
@@ -187,12 +190,23 @@ def build_pose_cond(src, traj_full=None, chan_keep=None, frame_lo=None, frame_hi
     if frame_lo is not None:
         lo_t = torch.as_tensor(frame_lo).to(device=dev, dtype=torch.int32).contiguous()
         hi_t = torch.as_tensor(frame_hi).to(device=dev, dtype=torch.int32).contiguous()
+    vis_T = 0
+    if vis_mask is not None:
+        if lengths is not None:
+            raise RohmB200Error("build_pose_cond: vis_mask applies to whole clips; it is refused with lengths")
+        if (not isinstance(vis_mask, torch.Tensor) or vis_mask.device != dev or vis_mask.dtype != torch.float32 or
+                vis_mask.dim() != 3 or vis_mask.shape[0] != B or vis_mask.shape[1] < Tp or vis_mask.shape[2] != BODY_FEAT_DIM):
+            raise RohmB200Error(f"build_pose_cond: vis_mask must be a float32 tensor [{B}, >={Tp}, {BODY_FEAT_DIM}] on {dev}, "
+                                f"got {getattr(vis_mask, 'dtype', type(vis_mask))} {tuple(getattr(vis_mask, 'shape', ()))} "
+                                f"on {getattr(vis_mask, 'device', None)}")
+        vis_mask = vis_mask.contiguous()
+        vis_T = int(vis_mask.shape[1])
     out = torch.empty(B, BODY_FEAT_DIM, 1, Tp, device=dev)
     lib, ctx = _lib.load(), _lib.ctx(dev.index)
     if lengths is not None:
         clip_layout(lengths, B, Tp, "build_pose_cond")
     rc = lib.rohm_build_pose_cond(ctx, _p(src), channel_major, Ts, _p(traj_full), _p(keep_t), _p(lo_t), _p(hi_t),
-                                  int(bool(zero_contact)), B, Tp, _p(lengths), _p(out), _stream(dev))
+                                  int(bool(zero_contact)), B, Tp, _p(lengths), _p(vis_mask), vis_T, _p(out), _stream(dev))
     _lib.check(rc, ctx)
     return out
 

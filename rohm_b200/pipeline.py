@@ -8,6 +8,9 @@ condition assembly of :313-370 is ``rohm_build_pose_cond``, the TrajControl cond
 ``rohm_pose_to_control_cond``.  ``reconstruct_outputs`` is the post-loop block :386-428 (joints / vertices of the clean,
 reconstructed and noisy motions) and ``result_dict`` the driver's pickle payload (:446-458).
 
+``run_video_rounds``, ``reconstruct_video_outputs`` and ``video_result_dicts`` do the same for the PROX / EgoBody driver
+(test_prox_egobody.py:214-384) on the windows of ``windows.encode_video``, any number of recordings per call.
+
 The reference loop cannot be replaced "unchanged" because it is inline driver code, not a function; INTEGRATION.md shows the
 5-line edit that swaps lines 218-384 for a call to ``run_rounds``.
 """
@@ -225,6 +228,166 @@ def reconstruct_outputs(args, pose_dataset, smplx_model, test_batch_pose, val_ou
         res = res if return_verts else (res, None)
         out['rec_ric_data_noisy'], out['smpl_verts_noisy'] = per_clip(res[0]), per_clip(res[1])
     return out
+
+
+VIDEO_POSE_KEYS = ('mask_vec_vis', 'keypoints_2d', 'transf_matrix', 'focal_length', 'camera_center')
+
+
+def run_video_rounds(args, model_posenet, model_trajnet, model_trajnet_control, diffusion_posenet, diffusion_trajnet,
+                     diffusion_trajnet_control, pose_dataset, traj_dataset, smplx_model, test_batch_pose, test_batch_traj,
+                     on_round=None):
+    """test_prox_egobody.py:214-324: ``args.sample_iter`` rounds of TrajNet / TrajControl -> glue -> guided PoseNet
+    (grad_type='prox') over the W video windows of ``windows.encode_video`` (any number of recordings), mutating the two
+    batch dicts as the driver does.  Returns (val_output_pose [W,294,1,143], val_output_traj [W,144,traj_dim]).
+
+    It differs from ``run_rounds`` (the AMASS driver) in three places: the trajectory composite is built on
+    test_batch_traj['motion_repr_noisy'] (round 0 stores it back there, so round 1 builds on round 0's composite); the
+    PoseNet condition is the noisy pose rows (round 0, and every round with iter2_cond_noisy_pose) or the previous PoseNet
+    output, with channels [0,22) from the glue, multiplied by test_batch_pose['mask_vec_vis'][:, 0:-2] and with its contact
+    channels zeroed in rounds < mask_iter_num (round 0 only unless iter2_cond_noisy_pose); and there is no occlusion scheme,
+    infill mask, clean motion or input-noise flag.  Where the reference writes the trajectory block into the previous
+    PoseNet output in place (round >= 1, iter2_cond_noisy_pose False), this builds a new tensor: nothing reads the
+    aliased one afterwards, and an output already handed to ``on_round`` stays as it was.
+
+    Flags read: sample_iter, iter2_cond_noisy_traj, iter2_cond_noisy_pose, early_stop, cond_fn_with_grad,
+    timestep_respacing_eval.  test_batch_traj['generators'] is honoured as in ``run_rounds``; with per-window generators,
+    model_posenet.guidance_normaliser = 'clip' and batch-invariant TrajNets, a window's rounds depend on that window only.
+    Refused before any sampling step: test_batch_traj['lengths'] (video windows are whole), a missing pose-batch key the
+    driver reads (VIDEO_POSE_KEYS) and pose / trajectory batches with different window counts."""
+    if test_batch_traj.get('lengths') is not None:
+        raise RohmB200Error("run_video_rounds: test_batch_traj['lengths'] is refused: video windows are whole clips")
+    missing = [k for k in VIDEO_POSE_KEYS if test_batch_pose.get(k) is None]
+    if missing:
+        raise RohmB200Error(f"run_video_rounds: test_batch_pose lacks {missing} (the video driver reads them)")
+    W = test_batch_traj['motion_repr_noisy'].shape[0]
+    if test_batch_pose['motion_repr_noisy'].shape[0] != W:
+        raise RohmB200Error(f"run_video_rounds: the trajectory batch holds {W} windows, the pose batch "
+                            f"{test_batch_pose['motion_repr_noisy'].shape[0]}")
+    dev = test_batch_traj['motion_repr_noisy'].device
+    tfd, pose_feat_dim = traj_dataset.traj_feat_dim, traj_dataset.pose_feat_dim
+    if test_batch_traj.get('generators') is not None:
+        from .noise_streams import check_generators
+        check_generators(test_batch_traj, W, dev)
+        test_batch_pose['generators'] = test_batch_traj['generators']
+    mask_iter_num = args.sample_iter if args.iter2_cond_noisy_pose else 1
+    val_output_traj = val_output_pose = None
+    for iter_idx in range(args.sample_iter):
+        # ---------------------------------------------------------------- trajectory network (:216-242)
+        shape = list(test_batch_traj['motion_repr_noisy'][:, :, 0:tfd].shape)
+        if iter_idx == 0:
+            _, val_output_traj = diffusion_trajnet.eval_losses(
+                model=model_trajnet, batch=test_batch_traj, shape=shape, progress=False, clip_denoised=False,
+                timestep_respacing=args.timestep_respacing_eval, cond_fn_with_grad=args.cond_fn_with_grad,
+                compute_loss=False, smplx_model=smplx_model)
+        else:
+            test_batch_traj['control_cond'] = glue.pose_to_control_cond(val_output_pose, shape[1], pose_feat_dim)
+            _, val_output_traj = diffusion_trajnet_control.eval_losses(
+                model=model_trajnet_control, batch=test_batch_traj, shape=shape, progress=False, clip_denoised=False,
+                timestep_respacing=args.timestep_respacing_eval, cond_fn_with_grad=args.cond_fn_with_grad,
+                compute_loss=False, smplx_model=smplx_model)
+
+        # ---------------------------------------------------------------- inter-round glue (:244-287)
+        composite, traj_rec_full = glue.traj_to_full_repr(smplx_model, val_output_traj, test_batch_traj['motion_repr_noisy'],
+                                                          traj_dataset, pose_dataset)
+        if iter_idx == 0:
+            test_batch_traj['motion_repr_noisy'] = composite
+        if iter_idx < args.sample_iter - 1 and not args.iter2_cond_noisy_traj:
+            test_batch_traj['cond'] = val_output_traj
+
+        # ---------------------------------------------------------------- PoseNet condition (:290-313)
+        if iter_idx == 0:
+            test_batch_pose['motion_repr_noisy'] = test_batch_pose['motion_repr_noisy'][:, 0:-1]
+        src = test_batch_pose['motion_repr_noisy'] if (args.iter2_cond_noisy_pose or iter_idx == 0) else val_output_pose
+        clip_len = traj_rec_full.shape[1]
+        if iter_idx < mask_iter_num:
+            cond = glue.build_pose_cond(src, traj_rec_full, zero_contact=True, frames=clip_len,
+                                        vis_mask=test_batch_pose['mask_vec_vis'])
+        else:
+            cond = glue.build_pose_cond(src, traj_rec_full, frames=clip_len)
+        test_batch_pose['cond'] = cond
+        if iter_idx == 0:
+            test_batch_pose['motion_repr_noisy'] = torch.permute(test_batch_pose['motion_repr_noisy'],
+                                                                 (0, 2, 1)).unsqueeze(-2)
+
+        # ---------------------------------------------------------------- PoseNet sampling (:315-324)
+        shape = list(test_batch_pose['motion_repr_noisy'].shape)
+        _, val_output_pose = diffusion_posenet.eval_losses(
+            model=model_posenet, batch=test_batch_pose, shape=shape, progress=False, clip_denoised=False,
+            timestep_respacing=args.timestep_respacing_eval, cond_fn_with_grad=args.cond_fn_with_grad,
+            early_stop=args.early_stop, compute_loss=False, grad_type='prox', smplx_model=smplx_model)
+        if on_round is not None:
+            # observer hook (tests): may return a tensor that replaces this round's PoseNet output for the next round
+            repl = on_round(iter_idx, val_output_traj, traj_rec_full, test_batch_pose['cond'], val_output_pose)
+            if repl is not None:
+                val_output_pose = repl
+    return val_output_pose, val_output_traj
+
+
+def reconstruct_video_outputs(pose_dataset, smplx_model, test_batch_pose, val_output_pose, return_verts=True):
+    """test_prox_egobody.py:326-354 on the device: de-normalise the noisy input (test_batch_pose['motion_repr_noisy'] as
+    ``run_video_rounds`` leaves it, [W,294,1,Tp]) and the PoseNet output, and recover joints (and vertices) of the noisy
+    motion from its SMPL-X parameters and of the reconstruction from its absolute trajectory and from its SMPL-X
+    parameters.  Returns a dict of device tensors."""
+    noisy = test_batch_pose['motion_repr_noisy']
+    if noisy.dim() != 4 or tuple(noisy.shape) != tuple(val_output_pose.shape):
+        raise RohmB200Error(f"reconstruct_video_outputs: test_batch_pose['motion_repr_noisy'] must be the [W, 294, 1, Tp] "
+                            f"rows run_video_rounds leaves, like val_output_pose {tuple(val_output_pose.shape)}; got "
+                            f"{tuple(noisy.shape)}")
+    mean, std = glue.stats_on(pose_dataset, val_output_pose.device)
+    noisy = noisy[:, :, 0].permute(0, 2, 1) * std + mean
+    rec = val_output_pose[:, :, 0].permute(0, 2, 1) * std + mean
+    out = {'motion_repr_noisy': noisy, 'motion_repr_rec': rec}
+    res = recover_from_repr_smpl(split_repr(noisy), 'smplx_params', smplx_model, return_verts=return_verts)
+    res = res if return_verts else (res, None)
+    out['rec_ric_data_noisy'], out['smpl_verts_noisy'] = res
+    out['rec_ric_data_rec_from_abs_traj'] = recover_from_repr_smpl(split_repr(rec), 'joint_abs_traj', smplx_model)
+    res = recover_from_repr_smpl(split_repr(rec), 'smplx_params', smplx_model, return_verts=return_verts)
+    res = res if return_verts else (res, None)
+    out['rec_ric_data_rec_from_smpl'], out['smpl_verts_rec'] = res
+    return out
+
+
+def video_result_dicts(windows, outputs, test_batch_pose, frame_names=None):
+    """The pickle payload of test_prox_egobody.py:356-384, one dict (numpy) per recording of ``windows`` (the Windows of
+    ``windows.encode_video``), holding that recording's windows in start order, each once.  outputs: the dict of
+    ``reconstruct_video_outputs``; test_batch_pose: the pose batch after ``run_video_rounds``.  frame_names (optional, one
+    list of frame names per recording) fills 'frame_name_list' [n, clip_len] from each window's start; recording_name and
+    gender_gt stay with the caller, who knows them.
+
+    Two deliberate differences from the reference: it stores only its last batch's frame names (the same as these whenever
+    a recording fits in one batch), and its ``len // batch_size + 1`` loop appends a wrapped-around duplicate batch when
+    the window count is a multiple of the batch size; here every window appears once."""
+    W, R = len(windows), len(windows.lengths)
+    if frame_names is not None and len(frame_names) != R:
+        raise RohmB200Error(f"video_result_dicts: frame_names must hold one name list per recording ({R}), got "
+                            f"{len(frame_names)}")
+    host = lambda t: t.detach().cpu().numpy()
+    per_window = {'trans_scene2cano_list': host(test_batch_pose['transf_matrix']),
+                  'rec_ric_data_noisy_list': host(outputs['rec_ric_data_noisy']),
+                  'rec_ric_data_rec_list_from_abs_traj': host(outputs['rec_ric_data_rec_from_abs_traj']),
+                  'rec_ric_data_rec_list_from_smpl': host(outputs['rec_ric_data_rec_from_smpl']),
+                  'joints_input_scene_coord_list': host(test_batch_pose['noisy_joints_scene_coord']),
+                  'motion_repr_noisy_list': host(outputs['motion_repr_noisy']),
+                  'motion_repr_rec_list': host(outputs['motion_repr_rec']),
+                  'mask_joint_vis_list': host(test_batch_pose['mask_joint_vis'][:, 0:-2])}
+    if test_batch_pose.get('gt_joints_scene_coord') is not None:
+        per_window['joints_gt_scene_coord_list'] = host(test_batch_pose['gt_joints_scene_coord'])
+    bad = [k for k, v in per_window.items() if v.shape[0] != W]
+    if bad:
+        raise RohmB200Error(f"video_result_dicts: {bad} do not hold the {W} windows")
+    rec, start = host(windows.recording).astype(np.int64), host(windows.start).astype(np.int64)
+    payloads = []
+    for r in range(R):
+        idx = np.flatnonzero(rec == r)
+        idx = idx[np.argsort(start[idx], kind='stable')]
+        save = {k: v[idx] for k, v in per_window.items()}
+        save['repr_name_list'], save['repr_dim_dict'] = REPR_LIST, REPR_DIM_DICT
+        if frame_names is not None:
+            names = np.asarray(frame_names[r])
+            save['frame_name_list'] = np.asarray([names[s:s + windows.clip_len] for s in start[idx]]).reshape(
+                len(idx), windows.clip_len)
+        payloads.append(save)
+    return payloads
 
 
 def result_dict(args, outputs_per_batch):

@@ -1038,13 +1038,231 @@ def gen_windows_video(ref):
     print("windows_video.npz", os.path.getsize(os.path.join(OUT, "windows_video.npz")), "bytes")
 
 
+# The video driver in miniature: one recording per case cut into two 17-frame windows (17 + 15 frames), the shipped
+# video flags (sample_iter 2, iter2_cond_noisy_traj / iter2_cond_noisy_pose False, early_stop), a 10-step TrajNet and
+# the 12-step respaced PoseNet of gen_pipeline (every step guided)
+VIDEO_PIPE_CASES = (("N3Office_00034_01", 'prox', 'N3Office'), ("recording_20210907_S02_S01_01", 'egobody', 'seminar_g110'))
+# Short windows keep the fixture small (every stored [windows, 294, frames] state scales with the window): the driver's
+# computation is the same at every window length whose trajectory frames are a multiple of 16, and the GPU tests run the
+# 145-frame windows of encode_video through the same rounds.
+VIDEO_PIPE_CLIP = 17
+VIDEO_PIPE_FRAMES = VIDEO_PIPE_CLIP + VIDEO_PIPE_CLIP - 2
+VIDEO_PIPE_RECORDED_STEPS = (1, 0)
+# the batch keys the video driver reads (test_prox_egobody.py:185-354), stored per case; the trajectory batch's cond and
+# control_cond are channels of its motion_repr_noisy (asserted), so only the rows are stored
+VIDEO_PIPE_POSE_KEYS = ('motion_repr_noisy', 'mask_vec_vis', 'mask_joint_vis', 'keypoints_2d', 'transf_matrix',
+                        'focal_length', 'camera_center', 'noisy_joints_scene_coord')
+VIDEO_PIPE_TRAJ_KEYS = ('motion_repr_noisy',)
+
+
+def gen_video_pipeline(ref):
+    """The call sequence of test_prox_egobody.py:214-354 through the UNMODIFIED reference, on windows its own
+    DataloaderVideo cut from recordings written to a temporary directory (the layout of gen_windows_video): TrajNet ->
+    host glue on motion_repr_noisy -> PoseNet conditioned on the visibility-masked noisy rows with 2-D projection and
+    skating guidance (grad_type 'prox') -> reconstruction, 2 rounds (round 2 through TrajControl)."""
+    import json
+    import pickle
+    import tempfile
+    sys.path.insert(0, '/root/reference')
+    import data_loaders.dataloader_video as dlv
+    sys.path.pop(0)
+    get_repr_smplx = ref.mr.get_repr_smplx
+    g = np.random.default_rng(121)
+    tn_steps, rounds = 10, 2
+    ds_pose = synthetic.make_dataset('pose', seed=3, realistic_std=True)
+    ds_traj = synthetic.make_dataset('traj', seed=3, realistic_std=True)
+    body = _StubBody()
+    mp, _ = build_ref_posenet(ref, seed=1)
+    mp.dataset, mp.device = ds_pose, 'cpu'
+    mt, _ = build_ref_trajnet(ref, seed=2, control=False)
+    mc, _ = build_ref_trajnet(ref, seed=4, control=True)
+    args = argparse.Namespace(noise_schedule='cosine', sigma_small=True)
+    mk = ref.model_util.create_gaussian_diffusion
+    dp = mk(args, gd=ref.gdp, return_class=ref.respace.SpacedDiffusionPoseNet, num_diffusion_timesteps=1000,
+            timestep_respacing=POSE_RESPACING, device='cpu')
+    dt = mk(args, gd=ref.gdt, return_class=ref.respace.SpacedDiffusionTrajNet, num_diffusion_timesteps=tn_steps, device='cpu')
+    dc = mk(args, gd=ref.gdt, return_class=ref.respace.SpacedDiffusionTrajNet, num_diffusion_timesteps=tn_steps, device='cpu')
+    n = VIDEO_PIPE_FRAMES
+    out = {"meta": np.array([len(VIDEO_PIPE_CASES), tn_steps, 12, rounds, n, VIDEO_PIPE_CLIP]),
+           "recorded_steps": np.array(VIDEO_PIPE_RECORDED_STEPS)}
+
+    def dump(path, obj, mode='w'):
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        with open(path, mode) as fh:
+            (pickle.dump if mode == 'wb' else json.dump)(obj, fh)
+
+    def write_fits(root, prm):
+        for fr in range(n):
+            dump(os.path.join(root, f"frame_{fr:05d}", "000.pkl"), {k: v[fr:fr + 1] for k, v in prm.items()}, 'wb')
+
+    with tempfile.TemporaryDirectory() as tmp:
+        base, init = os.path.join(tmp, "base"), os.path.join(tmp, "init")
+        logs = {}
+        for task, ds in (("pose", ds_pose), ("traj", ds_traj)):
+            logs[task] = os.path.join(tmp, f"log_{task}")
+            cur, mean, std = 0, {}, {}
+            for k in ko.REPR_LIST:
+                mean[k], std[k] = ds.Mean[cur:cur + ko.REPR_DIM_DICT[k]], ds.Std[cur:cur + ko.REPR_DIM_DICT[k]]
+                cur += ko.REPR_DIM_DICT[k]
+            dump(os.path.join(logs[task], "AMASS_mean.pkl"), mean, 'wb')
+            dump(os.path.join(logs[task], "AMASS_std.pkl"), std, 'wb')
+        dump(os.path.join(base, "calibration", "Color.json"), VIDEO_PROX_CAM)
+        dump(os.path.join(base, "kinect_cam_params", "kinect_master", "Color.json"), VIDEO_EGO_CAM)
+        import pandas as pd
+        ego = [c for c in VIDEO_PIPE_CASES if c[1] == 'egobody']
+        pd.DataFrame({'recording_name': [c[0] for c in ego], 'target_idx': [0], 'target_gender': ['male'],
+                      'view': ['master'], 'scene_name': [c[2] for c in ego],
+                      'body_idx_fpv': ['1 male']}).to_csv(os.path.join(base, "egobody_rohm_info.csv"))
+        pd.DataFrame({'train': ['a'], 'val': ['c'], 'test': [ego[0][0]]}).to_csv(os.path.join(base, "data_splits.csv"))
+        for c, (name, dataset, scene) in enumerate(VIDEO_PIPE_CASES):
+            y_up = dataset == 'egobody'
+            cam = _rigid([0.2, 2.9, 0.1], [0.5, 1.4, 2.0]) if y_up else _rigid([-2.0, 0.3, 0.4], [1.0, -2.0, 2.5])
+            heading = np.pi - 0.02 if c == 0 else -np.pi + 0.015
+            prm = video_recording(g, n, cam, y_up, heading)
+            kp = video_keypoints(g, n)
+            mask = g.uniform(0, 1, (n, 25)) > 0.15
+            if y_up:
+                fit_dir = os.path.join(init, name, "body_idx_0", "results")
+                write_fits(os.path.join(base, "smplx_camera_wearer_test", name, "body_idx_0", "results"),
+                           video_recording(g, n, cam, True, heading + 0.1))
+                dump(os.path.join(base, "calibrations", name, "cal_trans", "kinect12_to_world", scene + ".json"),
+                     {'trans': cam.tolist()})
+                kp_dir = os.path.join(base, "keypoints_cleaned", name, "master")
+                mask_path = os.path.join(base, "mask_joint", name, "master", "mask_joint.npy")
+            else:
+                fit_dir = os.path.join(init, name, "results")
+                dump(os.path.join(base, "cam2world", scene + ".json"), cam.tolist())
+                kp_dir = os.path.join(base, "keypoints_openpose", name)
+                mask_path = os.path.join(base, "mask_joint", name, "mask_joint.npy")
+            write_fits(fit_dir, prm)
+            for fr in range(n):
+                dump(os.path.join(kp_dir, f"frame_{fr:05d}_keypoints.json"),
+                     {'people': [{'pose_keypoints_2d': kp[fr].reshape(-1).tolist()}]})
+            os.makedirs(os.path.dirname(mask_path), exist_ok=True)
+            np.save(mask_path, mask)
+            loaders = {task: dlv.DataloaderVideo(dataset=dataset, init_root=init, base_dir=base, body_model_path='',
+                                                 recording_name=name, use_scene_floor_height=True,
+                                                 repr_abs_only=task == 'traj', task=task, overlap_len=2,
+                                                 clip_len=VIDEO_PIPE_CLIP,
+                                                 logdir=logs[task], device='cpu') for task in ("pose", "traj")}
+            items = {task: [d[w] for w in range(len(d))] for task, d in loaders.items()}
+            assert len(items['pose']) == 2, len(items['pose'])
+            stack = lambda its, key: torch.from_numpy(np.asarray([it[key] for it in its]))
+            pose = {k: stack(items['pose'], k) for k in VIDEO_PIPE_POSE_KEYS + (('gt_joints_scene_coord',) if y_up else ())}
+            traj = {k: stack(items['traj'], k) for k in ('motion_repr_noisy', 'cond', 'control_cond')}
+            assert torch.equal(traj['cond'], traj['motion_repr_noisy'][..., list(ABS_CHANNELS)])
+            assert torch.equal(traj['control_cond'], traj['motion_repr_noisy'][..., -ds_traj.pose_feat_dim:])
+            for k, v in list(pose.items()) + [('traj_' + k, traj[k]) for k in VIDEO_PIPE_TRAJ_KEYS]:
+                # the PROX loader's undistorted keypoints are float64, as the reference's guidance reads them: kept so
+                assert k == 'keypoints_2d' or v.dtype == torch.float32, (k, v.dtype)
+                out[f"c{c}_{'' if k.startswith('traj_') else 'pose_'}{k}"] = v.numpy()
+            # one camera per recording: the reference's guidance reads dataset.cam_R / cam_t
+            ds_pose.cam_R, ds_pose.cam_t = loaders['pose'].cam_R, loaders['pose'].cam_t
+            c2w = torch.eye(4)
+            c2w[:3, :3], c2w[:3, 3] = ds_pose.cam_R, ds_pose.cam_t.reshape(3)
+            out[f"c{c}_cam2world"] = c2w.numpy()
+            out[f"c{c}_meta"] = np.array([int(y_up), len(items['pose'])])
+            B = len(items['pose'])
+            tfd, pfd = ds_traj.traj_feat_dim, ds_traj.pose_feat_dim
+            val_pose = None
+            with _patched_th(ref.gdp, 130 + c), _patched_th(ref.gdt, 140 + c):
+                for it in range(rounds):
+                    shape = list(traj['motion_repr_noisy'][:, :, 0:tfd].shape)
+                    if it == 0:
+                        _, val_traj = dt.eval_losses(model=mt, batch=traj, shape=shape, progress=False, clip_denoised=False,
+                                                     timestep_respacing='', compute_loss=False, cond_fn_with_grad=True,
+                                                     smplx_model=body)
+                    else:
+                        traj['control_cond'] = torch.zeros([shape[0], shape[1], pfd])
+                        traj['control_cond'][:, 0:-1] = val_pose[:, :, 0].permute(0, 2, 1)[:, :, -pfd:]
+                        traj['control_cond'][:, -1] = traj['control_cond'][:, -2].clone()
+                        _, val_traj = dc.eval_losses(model=mc, batch=traj, shape=shape, progress=False, clip_denoised=False,
+                                                     timestep_respacing='', cond_fn_with_grad=True, compute_loss=False,
+                                                     smplx_model=body)
+                    comp = traj['motion_repr_noisy'].clone()
+                    comp[..., 0], comp[..., 2:4], comp[..., 6] = val_traj[..., 0], val_traj[..., 1:3], val_traj[..., 3]
+                    comp[..., 7:13], comp[..., 16:19] = val_traj[..., 4:10], val_traj[..., 10:13]
+                    if it == 0:
+                        traj['motion_repr_noisy'] = comp
+                    if it < rounds - 1:  # iter2_cond_noisy_traj False
+                        traj['cond'] = val_traj
+                    full = comp.detach().numpy() * ds_traj.Std + ds_traj.Mean
+                    rep = _rep_dict(torch.from_numpy(full))
+                    joints, _ = ref.mr.recover_from_repr_smpl(rep, recover_mode='smplx_params', smplx_model=_VertsBody(body),
+                                                             return_verts=True)
+                    joints = joints.detach().numpy()
+                    rows = []
+                    for i in range(B):
+                        go = ref.kt.rotation_matrix_to_angle_axis(ref.quat.rot6d_to_rotmat(rep['smplx_rot_6d'][i]))
+                        bp = ref.kt.rotation_matrix_to_angle_axis(
+                            ref.quat.rot6d_to_rotmat(rep['smplx_body_pose_6d'][i].reshape(-1, 6)))
+                        d = get_repr_smplx(positions=joints[i], smplx_params_dict={
+                            'transl': rep['smplx_trans'][i].numpy(), 'global_orient': go.numpy(),
+                            'body_pose': bp.reshape(-1, 63).numpy(), 'betas': rep['smplx_betas'][i].numpy()},
+                            feet_vel_thre=5e-5)
+                        row = np.concatenate([d[k] for k in ko.REPR_LIST], axis=-1)
+                        rows.append(((row - ds_pose.Mean) / ds_pose.Std)[:, 0:22])
+                    traj_full = torch.tensor(np.asarray(rows))
+                    if it == 0:
+                        pose['motion_repr_noisy'] = pose['motion_repr_noisy'][:, 0:-1]
+                        src = pose['motion_repr_noisy'].clone()
+                    else:  # iter2_cond_noisy_pose False: the previous PoseNet output (a permuted view, as the driver)
+                        src = val_pose[:, :, 0].permute(0, 2, 1)
+                    pose['cond'] = src
+                    pose['cond'][:, :, 0:22] = traj_full
+                    if it < 1:  # mask_iter_num = 1
+                        pose['cond'] = pose['cond'] * pose['mask_vec_vis'][:, 0:-2, :]
+                        pose['cond'][:, :, -4:] = 0.
+                    if it == 0:
+                        pose['motion_repr_noisy'] = torch.permute(pose['motion_repr_noisy'], (0, 2, 1)).unsqueeze(-2)
+                    pose['cond'] = torch.permute(pose['cond'], (0, 2, 1)).unsqueeze(-2)
+                    out[f"c{c}_r{it}_cond"] = pose['cond'].detach().numpy().copy()
+                    seen = {}
+                    orig = dp.p_sample_with_grad
+
+                    def recording(model, batch, x, t, **kw):
+                        seen[int(t[0])] = x.detach().clone()
+                        return orig(model, batch, x, t, **kw)
+
+                    dp.p_sample_with_grad = recording
+                    _, val_pose = dp.eval_losses(model=mp, batch=pose, shape=list(pose['motion_repr_noisy'].shape),
+                                                 progress=False, clip_denoised=False, timestep_respacing='',
+                                                 cond_fn_with_grad=True, early_stop=True, compute_loss=False,
+                                                 grad_type='prox', smplx_model=body)
+                    dp.p_sample_with_grad = orig
+                    for i in VIDEO_PIPE_RECORDED_STEPS:
+                        out[f"c{c}_r{it}_xt{i}"] = seen[i].numpy()
+                    out[f"c{c}_r{it}_val_traj"] = val_traj.detach().numpy()
+                    out[f"c{c}_r{it}_traj_full"] = traj_full.numpy().astype(np.float32)
+                    out[f"c{c}_r{it}_val_pose"] = val_pose.detach().numpy().copy()
+                    print(f"video pipeline case {c} ({dataset}) round {it}: |val_traj| {float(val_traj.abs().max()):.3f} "
+                          f"|val_pose| {float(val_pose.abs().max()):.3f}")
+            # :326-354: joints of the noisy input and of the reconstruction
+            rec = val_pose[:, :, 0].permute(0, 2, 1).detach().numpy() * ds_pose.Std + ds_pose.Mean
+            noisy = pose['motion_repr_noisy'][:, :, 0].permute(0, 2, 1).detach().numpy() * ds_pose.Std + ds_pose.Mean
+            rep_n, rep_r = _rep_dict(torch.from_numpy(noisy)), _rep_dict(torch.from_numpy(rec))
+            out[f"c{c}_rec_noisy"] = ref.mr.recover_from_repr_smpl(rep_n, recover_mode='smplx_params',
+                                                                   smplx_model=_VertsBody(body), return_verts=True)[0].detach().numpy()
+            out[f"c{c}_rec_from_abs_traj"] = ref.mr.recover_from_repr_smpl(rep_r, recover_mode='joint_abs_traj',
+                                                                           smplx_model=body).detach().numpy()
+            out[f"c{c}_rec_from_smpl"] = ref.mr.recover_from_repr_smpl(rep_r, recover_mode='smplx_params',
+                                                                       smplx_model=_VertsBody(body),
+                                                                       return_verts=True)[0].detach().numpy()
+    out = {k: (v.astype(np.float32) if v.dtype == np.float64 and not k.endswith('keypoints_2d') else v)
+           for k, v in out.items()}
+    path = os.path.join(OUT, "video_pipeline.npz")
+    np.savez_compressed(path, **out)
+    print("video_pipeline.npz", os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     ref = import_reference()
     which = sys.argv[1:] or ["schedules", "posenet", "trajnet", "sampling", "kinematics", "glue", "pipeline",
-                             "clip_guidance", "windows", "windows_noise", "windows_video"]
+                             "clip_guidance", "windows", "windows_noise", "windows_video", "video_pipeline"]
     for w in which:
         {"schedules": gen_schedules, "posenet": gen_posenet, "trajnet": gen_trajnet, "sampling": gen_sampling,
          "kinematics": gen_kinematics, "glue": gen_glue, "pipeline": gen_pipeline, "clip_guidance": gen_clip_guidance,
-         "windows": gen_windows, "windows_noise": gen_windows_noise, "windows_video": gen_windows_video}[w](ref)
+         "windows": gen_windows, "windows_noise": gen_windows_noise, "windows_video": gen_windows_video,
+         "video_pipeline": gen_video_pipeline}[w](ref)
