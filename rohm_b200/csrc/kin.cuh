@@ -37,17 +37,18 @@ __device__ __forceinline__ M3 rot6d_to_mat(const float* x, float* n1 = nullptr, 
   return {b1, b2, cross(b1, b2)};
 }
 
-// VJP of rot6d_to_mat: G = dL/dR (columns g1, g2, g3) -> dL/dx[6].
+// VJP of rot6d_to_mat: G = dL/dR (columns g1, g2, g3) -> dL/dx[6].  Below the 1e-12 clamp F.normalize divides by the
+// constant 1e-12 (clamp_min passes no gradient to the norm), so there the pull-back has no projection onto b's normal plane.
 __device__ __forceinline__ void rot6d_backward(const float* x, const M3& G, float* gx) {
   float l1, l2, s;
   const M3 R = rot6d_to_mat(x, &l1, &l2, &s);
   const V3 a2 = {x[1], x[3], x[5]};
   V3 gb1 = G.c0 + cross(R.c1, G.c2);   // b3 = b1 x b2
   V3 gb2 = G.c1 + cross(G.c2, R.c0);
-  const V3 gu2 = (1.0f / l2) * (gb2 - dot(gb2, R.c1) * R.c1);
+  const V3 gu2 = (1.0f / l2) * (l2 > 1e-12f ? gb2 - dot(gb2, R.c1) * R.c1 : gb2);
   const V3 ga2 = gu2 - dot(R.c0, gu2) * R.c0;
   gb1 = gb1 - s * gu2 - dot(gu2, R.c0) * a2;
-  const V3 ga1 = (1.0f / l1) * (gb1 - dot(gb1, R.c0) * R.c0);
+  const V3 ga1 = (1.0f / l1) * (l1 > 1e-12f ? gb1 - dot(gb1, R.c0) * R.c0 : gb1);
   gx[0] = ga1.x, gx[2] = ga1.y, gx[4] = ga1.z;
   gx[1] = ga2.x, gx[3] = ga2.y, gx[5] = ga2.z;
 }

@@ -1,6 +1,7 @@
 """ctypes driver of tests/native/libkernel_probe.so: the GEMM (rohm_b200/csrc/gemm.cu), attention (attention.cu) and
-GroupNorm + Mish (groupnorm.cu) kernels launched directly on torch device tensors, plus the operand packing the engines do
-(not collected by pytest).  The launching functions take `reps`: that many launches back to back on the default stream."""
+GroupNorm + Mish (groupnorm.cu) kernels launched directly on torch device tensors, the operand packing the engines do and
+the rotation / trajectory helpers of kin.cuh and repr.cuh one element at a time (not collected by pytest).  The launching functions take `reps`: that many launches back to
+back on the default stream."""
 import ctypes as C
 import os
 
@@ -72,6 +73,8 @@ def lib():
         _lib.probe_attention.argtypes = [C.POINTER(Attn), C.c_int]
         _lib.probe_group_norm.argtypes = [C.POINTER(GnArgs), C.c_int, C.c_int, C.c_int, C.c_void_p]
         _lib.probe_group_norm_cluster.argtypes = [C.c_int, C.c_int, C.c_int]
+        _lib.probe_kin.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+        _lib.probe_clip_of_frame.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
     return _lib
 
 
@@ -215,3 +218,74 @@ def group_norm(part, splits, split_stride, bias, gamma, beta, tp, tp_stride, r1,
 def group_norm_cluster(T, C_, groups=8):
     """The cluster size the TrajNet engine chooses for groups of T rows of C_ / groups channels."""
     return lib().probe_group_norm_cluster(T, C_, groups)
+
+
+# tests/native/kernel_probe.cu KinOp
+OP_ROT6D, OP_ROT6D_BACKWARD, OP_MAT_TO_AA, OP_RODRIGUES, OP_ROUND_TRIP, OP_ROTVEC, OP_HEADING, OP_QROT_Z, OP_TRAJ = range(9)
+
+
+def _kin(op, a, n_out, b=None, out2=None):
+    """One helper over the rows of the fp32 device tensor a ([n, k]) -> fp32 [n, n_out]."""
+    a = a.float().contiguous()
+    n = a.shape[0]
+    out = torch.empty(n, n_out, dtype=torch.float32, device=a.device)
+    b = None if b is None else b.float().contiguous()
+    assert lib().probe_kin(op, a.data_ptr(), _ptr(b), n, out.data_ptr(), _ptr(out2)) == 0
+    return out
+
+
+def rot6d_to_mat(x):
+    """kin::rot6d_to_mat on x [n, 6] -> (R [n, 3, 3], (l1, l2, s) [n, 3])."""
+    lls = torch.empty(x.shape[0], 3, dtype=torch.float32, device=x.device)
+    return _kin(OP_ROT6D, x, 9, out2=lls).view(-1, 3, 3), lls
+
+
+def rot6d_backward(x, G):
+    """kin::rot6d_backward: x [n, 6], G = dL/dR [n, 3, 3] -> dL/dx [n, 6]."""
+    return _kin(OP_ROT6D_BACKWARD, x, 6, b=G.reshape(-1, 9))
+
+
+def mat_to_aa(R):
+    """kin::mat_to_aa: R [n, 3, 3] -> axis-angle [n, 3]."""
+    return _kin(OP_MAT_TO_AA, R.reshape(-1, 9), 3)
+
+
+def rodrigues(r):
+    """kin::rodrigues: r [n, 3] -> R [n, 3, 3]."""
+    return _kin(OP_RODRIGUES, r, 9).view(-1, 3, 3)
+
+
+def rot6d_round_trip(x):
+    """kin::rodrigues(kin::mat_to_aa(kin::rot6d_to_mat(x))): x [n, 6] -> R [n, 3, 3]."""
+    return _kin(OP_ROUND_TRIP, x, 9).view(-1, 3, 3)
+
+
+def rotvec_to_mat(r):
+    """repr::rotvec_to_mat: r [n, 3] -> R [n, 3, 3]."""
+    return _kin(OP_ROTVEC, r, 9).view(-1, 3, 3)
+
+
+def heading_quat(j1, j2, j17, j16):
+    """repr::heading_quat on joints [n, 3] each -> (q0, q1, q3) [n, 3]."""
+    return _kin(OP_HEADING, torch.cat([j1, j2, j17, j16], dim=1), 3)
+
+
+def qrot_z(wz, v):
+    """repr::qrot_z: wz [n, 2] = (w, z), v [n, 3] -> [n, 3]."""
+    return _kin(OP_QROT_Z, wz, 3, b=v)
+
+
+def traj_channels(q, roots, rots, trs):
+    """repr::traj_channels of two frames: q [n, 4] = (w0, z0, w1, z1), roots [n, 2, 3], rots [n, 2, 3, 3], trs [n, 2, 3]
+    -> channels [n, 22]."""
+    n = q.shape[0]
+    return _kin(OP_TRAJ, torch.cat([q, roots.reshape(n, 6), rots.reshape(n, 18), trs.reshape(n, 6)], dim=1), 22)
+
+
+def clip_of_frame(clip_off, frames):
+    """kin::clip_of_frame over int32 device tensors: clip_off [B + 1], frames [n] -> clip ids [n] (int32)."""
+    clip_off, frames = clip_off.int().contiguous(), frames.int().contiguous()
+    out = torch.empty_like(frames)
+    B = clip_off.numel() - 1
+    assert lib().probe_clip_of_frame(clip_off.data_ptr(), B, frames.data_ptr(), frames.numel(), out.data_ptr()) == 0
+    return out

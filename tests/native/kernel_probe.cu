@@ -1,5 +1,5 @@
 // Test-only entry points into the GEMM, attention and GroupNorm kernels (rohm_b200/csrc/gemm.cu, attention.cu,
-// groupnorm.cu) and the operand-pair helpers of ptx.cuh, driven from Python through ctypes by tests/kernel_probe.py and
+// groupnorm.cu), the operand-pair helpers of ptx.cuh and the rotation / trajectory helpers of kin.cuh and repr.cuh, driven from Python through ctypes by tests/kernel_probe.py and
 // linked against the product's own objects of those sources.  Every function takes plain structs / device pointers, builds the tensor maps itself with the library's own
 // helpers and returns 0, a cudaError_t (> 0) or -CUresult of a failed tensor-map encoding.  The launching probes run their
 // launch `reps` >= 1 times back to back on the default stream, set-up done once, so that tools can time them.  The product
@@ -9,6 +9,8 @@
 #include "../../rohm_b200/csrc/attention.cuh"
 #include "../../rohm_b200/csrc/gemm.cuh"
 #include "../../rohm_b200/csrc/groupnorm.cuh"
+#include "../../rohm_b200/csrc/kin.cuh"
+#include "../../rohm_b200/csrc/repr.cuh"
 
 using namespace rohm;
 
@@ -45,9 +47,103 @@ __global__ void pair_forms_kernel(const float4* __restrict__ x, int64_t n4, __ha
   }
 }
 
+// The kin.cuh / repr.cuh helpers, one element per iteration of a grid-stride loop.  Matrices are row-major [9].
+using kin::M3;
+using kin::V3;
+
+__device__ __forceinline__ M3 load_m3(const float* m) {
+  return {{m[0], m[3], m[6]}, {m[1], m[4], m[7]}, {m[2], m[5], m[8]}};
+}
+__device__ __forceinline__ void store_m3(const M3& R, float* o) {
+  o[0] = R.c0.x, o[1] = R.c1.x, o[2] = R.c2.x, o[3] = R.c0.y, o[4] = R.c1.y, o[5] = R.c2.y;
+  o[6] = R.c0.z, o[7] = R.c1.z, o[8] = R.c2.z;
+}
+__device__ __forceinline__ V3 load_v3(const float* v) { return {v[0], v[1], v[2]}; }
+__device__ __forceinline__ void store_v3(V3 v, float* o) { o[0] = v.x, o[1] = v.y, o[2] = v.z; }
+
+enum KinOp { kOpRot6d, kOpRot6dBackward, kOpMatToAa, kOpRodrigues, kOpRoundTrip, kOpRotvec, kOpHeading, kOpQrotZ,
+             kOpTraj };
+
+// a: inputs of element i at a + i * in_stride, b: second input (G of the backward, v of qrot_z) at b + i * 9 or i * 3,
+// o: outputs at o + i * out_stride, o2: the (l1, l2, s) triple of rot6d_to_mat at o2 + i * 3.
+__global__ void kin_kernel(int op, const float* __restrict__ a, const float* __restrict__ b, int64_t n,
+                           float* __restrict__ o, float* __restrict__ o2) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    switch (op) {
+      case kOpRot6d: {
+        float x[6], l1, l2, s;
+        for (int e = 0; e < 6; ++e) x[e] = a[i * 6 + e];
+        store_m3(kin::rot6d_to_mat(x, &l1, &l2, &s), o + i * 9);
+        o2[i * 3] = l1, o2[i * 3 + 1] = l2, o2[i * 3 + 2] = s;
+        break;
+      }
+      case kOpRot6dBackward: {
+        float x[6], gx[6];
+        for (int e = 0; e < 6; ++e) x[e] = a[i * 6 + e];
+        kin::rot6d_backward(x, load_m3(b + i * 9), gx);
+        for (int e = 0; e < 6; ++e) o[i * 6 + e] = gx[e];
+        break;
+      }
+      case kOpMatToAa: store_v3(kin::mat_to_aa(load_m3(a + i * 9)), o + i * 3); break;
+      case kOpRodrigues: store_m3(kin::rodrigues(load_v3(a + i * 3)), o + i * 9); break;
+      case kOpRoundTrip: {
+        float x[6];
+        for (int e = 0; e < 6; ++e) x[e] = a[i * 6 + e];
+        store_m3(kin::rodrigues(kin::mat_to_aa(kin::rot6d_to_mat(x))), o + i * 9);
+        break;
+      }
+      case kOpRotvec: store_m3(repr::rotvec_to_mat(load_v3(a + i * 3)), o + i * 9); break;
+      case kOpHeading: {
+        const float* j = a + i * 12;  // joints 1, 2, 17, 16
+        repr::heading_quat(load_v3(j), load_v3(j + 3), load_v3(j + 6), load_v3(j + 9), o[i * 3], o[i * 3 + 1],
+                           o[i * 3 + 2]);
+        break;
+      }
+      case kOpQrotZ: store_v3(repr::qrot_z(a[i * 2], a[i * 2 + 1], load_v3(b + i * 3)), o + i * 3); break;
+      case kOpTraj: {
+        // w0, z0, w1, z1, root(0), root(1), rot(0), rot(1) (row-major), tr(0), tr(1)
+        const float* t = a + i * 34;
+        repr::traj_channels(
+            o + i * repr::kTrajFull, t[0], t[1], t[2], t[3], [&](int k) { return load_v3(t + 4 + 3 * k); },
+            [&](int k) { return load_m3(t + 10 + 9 * k); }, [&](int k, int c) { return t[28 + 3 * k + c]; });
+        break;
+      }
+    }
+  }
+}
+
+__global__ void clip_of_frame_kernel(const int* __restrict__ clip_off, int B, const int* __restrict__ f, int64_t n,
+                                     int* __restrict__ out) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
+    out[i] = kin::clip_of_frame(clip_off, B, f[i]);
+}
+
+unsigned grid_for(int64_t n) {
+  const int64_t blocks = (n + 255) / 256;
+  return static_cast<unsigned>(blocks < 4096 ? blocks : 4096);
+}
+
 }  // namespace
 
 extern "C" {
+
+// One kin.cuh / repr.cuh helper over n elements (KinOp, layouts at kin_kernel); n = 0 launches nothing.
+int probe_kin(int op, const float* a, const float* b, int64_t n, float* out, float* out2) {
+  if (n < 0 || op < kOpRot6d || op > kOpTraj) return static_cast<int>(cudaErrorInvalidValue);
+  if (n == 0) return 0;
+  kin_kernel<<<grid_for(n), 256>>>(op, a, b, n, out, out2);
+  return static_cast<int>(cudaGetLastError());
+}
+
+// kin::clip_of_frame(clip_off, B, f[i]) for n packed frame indices.
+int probe_clip_of_frame(const int* clip_off, int B, const int* f, int64_t n, int* out) {
+  if (n < 0 || B < 1) return static_cast<int>(cudaErrorInvalidValue);
+  if (n == 0) return 0;
+  clip_of_frame_kernel<<<grid_for(n), 256>>>(clip_off, B, f, n, out);
+  return static_cast<int>(cudaGetLastError());
+}
 
 // One A segment: rows of a row-major hi/lo matrix [rows, cols] with pitch ld (elements), read at row m * row_mul + row_shift.
 struct ProbeSeg {
