@@ -511,6 +511,42 @@ ROHM_API int rohm_window_scene_joints(rohm_ctx* ctx, const float* joints, const 
                                       const int* win_rec, const int* win_start, int W, int clip_len, float* out,
                                       void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Evaluation metrics (eval_amass_full.py:71-147, eval_prox_egobody.py:172-272), rohm_b200/metrics.py
+ * ------------------------------------------------------------------------------------------------------------ */
+
+/* B clips packed frame after frame: clip b is rows [frame_off[b], frame_off[b+1]) (device int64 [B+1]) of gt / rec
+ * [N,22,3] (rec_ric_data_clean / rec_ric_data_rec_from_smpl) and of repr_clean / repr_rec [N,repr_width] (the contact
+ * labels are the last 4 channels).  A (frame, joint) is occluded when bit j of occ_joints is set and occ_lo <= t < occ_hi
+ * (clamped to the clip).  Per clip: h0 [B] (the NaN-propagating minimum z of gt).  Per packed row: mpjpe [N,22], accerr
+ * [N,22] (rows t >= T-2 of a clip are 0), skate_gt / skate_rec [N] (row T-1 is 0), contact [N,4] matches, pene_freq [N,2]
+ * and pene_dist [N,2] (toes 10, 11).  sums [B,5] float64 (mpjpe, visible, occluded, accel error, pene dist) and counts
+ * [B,11] int64 (mpjpe n, visible n, occluded n, contact matches, contact n, skating gt, skating rec, skating n, accel n,
+ * pene freq, pene n), each in a fixed order. */
+ROHM_API int rohm_eval_amass(rohm_ctx* ctx, const float* gt, const float* rec, const float* repr_clean,
+                             const float* repr_rec, int repr_width, const int64_t* frame_off, int B, unsigned occ_joints,
+                             int occ_lo, int occ_hi, float* h0, float* mpjpe, float* accerr, unsigned char* skate_gt,
+                             unsigned char* skate_rec, unsigned char* contact, unsigned char* pene_freq,
+                             float* pene_dist, double* sums, int64_t* counts, void* stream);
+
+/* W video windows of T frames: rec [W,T,22,3] canonical joints, mapped to the scene by the float64 inverse of transf
+ * [W,4,4] rounded to float32; floor [R] per recording (win_rec [W] device int32); y_up = 1 for EgoBody (height y,
+ * horizontal xz), 0 for PROX (z; xy).  Optional ground truth gt [W,gt_frames,22,3] and visibility mask_vis
+ * [W,mask_frames,22] (first T frames used; the mask needs gt); without gt, accerr / gmpjpe / mpjpe may be NULL.  Outputs:
+ * skate [W,T-1], acc and accerr [W,T-2] (per frame, the mean over joints), gmpjpe and mpjpe [W,T,22], pene_freq and
+ * pene_dist [W,T]; sums [W,10] float64 (acc, acc error, gmpjpe, mpjpe, vis num, vis den, occ num, occ den, pene freq,
+ * pene dist) and counts [W,1] int64 (skating frames). */
+ROHM_API int rohm_eval_video(rohm_ctx* ctx, const float* rec, int T, const float* transf, const float* gt, int gt_frames,
+                             const float* mask_vis, int mask_frames, const int* win_rec, const float* floor, int W,
+                             int y_up, unsigned char* skate, float* acc, float* accerr, float* gmpjpe, float* mpjpe,
+                             float* pene_freq, float* pene_dist, double* sums, int64_t* counts, void* stream);
+
+/* Group sums of per-item rows sums [n,ks] / counts [n,kc]: group g sums items order[group_off[g] .. group_off[g+1]) in
+ * that order (device int32), row n_groups of out_sums [n_groups+1,ks] / out_counts [n_groups+1,kc] sums the groups in
+ * order. */
+ROHM_API int rohm_eval_reduce(rohm_ctx* ctx, const double* sums, int ks, const int64_t* counts, int kc, const int* order,
+                              const int* group_off, int n_groups, double* out_sums, int64_t* out_counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

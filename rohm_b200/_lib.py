@@ -98,6 +98,10 @@ SIGNATURES = {
                                       _i, C.POINTER(_i), _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "rohm_window_keypoints": (_i, [_p, _p, _p, _p, _p, _p, _i, _p, _p, _p, _i, _i, _p, _p, _p, _p]),
     "rohm_window_scene_joints": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p]),
+    "rohm_eval_amass": (_i, [_p, _p, _p, _p, _p, _i, _p, _i, C.c_uint, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
+                             _p]),
+    "rohm_eval_video": (_i, [_p, _p, _i, _p, _p, _i, _p, _i, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "rohm_eval_reduce": (_i, [_p, _p, _i, _p, _i, _p, _p, _i, _p, _p, _p]),
 }
 
 _lock = threading.Lock()

@@ -1255,14 +1255,257 @@ def gen_video_pipeline(ref):
     print("video_pipeline.npz", os.path.getsize(path), "bytes")
 
 
+# ------------------------------------------------------------------------------------------------------------ metrics
+EVAL_AMASS_RUNS = (('lower', 0.0), ('full', 0.1), ('full', 0.0), ('full', 0.7))
+EVAL_VIDEO_T = 20  # frames per synthetic window: the scripts take any clip length
+EVAL_VIDEO_WINDOWS = (1, 2, 1, 3, 1, 1, 2, 1, 1, 1, 1, 1, 2, 1, 1, 1, 1, 1, 1)  # per recording of --recording_name all
+
+
+def _eval_stubs():
+    """Stand-ins for what the evaluation scripts import but do not use for their numbers: configargparse (an argparse
+    shim), open3d / trimesh (empty) and pyrender (attribute lookups return a no-op class)."""
+    cap = types.ModuleType('configargparse')
+
+    class ArgParser(argparse.ArgumentParser):
+        def __init__(self, config_file_parser_class=None, **kw):
+            super().__init__(**kw)
+
+        def add_argument(self, *a, is_config_file=False, **kw):
+            return super().add_argument(*a, **kw)
+
+    cap.ArgParser, cap.ArgumentDefaultsHelpFormatter, cap.YAMLConfigFileParser = \
+        ArgParser, argparse.ArgumentDefaultsHelpFormatter, object
+    pyrender = types.ModuleType('pyrender')
+    pyrender.__getattr__ = lambda name: type(name, (), {'__init__': lambda self, *a, **k: None})
+    return {'configargparse': cap, 'open3d': types.ModuleType('open3d'), 'trimesh': types.ModuleType('trimesh'),
+            'pyrender': pyrender}
+
+
+def _run_reference_script(name, argv):
+    import runpy
+    old = sys.argv
+    sys.argv = [name] + argv
+    sys.path.insert(0, '/root/reference')
+    try:
+        return runpy.run_path(os.path.join('/root/reference', name), run_name='__main__')
+    finally:
+        sys.argv = old
+        sys.path.pop(0)
+
+
+def _threshold_speed(g):
+    """A float32 displacement dx with float32(|dx| * 30) == float32(0.1): a foot exactly at the speed threshold."""
+    dx = np.float32(0.1 / 30)
+    while np.float32(dx * np.float32(30)) != np.float32(0.1):
+        dx = np.nextafter(dx, np.float32(1))
+    return dx
+
+
+def eval_amass_clips(g, n, T, with_nan=False):
+    """Clean and reconstructed joints [n,T,22,3] with feet crossing every skating threshold, some exactly on one,
+    penetrating toes, and contact labels [n,T,4] (the reconstruction's around 0.5, one exactly 0.5, one NaN)."""
+    base = np.cumsum(g.normal(0, 0.004, (n, T, 1, 3)), axis=1) + g.normal(0, 0.3, (n, 1, 22, 3))
+    G = base + g.normal(0, 0.002, (n, T, 22, 3))
+    G[..., 2] = np.abs(G[..., 2]) + 0.2
+    G[:, :, [7, 10, 8, 11], 2] = g.uniform(0.0, 0.22, (n, T, 4))
+    G[:, 0, 0, 2] = 0.0  # h0 = 0 exactly, so that heights equal the joints' z
+    G = G.astype(np.float32)
+    P = (G + g.normal(0, 0.02, G.shape)).astype(np.float32)
+    P[:, :, [10, 11], 2] = g.uniform(-0.12, 0.2, (n, T, 2))
+    # exact thresholds: ankle at 0.15, toe at 0.1, a foot moving at exactly 0.1 m/s
+    G[0, 10:20, 7, 2], G[0, 10:20, 10, 2] = np.float32(0.15), np.float32(0.1)
+    dx = _threshold_speed(g)
+    for t in range(30, min(40, T - 1), 2):
+        for j in (7, 10, 8, 11):
+            G[0, t, j, 0:2] = 0.0
+            G[0, t + 1, j, 0:2] = (dx, 0.0)
+            G[0, t, j, 2] = G[0, t + 1, j, 2] = 0.01
+    P[1, 50:60] = G[1, 50:60]
+    lc = (g.uniform(0, 1, (n, T, 4)) > 0.5).astype(np.float32)
+    lc[0, 0, 0] = 0.5
+    lr = g.uniform(0, 1, (n, T, 4)).astype(np.float32)
+    lr[0, 1, 0], lr[0, 2, 1] = 0.5, np.nan
+    if with_nan:
+        G[0, 5, 3, 1] = np.nan  # poisons only mpjpe
+        G[0, 7, 4, 2] = np.nan  # poisons h0 of clip 0
+        P[1, 9, 10, 2] = np.nan
+    return G, P, lc, lr
+
+
+def eval_video_recordings(g, dataset, floors, T=EVAL_VIDEO_T):
+    """Per recording: canonical joints [n,T,22,3], transf [n,4,4] (a rigid scene -> canonical map), and for EgoBody the
+    scene ground truth [n,T+2,22,3] and visibility [n,T,22]; the scene feet hover around the recording's floor."""
+    up, horiz = (1, [0, 2]) if dataset == 'egobody' else (2, [0, 1])
+    out = []
+    for r, n in enumerate(EVAL_VIDEO_WINDOWS):
+        S = np.cumsum(g.normal(0, 0.004, (n, T + 2, 1, 3)), axis=1) + g.normal(0, 0.3, (n, 1, 22, 3))
+        S = S + g.normal(0, 0.002, S.shape)
+        S[..., up] = floors[r] + np.abs(S[..., up]) + 0.2
+        S[:, :, [7, 10, 8, 11], up] = floors[r] + g.uniform(-0.1, 0.25, (n, T + 2, 4))
+        drift = np.cumsum(g.normal(0, 0.006, (n, T + 2, 4, 2)), axis=1)
+        for f, j in enumerate((7, 10, 8, 11)):
+            for a, axis in enumerate(horiz):
+                S[:, :, j, axis] += drift[:, :, f, a]
+        transf = np.zeros((n, 4, 4))
+        for w in range(n):
+            transf[w, :3, :3] = ref_rotation.from_rotvec(g.normal(0, 1.0, 3)).as_matrix()
+            transf[w, :3, 3] = g.normal(0, 1.0, 3)
+            transf[w, 3, 3] = 1.0
+        transf = transf.astype(np.float32)
+        rec = np.einsum('wij,wtkj->wtki', transf[:, :3, :3].astype(np.float64), S[:, :T]) + transf[:, None, None, :3, 3]
+        rec = (rec + g.normal(0, 0.01, rec.shape)).astype(np.float32)
+        item = {'rec': rec, 'transf': transf}
+        if dataset == 'egobody':
+            item['gt'] = S.astype(np.float32)
+            item['mask'] = (g.uniform(0, 1, (n, T, 22)) > 0.3).astype(np.float32)
+        out.append(item)
+    return out
+
+
+def gen_eval_metrics(ref):
+    """The unmodified eval_amass_full.py and eval_prox_egobody.py (runpy) on synthetic pickles in a temporary directory,
+    with a dataset root holding egobody_rohm_info.csv, the calibration and the cam2world JSONs.  Keeps the scripts'
+    per-frame arrays and final numbers, their inputs, and the floor height each recording used."""
+    import json
+    import pickle
+    import tempfile
+    sys.modules.update(_eval_stubs())
+    g = np.random.default_rng(2024)
+    out = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        # ---------------------------------------------------------------- AMASS
+        for tag, n, T, with_nan in (('amass', 4, 143, False), ('amass_nan', 2, 40, True)):
+            G, P, lc, lr = eval_amass_clips(g, n, T, with_nan)
+            out[f"{tag}_gt"], out[f"{tag}_rec"], out[f"{tag}_label_clean"], out[f"{tag}_label_rec"] = G, P, lc, lr
+            repr_c, repr_r = np.zeros((n, T, 294), np.float32), np.zeros((n, T, 294), np.float32)
+            repr_c[..., -4:], repr_r[..., -4:] = lc, lr
+            path = os.path.join(tmp, f"{tag}.pkl")
+            with open(path, 'wb') as f:
+                pickle.dump({'repr_name_list': ko.REPR_LIST, 'repr_dim_dict': {}, 'rec_ric_data_clean_list': G,
+                             'rec_ric_data_rec_list_from_abs_traj': P, 'rec_ric_data_rec_list_from_smpl': P,
+                             'motion_repr_clean_list': repr_c, 'motion_repr_rec_list': repr_r}, f)
+            runs = EVAL_AMASS_RUNS if tag == 'amass' else (('lower', 0.0),)
+            for k, (scheme, ratio) in enumerate(runs):
+                res = _run_reference_script('eval_amass_full.py', ['--saved_data_path', path, '--mask_scheme', scheme,
+                                                                   '--traj_mask_ratio', str(ratio)])
+                key = f"{tag}_run{k}"
+                out[f"{key}_scheme"], out[f"{key}_ratio"] = np.array(scheme), np.float64(ratio)
+                out[f"{key}_mpjpe_global"] = np.float64(np.mean(res['joints_mpjpe_global']))
+                out[f"{key}_mpjpe_global_vis"] = np.float64(np.mean(res['joints_mpjpe_global_vis']))
+                out[f"{key}_mpjpe_global_occ"] = np.float64(np.mean(res['joints_mpjpe_global_invis']))
+                for name in ('skating_gt_ratio', 'skating_rec_ratio', 'acc_error', 'pene_freq', 'pene_dist'):
+                    out[f"{key}_{name}"] = np.float64(res[name])
+                out[f"{key}_contact_lbl_acc"] = np.float64(np.mean(res['contact_lbl_acc']))
+                if k == 0:
+                    out[f"{tag}_mpjpe"] = res['joints_mpjpe_global']
+                    out[f"{tag}_contact_match"] = res['contact_lbl_acc']
+                    out[f"{tag}_skating_gt"], out[f"{tag}_skating_rec"] = res['skating_gt'], res['skating_rec']
+                    out[f"{tag}_accel_error"] = np.linalg.norm(res['acc_rec'] - res['acc_gt'], axis=-1)
+                    out[f"{tag}_h0"] = res['min_height_gt']
+                print(f"eval {tag} {scheme} {ratio}: mpjpe {out[f'{key}_mpjpe_global']:.5f} skating "
+                      f"{out[f'{key}_skating_gt_ratio']:.4f}/{out[f'{key}_skating_rec_ratio']:.4f} pene "
+                      f"{out[f'{key}_pene_freq']:.4f} {out[f'{key}_pene_dist']:.5f}")
+
+        # ---------------------------------------------------------------- PROX / EgoBody
+        root = os.path.join(tmp, 'dataset')
+        scenes = {'prox': ['MPH1Library', 'N0Sofa', 'N3Library', 'N3Office'], 'egobody': sorted(ref.ou.egobody_floor_height)}
+        for dataset in ('prox', 'egobody'):
+            res_dir = os.path.join(tmp, dataset)
+            os.makedirs(res_dir)
+            # the recording list the script evaluates with --recording_name all, read back from the script itself
+            src = open('/root/reference/eval_prox_egobody.py').read()
+            names = _recording_names(src, dataset)
+            rows = []
+            floors = []
+            for r, name in enumerate(names):
+                if dataset == 'prox':
+                    scene = name.split('_')[0]
+                    floors.append(ref.ou.prox_floor_height[scene])
+                    os.makedirs(os.path.join(root, 'cam2world'), exist_ok=True)
+                    with open(os.path.join(root, 'cam2world', scene + '.json'), 'w') as f:
+                        json.dump(np.eye(4).tolist(), f)
+                else:
+                    scene = scenes['egobody'][r % len(scenes['egobody'])]
+                    floors.append(ref.ou.egobody_floor_height[scene])
+                    view = 'sub_1' if r == 3 else 'master'
+                    rows.append((name, 0, 100, 0, 'male', view, scene, 1))
+                    cal = os.path.join(root, 'calibrations', name, 'cal_trans')
+                    os.makedirs(os.path.join(cal, 'kinect12_to_world'), exist_ok=True)
+                    with open(os.path.join(cal, 'kinect12_to_world', scene + '.json'), 'w') as f:
+                        json.dump({'trans': np.eye(4).tolist()}, f)
+                    with open(os.path.join(cal, 'kinect_11to12_color.json'), 'w') as f:
+                        json.dump({'trans': np.eye(4).tolist()}, f)
+            if rows:
+                import pandas as pd
+                pd.DataFrame(rows, columns=['recording_name', 'target_start_frame', 'target_end_frame', 'target_idx',
+                                            'target_gender', 'view', 'scene_name', 'body_idx_fpv']).to_csv(
+                    os.path.join(root, 'egobody_rohm_info.csv'), index=False)
+            recs = eval_video_recordings(g, dataset, floors)
+            for r, (name, item) in enumerate(zip(names, recs)):
+                n = item['rec'].shape[0]
+                save = {'repr_name_list': ko.REPR_LIST, 'repr_dim_dict': {}, 'rec_ric_data_noisy_list': item['rec'].copy(),
+                        'rec_ric_data_rec_list_from_smpl': item['rec'].copy(),
+                        'joints_input_scene_coord_list': item['rec'].copy(),
+                        'motion_repr_rec_list': np.zeros((n, EVAL_VIDEO_T, 294), np.float32),
+                        'motion_repr_noisy_list': np.zeros((n, EVAL_VIDEO_T, 294), np.float32),
+                        'mask_joint_vis_list': item.get('mask', np.ones((n, EVAL_VIDEO_T, 22), np.float32)),
+                        'trans_scene2cano_list': item['transf']}
+                if dataset == 'egobody':
+                    save['joints_gt_scene_coord_list'] = item['gt']
+                    save['frame_name_list'] = np.zeros((n, EVAL_VIDEO_T), dtype='<U8')
+                with open(os.path.join(res_dir, name + '.pkl'), 'wb') as f:
+                    pickle.dump(save, f)
+                for k, v in item.items():
+                    out[f"{dataset}_r{r}_{k}"] = v
+            out[f"{dataset}_floor"] = np.asarray(floors, np.float64)
+            res = _run_reference_script('eval_prox_egobody.py', ['--dataset', dataset, '--dataset_root', root,
+                                                                 '--saved_data_dir', res_dir, '--recording_name', 'all'])
+            lists = ['skating_list', 'acc_list', 'ground_pene_freq_list', 'ground_pene_dist_list']
+            if dataset == 'egobody':
+                lists += ['acc_error_list', 'gmpjpe_list', 'mpjpe_list', 'mpjpe_list_vis', 'mpjpe_list_occ',
+                          'joint_mask_list']
+            for lst in lists:
+                for r, name in enumerate(names):
+                    out[f"{dataset}_r{r}_{lst}"] = res[lst][name]
+            out[f"{dataset}_all_skating"] = np.float64(res['skating_list']['all'].mean())
+            out[f"{dataset}_all_acc"] = np.float64(res['acc_list']['all'].mean())
+            out[f"{dataset}_all_ground_pene_freq"] = np.float64(res['ground_pene_freq_list']['all'].mean())
+            out[f"{dataset}_all_ground_pene_dist"] = np.float64(res['ground_pene_dist_list']['all'].mean())
+            if dataset == 'egobody':
+                m = res['joint_mask_list']['all']
+                out["egobody_all_acc_error"] = np.float64(res['acc_error_list']['all'].mean())
+                out["egobody_all_gmpjpe"] = np.float64(res['gmpjpe_list']['all'].mean())
+                out["egobody_all_mpjpe"] = np.float64(res['mpjpe_list']['all'].mean())
+                out["egobody_all_mpjpe_vis"] = np.float64(res['mpjpe_list_vis']['all'].sum() / m.sum())
+                out["egobody_all_mpjpe_occ"] = np.float64(res['mpjpe_list_occ']['all'].sum() / (1 - m).sum())
+            print(f"eval {dataset}: {len(names)} recordings, skating {out[f'{dataset}_all_skating']:.4f} acc "
+                  f"{out[f'{dataset}_all_acc']:.3f}")
+    path = os.path.join(OUT, "eval_metrics.npz")
+    np.savez_compressed(path, **out)
+    print("eval_metrics.npz", os.path.getsize(path), "bytes")
+
+
+def _recording_names(src, dataset):
+    """The script's --recording_name all list for `dataset`, parsed from its source (only to name the pickles)."""
+    import ast
+    tree = ast.parse(src)
+    for node in ast.walk(tree):
+        if isinstance(node, ast.If) and isinstance(node.test, ast.Compare) and \
+                isinstance(node.test.comparators[0], ast.Constant) and node.test.comparators[0].value == dataset and \
+                node.body and isinstance(node.body[0], ast.Assign) and \
+                getattr(node.body[0].targets[0], 'id', None) == 'test_recording_name_list':
+            return ast.literal_eval(node.body[0].value)
+    raise RuntimeError(f"no recording list for {dataset}")
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     ref = import_reference()
     which = sys.argv[1:] or ["schedules", "posenet", "trajnet", "sampling", "kinematics", "glue", "pipeline",
-                             "clip_guidance", "windows", "windows_noise", "windows_video", "video_pipeline"]
+                             "clip_guidance", "windows", "windows_noise", "windows_video", "video_pipeline", "eval_metrics"]
     for w in which:
         {"schedules": gen_schedules, "posenet": gen_posenet, "trajnet": gen_trajnet, "sampling": gen_sampling,
          "kinematics": gen_kinematics, "glue": gen_glue, "pipeline": gen_pipeline, "clip_guidance": gen_clip_guidance,
          "windows": gen_windows, "windows_noise": gen_windows_noise, "windows_video": gen_windows_video,
-         "video_pipeline": gen_video_pipeline}[w](ref)
+         "video_pipeline": gen_video_pipeline, "eval_metrics": gen_eval_metrics}[w](ref)
