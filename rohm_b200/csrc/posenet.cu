@@ -23,6 +23,7 @@
 
 #include "attention.cuh"
 #include "common.h"
+#include "engine_kernels.cuh"
 #include "gemm.cuh"
 #include "graph.cuh"
 #include "ptx.cuh"
@@ -171,79 +172,6 @@ __global__ void add_vec_kernel(const float* __restrict__ a, const float* __restr
   if (i < n) out[i] = a[i] + b[i];
 }
 
-// LayerNorm over the last dim (eps 1e-5) of in + res (res = the residual stream, may be null), one warp per row; writes
-// fp32 and the hi/lo pair.  `out` may alias `res` (each row is read completely before it is written).
-template <int D>
-__global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ in, const float* res,
-                                                        const float* __restrict__ gamma,
-                                                        const float* __restrict__ beta, float* out,
-                                                        float* __restrict__ out_hi, float* __restrict__ out_lo,
-                                                        int rows, int f16) {
-  static_assert(D % 128 == 0, "row must be a multiple of 32 lanes x float4");
-  ptx::pdl_launch_dependents();
-  ptx::pdl_wait_prior_grid();
-  constexpr int V = D / 128;
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  const float4* src = reinterpret_cast<const float4*>(in + static_cast<int64_t>(row) * D);
-  float4 x[V];
-#pragma unroll
-  for (int i = 0; i < V; ++i) x[i] = src[lane + 32 * i];
-  if (res != nullptr) {  // x = sublayer output + residual stream (torch: x + sa_block(x) / x + ff_block(x))
-    const float4* rs = reinterpret_cast<const float4*>(res + static_cast<int64_t>(row) * D);
-#pragma unroll
-    for (int i = 0; i < V; ++i) {
-      const float4 r = rs[lane + 32 * i];
-      x[i].x += r.x, x[i].y += r.y, x[i].z += r.z, x[i].w += r.w;
-    }
-  }
-  float sum = 0.0f;
-#pragma unroll
-  for (int i = 0; i < V; ++i) sum += (x[i].x + x[i].y) + (x[i].z + x[i].w);
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
-  const float mean = sum * (1.0f / D);
-  float sq = 0.0f;
-#pragma unroll
-  for (int i = 0; i < V; ++i) {
-    const float a = x[i].x - mean, b = x[i].y - mean, c = x[i].z - mean, d = x[i].w - mean;
-    sq += (a * a + b * b) + (c * c + d * d);
-  }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, off);
-  const float rstd = rsqrtf(sq * (1.0f / D) + 1e-5f);
-  const float4* g4 = reinterpret_cast<const float4*>(gamma);
-  const float4* b4 = reinterpret_cast<const float4*>(beta);
-  float4* o = reinterpret_cast<float4*>(out + static_cast<int64_t>(row) * D);
-  float4* oh = reinterpret_cast<float4*>(out_hi + static_cast<int64_t>(row) * D);
-  float4* ol = reinterpret_cast<float4*>(out_lo + static_cast<int64_t>(row) * D);
-  uint2* oh16 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(out_hi) + static_cast<int64_t>(row) * D);
-  uint2* ol16 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(out_lo) + static_cast<int64_t>(row) * D);
-#pragma unroll
-  for (int i = 0; i < V; ++i) {
-    const float4 g = g4[lane + 32 * i], bb = b4[lane + 32 * i];
-    float4 y;
-    y.x = (x[i].x - mean) * rstd * g.x + bb.x;
-    y.y = (x[i].y - mean) * rstd * g.y + bb.y;
-    y.z = (x[i].z - mean) * rstd * g.z + bb.z;
-    y.w = (x[i].w - mean) * rstd * g.w + bb.w;
-    o[lane + 32 * i] = y;
-    if (f16) {
-      uint2 h, l;
-      ptx::split_f16x4(y, h, l);
-      oh16[lane + 32 * i] = h;
-      ol16[lane + 32 * i] = l;
-    } else {
-      float4 h, l;
-      h.x = ptx::to_tf32(y.x), h.y = ptx::to_tf32(y.y), h.z = ptx::to_tf32(y.z), h.w = ptx::to_tf32(y.w);
-      l.x = y.x - h.x, l.y = y.y - h.y, l.z = y.z - h.z, l.w = y.w - h.w;
-      oh[lane + 32 * i] = h;
-      ol[lane + 32 * i] = l;
-    }
-  }
-}
-
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------------
@@ -389,33 +317,6 @@ static __global__ void pack_weight_kernel(const float* __restrict__ w, float* __
   }
 }
 
-// LayerNorm folding of a consumer GEMM y = LN(u) W^T + b, LN(u) = (u - mean) rstd gamma + beta:
-//   Wf[n,k] = gamma_k W[n,k],  c_n = sum_k Wf[n,k],  d_n = b_n + sum_k beta_k W[n,k]      (one CTA per output row n)
-static __global__ void fold_ln_kernel(const float* __restrict__ W, const float* __restrict__ gamma,
-                                      const float* __restrict__ beta, const float* __restrict__ bias, int K,
-                                      float* __restrict__ Wf, float* __restrict__ c, float* __restrict__ d) {
-  const int n = blockIdx.x;
-  double sc = 0.0, sd = 0.0;
-  for (int k = threadIdx.x; k < K; k += blockDim.x) {
-    const float w = W[static_cast<int64_t>(n) * K + k];
-    const float wf = gamma[k] * w;
-    Wf[static_cast<int64_t>(n) * K + k] = wf;
-    sc += static_cast<double>(wf);
-    sd += static_cast<double>(beta[k]) * static_cast<double>(w);
-  }
-  __shared__ double rc[256], rd[256];
-  rc[threadIdx.x] = sc, rd[threadIdx.x] = sd;
-  __syncthreads();
-  for (int s = blockDim.x / 2; s > 0; s >>= 1) {
-    if (threadIdx.x < s) rc[threadIdx.x] += rc[threadIdx.x + s], rd[threadIdx.x] += rd[threadIdx.x + s];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    c[n] = static_cast<float>(rc[0]);
-    d[n] = static_cast<float>(static_cast<double>(bias[n]) + rd[0]);
-  }
-}
-
 static int pack_weight(rohm_posenet* pn, const float* w, int N, int K, PackedWeight* out, int kind);
 
 // Packs gamma-folded weights of a [N, K] linear layer and produces its c / d vectors (library-owned).
@@ -429,8 +330,8 @@ static int pack_folded(rohm_posenet* pn, const float* w, const float* bias, cons
   if (*c == nullptr || *d == nullptr) {
     rc = fail(pn->ctx, ROHM_ERR_CUDA, "alloc failed: %s", cudaGetErrorString(pn->pool.last_error()));
   } else {
-    fold_ln_kernel<<<N, 256>>>(w, gamma, beta, bias, K, wf, *c, *d);
-    if (cudaGetLastError() != cudaSuccess) rc = fail(pn->ctx, ROHM_ERR_CUDA, "fold_ln_kernel launch failed");
+    if (launch_fold_ln(w, gamma, beta, bias, N, K, wf, *c, *d) != cudaSuccess)
+      rc = fail(pn->ctx, ROHM_ERR_CUDA, "fold_ln_kernel launch failed");
     if (rc == ROHM_OK) rc = pack_weight(pn, wf, N, K, out, pn->kind);
     if (rc == ROHM_OK && cudaDeviceSynchronize() != cudaSuccess) rc = fail(pn->ctx, ROHM_ERR_CUDA, "weight folding failed");
   }
@@ -499,24 +400,13 @@ static int run_gemm(rohm_posenet* pn, GemmParams& g, const PackedWeight& w, int 
   return ROHM_OK;
 }
 
-template <int D>
-static void launch_ln(const float* in, const float* res, const float* g, const float* b, float* out, float* oh, float* ol,
-               int rows, cudaStream_t st, int f16, bool pdl) {
-  launch_chain(layernorm_kernel<D>, dim3((rows + 7) / 8), dim3(256), 0, st, pdl, in, res, g, b, out, oh, ol, rows, f16);
-}
-
 static int run_ln(rohm_posenet* pn, const float* in, const float* res, const float* g, const float* b, float* out, float* oh,
            float* ol, int rows, cudaStream_t st) {
   prof_begin(pn, kCatLayerNorm, st);
   const int f16 = pn->kind == kKindF16 ? 1 : 0;
   const bool pdl = pn->use_pdl && !pn->profiling;
-  switch (pn->D) {
-    case 128: launch_ln<128>(in, res, g, b, out, oh, ol, rows, st, f16, pdl); break;
-    case 256: launch_ln<256>(in, res, g, b, out, oh, ol, rows, st, f16, pdl); break;
-    case 512: launch_ln<512>(in, res, g, b, out, oh, ol, rows, st, f16, pdl); break;
-    case 1024: launch_ln<1024>(in, res, g, b, out, oh, ol, rows, st, f16, pdl); break;
-    default: return fail(pn->ctx, ROHM_ERR_INVALID, "unsupported d_model %d for LayerNorm", pn->D);
-  }
+  if (launch_layernorm(pn->D, in, res, g, b, out, oh, ol, rows, f16, st, pdl) == cudaErrorInvalidValue)
+    return fail(pn->ctx, ROHM_ERR_INVALID, "unsupported d_model %d for LayerNorm", pn->D);
   prof_end(pn, st);
   ROHM_CUDA(pn->ctx, cudaGetLastError());
   pn->launches++;

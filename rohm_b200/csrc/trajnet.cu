@@ -29,6 +29,7 @@
 #include <string>
 
 #include "common.h"
+#include "engine_kernels.cuh"
 #include "gemm.cuh"
 #include "graph.cuh"
 #include "groupnorm.cuh"
@@ -76,97 +77,6 @@ __global__ void pack_rows_kernel(const float* __restrict__ x, float* __restrict_
   }
 }
 constexpr size_t kPackRowsX = 0;  // the argument replaced on every replay of a cached forward graph
-
-// Timestep path of TrajNet (trajnet.py:120-125, 189) and the per-block time projections (heads.py:34-38, 51-52):
-//   temb = W3 mish(W1 sinusoid(t) + b1) + b3;  tp[b, :] = Wcat mish(temb) + bcat   (all blocks' Linear(32,out) stacked)
-__device__ __forceinline__ void trajnet_time_compute(float t, int b, int time_dim, const float* __restrict__ w1,
-                                                     const float* __restrict__ b1, const float* __restrict__ w3,
-                                                     const float* __restrict__ b3, const float* __restrict__ wcat,
-                                                     const float* __restrict__ bcat, int total_out, float* __restrict__ tp,
-                                                     float* sm) {
-  float* e = sm;                  // [time_dim]
-  float* h = e + time_dim;        // [4 * time_dim]
-  float* m = h + 4 * time_dim;    // [time_dim]  mish(temb)
-  const int half = time_dim / 2;
-  if (threadIdx.x < half) {
-    const float f = expf(static_cast<float>(threadIdx.x) * -(logf(10000.0f) / static_cast<float>(half - 1)));
-    const float a = t * f;
-    e[threadIdx.x] = sinf(a);
-    e[half + threadIdx.x] = cosf(a);
-  }
-  __syncthreads();
-  for (int n = threadIdx.x; n < 4 * time_dim; n += blockDim.x) {
-    float acc = b1[n];
-    for (int k = 0; k < time_dim; ++k) acc = fmaf(w1[n * time_dim + k], e[k], acc);
-    h[n] = mish_f(acc);
-  }
-  __syncthreads();
-  for (int n = threadIdx.x; n < time_dim; n += blockDim.x) {
-    float acc = b3[n];
-    for (int k = 0; k < 4 * time_dim; ++k) acc = fmaf(w3[n * 4 * time_dim + k], h[k], acc);
-    m[n] = mish_f(acc);
-  }
-  __syncthreads();
-  // the stacked projections are split over blockIdx.y (each CTA recomputes the small time MLP above)
-  for (int n = blockIdx.y * blockDim.x + threadIdx.x; n < total_out; n += blockDim.x * gridDim.y) {
-    float acc = bcat[n];
-    for (int k = 0; k < time_dim; ++k) acc = fmaf(wcat[n * time_dim + k], m[k], acc);
-    tp[static_cast<int64_t>(b) * total_out + n] = acc;
-  }
-}
-
-// Per step the embedding depends on the (integer) timestep only, so the whole path is tabulated at create time for
-// t in [0, table_rows) (the direct evaluation is latency-bound) and the per-forward kernel is a row
-// gather; timesteps outside the table are evaluated directly.  `table` == nullptr: always evaluate (used to build the table).
-__global__ void __launch_bounds__(256) trajnet_time_kernel(const int64_t* __restrict__ time, int time_dim,
-                                                           const float* __restrict__ w1, const float* __restrict__ b1,
-                                                           const float* __restrict__ w3, const float* __restrict__ b3,
-                                                           const float* __restrict__ wcat, const float* __restrict__ bcat,
-                                                           int total_out, float* __restrict__ tp,
-                                                           const float* __restrict__ table, int table_rows) {
-  extern __shared__ float sm[];
-  const int b = blockIdx.x;
-  const int64_t ti = time[b];
-  if (table != nullptr && ti >= 0 && ti < table_rows) {  // block-uniform
-    const float4* src = reinterpret_cast<const float4*>(table + ti * total_out);
-    float4* dst = reinterpret_cast<float4*>(tp + static_cast<int64_t>(b) * total_out);
-    for (int n = blockIdx.y * blockDim.x + threadIdx.x; n < total_out / 4; n += blockDim.x * gridDim.y) dst[n] = src[n];
-    return;
-  }
-  trajnet_time_compute(static_cast<float>(ti), b, time_dim, w1, b1, w3, b3, wcat, bcat, total_out, tp, sm);
-}
-constexpr size_t kTrajnetTimeT = 0;  // the argument replaced on every replay of a cached forward graph
-
-// Split-K convolution without a GroupNorm behind it (the stride-2 downsampling convolutions): out = bias + the partials (in
-// split order) on real rows, 0 on pad rows.  4 channels per thread over the [B * Tp, C] output.  kPacked: row r is real iff
-// row_mask[r] != 0.
-template <bool kPacked>
-__global__ void __launch_bounds__(256) sum_split_kernel(const float* __restrict__ part, int splits, int64_t split_stride,
-                                                        const float* __restrict__ bias, float* __restrict__ out,
-                                                        float* __restrict__ out_hi, float* __restrict__ out_lo, int C, int Tp,
-                                                        int T, int64_t total4, int f16,
-                                                        const unsigned char* __restrict__ row_mask) {
-  ptx::pdl_launch_dependents();
-  ptx::pdl_wait_prior_grid();
-  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= total4) return;
-  const int c4 = C / 4;
-  const int64_t row = i / c4;
-  const int c = static_cast<int>(i - row * c4) * 4;
-  const bool real = kPacked ? row_mask[row] != 0 : static_cast<int>(row % Tp) < T;
-  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (real) {
-    float4 a[kMaxSplitsDev];
-#pragma unroll
-    for (int sp = 0; sp < kMaxSplitsDev; ++sp)
-      if (sp < splits) a[sp] = __ldcg(reinterpret_cast<const float4*>(part + sp * split_stride) + i);
-    v = *reinterpret_cast<const float4*>(bias + c);
-#pragma unroll
-    for (int sp = 0; sp < kMaxSplitsDev; ++sp)
-      if (sp < splits) v.x += a[sp].x, v.y += a[sp].y, v.z += a[sp].z, v.w += a[sp].w;
-  }
-  store_act4(out, out_hi, out_lo, i, v, f16);
-}
 
 // padded-clip rows [B * Tp, ld] -> compact [B, T, C]; kPacked (clip_off: packed clips): frames past a clip are zero
 template <bool kPacked>
@@ -606,11 +516,9 @@ int run_conv(rohm_trajnet* tn, Conv& cv, int B, cudaStream_t st) {
   tn->launches++;
   if (cv.sum_after) {
     const int C = cv.w.N;
-    const int64_t total4 = static_cast<int64_t>(rows) * C / 4;
-    ROHM_CUDA(tn->ctx, launch_chain(packed ? sum_split_kernel<true> : sum_split_kernel<false>, dim3(static_cast<unsigned>((total4 + 255) / 256)), dim3(256), 0, st,
-                                    tn->use_pdl, cv.partial, cv.splits, cv.split_rows * C, cv.bias, cv.out.f32, cv.out.hi,
-                                    cv.out.lo, C, tn->Tp[cv.level_out], tn->Tl[cv.level_out], total4,
-                                    tn->kind == kKindF16 ? 1 : 0, mask));
+    ROHM_CUDA(tn->ctx, launch_sum_split(cv.partial, cv.splits, cv.split_rows * C, cv.bias, cv.out.f32, cv.out.hi, cv.out.lo,
+                                        C, tn->Tp[cv.level_out], tn->Tl[cv.level_out], rows, tn->kind == kKindF16 ? 1 : 0,
+                                        mask, st, tn->use_pdl));
     tn->launches++;
   }
   return ROHM_OK;

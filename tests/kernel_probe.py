@@ -1,5 +1,5 @@
-"""ctypes driver of tests/native/libkernel_probe.so: the GEMM (rohm_b200/csrc/gemm.cu), attention (attention.cu) and
-GroupNorm + Mish (groupnorm.cu) kernels launched directly on torch device tensors, the operand packing the engines do and
+"""ctypes driver of tests/native/libkernel_probe.so: the GEMM (rohm_b200/csrc/gemm.cu), attention (attention.cu),
+GroupNorm + Mish (groupnorm.cu) and engine (engine_kernels.cu) kernels launched directly on torch device tensors, the operand packing the engines do and
 the rotation / trajectory helpers of kin.cuh and repr.cuh one element at a time (not collected by pytest).  The launching functions take `reps`: that many launches back to
 back on the default stream."""
 import ctypes as C
@@ -72,7 +72,15 @@ def lib():
         _lib.probe_f16_weight_scale.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_float)]
         _lib.probe_attention.argtypes = [C.POINTER(Attn), C.c_int]
         _lib.probe_group_norm.argtypes = [C.POINTER(GnArgs), C.c_int, C.c_int, C.c_int, C.c_void_p]
+        _lib.probe_group_norm_clip_slices.argtypes = [C.POINTER(GnArgs), C.c_int, C.c_int, C.POINTER(C.c_int), C.c_void_p,
+                                                      C.c_int]
         _lib.probe_group_norm_cluster.argtypes = [C.c_int, C.c_int, C.c_int]
+        _lib.probe_layernorm.argtypes = [C.c_int] + [C.c_void_p] * 7 + [C.c_int, C.c_int]
+        _lib.probe_fold_ln.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_void_p] * 3
+        _lib.probe_trajnet_time.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 6 + [
+            C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+        _lib.probe_sum_split.argtypes = [C.c_void_p, C.c_int, C.c_int64] + [C.c_void_p] * 4 + [
+            C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_void_p]
         _lib.probe_kin.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
         _lib.probe_clip_of_frame.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
     return _lib
@@ -215,6 +223,18 @@ def group_norm(part, splits, split_stride, bias, gamma, beta, tp, tp_stride, r1,
     return lib().probe_group_norm(C.byref(a), B, n, reps, p(clip_off))
 
 
+def group_norm_clip_slices(part, splits, split_stride, bias, gamma, beta, tp, tp_stride, r1, r2, out, out_hi, out_lo, C_, Tp,
+                           T, n, f16, clip_off, real_rows, groups=8, reps=1):
+    """launch_gn_mish_clip_slices (the batch-invariant engines' instance) over packed clips, n >= 2 CTAs per (clip, group),
+    `reps` times; real_rows: the clips' real rows (a list), clip_off as for group_norm.  Returns 0 or the CUDA error code."""
+    p = _ptr
+    a = GnArgs(p(part), splits, split_stride, p(bias), p(gamma), p(beta), p(tp), tp_stride, p(r1), p(r2), p(out), p(out_hi),
+               p(out_lo), C_, Tp, T, groups, int(f16))
+    B = len(real_rows)
+    rows = (C.c_int * B)(*real_rows)
+    return lib().probe_group_norm_clip_slices(C.byref(a), B, n, rows, p(clip_off), reps)
+
+
 def group_norm_cluster(T, C_, groups=8):
     """The cluster size the TrajNet engine chooses for groups of T rows of C_ / groups channels."""
     return lib().probe_group_norm_cluster(T, C_, groups)
@@ -289,3 +309,29 @@ def clip_of_frame(clip_off, frames):
     B = clip_off.numel() - 1
     assert lib().probe_clip_of_frame(clip_off.data_ptr(), B, frames.data_ptr(), frames.numel(), out.data_ptr()) == 0
     return out
+
+
+def layernorm(D, x, res, gamma, beta, out, out_hi, out_lo, rows, f16):
+    """layernorm_kernel<D> of x + res (res may be None or `out` itself) over `rows` rows; returns 0 or the error code."""
+    return lib().probe_layernorm(D, _ptr(x), _ptr(res), _ptr(gamma), _ptr(beta), _ptr(out), _ptr(out_hi), _ptr(out_lo), rows,
+                                 int(f16))
+
+
+def fold_ln(W, gamma, beta, bias, Wf, c, d):
+    """fold_ln_kernel of the [N, K] weight W into Wf, c, d; returns 0 or the error code."""
+    N, K = W.shape
+    return lib().probe_fold_ln(_ptr(W), _ptr(gamma), _ptr(beta), _ptr(bias), N, K, _ptr(Wf), _ptr(c), _ptr(d))
+
+
+def trajnet_time(time, ctas_per_clip, time_dim, w1, b1, w3, b3, wcat, bcat, tp, table=None, table_rows=0):
+    """trajnet_time_kernel for the int64 timesteps `time` into tp [B, total_out] (total_out = bcat's length); returns 0 or
+    the error code."""
+    return lib().probe_trajnet_time(_ptr(time), time.numel(), ctas_per_clip, time_dim, _ptr(w1), _ptr(b1), _ptr(w3),
+                                    _ptr(b3), _ptr(wcat), _ptr(bcat), bcat.numel(), _ptr(tp), _ptr(table), table_rows)
+
+
+def sum_split(part, splits, split_stride, bias, out, out_hi, out_lo, C_, Tp, T, rows, f16, row_mask=None):
+    """sum_split_kernel over `rows` rows of C_ channels (row_mask: uint8 device tensor of the real rows, or None for
+    uniform clips of Tp rows with T real ones); returns 0 or the error code."""
+    return lib().probe_sum_split(_ptr(part), splits, split_stride, _ptr(bias), _ptr(out), _ptr(out_hi), _ptr(out_lo), C_, Tp,
+                                 T, rows, int(f16), _ptr(row_mask))

@@ -1,12 +1,16 @@
-// Test-only entry points into the GEMM, attention and GroupNorm kernels (rohm_b200/csrc/gemm.cu, attention.cu,
-// groupnorm.cu), the operand-pair helpers of ptx.cuh and the rotation / trajectory helpers of kin.cuh and repr.cuh, driven from Python through ctypes by tests/kernel_probe.py and
+// Test-only entry points into the GEMM, attention, GroupNorm and engine kernels (rohm_b200/csrc/gemm.cu, attention.cu,
+// groupnorm.cu, engine_kernels.cu), the operand-pair helpers of ptx.cuh and the rotation / trajectory helpers of kin.cuh and repr.cuh, driven from Python through ctypes by tests/kernel_probe.py and
 // linked against the product's own objects of those sources.  Every function takes plain structs / device pointers, builds the tensor maps itself with the library's own
-// helpers and returns 0, a cudaError_t (> 0) or -CUresult of a failed tensor-map encoding.  The launching probes run their
-// launch `reps` >= 1 times back to back on the default stream, set-up done once, so that tools can time them.  The product
+// helpers and returns 0, a cudaError_t (> 0) or -CUresult of a failed tensor-map encoding.  Every launch goes to the default
+// stream; the probes that take `reps` run their launch that many times back to back, set-up done once, so that tools can
+// time them.  The product
 // library (librohm_b200.so, include/rohm_b200.h) exports none of this.
 #include <cstdint>
 
+#include <algorithm>
+
 #include "../../rohm_b200/csrc/attention.cuh"
+#include "../../rohm_b200/csrc/engine_kernels.cuh"
 #include "../../rohm_b200/csrc/gemm.cuh"
 #include "../../rohm_b200/csrc/groupnorm.cuh"
 #include "../../rohm_b200/csrc/kin.cuh"
@@ -310,11 +314,59 @@ int probe_group_norm(const GnArgs* a, int B, int n, int reps, const int* clip_of
   return repeat(reps, [&] { return launch_gn_mish(*a, B, n, nullptr, false, clip_off); });
 }
 
+// The batch-invariant engines' GroupNorm + Mish of packed clips (launch_gn_mish_clip_slices), n >= 2 CTAs per (clip, group),
+// with the dynamic shared memory run_gn (trajnet.cu) gives it: the largest slice of any clip's own cluster.  real_rows (host
+// int[B]): clip b's real rows, clip_off[b + 1] - clip_off[b] - (Tp - T).
+int probe_group_norm_clip_slices(const GnArgs* a, int B, int n, const int* real_rows, const int* clip_off, int reps) {
+  if (reps < 1 || B < 1) return static_cast<int>(cudaErrorInvalidValue);
+  size_t smem = 0;
+  for (int b = 0; b < B; ++b) {
+    const int Tc = real_rows[b];
+    smem = std::max(smem, gn_slice_bytes(Tc, a->C, a->groups, gn_pick_cluster(Tc, a->C, a->groups, kGnClipBudget)));
+  }
+  return repeat(reps, [&] { return launch_gn_mish_clip_slices(*a, B, n, smem, nullptr, false, clip_off); });
+}
+
 // The cluster size rohm_trajnet_create chooses for a (clip, group) of T rows of C / groups channels; 0 on error.
 int probe_group_norm_cluster(int T, int C, int groups) {
   size_t budget = 0, max_budget = 0;
   if (gn_smem_budgets(&budget, &max_budget) != cudaSuccess) return 0;
   return gn_pick_cluster(T, C, groups, budget);
+}
+
+// PoseNet's LayerNorm (layernorm_kernel<D>) of in + res over `rows` rows of D floats: fp32 out and the hi/lo pair (fp16
+// when f16, else tf32 in fp32 containers).  res may be NULL or alias out.
+int probe_layernorm(int D, const float* in, const float* res, const float* gamma, const float* beta, float* out, void* out_hi,
+                    void* out_lo, int rows, int f16) {
+  if (rows < 1) return static_cast<int>(cudaErrorInvalidValue);
+  return static_cast<int>(launch_layernorm(D, in, res, gamma, beta, out, static_cast<float*>(out_hi),
+                                           static_cast<float*>(out_lo), rows, f16, nullptr, false));
+}
+
+// LayerNorm folding (fold_ln_kernel) of a [N, K] weight: Wf [N, K], c [N], d [N].
+int probe_fold_ln(const float* W, const float* gamma, const float* beta, const float* bias, int N, int K, float* Wf, float* c,
+                  float* d) {
+  if (N < 1 || K < 1) return static_cast<int>(cudaErrorInvalidValue);
+  return static_cast<int>(launch_fold_ln(W, gamma, beta, bias, N, K, Wf, c, d));
+}
+
+// TrajNet's time path (trajnet_time_kernel) for the B timesteps time[0 .. B), ctas_per_clip CTAs per clip as gridDim.y, into
+// tp [B, total_out]; table (NULL: every timestep evaluated directly) [table_rows, total_out].
+int probe_trajnet_time(const int64_t* time, int B, int ctas_per_clip, int time_dim, const float* w1, const float* b1,
+                       const float* w3, const float* b3, const float* wcat, const float* bcat, int total_out, float* tp,
+                       const float* table, int table_rows) {
+  if (B < 1 || ctas_per_clip < 1) return static_cast<int>(cudaErrorInvalidValue);
+  trajnet_time_kernel<<<dim3(B, ctas_per_clip), 256, sizeof(float) * 6 * time_dim>>>(time, time_dim, w1, b1, w3, b3, wcat,
+                                                                                      bcat, total_out, tp, table, table_rows);
+  return static_cast<int>(cudaGetLastError());
+}
+
+// The split-K sum (sum_split_kernel) over `rows` rows of C channels; row_mask NULL: uniform clips of Tp rows, T real.
+int probe_sum_split(const float* part, int splits, int64_t split_stride, const float* bias, float* out, void* out_hi,
+                    void* out_lo, int C, int Tp, int T, int64_t rows, int f16, const unsigned char* row_mask) {
+  if (rows < 1 || splits < 1 || splits > kMaxSplitsDev || C % 4 != 0) return static_cast<int>(cudaErrorInvalidValue);
+  return static_cast<int>(launch_sum_split(part, splits, split_stride, bias, out, static_cast<float*>(out_hi),
+                                           static_cast<float*>(out_lo), C, Tp, T, rows, f16, row_mask, nullptr, false));
 }
 
 }  // extern "C"

@@ -1,7 +1,8 @@
 """GPU: TrajNet, the inter-round glue and the round pipeline on clips longer than 1024 frames.
 
 * The cluster GroupNorm + Mish kernel (gn_mish_split_kernel, rohm_b200/csrc/groupnorm.cu) through its test probe,
-  against a float64 GroupNorm + Mish, for every cluster size.
+  against a float64 GroupNorm + Mish, for every cluster size, on uniform and packed clips; and the batch-invariant
+  engines' instance (gn_mish_split_clip_kernel), which must give each packed clip the bits it gets alone.
 * TrajNet / TrajNet+TrajControl forwards up to 4992 frames against oracle/trajnet_oracle, and the frame limit.
 * traj_repr_from_joints / traj_to_full_repr (a cluster of ceil(T / 1024) CTAs per clip) up to 4992 frames with planted
   degenerate frames, against oracle/glue_oracle.
@@ -141,6 +142,137 @@ def test_cluster_group_norm_matches_float64(cuda_device, T, C, div):
                 again = _gn_run(c, 8)[0][:rows * C].view(B, Tp, C)[:, :TL].double()
                 assert torch.equal(again, got[8])
     print(f"GroupNorm T={T} C={C} T_L={T // div}: worst error / bound = {worst:.3f}")
+
+
+def _gn_clip_cluster(Tc, C, groups=8):
+    """gn_pick_cluster(Tc, C, groups, kGnClipBudget): the cluster a clip of Tc real rows gets alone in a batch-invariant
+    engine, the smallest power of two whose slice of ceil(Tc / n) rows fits 47 KB."""
+    n = 1
+    while n < 8 and -(-Tc // n) * (C // groups) * 4 > 47 * 1024:
+        n *= 2
+    return n
+
+
+def _packed_gn_case(dev, lengths, L, C, splits, f16, gen, offset=0.0):
+    """Packed clips of the given frame counts at pyramid level L, laid out as a TrajNet engine lays them out: clip b takes
+    (lengths[b] + 32) >> L rows from clip_off[b], its lengths[b] >> L real rows first.  offset: added to the bias."""
+    rows_b = [(n + 32) >> L for n in lengths]
+    off = np.concatenate([[0], np.cumsum(rows_b)]).tolist()
+    T = max(lengths)
+    rows = off[-1]
+    rnd = lambda *s: torch.randn(*s, generator=gen).to(dev)
+    B = len(lengths)
+    return dict(B=B, Tp=(T + 32) >> L, TL=T >> L, rows=rows, C=C, splits=splits, f16=f16, off=off, rows_b=rows_b,
+                real=[n >> L for n in lengths], clip_off=torch.tensor(off, dtype=torch.int32, device=dev),
+                part=rnd(splits, rows * C), bias=rnd(C) * 0.5 + offset, gamma=1.0 + 0.2 * rnd(C), beta=0.3 * rnd(C),
+                tp=rnd(B, C + 4), r1=rnd(rows * C), r2=rnd(rows * C),
+                pair_dtype=torch.float16 if f16 else torch.float32)
+
+
+def _packed_gn_run(c, n, clip_slices):
+    """One launch over the packed clips into sentinel-filled buffers: launch_gn_mish with clip_off, or the clip-slice
+    instance; returns (out, hi, lo) of rows * C elements."""
+    m = c["rows"] * c["C"]
+    extra = 64
+    dev = c["part"].device
+    out = torch.full((m + extra,), SENTINEL, device=dev)
+    hi = torch.full((m + extra,), SENTINEL, device=dev, dtype=c["pair_dtype"])
+    lo = torch.full_like(hi, SENTINEL)
+    args = (c["part"], c["splits"], m, c["bias"], c["gamma"], c["beta"], c["tp"], c["C"] + 4, c["r1"], c["r2"], out, hi, lo,
+            c["C"], c["Tp"], c["TL"])
+    if clip_slices:
+        rc = kp.group_norm_clip_slices(*args, n, c["f16"], c["clip_off"], c["real"])
+    else:
+        rc = kp.group_norm(*args, c["B"], n, c["f16"], clip_off=c["clip_off"])
+    torch.cuda.synchronize()
+    assert rc == 0, rc
+    for buf in (out, hi, lo):
+        assert bool((buf[m:].float() == SENTINEL).all()), (n, clip_slices, "wrote past the matrix")
+    return out[:m], hi[:m], lo[:m]
+
+
+def _clip(c, t, b):
+    """Clip b's rows of a [rows * C] tensor, as [rows_b, C]."""
+    return t.view(c["rows"], c["C"])[c["off"][b]:c["off"][b + 1]]
+
+
+# Frame counts whose real rows straddle the clip-slice thresholds: at level 0, C = 64 (32 bytes per row of a group) the
+# clip's own cluster grows after 1504 and 3008 rows; at level 1, C = 128 (64 bytes) after 752 and 1504; mixed with 16.
+PACKED_LENGTHS = [1504, 16, 1520, 3008, 16, 3024, 4992]
+
+
+@pytest.mark.parametrize("L,C", [(0, 64), (1, 128)])
+def test_packed_group_norm_matches_float64_per_clip(cuda_device, L, C):
+    """Packed clips of different lengths in one launch, fp16 and tf32 pairs, 3 split-K partials, time projection and both
+    residuals: launch_gn_mish with clip_off at n = 1, 2, 4, 8 and the clip-slice instance at the largest own cluster and
+    at n = 8 against a float64 GroupNorm + Mish over each clip's own real rows (_gn_reference of that clip alone), within
+    its bound; pad rows exactly zero in every output, nothing written past the matrix, a repeated launch bit-identical."""
+    gen = torch.Generator().manual_seed(97 + L)
+    worst = 0.0
+    for f16 in (1, 0):
+        c = _packed_gn_case(cuda_device, PACKED_LENGTHS, L, C, 3, f16, gen)
+        B = c["B"]
+        refs = []
+        for b in range(B):
+            part_b = [_clip(c, p, b).reshape(-1) for p in c["part"]]
+            refs.append(_gn_reference(part_b, c["bias"], c["gamma"], c["beta"], c["tp"][b:b + 1], _clip(c, c["r1"], b),
+                                      _clip(c, c["r2"], b), 1, c["rows_b"][b], c["real"][b], C))
+        vmax = max(_gn_clip_cluster(Tc, C) for Tc in c["real"])
+        assert vmax >= 2
+        launches = [(n, False) for n in (1, 2, 4, 8)] + [(vmax, True), (8, True)]
+        for n, slices in launches:
+            out, hi, lo = _packed_gn_run(c, n, slices)
+            for b in range(B):
+                Tc = c["real"][b]
+                for buf in (out, hi, lo):
+                    assert bool((_clip(c, buf, b)[Tc:] == 0).all()), (n, slices, b, "pad rows must be zero")
+                ref, bound = refs[b]
+                o = _clip(c, out, b)[:Tc].double()
+                err = (o - ref[0]).abs()
+                assert bool((err <= bound[0]).all()), (n, slices, b, Tc, float(err.max()), float((err / bound[0]).max()))
+                worst = max(worst, float((err / bound[0]).max()))
+                pair = _clip(c, hi, b)[:Tc].double() + _clip(c, lo, b)[:Tc].double()
+                if f16:
+                    assert bool(((pair - o).abs() <= 2.0 ** -21 * o.abs() + 2.0 ** -24).all()), (n, slices, b)
+                else:
+                    assert torch.equal(pair, o), (n, slices, b)
+        for slices in (False, True):
+            first, again = _packed_gn_run(c, 8, slices), _packed_gn_run(c, 8, slices)
+            for x, y in zip(first, again):
+                assert torch.equal(x, y), slices
+    print(f"packed GroupNorm L={L} C={C}: worst error / bound = {worst:.3f}")
+
+
+@pytest.mark.parametrize("offset", [0.0, 3e4])
+@pytest.mark.parametrize("L,C", [(0, 64), (1, 128)])
+def test_clip_slice_group_norm_gives_each_clip_its_bits_alone(cuda_device, L, C, offset):
+    """The batch-invariant engines' instance at n = 8 and at the largest own cluster: every packed clip's rows (real and
+    pad, fp32 and pair) equal bit for bit those of the clip launched alone as one uniform clip with n = v, its own
+    cluster.  offset 3e4 puts the groups' mean far above their spread, so the variance s2 / cnt - mean^2 cancels most of
+    its digits and a change in how the double sums are split shows in the fp32 statistics."""
+    gen = torch.Generator().manual_seed(131 + L)
+    for f16 in (1, 0):
+        c = _packed_gn_case(cuda_device, PACKED_LENGTHS, L, C, 3, f16, gen, offset)
+        vmax = max(_gn_clip_cluster(Tc, C) for Tc in c["real"])
+        packed = {n: _packed_gn_run(c, n, True) for n in (vmax, 8)}
+        for b in range(c["B"]):
+            Tc, rows_b = c["real"][b], c["rows_b"][b]
+            alone = dict(c, B=1, Tp=rows_b, TL=Tc, rows=rows_b, off=[0, rows_b],
+                         part=torch.stack([_clip(c, p, b).reshape(-1) for p in c["part"]]),
+                         tp=c["tp"][b:b + 1].contiguous(), r1=_clip(c, c["r1"], b).reshape(-1).contiguous(),
+                         r2=_clip(c, c["r2"], b).reshape(-1).contiguous())
+            m = rows_b * C
+            out = torch.full((m,), SENTINEL, device=cuda_device)
+            hi = torch.full((m,), SENTINEL, device=cuda_device, dtype=c["pair_dtype"])
+            lo = torch.full_like(hi, SENTINEL)
+            rc = kp.group_norm(alone["part"], 3, m, c["bias"], c["gamma"], c["beta"], alone["tp"], C + 4, alone["r1"],
+                               alone["r2"], out, hi, lo, C, rows_b, Tc, 1, _gn_clip_cluster(Tc, C), f16)
+            torch.cuda.synchronize()
+            assert rc == 0, rc
+            for n, bufs in packed.items():
+                for got, want in zip(bufs, (out, hi, lo)):
+                    bits = torch.int16 if want.dtype == torch.float16 else torch.int32
+                    assert torch.equal(_clip(c, got, b).reshape(-1).view(bits), want.view(bits)), (f16, n, b, Tc)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
