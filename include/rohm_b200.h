@@ -547,6 +547,39 @@ ROHM_API int rohm_eval_video(rohm_ctx* ctx, const float* rec, int T, const float
 ROHM_API int rohm_eval_reduce(rohm_ctx* ctx, const double* sums, int ks, const int64_t* counts, int kc, const int* order,
                               const int* group_off, int n_groups, double* out_sums, int64_t* out_counts, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Joint occlusion masks (utils/get_occlusion_mask.py:55-144), rohm_b200/occlusion.py, DESIGN §4.17
+ * ------------------------------------------------------------------------------------------------------------ */
+
+/* Bytes of the workspace rohm_scene_depth needs for a scene of n_verts vertices and n_faces triangles rendered at
+ * width x height (-1 for a negative count or an empty viewport). */
+ROHM_API int64_t rohm_scene_depth_workspace_bytes(int64_t n_verts, int64_t n_faces, int width, int height);
+
+/* The depth map of a scene mesh: vertices [n_verts,3] in the world frame, faces [n_faces,3] int32 (indices in range),
+ * world2cam_host: host float64 [3,4] to the camera frame (x right, y down, z forward).  Each pixel holds, rounded to
+ * float32, the smallest z in [znear, zfar] at which the ray through its centre, ((x + 0.5 - cx) / fx, (y + 0.5 - cy) / fy,
+ * 1), hits a front-facing triangle (edges and vertices included), 0 where none is hit: depth [height,width].  Bit-
+ * deterministic.  workspace: device memory of rohm_scene_depth_workspace_bytes bytes. */
+ROHM_API int rohm_scene_depth(rohm_ctx* ctx, const float* vertices, int64_t n_verts, const int* faces, int64_t n_faces,
+                              const double* world2cam_host, double fx, double fy, double cx, double cy, int width,
+                              int height, double znear, double zfar, void* workspace, int64_t workspace_bytes,
+                              float* depth, void* stream);
+
+/* The occlusion masks of N frames of R recordings.  Per frame: joints [N,joints_per_frame,3] (the first 25 are used) and
+ * vertices (frame f's row starts at f * vertex_pitch floats, [V,3] dense) in its recording's camera frame; faces
+ * [n_faces,3] int32 (indices in range); frame_rec [N] int32.  Per recording: camera_mtx [R,3,3] and dist [R,14] float64
+ * (zero-padded OpenCV coefficients) project the joints as cv2.projectPoints does; map_of_rec [R] int32 picks its scene
+ * map in depth_maps [S,height,width] (rohm_scene_depth of the same render camera fx, fy, cx, cy, znear, zfar).
+ * mask [N,25]: 0 where the joint's pixel is on screen, the scene depth there is not 0 and the body's depth minus the
+ * scene's exceeds 0.1 m, else 1.  Optional (NULL to skip): pixel [N,25,2] int32 (the truncated coordinates, INT_MIN
+ * where non-finite or beyond int32), depth_body and depth_scene [N,25] at the pixel (0 off screen). */
+ROHM_API int rohm_joint_occlusion(rohm_ctx* ctx, const float* joints, int joints_per_frame, const float* vertices,
+                                  int64_t vertex_pitch, const int* faces, int n_faces, const int* frame_rec, int N,
+                                  const double* camera_mtx, const double* dist, const float* depth_maps,
+                                  const int* map_of_rec, double fx, double fy, double cx, double cy, int width,
+                                  int height, double znear, double zfar, float* mask, int* pixel, float* depth_body,
+                                  float* depth_scene, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -37,7 +37,7 @@ class PoseNetW(C.Structure):
 
 
 # name -> (restype, argtypes).  Kept in one table so tests can check it against the header.
-_p, _i, _i64, _f = C.c_void_p, C.c_int, C.c_int64, C.c_float
+_p, _i, _i64, _f, _d = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double
 SIGNATURES = {
     "rohm_version": (_i, []),
     "rohm_ctx_create": (_i, [_i, C.POINTER(_p)]),
@@ -102,6 +102,10 @@ SIGNATURES = {
                              _p]),
     "rohm_eval_video": (_i, [_p, _p, _i, _p, _p, _i, _p, _i, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "rohm_eval_reduce": (_i, [_p, _p, _i, _p, _i, _p, _p, _i, _p, _p, _p]),
+    "rohm_scene_depth_workspace_bytes": (_i64, [_i64, _i64, _i, _i]),
+    "rohm_scene_depth": (_i, [_p, _p, _i64, _p, _i64, _p, _d, _d, _d, _d, _i, _i, _d, _d, _p, _i64, _p, _p]),
+    "rohm_joint_occlusion": (_i, [_p, _p, _i, _p, _i64, _p, _i, _p, _i, _p, _p, _p, _p, _d, _d, _d, _d, _i, _i, _d, _d,
+                                  _p, _p, _p, _p, _p]),
 }
 
 _lock = threading.Lock()

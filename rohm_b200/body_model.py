@@ -199,6 +199,19 @@ def kernels_for(model, device, frames, with_vertices):
     return k
 
 
+def load_faces(path):
+    """The SMPL-X triangles [F,3] (int64) of a model file: ``f`` of ``SMPLX_NEUTRAL.npz``, or of
+    ``<path>/smplx/SMPLX_NEUTRAL.npz`` for the directory ``BodyModel.create`` takes.  They are not a ``BodyModel`` buffer,
+    so checkpoints keep their state-dict keys."""
+    npz = path if os.path.isfile(path) else os.path.join(path, 'smplx', 'SMPLX_NEUTRAL.npz')
+    if not os.path.exists(npz):
+        raise RohmB200Error(f"load_faces: {npz} not found")
+    f = np.asarray(np.load(npz, allow_pickle=True)['f'], dtype=np.int64)
+    if f.ndim != 2 or f.shape[1] != 3:
+        raise RohmB200Error(f"load_faces: {npz}: 'f' must be [F,3], got {f.shape}")
+    return f
+
+
 class BodyModel(nn.Module):
     NUM_JOINTS = 55
     NUM_BODY_JOINTS = 21

@@ -4,7 +4,7 @@
 
 #include "common.h"
 
-extern "C" int rohm_version(void) { return 108; }
+extern "C" int rohm_version(void) { return 109; }
 
 extern "C" int rohm_ctx_create(int device, rohm_ctx** out) {
   if (out == nullptr) return ROHM_ERR_INVALID;

@@ -129,13 +129,7 @@ def pipeline_batches(B, seed, ds_pose, frames=144, device="cpu"):
     return pose, traj
 
 
-def smplx_like_model(seed=0, num_verts=10475, dtype=torch.float32):
-    """A synthetic body model with SMPL-X's exact tensor shapes, kinematic tree and sparsity pattern:
-    v_template [V,3], shapedirs [V,3,20], posedirs [486, V*3], J_regressor [55,V] (sparse rows, convex weights),
-    lbs_weights [V,55] (<= 4 bones per vertex, convex), parents[55].  NOT the licensed SMPL-X data."""
-    g = torch.Generator(device="cpu")
-    g.manual_seed(int(seed))
-    J, V = 55, int(num_verts)
+def _rest_and_owner(g, J, V):
     # rest joints: a random tree embedding with bone lengths ~10-25 cm
     rest = torch.zeros(J, 3)
     for j in range(1, J):
@@ -144,6 +138,38 @@ def smplx_like_model(seed=0, num_verts=10475, dtype=torch.float32):
     # every vertex belongs to a primary bone and lies near it
     owner = torch.randint(0, J, (V,), generator=g)
     owner[:J] = torch.arange(J)
+    return rest, owner
+
+
+def smplx_like_faces(seed=0, num_faces=20908, num_verts=10475):
+    """SMPL-X's triangle count [num_faces, 3] (int64) over the vertices of ``smplx_like_model(seed)``: each triangle joins
+    three distinct vertices of one bone (the model orders its vertices by bone), so every surface stays local to a bone
+    as a real mesh's does.  Bones get triangles in proportion to their vertex counts.  NOT the SMPL-X topology."""
+    g = torch.Generator(device="cpu")
+    g.manual_seed(int(seed))
+    J, V = 55, int(num_verts)
+    _, owner = _rest_and_owner(g, J, V)
+    counts = np.bincount(owner.numpy(), minlength=J)
+    start = np.concatenate([[0], np.cumsum(counts)])
+    rng = np.random.RandomState(int(seed))
+    usable = np.nonzero(counts >= 3)[0]
+    share = np.floor(num_faces * counts[usable] / counts[usable].sum()).astype(np.int64)
+    share[:num_faces - int(share.sum())] += 1
+    faces = []
+    for j, n in zip(usable, share):
+        for _ in range(int(n)):
+            faces.append(start[j] + rng.choice(counts[j], 3, replace=False))
+    return np.asarray(faces, np.int64).reshape(-1, 3)
+
+
+def smplx_like_model(seed=0, num_verts=10475, dtype=torch.float32):
+    """A synthetic body model with SMPL-X's exact tensor shapes, kinematic tree and sparsity pattern:
+    v_template [V,3], shapedirs [V,3,20], posedirs [486, V*3], J_regressor [55,V] (sparse rows, convex weights),
+    lbs_weights [V,55] (<= 4 bones per vertex, convex), parents[55].  NOT the licensed SMPL-X data."""
+    g = torch.Generator(device="cpu")
+    g.manual_seed(int(seed))
+    J, V = 55, int(num_verts)
+    rest, owner = _rest_and_owner(g, J, V)
     v_template = rest[owner] + 0.05 * torch.randn(V, 3, generator=g)
     # skinning weights are spatially local in SMPL-X: a vertex is driven by its primary bone and that bone's
     # neighbours in the kinematic tree (parent, grand-parent, a child) -- not by arbitrary bones
