@@ -59,12 +59,13 @@ class LossType(enum.Enum):
         return self == LossType.KL or self == LossType.RESCALED_KL
 
 
-# Guidance schedule hard-coded by the reference (p_sample_with_grad, gaussian_diffusion_posenet.py:461-477):
+# Guidance schedule hard-coded by the reference (p_sample_with_grad, gaussian_diffusion_posenet.py:461-477), as
+# (denoiser hook, weight, last respaced step index it applies on):
 #   'amass': skating guidance, weight 3e6, on respaced step indices t <= 50
 #   'prox' : 2-D reprojection guidance weight 3e5 then skating guidance weight 1e5, both on t <= 100
 _GUIDANCE = {
-    'amass': (('skating', 3e6, 50),),
-    'prox': (('projection', 3e5, 100), ('skating', 1e5, 100)),
+    'amass': (('guide_skating_with_smpl', 3e6, 50),),
+    'prox': (('guide_2d_projection_with_smpl', 3e5, 100), ('guide_skating_with_smpl', 1e5, 100)),
 }
 
 
@@ -234,7 +235,6 @@ class _GaussianDiffusion:
     def _wrap_model(self, model):
         return model  # the respaced subclasses wrap the denoiser so that it sees original timesteps
 
-    # ------------------------------------------------------------------ fused step (one launch per step)
     def _noise_in_kernel(self, x):
         """The noise may be drawn inside the update kernel when it comes from torch's own CUDA generator (bit-identical
         stream, see ops.ddpm_step_philox); an injected noise source (tests, sharded parity noise) keeps the explicit tensor."""
@@ -248,11 +248,7 @@ class _GaussianDiffusion:
         """The per-clip lengths the draws of a [B, ...] batch follow (the denoiser's check of batch['lengths']), or None."""
         if batch.get('lengths') is None:
             return None
-        inner = model.model if isinstance(model, _WrappedModel) else model
-        if self._POSENET:
-            return inner.clip_lengths(batch, shape)
-        from .trajnet_engine import clip_lengths
-        return clip_lengths(batch, shape)
+        return _inner(model).clip_lengths(batch, shape)
 
     def _open_streams(self, batch, shape, device, const_noise=False):
         """NoiseStreams of batch['generators'] after the validator's checks, or None without the key."""
@@ -270,7 +266,10 @@ class _GaussianDiffusion:
             return ls[1], False
         return self._open_streams(batch, x.shape, x.device, const_noise), True
 
-    def _randn_clips(self, model, batch, x, streams):
+    def _draw_noise(self, model, batch, x, streams):
+        """An explicit noise tensor like x: each clip's draw from its stream, else self._randn_like."""
+        if streams is None:
+            return self._randn_like(x)
         return ops.randn_clips(streams, x.shape, self._channels_last(), self._draw_lengths(model, batch, x.shape),
                                device=x.device)
 
@@ -281,40 +280,69 @@ class _GaussianDiffusion:
             return self._dev(t.device)["coef"][int(step_index)]
         return self._coef_for(t)
 
-    def _fused_posenet_step(self, model, batch, x, t, step_index, model_kwargs, streams=None):
-        """PoseNet, unguided step, noise from torch's generator (or the per-clip streams), no model kwargs: forward + update
-        as ONE graph launch."""
-        if not (self._POSENET and step_index is not None and not model_kwargs and self._noise_in_kernel(x)):
-            return None
-        model = self._wrap_model(model)  # respaced schedules: step index -> original timestep
-        inner = model.model if isinstance(model, _WrappedModel) else model
-        prep = getattr(inner, "prepare_cond", None)
-        if prep is None or x.dim() != 4 or self.rescale_timesteps or t.is_floating_point():
-            return None
-        x = x if (x.is_contiguous() and x.dtype == th.float32) else x.contiguous().float()
-        batch['x_t'] = x
-        ts = model.map_timesteps(t) if isinstance(model, _WrappedModel) else t
-        e = prep(batch['cond'], inner.clip_lengths(batch, x.shape))
-        x0, nxt = e.sample_step(x, ts.to(th.int64).contiguous(), self._coef_row(t, step_index), streams=streams)
-        return {"sample": nxt, "pred_xstart": x0, "x_t": x}
+    # ------------------------------------------------------------------ one ancestral step
+    def _step(self, model, batch, x, t, step_index, streams, terms=(), cond_fn=None, const_noise=False,
+              model_kwargs=None):
+        """x_{t-1} = coef1[t] x0 + coef2[t] x_t (+ guidance) + (t != 0) exp(0.5 logvar[t]) noise, x0 = model(batch | x_t, t)
+        -> {'sample', 'pred_xstart', 'x_t'}.  Decides, in this order:
 
-    def _fused_trajnet_step(self, model, batch, x, t, step_index, model_kwargs, streams=None):
-        """TrajNet, step without cond_fn, noise from torch's generator, no model kwargs: forward + update as ONE graph launch
-        (rohm_trajnet_sample_step); the same arithmetic and the same noise as the separate launches below."""
-        if self._POSENET or step_index is None or model_kwargs or not self._noise_in_kernel(x):
-            return None
-        model = self._wrap_model(model)  # respaced schedules: step index -> original timestep
-        inner = model.model if isinstance(model, _WrappedModel) else model
-        if not hasattr(inner, "traj_feat_dim") or not hasattr(inner, "_engine") or x.dim() != 3 or self.rescale_timesteps or \
-                t.is_floating_point():
-            return None
-        from .trajnet_engine import prepare
-        batch['x_t'] = x
-        ts = model.map_timesteps(t) if isinstance(model, _WrappedModel) else t
-        e, xc, tsc = prepare(inner, batch, ts)
-        batch['x_t'] = xc
-        x0, nxt = e.sample_step(xc, tsc, self._coef_row(t, step_index), streams=streams)
-        return {"sample": nxt, "pred_xstart": x0, "x_t": xc}
+        1. the fused step: the denoiser's forward and the update as ONE graph launch (engine.sample_step), when there are
+           no guidance terms, no cond_fn, no const_noise and no model kwargs, the step index is known to the host, the
+           noise is drawn in the kernel (_noise_in_kernel), t holds integer step indices that are not rescaled, and the
+           denoiser has prepare().  The same arithmetic and the same noise as the separate launches below;
+        2. otherwise the denoiser call, then the noise: drawn inside the update kernel from torch's generator or from the
+           per-clip streams, or an explicit tensor when the noise source is replaced, _FUSED_STEP is off, const_noise is
+           on (clip 0's noise for every clip) or a cond_fn is given;
+        3. guidance: `terms` are (hook, weight) pairs; hook k's gradient w.r.t. pred_xstart enters the update scaled by
+           the fp32 product weight * variance[t] (coefficient column 3 + k), as the reference forms it.  A 0-dim gradient
+           ("nothing skates") adds nothing;
+        4. one update launch.  A TrajNet cond_fn instead shifts the posterior mean by condition_mean (reference
+           gaussian_diffusion_trajnet.py:433-436); a PoseNet cond_fn is not applied, as in the reference's p_sample."""
+        if (not terms and cond_fn is None and not const_noise and not model_kwargs and step_index is not None and
+                self._noise_in_kernel(x) and not t.is_floating_point() and not self.rescale_timesteps):
+            wrapped = self._wrap_model(model)  # respaced schedules: step index -> original timestep
+            prepare = getattr(_inner(wrapped), "prepare", None)
+            if prepare is not None:
+                batch['x_t'] = x
+                e, x, ts = prepare(batch, wrapped.map_timesteps(t) if isinstance(wrapped, _WrappedModel) else t)
+                batch['x_t'] = x
+                x0, nxt = e.sample_step(x, ts, self._coef_row(t, step_index), streams=streams)
+                return {"sample": nxt, "pred_xstart": x0, "x_t": x}
+        x, x0 = self._denoise(model, batch, x, t, model_kwargs)
+        noise = None
+        if const_noise or cond_fn is not None or not self._noise_in_kernel(x):
+            noise = self._draw_noise(model, batch, x, streams)
+            if const_noise:
+                noise = noise[[0]].repeat(x.shape[0], *([1] * (x.dim() - 1)))
+        if cond_fn is not None and not self._POSENET:
+            mean, var, logvar = self.q_posterior_mean_variance(x0, x, t)
+            out = {"mean": mean, "variance": var, "log_variance": logvar, "pred_xstart": x0}
+            mean = self.condition_mean(cond_fn, out, x, t, model_kwargs=model_kwargs)
+            nonzero = (t != 0).float().view(-1, *([1] * (x.dim() - 1)))
+            sample = mean + nonzero * th.exp(0.5 * logvar) * noise
+            return {"sample": sample, "pred_xstart": x0, "x_t": x}
+        coef = self._coef_row(t, step_index)
+        grads, scales = [], []
+        for hook, weight in terms:
+            g = hook(batch, {"pred_xstart": x0}, t, compute_grad='x_0')
+            if g.dim() != 0:
+                grads.append(g.contiguous().float())
+                scales.append(weight)
+        if grads:
+            coef = coef.expand(x.shape[0], -1) if coef.dim() == 1 else coef
+            var = coef[:, 3].clone()
+            coef = coef.clone()
+            for k, w in enumerate(scales):
+                coef[:, 3 + k] = w * var  # fp32 product weight * variance[t], as the reference forms it
+        grads = tuple(grads)
+        if noise is not None:
+            sample = ops.ddpm_step(x0, x, noise, coef, grads=grads)
+        elif streams is not None:
+            sample = ops.ddpm_step_philox_clips(x0, x, coef, streams, self._channels_last(),
+                                                self._draw_lengths(model, batch, x.shape), grads=grads)
+        else:
+            sample = ops.ddpm_step_philox(x0, x, coef, grads=grads)
+        return {"sample": sample, "pred_xstart": x0, "x_t": x}
 
     def p_sample(self, model, batch, x, t, clip_denoised=True, denoised_fn=None, cond_fn=None, model_kwargs=None,
                  const_noise=False, _step_index=None):
@@ -323,110 +351,27 @@ class _GaussianDiffusion:
         (rohm_b200.noise_streams)."""
         streams, owned = self._step_streams(batch, x, const_noise)
         try:
-            return self._p_sample(model, batch, x, t, cond_fn, model_kwargs, const_noise, _step_index, streams)
+            return self._step(model, batch, x, t, _step_index, streams, cond_fn=cond_fn, const_noise=const_noise,
+                              model_kwargs=model_kwargs)
         finally:
             if owned:
                 streams.close()
-
-    def _p_sample(self, model, batch, x, t, cond_fn, model_kwargs, const_noise, _step_index, streams):
-        if cond_fn is None and not const_noise:
-            fused = self._fused_posenet_step(model, batch, x, t, _step_index, model_kwargs, streams)
-            if fused is None:
-                fused = self._fused_trajnet_step(model, batch, x, t, _step_index, model_kwargs, streams)
-            if fused is not None:
-                return fused
-        x, x0 = self._denoise(model, batch, x, t, model_kwargs)
-        if cond_fn is None and not const_noise and self._noise_in_kernel(x):
-            coef = self._coef_row(t, _step_index)
-            if streams is not None:
-                sample = ops.ddpm_step_philox_clips(x0, x, coef, streams, self._channels_last(),
-                                                    self._draw_lengths(model, batch, x.shape))
-            else:
-                sample = ops.ddpm_step_philox(x0, x, coef)
-            return {"sample": sample, "pred_xstart": x0, "x_t": x}
-        noise = self._randn_like(x) if streams is None else self._randn_clips(model, batch, x, streams)
-        if const_noise:
-            noise = noise[[0]].repeat(x.shape[0], *([1] * (x.dim() - 1)))
-        coef = self._coef_row(t, _step_index)
-        if cond_fn is not None and not self._POSENET:
-            # TrajNet variant only (reference _trajnet.py:433-436): mean <- condition_mean(cond_fn, ...)
-            coef = self._coef_for(t)
-            rows = coef.clone()
-            rows[:, 2:] = 0
-            mean = ops.ddpm_step(x0, x, x0, rows)
-            var = self._extract("posterior_variance", t, x.shape)
-            logvar = self._extract("posterior_log_variance_clipped", t, x.shape)
-            out = {"mean": mean, "variance": var, "log_variance": logvar, "pred_xstart": x0}
-            mean = self.condition_mean(cond_fn, out, x, t, model_kwargs=model_kwargs)
-            nonzero = (t != 0).float().view(-1, *([1] * (x.dim() - 1)))
-            sample = mean + nonzero * th.exp(0.5 * logvar) * noise
-            return {"sample": sample, "pred_xstart": x0, "x_t": x}
-        sample = ops.ddpm_step(x0, x, noise, coef)
-        return {"sample": sample, "pred_xstart": x0, "x_t": x}
 
     def p_sample_with_grad(self, model, batch, x, t, clip_denoised=True, denoised_fn=None, cond_fn=None, grad_type=None,
                            model_kwargs=None, const_noise=False, _step_index=None):
-        """PoseNet: p_sample plus the hard-coded test-time guidance schedule; TrajNet: identical to p_sample without
-        const_noise / cond_fn (the reference's TrajNet variant contains no guidance).  batch['generators']: as p_sample."""
+        """PoseNet: p_sample plus the hard-coded test-time guidance schedule _GUIDANCE[grad_type] (an unknown grad_type
+        applies none, as in the reference); TrajNet: p_sample without guidance.  The update ignores cond_fn and
+        const_noise, as the reference's does; const_noise with batch['generators'] is still refused."""
         streams, owned = self._step_streams(batch, x, const_noise)
         try:
-            return self._p_sample_with_grad(model, batch, x, t, cond_fn, grad_type, model_kwargs, const_noise, _step_index,
-                                            streams)
+            terms = ()
+            if grad_type in _GUIDANCE:
+                step = int(t[0]) if _step_index is None else int(_step_index)  # the reference syncs on t[0] every step
+                terms = [(getattr(model, hook), weight) for hook, weight, last in _GUIDANCE[grad_type] if step <= last]
+            return self._step(model, batch, x, t, _step_index, streams, terms, model_kwargs=model_kwargs)
         finally:
             if owned:
                 streams.close()
-
-    def _p_sample_with_grad(self, model, batch, x, t, cond_fn, grad_type, model_kwargs, const_noise, _step_index, streams):
-        step = None if _step_index is None else int(_step_index)
-        guided_now = (self._POSENET and grad_type in _GUIDANCE and
-                      (step is None or any(step <= last for _, _, last in _GUIDANCE[grad_type])))
-        if not guided_now:
-            fused = self._fused_posenet_step(model, batch, x, t, _step_index, model_kwargs, streams)
-            if fused is None and cond_fn is None and not const_noise:
-                fused = self._fused_trajnet_step(model, batch, x, t, _step_index, model_kwargs, streams)
-            if fused is not None:
-                return fused
-        x, x0 = self._denoise(model, batch, x, t, model_kwargs)
-        in_kernel = self._noise_in_kernel(x)
-        if in_kernel:
-            noise = None
-        else:
-            noise = self._randn_like(x) if streams is None else self._randn_clips(model, batch, x, streams)
-        coef = self._coef_row(t, _step_index)
-        if coef.dim() == 1:
-            coef = coef.unsqueeze(0).expand(x.shape[0], -1)  # guidance scales are written per clip below
-        grads = []
-        if self._POSENET and grad_type in _GUIDANCE:
-            step = int(t[0]) if _step_index is None else _step_index  # the reference syncs on t[0] every step
-            out = {"pred_xstart": x0}
-            scales = []
-            for kind, weight, last_step in _GUIDANCE[grad_type]:
-                if step > last_step:
-                    continue
-                if kind == 'skating':
-                    g = model.guide_skating_with_smpl(batch, out, t, compute_grad='x_0')
-                else:
-                    g = model.guide_2d_projection_with_smpl(batch, out, t, compute_grad='x_0')
-                if g.dim() == 0:  # "nothing skates": the reference adds weight*variance*0
-                    continue
-                grads.append(g.contiguous().float())
-                scales.append(weight)
-            if grads:
-                var = coef[:, 3].clone()
-                coef = coef.clone()
-                for k, w in enumerate(scales):
-                    coef[:, 3 + k] = w * var  # fp32 product weight * variance[t], as the reference forms it
-        elif grad_type is not None and self._POSENET:
-            pass  # unknown grad_type: the reference silently applies no guidance
-        coef = coef.contiguous()
-        if in_kernel and streams is not None:
-            sample = ops.ddpm_step_philox_clips(x0, x, coef, streams, self._channels_last(),
-                                                self._draw_lengths(model, batch, x.shape), grads=tuple(grads))
-        elif in_kernel:
-            sample = ops.ddpm_step_philox(x0, x, coef, grads=tuple(grads))
-        else:
-            sample = ops.ddpm_step(x0, x, noise, coef, grads=tuple(grads))
-        return {"sample": sample, "pred_xstart": x0, "x_t": x}
 
     # ------------------------------------------------------------------ loops
     def _begin_loop(self, model, grad_type=None, batch=None, shape=None, device=None, const_noise=False):
@@ -435,7 +380,7 @@ class _GaussianDiffusion:
         denoiser steps are spent (the reference would fail, or silently do nothing, at the first guided step), per-clip
         lengths and generators included.  Returns the loop's NoiseStreams with batch['generators'] (the caller closes
         them when the loop ends), else None."""
-        inner = model.model if isinstance(model, _WrappedModel) else model
+        inner = _inner(model)
         if grad_type is not None and self._POSENET and hasattr(inner, "guidance_per_clip"):
             inner.guidance_per_clip()  # a bad guidance_normaliser, or 'clip' with global_guidance
         if not self._POSENET and hasattr(inner, "batch_invariant"):
@@ -445,17 +390,13 @@ class _GaussianDiffusion:
             inner.clip_lengths(batch, shape, grad_type=grad_type)
         streams = None
         if batch is not None and batch.get('generators') is not None:
-            if batch.get('lengths') is not None and not self._POSENET:
-                from .trajnet_engine import clip_lengths
-                clip_lengths(batch, shape)
             from .noise_streams import check_generators
             check_generators(batch, shape[0], device, diffusion=self, const_noise=const_noise)
         inv = getattr(inner, "invalidate_cond", None)
         if inv is not None:
             inv()
         if grad_type is not None and self._POSENET and grad_type in _GUIDANCE:
-            for kind, _, _ in _GUIDANCE[grad_type]:
-                hook = 'guide_skating_with_smpl' if kind == 'skating' else 'guide_2d_projection_with_smpl'
+            for hook, _, _ in _GUIDANCE[grad_type]:
                 if not hasattr(inner, hook):
                     raise RohmB200Error(f"grad_type={grad_type!r} needs model.{hook}")
         tmap = getattr(self, "timestep_map", None)
@@ -484,6 +425,36 @@ class _GaussianDiffusion:
             return ops.randn_clips(streams, shape, self._channels_last(), self._draw_lengths(model, batch, shape),
                                    device=device)
         return self._randn(*shape, device=device)
+
+    def _loop(self, model, batch, shape, noise, device, progress, skip_timesteps, init_image, step, grad_type=None,
+              const_noise=False, early_stop=False):
+        """The loop structure the ancestral and DDIM samplers share: x_T (or init_image noised to the first step), then
+        step(x, t, i) -> out from i = T-1 - skip_timesteps down to 0 (the first 980 steps with early_stop), yielding each
+        out and continuing from out['sample']."""
+        if device is None:
+            device = next(model.parameters()).device
+        assert isinstance(shape, (tuple, list))
+        streams = self._begin_loop(model, grad_type, batch, shape, device, const_noise)
+        try:
+            img = self._initial_noise(model, batch, shape, device, noise, streams)
+            if skip_timesteps and init_image is None:
+                init_image = th.zeros_like(img)
+            indices = list(range(self.num_timesteps - skip_timesteps))[::-1]
+            t_rows = self._t_rows(shape[0], device)
+            if init_image is not None:
+                img = self.q_sample(init_image, t_rows[indices[0]], img)
+            if early_stop:
+                indices = indices[0:980]
+            if progress:
+                from tqdm.auto import tqdm
+                indices = tqdm(indices)
+            for i in indices:
+                with th.no_grad():
+                    out = step(img, t_rows[i], i)
+                    yield out
+                    img = out["sample"]
+        finally:
+            self._end_loop(streams)
 
     def p_sample_loop(self, model, batch, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
                       model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
@@ -523,45 +494,14 @@ class _GaussianDiffusion:
                                   init_image=None, randomize_class=False, cond_fn_with_grad=False, grad_type=None,
                                   early_stop=False, const_noise=False):
         """Generator over the per-step dicts, from t = T-1 down to 0 (or the first 980 steps with early_stop)."""
-        if device is None:
-            device = next(model.parameters()).device
-        assert isinstance(shape, (tuple, list))
-        streams = self._begin_loop(model, grad_type if cond_fn_with_grad else None, batch, shape, device, const_noise)
-        try:
-            img = self._initial_noise(model, batch, shape, device, noise, streams)
-            if skip_timesteps and init_image is None:
-                init_image = th.zeros_like(img)
-            indices = list(range(self.num_timesteps - skip_timesteps))[::-1]
-            t_rows = self._t_rows(shape[0], device)
-            if init_image is not None:
-                img = self.q_sample(init_image, t_rows[indices[0]], img)
-            if early_stop:
-                indices = indices[0:980]
-            if progress:
-                from tqdm.auto import tqdm
-                indices = tqdm(indices)
-            for i in indices:
-                t = t_rows[i]
-                with th.no_grad():
-                    if cond_fn_with_grad:
-                        if self._POSENET:
-                            out = self.p_sample_with_grad(model, batch, img, t, clip_denoised=clip_denoised,
-                                                          denoised_fn=denoised_fn, cond_fn=cond_fn, grad_type=grad_type,
-                                                          model_kwargs=model_kwargs, const_noise=const_noise,
-                                                          _step_index=i)
-                        else:
-                            out = self.p_sample_with_grad(model, batch, img, t, clip_denoised=clip_denoised,
-                                                          denoised_fn=denoised_fn, cond_fn=cond_fn,
-                                                          model_kwargs=model_kwargs, const_noise=const_noise,
-                                                          _step_index=i)
-                    else:
-                        out = self.p_sample(model, batch, img, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
-                                            cond_fn=cond_fn, model_kwargs=model_kwargs, const_noise=const_noise,
-                                            _step_index=i)
-                    yield out
-                    img = out["sample"]
-        finally:
-            self._end_loop(streams)
+        sample_fn = self.p_sample_with_grad if cond_fn_with_grad else self.p_sample
+        kw = dict(grad_type=grad_type) if cond_fn_with_grad and self._POSENET else {}
+        yield from self._loop(
+            model, batch, shape, noise, device, progress, skip_timesteps, init_image,
+            lambda x, t, i: sample_fn(model, batch, x, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
+                                      cond_fn=cond_fn, model_kwargs=model_kwargs, const_noise=const_noise,
+                                      _step_index=i, **kw),
+            grad_type if cond_fn_with_grad else None, const_noise, early_stop)
 
     # ------------------------------------------------------------------ DDIM
     # The reference's ddim_* methods cannot run (they call p_mean_variance without `batch`, and eval_losses never
@@ -573,7 +513,7 @@ class _GaussianDiffusion:
         streams, owned = self._step_streams(batch, x)
         try:
             x, x0 = self._denoise(model, batch, x, t, model_kwargs)
-            noise = self._randn_like(x) if streams is None else self._randn_clips(model, batch, x, streams)
+            noise = self._draw_noise(model, batch, x, streams)
         finally:
             if owned:
                 streams.close()
@@ -601,30 +541,10 @@ class _GaussianDiffusion:
     def ddim_sample_loop_progressive(self, model, batch, shape, noise=None, clip_denoised=True, denoised_fn=None,
                                      cond_fn=None, model_kwargs=None, device=None, progress=False, eta=0.0,
                                      skip_timesteps=0, init_image=None, randomize_class=False, cond_fn_with_grad=False):
-        if device is None:
-            device = next(model.parameters()).device
-        assert isinstance(shape, (tuple, list))
-        streams = self._begin_loop(model, batch=batch, shape=shape, device=device)
-        try:
-            img = self._initial_noise(model, batch, shape, device, noise, streams)
-            if skip_timesteps and init_image is None:
-                init_image = th.zeros_like(img)
-            indices = list(range(self.num_timesteps - skip_timesteps))[::-1]
-            t_rows = self._t_rows(shape[0], device)
-            if init_image is not None:
-                img = self.q_sample(init_image, t_rows[indices[0]], img)
-            if progress:
-                from tqdm.auto import tqdm
-                indices = tqdm(indices)
-            for i in indices:
-                with th.no_grad():
-                    out = self.ddim_sample(model, batch, img, t_rows[i], clip_denoised=clip_denoised,
-                                           denoised_fn=denoised_fn, cond_fn=cond_fn, model_kwargs=model_kwargs, eta=eta,
-                                           _step_index=i)
-                    yield out
-                    img = out["sample"]
-        finally:
-            self._end_loop(streams)
+        yield from self._loop(
+            model, batch, shape, noise, device, progress, skip_timesteps, init_image,
+            lambda x, t, i: self.ddim_sample(model, batch, x, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
+                                             cond_fn=cond_fn, model_kwargs=model_kwargs, eta=eta, _step_index=i))
 
     # ------------------------------------------------------------------ entry points used by the drivers
     def training_losses(self, *a, **k):
@@ -633,7 +553,7 @@ class _GaussianDiffusion:
 
     def _sample_for_eval(self, model, batch, shape, progress, clip_denoised, cond_fn_with_grad, timestep_respacing,
                          grad_type=None, early_stop=False):
-        inner = model.model if isinstance(model, _WrappedModel) else model
+        inner = _inner(model)
         if isinstance(timestep_respacing, str) and timestep_respacing.startswith('ddim'):
             # the branch the reference left commented out (:949-952); it has no guidance / early-stop variant, so asking
             # for them is an error rather than a silently unguided run
@@ -665,7 +585,7 @@ class GaussianDiffusionPoseNet(_GaussianDiffusion):
         _refuse_losses_with_lengths(batch, compute_loss)
         model_output = self._sample_for_eval(model, batch, shape, progress, clip_denoised, cond_fn_with_grad,
                                              timestep_respacing, grad_type=grad_type, early_stop=early_stop)
-        inner = model.model if isinstance(model, _WrappedModel) else model
+        inner = _inner(model)
         loss_dict = inner.compute_losses_with_smpl(batch, model_output, smplx_model, epoch) if compute_loss else None
         return loss_dict, model_output
 
@@ -698,7 +618,7 @@ class GaussianDiffusionTrajNet(_GaussianDiffusion):
         _refuse_losses_with_lengths(batch, compute_loss)
         model_output = self._sample_for_eval(model, batch, shape, progress, clip_denoised, cond_fn_with_grad,
                                              timestep_respacing)
-        inner = model.model if isinstance(model, _WrappedModel) else model
+        inner = _inner(model)
         loss_dict = inner.compute_losses_with_smpl(batch, model_output, smplx_model) if compute_loss else None
         return loss_dict, model_output
 
@@ -744,6 +664,11 @@ class _WrappedModel:
     def __getattr__(self, name):
         # guidance hooks (guide_skating_with_smpl, ...) are looked up on the wrapped denoiser
         return getattr(self.__dict__["model"], name)
+
+
+def _inner(model):
+    """The denoiser behind a respacing wrapper."""
+    return model.model if isinstance(model, _WrappedModel) else model
 
 
 def _spaced(base_cls):

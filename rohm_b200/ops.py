@@ -29,31 +29,37 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
-def ddpm_step(x0, x_t, noise, coef, grads=(), out=None):
-    """out = c1*x0 + c2*x_t (+ gs_k*grad_k) + sigma*noise; coef: fp32 CUDA [8] (shared) or [B, 8] (per clip)."""
-    for n, t in (("x0", x0), ("x_t", x_t), ("noise", noise), ("coef", coef)):
+def _update_args(name, x0, x_t, coef, grads, noise=None):
+    """The checks the update wrappers share, all before any launch: -> (B, elements per clip, coef stride, grad 0,
+    grad 1).  coef is one shared row [8] (stride 0) or one row per clip [B, 8]; at most two guidance gradients."""
+    tensors = (("x0", x0), ("x_t", x_t)) + ((("noise", noise),) if noise is not None else ()) + (("coef", coef),)
+    for n, t in tensors:
         _require_cuda(n, t)
-    if not (x0.shape == x_t.shape == noise.shape):
-        raise RohmB200Error("ddpm_step: x0, x_t and noise must have the same shape")
+    if x0.shape != x_t.shape or (noise is not None and noise.shape != x0.shape):
+        raise RohmB200Error(f"{name}: {'x0, x_t and noise' if noise is not None else 'x0 and x_t'} must have the same "
+                            "shape")
     for g in grads:
         _require_cuda("grad", g)
         if g.shape != x0.shape:
-            raise RohmB200Error("ddpm_step: grad shape mismatch")
+            raise RohmB200Error(f"{name}: grad shape mismatch")
     B = x0.shape[0]
-    clip_elems = x0.numel() // max(B, 1)
     if coef.dim() == 1:
-        stride = 0
         if coef.numel() < _lib.DDPM_COEFS:
-            raise RohmB200Error("ddpm_step: coef row must hold 8 floats")
+            raise RohmB200Error(f"{name}: coef row must hold 8 floats")
+        stride = 0
+    elif coef.shape != (B, _lib.DDPM_COEFS):
+        raise RohmB200Error(f"{name}: per-clip coef must be [{B}, 8]")
     else:
-        if coef.shape != (B, _lib.DDPM_COEFS):
-            raise RohmB200Error(f"ddpm_step: per-clip coef must be [{B}, 8]")
         stride = _lib.DDPM_COEFS
+    return B, x0.numel() // max(B, 1), stride, (grads[0] if grads else None), (grads[1] if len(grads) > 1 else None)
+
+
+def ddpm_step(x0, x_t, noise, coef, grads=(), out=None):
+    """out = c1*x0 + c2*x_t (+ gs_k*grad_k) + sigma*noise; coef: fp32 CUDA [8] (shared) or [B, 8] (per clip)."""
+    B, clip_elems, stride, g0, g1 = _update_args("ddpm_step", x0, x_t, coef, grads, noise)
     if out is None:
         out = torch.empty_like(x0)
     lib, c = _lib.load(), _lib.ctx(x0.device.index)
-    g0 = grads[0] if len(grads) > 0 else None
-    g1 = grads[1] if len(grads) > 1 else None
     rc = lib.rohm_ddpm_step(c, _ptr(x0), _ptr(x_t), _ptr(noise), _ptr(g0), _ptr(g1), len(grads), _ptr(out), B,
                             clip_elems, _ptr(coef), stride, _stream(x0.device))
     _lib.check(rc, c)
@@ -69,31 +75,12 @@ def cuda_generator_state(device):
 def ddpm_step_philox(x0, x_t, coef, grads=(), out=None):
     """ddpm_step with noise = torch.randn_like(x_t) drawn inside the kernel from torch's CUDA generator (same values, same
     generator advance as the explicit call), saving the noise tensor's launch and its HBM round trip."""
-    for n, t in (("x0", x0), ("x_t", x_t), ("coef", coef)):
-        _require_cuda(n, t)
-    if x0.shape != x_t.shape:
-        raise RohmB200Error("ddpm_step_philox: x0 and x_t must have the same shape")
-    for g in grads:
-        _require_cuda("grad", g)
-        if g.shape != x0.shape:
-            raise RohmB200Error("ddpm_step_philox: grad shape mismatch")
-    B = x0.shape[0]
-    clip_elems = x0.numel() // max(B, 1)
-    if coef.dim() == 1:
-        stride = 0
-        if coef.numel() < _lib.DDPM_COEFS:
-            raise RohmB200Error("ddpm_step_philox: coef row must hold 8 floats")
-    else:
-        if coef.shape != (B, _lib.DDPM_COEFS):
-            raise RohmB200Error(f"ddpm_step_philox: per-clip coef must be [{B}, 8]")
-        stride = _lib.DDPM_COEFS
+    B, clip_elems, stride, g0, g1 = _update_args("ddpm_step_philox", x0, x_t, coef, grads)
     if out is None:
         out = torch.empty_like(x0)
     lib, c = _lib.load(), _lib.ctx(x0.device.index)
     gen, seed, offset = cuda_generator_state(x0.device)
     inc = C.c_uint64(0)
-    g0 = grads[0] if len(grads) > 0 else None
-    g1 = grads[1] if len(grads) > 1 else None
     rc = lib.rohm_ddpm_step_philox(c, _ptr(x0), _ptr(x_t), _ptr(g0), _ptr(g1), len(grads), _ptr(out), B, clip_elems,
                                    _ptr(coef), stride, seed, offset, C.byref(inc), _stream(x0.device))
     _lib.check(rc, c)
@@ -131,31 +118,14 @@ def randn_clips(streams, shape, channels_last, lengths=None, device=None):
 def ddpm_step_philox_clips(x0, x_t, coef, streams, channels_last, lengths=None, grads=(), out=None):
     """ddpm_step with noise = randn_clips(streams, x_t.shape, channels_last, lengths) drawn inside the kernel (same bits),
     and zero in every clip's padded frames."""
-    for n, t in (("x0", x0), ("x_t", x_t), ("coef", coef)):
-        _require_cuda(n, t)
-    if x0.shape != x_t.shape:
-        raise RohmB200Error("ddpm_step_philox_clips: x0 and x_t must have the same shape")
-    for g in grads:
-        _require_cuda("grad", g)
-        if g.shape != x0.shape:
-            raise RohmB200Error("ddpm_step_philox_clips: grad shape mismatch")
+    _, _, stride, g0, g1 = _update_args("ddpm_step_philox_clips", x0, x_t, coef, grads)
     B, Cc, T = _clip_layout(x0.shape, channels_last)
     if B != len(streams):
         raise RohmB200Error(f"ddpm_step_philox_clips: {len(streams)} streams for a batch of {B} clips")
-    if coef.dim() == 1:
-        stride = 0
-        if coef.numel() < _lib.DDPM_COEFS:
-            raise RohmB200Error("ddpm_step_philox_clips: coef row must hold 8 floats")
-    else:
-        if coef.shape != (B, _lib.DDPM_COEFS):
-            raise RohmB200Error(f"ddpm_step_philox_clips: per-clip coef must be [{B}, 8]")
-        stride = _lib.DDPM_COEFS
     if out is None:
         out = torch.empty_like(x0)
     draw = streams.next_draw((Cc, T, bool(channels_last), lengths))
     lib, c = _lib.load(), _lib.ctx(x0.device.index)
-    g0 = grads[0] if len(grads) > 0 else None
-    g1 = grads[1] if len(grads) > 1 else None
     rc = lib.rohm_ddpm_step_philox_clips(c, _ptr(x0), _ptr(x_t), _ptr(g0), _ptr(g1), len(grads), _ptr(out), B, Cc, T,
                                          int(bool(channels_last)), streams.lengths_c(lengths), _ptr(coef), stride,
                                          _ptr(streams.table), draw, streams.incs, _stream(x0.device))

@@ -518,6 +518,12 @@ class PoseNet(nn.Module):
         (channels [0, traj_feat_dim) are batch['cond'][:, :traj_feat_dim], the rest is the denoised pose).
         batch['lengths'] (optional, integer [bs], 1 <= lengths[b] <= T): clip b has lengths[b] real frames; those come out
         bit-identical to running the clip alone, later frames come out zero and their inputs are never read."""
+        e, x, ts = self.prepare(batch, timesteps)
+        return e.forward(x, ts)
+
+    def prepare(self, batch, timesteps):
+        """forward up to the engine call: argument checks (host attribute reads), engine lookup and the step-invariant
+        condition embedding (prepare_cond) -> (engine, x_t as a contiguous fp32 tensor, timesteps as contiguous int64)."""
         x_t, cond = batch['x_t'], batch['cond']
         if x_t.dim() != 4 or x_t.shape[2] != 1 or x_t.shape != cond.shape or x_t.shape[1] != self.input_feats:
             raise RohmB200Error(f"PoseNet: expected x_t/cond of shape [B, {self.input_feats}, 1, T], got "
@@ -534,4 +540,4 @@ class PoseNet(nn.Module):
         e = self.prepare_cond(cond, lengths)
         x = x_t if (x_t.is_contiguous() and x_t.dtype == torch.float32) else x_t.contiguous().float()
         ts = timesteps.to(device=x.device, dtype=torch.int64).contiguous()
-        return e.forward(x, ts)
+        return e, x, ts

@@ -156,5 +156,10 @@ class TrajNet(nn.Module):
         time: [bs] int -> [bs, T, traj_dim] (reconstructed trajectory representation at timestep 0).
         batch['lengths'] (optional, integer [bs], multiples of 16 with 16 <= lengths[b] <= T): clip b has lengths[b] real
         frames; those depend on that clip alone, later frames come out zero and their inputs are never read."""
-        from .trajnet_engine import run_forward
-        return run_forward(self, batch, time)
+        e, x, ts = self.prepare(batch, time)
+        return e.forward(x, ts)
+
+    def prepare(self, batch, time):
+        """trajnet_engine.prepare: -> (engine, x_t as a contiguous fp32 tensor, time as contiguous int64)."""
+        from .trajnet_engine import prepare
+        return prepare(self, batch, time)

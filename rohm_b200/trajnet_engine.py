@@ -152,11 +152,6 @@ def batch_invariant(module):
     return v
 
 
-def run_forward(module, batch, time):
-    e, x_t, ts = prepare(module, batch, time)
-    return e.forward(x_t, ts)
-
-
 def prepare(module, batch, time):
     """Argument checks, engine lookup and the step-invariant condition pyramid of one denoiser call: -> (engine, x_t as a
     contiguous fp32 tensor, time as contiguous int64)."""
